@@ -95,7 +95,7 @@ def _load():
     if not os.path.exists(_LIB_PATH):
         raise ImportError(
             f"{_LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback."
+            "(nvcc, sm_90a). There is no CPU fallback."
         )
     lib = ctypes.CDLL(_LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -1,4 +1,4 @@
-"""In-tree build of libb200awq.so (nvcc, sm_100a only) and of the C oracle (gcc).  No JIT cache:
+"""In-tree build of libb200awq.so (nvcc, sm_90a only) and of the C oracle (gcc).  No JIT cache:
 the .so lands in autoawq_b200/lib/ so it travels to the GPU box with the snapshot."""
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ LIB = os.path.join(HERE, "lib", "libb200awq.so")
 SOURCES = ["cabi.cu", "dequant.cu", "gemv.cu", "gemm_tc.cu", "aux.cu", "program.cu", "moe.cu", "comm.cu"]
 HEADERS = ["common.cuh", "gemv_tile.cuh", "program_stream.cuh", "kernels.h", os.path.join(ROOT, "include", "b200awq.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

@@ -74,7 +74,7 @@ const char* b200awq_error_string(int code) {
     case B200AWQ_EUNSUPPORTED: return "shape not supported by this path";
     case B200AWQ_EWORKSPACE: return "workspace missing or too small (see b200awq_workspace_bytes)";
     case B200AWQ_ECUDA: return "CUDA error (see b200awq_last_cuda_error)";
-    case B200AWQ_EARCH: return "device is not sm_100";
+    case B200AWQ_EARCH: return "device is not sm_90";
     default: return "unknown error code";
   }
 }
@@ -125,8 +125,9 @@ int b200awq_gemm_forward(const void* x, int64_t ldx, const int32_t* qweight, con
   const bool have_ws = carve(workspace, workspace_bytes, M, N, &ws);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // M <= 8 (knob 2): the persistent TMA-ring GEMV.  At its default the threshold drops to 4 where the small-M tensor-core
-  // kernel applies: from 5 tokens on it is faster on every Llama shape (profiles/r02_tcq_sweep.json: 13 vs 20 us on
-  // 4096 x 4096, 33 vs 47 us on 4096 x 28672 at M = 8; at M = 4 the GEMV still wins on three of four shapes).
+  // kernel applies.  Measured on an H100 (400 W), the four Llama-3-8B linears of one layer take 93 us on the GEMV vs
+  // 111 us on the small-M kernel at M = 4, and 114 vs 112 us at M = 5 (4096 x 4096 alone already favours the small-M
+  // kernel from M = 3, 4096 x 28672 the GEMV up to M = 7).
   int gemv_max = knob(2);
   if (gemv_max == 8 && M > 4 && have_ws && gemm_tcq_applicable(a, ws.acc, ws.tickets)) gemv_max = 4;
   if (M <= gemv_max && M <= 8 && gemv_gemm_layout_supported(a)) {
@@ -158,8 +159,9 @@ int b200awq_gemv_forward(const void* x, int64_t ldx, const int32_t* qweight, con
   if (!x || !qweight || !scales || !qzeros || !y) return B200AWQ_EINVAL;
   GemmArgs a{x, ldx, qweight, scales, qzeros, bias, y, M, K, N, G};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the warp-per-row FHFMA kernel does M x the FMA work (7.5 us at M = 1, 35 us at M = 8 on 4096 x 4096, 135 us on
-  // 14336 x 4096): beyond two tokens the tcgen05 kernel with the GEMV-layout loader is faster (it needs K % 64 == 0)
+  // the warp-per-row fp32-FMA kernel does M x the FMA work per weight while the wgmma kernel with the GEMV-layout loader
+  // (it needs K % 64 == 0) does the same work for any M up to its token tile: the GEMV kernel serves M <= 2.  (This
+  // crossover was carried over from the kernels' earlier tuning; it has not been re-measured on H100.)
   if (M <= knob(2) && (M <= 2 || (K % 64) != 0)) return fold(gemv_gemv_layout(a, st));
   Ws ws;
   carve(workspace, workspace_bytes, M, N, &ws);
@@ -175,8 +177,8 @@ int b200awq_fast_forward(const void* x, int64_t ldx, const int16_t* qweight, con
   if (M == 0) return B200AWQ_OK;
   if (!x || !qweight || !scales || !scaled_zeros || !y) return B200AWQ_EINVAL;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the warp-per-row FHFMA kernel does M x the FMA work (measured: 10 us at M = 1, 35 us at M = 8 on 4096 x 4096,
-  // 124 us on 14336 x 4096): beyond two tokens the tcgen05 kernel with the FAST-layout loader is faster
+  // as for the GEMV layout: the warp-per-row kernel does M x the FMA work, the wgmma kernel with the FAST-layout loader
+  // does not; M <= 2 stays on the former (carried over from the earlier tuning, not re-measured on H100)
   if (M <= (knob(2) < 2 ? knob(2) : 2)) {
     FastArgs f{x, ldx, qweight, scales, scaled_zeros, bias, y, M, K, N, G};
     return fold(gemv_fast_layout(f, st));

@@ -2,8 +2,8 @@
 //
 // A row-parallel linear (o_proj / down_proj split along K, autoawq_b200/shard.py) leaves a PARTIAL fp16 [M, hidden]
 // output on every GPU; the block's result is their sum.  At decode that is 16 KB per collective, 160 collectives per
-// token for Llama-3-70B: pure latency.  ncclAllReduce inside a CUDA graph measured 22.8 us per call on 2 x B200
-// (profiles/r02_tp70b_n2.json) - 3.6 ms of a 9.9 ms step.  This kernel does the same sum in one launch of one CTA:
+// token for Llama-3-70B: pure latency, and a general collective library call inside a CUDA graph costs several of its own
+// protocol round trips per call.  This kernel does the same sum in one launch of one CTA:
 //
 //   every rank owns a SYMMETRIC buffer (cudaMalloc + CUDA IPC: each process maps all peers' buffers):
 //       inbox[2 parities][world slots][max_elems] fp16, flags[2][world] u32
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(kCommThreads, 1)
 
 // ---------------------------------------------------------------------------------------------- LL protocol
 // The flag protocol above pays for: push, CTA barrier, fence.sys, flag store, flag poll, CTA barrier, reduce - two
-// NVLink hops and two fences in sequence (8.1 us at N = 2, 11.6 us at N = 8).  Here every 8-byte word carries its own
+// NVLink hops and two fences in sequence.  Here every 8-byte word carries its own
 // validity (NCCL's LL idea): {two fp16 values, 32-bit call number}.  A rank stores such words straight into every
 // peer's slot and polls its own slots word by word until the call number matches: ONE hop, no barrier, no fence, no
 // flag.  8-byte aligned stores do not tear; 16-byte vectors (two words) are used on both sides.  Same parity

@@ -1,5 +1,5 @@
-// Shared device helpers for the B200 (sm_100a) AWQ W4A16 kernels.
-// Raw PTX wrappers only: mbarrier, TMA (cp.async.bulk[.tensor]), tcgen05 (alloc/mma/commit/ld),
+// Shared device helpers for the H100 (sm_90a) AWQ W4A16 kernels.
+// Raw PTX wrappers only: mbarrier, TMA (cp.async.bulk[.tensor]), wgmma (warpgroup MMA, descriptors),
 // int4 -> fp16 unpack tricks.  No CUTLASS/CuTe, no torch.
 #pragma once
 #include <cuda_fp16.h>
@@ -9,7 +9,7 @@
 namespace b200awq {
 
 #ifndef B200AWQ_SM_COUNT_FALLBACK
-#define B200AWQ_SM_COUNT_FALLBACK 148
+#define B200AWQ_SM_COUNT_FALLBACK 132
 #endif
 
 // ------------------------------------------------------------------------------------ misc
@@ -57,7 +57,7 @@ __device__ __forceinline__ float ldcg_f1(const void* p) {
 }
 
 // Split-K hand-off without sequentially-consistent fences (__threadfence() = fence.sc.gpu = MEMBAR.SC.GPU +
-// L1 invalidate, measured at microseconds in the GEMV tail): contributors add with relaxed REDs, synchronise
+// L1 invalidate, microseconds in the GEMV tail): contributors add with relaxed REDs, synchronise
 // on a CTA barrier, ONE thread bumps the ticket with acq_rel at gpu scope (release is cumulative over what the
 // barrier ordered before it); the thread that sees the final count acquires, and the barrier after it orders
 // the rest of the CTA.
@@ -113,11 +113,10 @@ __device__ __forceinline__ uint32_t lop3_and_or(uint32_t a, uint32_t b, uint32_t
 __device__ __forceinline__ __half2 u32_as_h2(uint32_t v) { return *reinterpret_cast<__half2*>(&v); }
 __device__ __forceinline__ uint32_t h2_as_u32(__half2 v) { return *reinterpret_cast<uint32_t*>(&v); }
 
-// f32 += f16 * f16 (exact product, single fp32 rounding); SASS: FHFMA (sm_100+)
+// f32 += f16 * f16 (exact product, single fp32 rounding).  sm_90 has no mixed-precision FMA: both fp16 operands are
+// widened (exact) and multiplied in fp32 - an fp16 x fp16 product has at most 22 significant bits, so it is exact there.
 __device__ __forceinline__ float fhfma(uint16_t a, uint16_t b, float c) {
-  float d;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(d) : "h"(a), "h"(b), "f"(c));
-  return d;
+  return fmaf(__half2float(__ushort_as_half(a)), __half2float(__ushort_as_half(b)), c);
 }
 __device__ __forceinline__ uint16_t lo16(uint32_t v) { return static_cast<uint16_t>(v & 0xffffu); }
 __device__ __forceinline__ uint16_t hi16(uint32_t v) { return static_cast<uint16_t>(v >> 16); }
@@ -208,7 +207,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------- TMA
@@ -242,73 +241,78 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
       : "memory");
 }
 
-// ------------------------------------------------------------------------------------ tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// -------------------------------------------------------------------------------------- wgmma
+// Warpgroup MMA (sm_90a): four consecutive warps, aligned to a multiple of four, issue one D[64 x N] (+)= A[64 x 16] .
+// B[16 x N] together; A and B are read from shared memory through matrix descriptors, D lives in the 128 threads'
+// registers.  Accumulator fragment of m64nNk16 (fp32): thread t of the warpgroup (warp w = t / 32, lane l) holds
+// d[4 j + r] = D[16 w + l / 4 + 8 (r / 2)][8 j + 2 (l % 4) + (r % 2)].
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued tcgen05.mma of this thread arrive on the mbarrier when complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp gets lane (base_lane + i), 32 consecutive columns
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory matrix descriptor (sm_100): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
-// version=1 [46,48) | layout type [61,64) (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// GMMA shared-memory matrix descriptor (sm_90): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | base offset [49,52)
+// (0: every stage is 1024-byte aligned) | layout type [62,64) (1 = SWIZZLE_128B).  128B-swizzled canonical layouts of
+// 16-bit elements: K-major = rows of 64 k (128 B), SBO = stride between 8-row groups; MN-major = 64-element rows along
+// MN per k, LBO = stride between 64-element MN blocks, SBO = stride between 8-k groups.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// kind::f16 instruction descriptor: D fp32, A/B fp16; majors: 0 = K-major, 1 = MN-major
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (static_cast<uint32_t>(a_mn_major) << 15) | (static_cast<uint32_t>(b_mn_major) << 16) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
+
+// D (fp32, registers) += A (fp16, smem desc) . B (fp16, smem desc); TA = 1: A is MN-major, 0: K-major; B K-major.
+template <int TA>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, 1, 1, 1, %10, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "n"(TA)
+      : "memory");
+}
+template <int TA>
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, 1, 1, 1, %18, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "n"(TA)
+      : "memory");
+}
+template <int TA>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, 1, 1, 1, %34, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "n"(TA)
+      : "memory");
+}
+template <int TA>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, 1, 1, 1, %66, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "n"(TA)
+      : "memory");
+}
+
+template <int N, int TA>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 16 || N == 32 || N == 64 || N == 128, "token tile");
+  if constexpr (N == 16) wgmma_m64n16k16<TA>(d, da, db);
+  else if constexpr (N == 32) wgmma_m64n32k16<TA>(d, da, db);
+  else if constexpr (N == 64) wgmma_m64n64k16<TA>(d, da, db);
+  else wgmma_m64n128k16<TA>(d, da, db);
 }
 
 }  // namespace b200awq

@@ -1,22 +1,21 @@
-// Tensor-core path (M > 8 tokens): Y[M, N] = X[M, K] . deq(W), fp16 x fp16 -> fp32 in TMEM (tcgen05).
+// Tensor-core path (M > 4 tokens): Y[M, N] = X[M, K] . deq(W), fp16 x fp16 -> fp32 on the warpgroup MMA (wgmma, sm_90a).
 //
-// Orientation ("swap-AB"): the MMA's M dimension is the OUTPUT-FEATURE axis n (128 per tile, the only
-// M the 1-CTA UMMA runs at full rate), the MMA's N dimension is the token axis (BT = 32..256 per tile).
-//   A operand = W^T tile [128 n x 64 k]  - produced IN-KERNEL: 4 warps read packed int4 words, dequantise
-//               in registers (bit-exact with the dequant kernel) and store fp16 into shared memory in the
-//               UMMA canonical 128B-swizzled layout (MN-major for the GEMM layout, whose words hold 8
-//               consecutive n of one k; K-major for the GEMV / GEMVFast layouts, whose words hold
-//               consecutive k of one n).
+// Orientation ("swap-AB"): the MMA's M dimension is the OUTPUT-FEATURE axis n (128 per tile = two warpgroups of
+// m64), the MMA's N dimension is the token axis (BT = 16..128 per tile).
+//   A operand = W^T tile [128 n x 64 k]  - produced IN-KERNEL: producer warps read packed int4 words, dequantise in
+//               registers (bit-exact with the dequant kernel) and store fp16 into shared memory in the 128B-swizzled
+//               canonical layout (MN-major for the GEMM layout, whose words hold 8 consecutive n of one k; K-major for
+//               the GEMV / GEMVFast layouts, whose words hold consecutive k of one n).
 //   B operand = X tile [BT tokens x 64 k], K-major, 128B swizzle, loaded by TMA (cp.async.bulk.tensor.2d).
-//   D         = [128 lanes (n) x BT columns (tokens)] fp32 in tensor memory.
-// Warp roles (448 threads): warp 0 = TMA producer, warp 1 = TMEM owner + single-thread MMA issuer,
-// warps 2..5 = epilogue (tcgen05.ld -> +bias -> fp16 -> global), warps 6.. = dequant producers (16 for the GEMM layout).
-// Pipeline: NS smem stages, one "full" mbarrier per stage (8 producer-warp arrivals + 1 TMA expect_tx),
-// one "empty" mbarrier per stage (tcgen05.commit); two TMEM accumulator buffers with tmem_full /
-// tmem_empty mbarriers, so the epilogue of one tile overlaps the main loop of the next.
+//   D         = [128 n x BT tokens] fp32 in the registers of two consumer warpgroups (64 n each), which also run the
+//               epilogue (+bias -> fp16 -> global, or the split-K reduction).
+// Warp roles (512 threads): warpgroups 0-1 = MMA + epilogue, warpgroups 2-3 = dequant producers; producer warp 0 also
+// issues the activation TMA and the L2 prefetch of the packed weights.
+// Pipeline: NS smem stages, one "full" mbarrier per stage (8 producer-warp arrivals + 1 TMA expect_tx), one "empty"
+// mbarrier per stage (8 consumer-warp arrivals once the wgmma reading the stage has retired).
 // Persistent CTAs walk (n_tile, m_tile, k_split) work items.  Split-K (only for M <= 256 and fewer tiles than SMs, where
-// the problem is HBM-bound and 148 SMs must all stream weights) reduces through fp32 atomics into the
-// caller's zeroed workspace; the last CTA of a tile rounds to fp16 and restores the zeros.
+// the problem is HBM-bound and every SM must stream weights) reduces through fp32 atomics into the caller's zeroed
+// workspace; the last CTA of a tile rounds to fp16 and restores the zeros.
 #include <cuda.h>
 
 #include <mutex>
@@ -27,9 +26,10 @@
 
 namespace b200awq {
 
-constexpr int kTileN = 128;  // output features per tile (UMMA M)
+constexpr int kTileN = 128;  // output features per tile (two m64 warpgroups)
 constexpr int kBK = 64;      // k per pipeline stage (one 128B swizzle row of fp16)
 constexpr int kAStageBytes = kTileN * kBK * 2;  // 16 KB
+constexpr uint32_t kAHalfBytes = 64 * kBK * 2;  // the 64 output features of one consumer warpgroup (either layout)
 
 struct TcParams {
   const int32_t* qweight;
@@ -47,17 +47,39 @@ struct TcParams {
   int dbg;         // small-M kernel: record phase timestamps (knob 3 == 9)
 };
 
+// Accumulators live in registers (BT / 2 fp32 per consumer thread): BT <= 128 keeps them next to the loop's addresses
+// within the 128 registers a thread of a 512-thread CTA may use.
 template <int BT>
 struct TcCfg {
   static constexpr int kXStageBytes = BT * kBK * 2;
   static constexpr int kStageBytes = kAStageBytes + kXStageBytes;
-  static constexpr int kStages = (BT >= 256) ? 4 : (BT >= 128 ? 6 : 8);
-  static constexpr int kTmemCols = 2 * (BT < 32 ? 32 : BT);  // two accumulator buffers
+  static constexpr int kStages = BT >= 128 ? 6 : 8;
   static constexpr size_t kSmemBytes = (size_t)kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 232448, "shared memory per CTA");
 };
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// A-operand descriptor of one consumer warpgroup's 64 output features at smem address `a` (see the loaders' layouts):
+// MN-major SW128 (GEMM layout): 8-k groups 1024 B apart; K-major SW128: 8-row groups 1024 B apart.  k16 steps advance the
+// start address by 2048 B (MN-major: two 8-k groups) or 32 B (K-major: inside the swizzled 128-byte row).
+template <bool kMnMajorA>
+__device__ __forceinline__ uint64_t tc_desc_a(uint32_t a) {
+  return kMnMajorA ? gmma_desc(a, 8192, 1024) : gmma_desc(a, 16, 1024);
+}
+template <bool kMnMajorA>
+__host__ __device__ constexpr uint32_t tc_a_k16_step() { return kMnMajorA ? (2048u >> 4) : (32u >> 4); }
+
+// Issues the four k16 MMAs of one 64-k stage for one warpgroup (no commit).
+template <int BT, bool kMnMajorA>
+__device__ __forceinline__ void tc_mma_stage(float (&acc)[BT / 2], uint32_t a_addr, uint32_t x_addr) {
+  const uint64_t da = tc_desc_a<kMnMajorA>(a_addr);
+  const uint64_t db = gmma_desc(x_addr, 16, 1024);
+#pragma unroll
+  for (int k16 = 0; k16 < kBK / 16; ++k16)
+    wgmma_f16<BT, kMnMajorA ? 1 : 0>(acc, da + (uint64_t)(k16 * tc_a_k16_step<kMnMajorA>()), db + (uint64_t)(k16 * (32 >> 4)));
 }
 
 // ------------------------------------------------------------------------------- A-tile producers
@@ -66,7 +88,6 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 // dequantises from registers and writes the swizzled fp16 tile: no global latency on the critical path.
 
 // GEMM layout: thread dt owns word column c = dt % 16 (8 n) and rows kk = dt/16 + 16 j, j = 0..3.
-// (A 512-thread variant with 2 rows per thread measured slower: 725 vs 838 TFLOP/s at M = 4096.)
 // NG = quantisation groups per 64-row k-step: 1 for G >= 64, 2 for G == 32 (rows < 32 / >= 32).  Keeping the
 // slot small (9 registers for NG = 1) is what allows a 6-deep register prefetch ring.
 template <int NG>
@@ -233,19 +254,19 @@ template <> struct LoaderOf<1> { using T = GemvLayoutLoader; };
 template <> struct LoaderOf<2> { using T = FastLayoutLoader; };
 
 // --------------------------------------------------------------------------------------- kernel
-// warps: 0 = TMA producer, 1 = MMA issuer / TMEM owner, 2..5 = epilogue (TMEM lane quadrant = warp % 4),
-// 6..13 = dequant producers.  Two TMEM accumulator buffers: the epilogue of tile i overlaps the main loop
-// of tile i+1.
-template <int LAYOUT>
-constexpr int tc_threads() { return 64 + 128 + LoaderOf<LAYOUT>::T::kThreads; }
+// warpgroups 0-1: consumers (wgmma on 64 output features each, accumulators in registers, epilogue); warpgroups 2-3: the
+// dequant producers (8 warps).  The producers' register ring runs ahead across tile boundaries, so the epilogue of one
+// tile overlaps the production of the next tile's first stages.
+constexpr int kTcThreads = 512;
 
 template <int BT, int LAYOUT>
-__global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmq,
                    const TcParams p) {
   using Cfg = TcCfg<BT>;
   constexpr int NS = Cfg::kStages;
-  constexpr int NPROD = LoaderOf<LAYOUT>::T::kThreads;
+  constexpr bool kMnMajorA = (LAYOUT == 0 || LAYOUT == 3);
+  static_assert(LoaderOf<LAYOUT>::T::kThreads == 256, "two producer warpgroups");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_base = smem;                                  // NS x 16 KB
@@ -253,183 +274,92 @@ __global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)NS * Cfg::kStageBytes);
   uint64_t* full = bars;            // [NS]
   uint64_t* empty = bars + NS;      // [NS]
-  uint64_t* tmem_full = bars + 2 * NS;       // [2]
-  uint64_t* tmem_empty = bars + 2 * NS + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NS + 4);
-  int* s_flag = reinterpret_cast<int*>(bars + 2 * NS + 5);
+  int* s_flag = reinterpret_cast<int*>(bars + 2 * NS);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   pdl_trigger();
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmx);
     for (int s = 0; s < NS; ++s) {
-      mbar_init(&full[s], NPROD / 32 + 1);  // one elected arrival per producer warp + the TMA expect_tx
-      mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full[b], 1);
-      mbar_init(&tmem_empty[b], 128);
+      mbar_init(&full[s], 8 + 1);  // one elected arrival per producer warp + the TMA expect_tx
+      mbar_init(&empty[s], 8);     // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int KS = p.K / kBK;  // k-steps in total
   const int n_work = p.n_tiles * p.m_tiles * p.ksplit;
 
-  if (warp == 0) {
-    // ================================================================= TMA producer (X tiles)
-    // The whole warp walks the loop and one elected lane issues (see the MMA warp below for why).
-    {
-      const bool leader = elect_one();
-      // GEMM layout: pull the packed weights of the next kL2Ahead k-steps from HBM into L2 (TMA prefetch, no
-      // smem destination) so that the producers' register prefetch only has to cover L2 latency.  Weights
-      // do not depend on the predecessor kernel: this starts before the PDL wait.
-      constexpr int kL2Ahead = 16;
-      int wp = blockIdx.x, sp = 0, sp_end = 0;
-      bool pf_valid = (LAYOUT == 0 || LAYOUT == 3) && p.has_tmq && wp < n_work;
-      auto pf_range = [&]() {
-        const int ks = wp % p.ksplit;
-        sp = (int)((int64_t)KS * ks / p.ksplit);
-        sp_end = (int)((int64_t)KS * (ks + 1) / p.ksplit);
-      };
-      auto pf_step = [&]() {
-        const int nt = wp / (p.ksplit * p.m_tiles);
-        if (leader) tma_prefetch_l2_2d(&tmq, nt * 16, sp * kBK);
-        if (++sp == sp_end) {
-          wp += gridDim.x;
-          if (wp < n_work) pf_range(); else pf_valid = false;
-        }
-      };
-      if (pf_valid) pf_range();
-      for (int i = 0; i < kL2Ahead && pf_valid; ++i) pf_step();
-      pdl_wait();  // the activations are the predecessor's output
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int ks = w % p.ksplit;
-        const int mt = (w / p.ksplit) % p.m_tiles;
-        const int s_begin = (int)((int64_t)KS * ks / p.ksplit), s_end = (int)((int64_t)KS * (ks + 1) / p.ksplit);
-        for (int s = s_begin; s < s_end; ++s) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          if (leader) {
-            mbar_arrive_expect_tx(&full[stage], Cfg::kXStageBytes);
-            tma_load_2d(x_base + (size_t)stage * Cfg::kXStageBytes, &tmx, &full[stage], s * kBK, mt * BT);
-          }
-          __syncwarp();
-          if (++stage == NS) { stage = 0; phase ^= 1; }
-          if (pf_valid) pf_step();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================================================= MMA issuer
-    // The WHOLE warp walks the loop (waits, stage bookkeeping, descriptors) and one elected lane issues, so that every
-    // operand of the tcgen05 instructions is warp-uniform for the compiler (uniform registers).  Under `if (lane == 0)`
-    // the same operands are divergent values and each UTCHMMA / UTCBAR came wrapped in an ELECT + 5 x R2UR + retry loop:
-    // ~130 instructions and ~700 clk per k-step on ONE thread, more than the 512 clk the four 128x256x16 MMAs of a
-    // k-step take (r2 ncu: tensor pipe 57 % active at M = 4096) - the issue loop, not the tensor pipe, set the pace.
-    {
-      constexpr uint32_t idesc = umma_idesc_f16(kTileN, BT, (LAYOUT == 0 || LAYOUT == 3) ? 1 : 0, 0);
-      constexpr bool kMnMajorA = (LAYOUT == 0 || LAYOUT == 3);
-      const bool leader = elect_one();
-      // MN-major, SW128: LBO = stride between 64-n atoms (8192), SBO = stride between 8-k atoms (1024); K-major SW128
-      // otherwise.  Descriptors advance by adding (byte offset >> 4) to the start-address field (smem < 256 KB: no carry).
-      const uint64_t da0 = kMnMajorA ? umma_smem_desc(smem_u32(a_base), 8192, 1024) : umma_smem_desc(smem_u32(a_base), 16, 1024);
-      const uint64_t db0 = umma_smem_desc(smem_u32(x_base), 16, 1024);
-      constexpr uint32_t kAStep = kMnMajorA ? (2048u >> 4) : (32u >> 4);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
-        const int ks = w % p.ksplit;
-        const int s_begin = (int)((int64_t)KS * ks / p.ksplit), s_end = (int)((int64_t)KS * (ks + 1) / p.ksplit);
-        const int buf = it & 1;
-        const uint32_t use = (uint32_t)(it >> 1) & 1u;
-        mbar_wait(&tmem_empty[buf], use ^ 1);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BT);
-        for (int s = s_begin; s < s_end; ++s) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t da = da0 + (uint64_t)((uint32_t)(stage * kAStageBytes) >> 4);
-          const uint64_t db = db0 + (uint64_t)((uint32_t)(stage * Cfg::kXStageBytes) >> 4);
-          if (leader) {
-#pragma unroll
-            for (int k16 = 0; k16 < kBK / 16; ++k16)
-              umma_f16_ss(d_tmem, da + (uint64_t)(k16 * kAStep), db + (uint64_t)(k16 * (32 >> 4)), idesc,
-                          (s > s_begin || k16 > 0) ? 1u : 0u);
-            umma_commit(&empty[stage]);  // frees this smem stage when the MMAs above retire
-          }
-          __syncwarp();
-          if (++stage == NS) { stage = 0; phase ^= 1; }
-        }
-        if (leader) umma_commit(&tmem_full[buf]);  // accumulator complete
-        __syncwarp();
-      }
-    }
-  } else if (warp < 6) {
-    // ================================================================= epilogue (4 warps)
-    const int et = threadIdx.x - 64;  // 0..127
-    const int q4 = warp & 3;          // TMEM lane quadrant this warp may read
-    pdl_wait();                       // outputs / workspace may alias memory the predecessor still uses
-    int it = 0;
-    for (int w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
+  if (warp < 8) {
+    // ================================================================= consumers: wgmma + epilogue (2 warpgroups)
+    const int wg = warp >> 2;
+    const int et = threadIdx.x;  // 0..255
+    const uint32_t a_s = smem_u32(a_base) + (uint32_t)wg * kAHalfBytes;
+    const uint32_t x_s = smem_u32(x_base);
+    pdl_wait();  // outputs / workspace may alias memory the predecessor still uses
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+      const int ks = w % p.ksplit;
       const int mt = (w / p.ksplit) % p.m_tiles;
       const int nt = w / (p.ksplit * p.m_tiles);
-      const int buf = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(&tmem_full[buf], use);
-      tc_fence_after();
-      const int n = nt * kTileN + q4 * 32 + lane;
-      const bool n_ok = n < p.N;
-      const float bias_v = (p.bias != nullptr && n_ok) ? __half2float(p.bias[n]) : 0.f;
-      const int m0 = mt * BT;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BT; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(buf * BT + c0), v);
-        tmem_ld_wait();
-        if (n_ok && m0 + c0 < p.M) {
+      const int s_begin = (int)((int64_t)KS * ks / p.ksplit), s_end = (int)((int64_t)KS * (ks + 1) / p.ksplit);
+      float acc[BT / 2];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int m = m0 + c0 + j;
-            if (m < p.M) {
-              const float f = __uint_as_float(v[j]);
-              if (p.ksplit == 1)
-                p.y[(int64_t)m * p.N + n] = __float2half_rn(f + bias_v);
-              else
-                atomicAdd(&p.acc_ws[(int64_t)m * p.N + n], f);
-            }
-          }
+      for (int i = 0; i < BT / 2; ++i) acc[i] = 0.f;
+      // one group of MMAs in flight: a stage is released once the group after it has been issued
+      int prev = -1;
+      for (int s = s_begin; s < s_end; ++s) {
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        tc_mma_stage<BT, kMnMajorA>(acc, a_s + (uint32_t)stage * kAStageBytes, x_s + (uint32_t)stage * Cfg::kXStageBytes);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == NS) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+      // accumulator element i of this thread: feature n_a (+8 when i & 2), token m_a + 8 (i / 4) + (i & 1)
+      const int n_a = nt * kTileN + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      const int m0 = mt * BT;
+      const int m_a = m0 + 2 * (lane & 3);
+      const float bias_a = (p.bias != nullptr && n_a < p.N) ? __half2float(p.bias[n_a]) : 0.f;
+      const float bias_b = (p.bias != nullptr && n_a + 8 < p.N) ? __half2float(p.bias[n_a + 8]) : 0.f;
+#pragma unroll
+      for (int i = 0; i < BT / 2; ++i) {
+        const int n = n_a + ((i & 2) ? 8 : 0);
+        const int m = m_a + 8 * (i >> 2) + (i & 1);
+        if (n < p.N && m < p.M) {
+          if (p.ksplit == 1)
+            p.y[(int64_t)m * p.N + n] = __float2half_rn(acc[i] + ((i & 2) ? bias_b : bias_a));
+          else
+            atomicAdd(&p.acc_ws[(int64_t)m * p.N + n], acc[i]);
         }
       }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[buf]);
       if (p.ksplit > 1) {
         __threadfence();
-        named_bar_sync(1, 128);
+        named_bar_sync(1, 256);
         if (et == 0) {
-          const int prev = atomicAdd(&p.tickets[nt * p.m_tiles + mt], 1);
-          *s_flag = (prev == p.ksplit - 1);
+          const int prev_t = atomicAdd(&p.tickets[nt * p.m_tiles + mt], 1);
+          *s_flag = (prev_t == p.ksplit - 1);
         }
-        named_bar_sync(1, 128);
+        named_bar_sync(1, 256);
         const bool last = *s_flag != 0;
-        named_bar_sync(1, 128);  // everyone has read the flag before a later item rewrites it
+        named_bar_sync(1, 256);  // everyone has read the flag before a later item rewrites it
         if (last) {
           __threadfence();
-          if (n_ok) {
-            // 16 tokens per L2 round trip (loads first, then the stores): one token at a time cost ~0.45 us each
-            for (int j0 = 0; j0 < BT && m0 + j0 < p.M; j0 += 16) {
+          // thread et finalises feature (et % 128) for the tokens of its half of every 32-token batch; 16 tokens per L2
+          // round trip (loads first, then the stores), not one round trip per token
+          const int n = nt * kTileN + (et & 127);
+          const float bias_v = (p.bias != nullptr && n < p.N) ? __half2float(p.bias[n]) : 0.f;
+          if (n < p.N) {
+            for (int j0 = 16 * (et >> 7); j0 < BT && m0 + j0 < p.M; j0 += 32) {
               float f[16];
 #pragma unroll
               for (int j = 0; j < 16; ++j) {
@@ -452,21 +382,24 @@ __global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
     }
   } else {
     // ================================================================= dequant producers (8 warps)
-    // Global loads run kPrefetch k-steps ahead of the dequantisation (register ring): a k-step is only
-    // ~500 MMA cycles, well below the DRAM / L2 latency a 1-deep prefetch would expose every step.
+    // Global loads run kPrefetch k-steps ahead of the dequantisation (register ring): a k-step is only a few hundred
+    // MMA cycles, well below the DRAM / L2 latency a 1-deep prefetch would expose every step.
     constexpr int kPrefetch = LoaderOf<LAYOUT>::T::kDepth;
-    const int dt = threadIdx.x - 192;  // 0..255
+    const int dt = threadIdx.x - 256;  // 0..255
+    const int pw = dt >> 5;            // producer warp; warp 0 also issues the activation TMA and the L2 prefetch
+    const bool leader = pw == 0 && elect_one();
     const uint32_t a_base_s = smem_u32(a_base);
     typename LoaderOf<LAYOUT>::T ring[kPrefetch];
     // The (work item, k-step) sequence of this CTA is ONE stream: the load cursor runs kPrefetch steps ahead
     // of the store cursor straight through tile boundaries, so the ring never drains between tiles.
     struct Cursor {
-      int w, s, s_end, nt;
+      int w, s, s_end, nt, mt;
       bool valid;
     };
     auto set_range = [&](Cursor& c) {
       const int ks = c.w % p.ksplit;
       c.nt = c.w / (p.ksplit * p.m_tiles);
+      c.mt = (c.w / p.ksplit) % p.m_tiles;
       c.s = (int)((int64_t)KS * ks / p.ksplit);
       c.s_end = (int)((int64_t)KS * (ks + 1) / p.ksplit);
     };
@@ -477,10 +410,19 @@ __global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
         if (c.valid) set_range(c);
       }
     };
-    Cursor L, S;
-    L.w = S.w = blockIdx.x;
+    Cursor L, S, P;
+    L.w = S.w = P.w = blockIdx.x;
     L.valid = S.valid = blockIdx.x < n_work;
-    if (L.valid) { set_range(L); set_range(S); }
+    if (L.valid) { set_range(L); set_range(S); set_range(P); }
+    // GEMM layout: pull the packed weights of the next kL2Ahead k-steps from HBM into L2 (TMA prefetch, no smem
+    // destination) so that the register prefetch only has to cover L2 latency.  Weights do not depend on the
+    // predecessor kernel: this starts before the PDL wait.
+    constexpr int kL2Ahead = 16;
+    P.valid = kMnMajorA && p.has_tmq && pw == 0 && L.valid;
+    for (int i = 0; i < kL2Ahead && P.valid; ++i) {
+      if (leader) tma_prefetch_l2_2d(&tmq, P.nt * 16, P.s * kBK);
+      advance(P);
+    }
 #pragma unroll
     for (int d = 0; d < kPrefetch; ++d) {
       ring[d].init();
@@ -489,6 +431,7 @@ __global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
         advance(L);
       }
     }
+    if (pw == 0) pdl_wait();  // the activations are the predecessor's output
     int stage = 0;
     uint32_t phase = 0;
     while (S.valid) {
@@ -496,6 +439,12 @@ __global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
       for (int d = 0; d < kPrefetch; ++d) {
         if (S.valid) {
           mbar_wait(&empty[stage], phase ^ 1);
+          if (leader) {
+            mbar_arrive_expect_tx(&full[stage], Cfg::kXStageBytes);
+            tma_load_2d(x_base + (size_t)stage * Cfg::kXStageBytes, &tmx, &full[stage], S.s * kBK, S.mt * BT);
+            if (P.valid) tma_prefetch_l2_2d(&tmq, P.nt * 16, P.s * kBK);
+          }
+          if (P.valid) advance(P);
           ring[d].store(p, S.nt, S.s * kBK, dt, a_base_s + (uint32_t)stage * kAStageBytes);
           fence_proxy_async_smem();   // every writer: generic-proxy stores -> visible to the tensor core
           __syncwarp();
@@ -510,55 +459,38 @@ __global__ void __launch_bounds__(tc_threads<LAYOUT>(), 1)
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
 }
 
 // ------------------------------------------------------------ small-M kernel (TMA-staged packed weights)
 // M <= 128 on the GEMM layout is HBM-bound; the kernel above is latency-bound there (its producers pull the packed
-// words L2 -> registers through a 6-deep ring: ~500-900 clk per k-step whatever the token count, r2 M sweep).  This
-// variant keeps the MMA / descriptor / epilogue machinery and changes what bounded it:
+// words L2 -> registers through a shallow register ring whatever the token count).  This variant keeps the MMA /
+// descriptor / epilogue machinery and changes what bounds it:
 //   * the packed weights arrive by TMA in a deep shared-memory ring, one stage = a PAIR of k-steps (128 rows x 16 words
 //     = 8 KB, plus the rows' group constants: 256 B of scales + 64 B of zeros per group), 11-14 stages = 96-123 KB in
-//     flight per SM independent of registers (a read-only probe with the same ring moves 2.5 TB/s with 64 KB in flight
-//     and 3.9 TB/s with 128 KB: profiles/r02_membw_box_shapes.log), issued by a dedicated warp that never waits for
-//     activations (weights do not depend on the predecessor kernel);
-//   * two producer teams of 8 warps: team t dequantises rows 64 t .. 64 t + 63 of every stage (conflict-free LDS, the
-//     exact arithmetic of the dequant kernel: the A tile is bit-identical), one step ahead of its own stores, into its own
-//     A stages; the activation tiles have their own ring (they come from L2 with ~1 us of latency);
-//   * the MMA / TMA issue loops are walked by the whole warp with one elected lane issuing (uniform operands);
+//     flight per SM independent of registers, issued by a dedicated warp that never waits for activations (weights do
+//     not depend on the predecessor kernel);
+//   * 8 producer warps dequantise both k-steps of every stage (conflict-free LDS, the exact arithmetic of the dequant
+//     kernel: the A tile is bit-identical) into the A stages; the activation tiles have their own ring and TMA warp
+//     (they come from L2, with its latency under load);
 //   * work is cut into CONTIGUOUS RANGES of the linearised (n-tile, k-step pair) sequence, one range per SM: every SM
-//     streams the same number of bytes whatever N / 128 is (the (tile, k-split) items of the kernel above leave
-//     224 tiles on 148 SMs two waves deep).  A range crosses at most a few n-tiles = segments; a segment that holds a
-//     whole K column stores fp16 directly, a partial one adds fp32 into the caller's zeroed workspace and bumps the
-//     tile's ticket by its number of k-step pairs; the contributor that completes K rounds, adds the bias, restores
-//     zeros.  Wherever N / 128 <= SM count (and from 64 tokens on) the ranges are tile-aligned instead: gemm_tcq_grid.
-//   * knob 22 = optional HBM -> L2 prefetch ahead of the ring: measured, no gain (profiles/r02_tcq_knob20.json).
+//     streams the same number of bytes whatever N / 128 is.  A range crosses at most a few n-tiles = segments; a
+//     segment that holds a whole K column stores fp16 directly, a partial one adds fp32 into the caller's zeroed
+//     workspace and bumps the tile's ticket by its number of k-step pairs; the contributor that completes K rounds,
+//     adds the bias, restores zeros.  Wherever N / 128 <= SM count (and from 64 tokens on) the ranges are tile-aligned
+//     instead: gemm_tcq_grid.
+//   * knob 22 = optional HBM -> L2 prefetch ahead of the ring.
 template <int BT>
 struct TcqCfg {
-  static constexpr int kNS = 4;                                            // A stages (producers -> MMA), 2 per team
-  static constexpr int kNX = BT <= 16 ? 16 : (BT == 32 ? 8 : (BT == 64 ? 8 : 4));   // X stages (TMA -> MMA), own ring
+  static constexpr int kNS = 4;                                            // A stages (producers -> MMA)
+  static constexpr int kNX = BT <= 16 ? 16 : (BT <= 64 ? 8 : 4);           // X stages (TMA -> MMA), own ring
   static constexpr int kNQ = BT <= 32 ? 14 : 11;                           // packed-weight stages (TMA -> producers)
   static constexpr int kXStageBytes = BT * kBK * 2;
-  static constexpr int kQRows = 2 * kBK;                                   // rows per packed stage: one k-step per team
+  static constexpr int kQRows = 2 * kBK;                                   // rows per packed stage: two k-steps
   static constexpr int kQTileBytes = 16 * 4 * kQRows;                      // 128 rows x 16 words = 8 KB
   static constexpr int kQStageBytes = kQTileBytes + 2 * 256 + 2 * 64 + 128;   // up to 2 groups of constants; 128-B multiple
-  static constexpr int kAccCols = BT < 32 ? 32 : BT;
-  static constexpr int kTeams = 2;
-  // One MMA-issuing warp per team, each with its own accumulator (the epilogue adds the two): the issue loop of ONE
-  // warp (two barrier waits, descriptor arithmetic on the uniform datapath, 4 MMAs, 2 commits: ~55 dependent
-  // instructions) takes ~300 ns per k-step however little the tensor pipe has to do - with every other stage removed
-  // (no dequantisation, no MMAs) the kernel still ran at that pace (profiles/r02_tcq_experiments.md).
-  static constexpr int kTmemCols = 2 * kTeams * kAccCols;                  // two buffers x one accumulator per team
-  static_assert(kTmemCols <= 512 && (kTmemCols & (kTmemCols - 1)) == 0, "TMEM allocation: power of two <= 512");
-  static constexpr int kThreads = 192 + 256 * kTeams + 64;   // X-TMA, MMA 0, 4 epilogue, 16 producer warps, Q-TMA, MMA 1
+  static constexpr int kThreads = 256 + 256 + 64;   // 2 consumer warpgroups, 8 producer warps, Q-TMA warp, X-TMA warp
   static constexpr size_t kSmemBytes = (size_t)kNS * kAStageBytes + (size_t)kNX * kXStageBytes +
                                        (size_t)kNQ * kQStageBytes + 1024 /*align slack*/ + 1024 /*barriers*/;
-  static_assert(kNS % kTeams == 0 && kNX % kTeams == 0, "team t owns A stages / X stages t, t + 2, ...");
   static_assert(kQStageBytes % 128 == 0, "TMA destination alignment");
   static_assert(kSmemBytes <= 232448, "shared memory per CTA");
 };
@@ -575,8 +507,8 @@ __device__ __forceinline__ uint4 lds_u4(uint32_t saddr) {
 }
 
 // Phase timestamps (globaltimer, ns) of the last small-M launch, 8 per CTA, written only when knob 3 == 9 (TcParams::dbg):
-// [0] entry, [1] setup done (barriers, TMEM), [2] first packed stage landed, [3] producers done, [4] MMA issuer done,
-// [5] last accumulator drained, [6] epilogue done (incl. finalisation), [7] number of segments.
+// [0] entry, [1] setup done (barriers), [2] first packed stage landed, [3] producers done, [4] MMA issue done,
+// [5] last accumulator complete, [6] epilogue done (incl. finalisation), [7] number of segments.
 __device__ unsigned long long g_tcq_dbg[256 * 8];
 __device__ __forceinline__ unsigned long long tcq_timer() {
   unsigned long long t;
@@ -599,16 +531,13 @@ __global__ void __launch_bounds__(TcqCfg<BT>::kThreads, 1)
   uint8_t* x_base = a_base + (size_t)NS * kAStageBytes;                // NX x BT*128 B
   uint8_t* q_base = x_base + (size_t)NX * Cfg::kXStageBytes;           // NQ x kQStageBytes
   uint64_t* bars = reinterpret_cast<uint64_t*>(q_base + (size_t)NQ * Cfg::kQStageBytes);
-  uint64_t* full = bars;                     // [NS]  8 producer warps (one team)
-  uint64_t* empty = full + NS;               // [NS]  tcgen05.commit
+  uint64_t* full = bars;                     // [NS]  8 producer warps
+  uint64_t* empty = full + NS;               // [NS]  8 consumer warps
   uint64_t* xfull = empty + NS;              // [NX]  expect_tx of the activation tile
-  uint64_t* xempty = xfull + NX;             // [NX]  tcgen05.commit
+  uint64_t* xempty = xfull + NX;             // [NX]  8 consumer warps
   uint64_t* qfull = xempty + NX;             // [NQ]  expect_tx of the packed stage
-  uint64_t* qempty = qfull + NQ;             // [NQ]  16 producer warps (both teams)
-  uint64_t* tmem_full = qempty + NQ;         // [2]
-  uint64_t* tmem_empty = tmem_full + 2;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  int* s_flag = reinterpret_cast<int*>(tmem_empty + 3);
+  uint64_t* qempty = qfull + NQ;             // [NQ]  8 producer warps
+  int* s_flag = reinterpret_cast<int*>(qempty + NQ);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -617,35 +546,24 @@ __global__ void __launch_bounds__(TcqCfg<BT>::kThreads, 1)
   unsigned long long* dbg_row = g_tcq_dbg + blockIdx.x * 8;
   if (dbg && threadIdx.x == 0) dbg_row[0] = tcq_timer();
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmx);
     tma_prefetch_desc(&tmq);
     for (int s = 0; s < NS; ++s) {
       mbar_init(&full[s], 8);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);
     }
     for (int s = 0; s < NX; ++s) {
       mbar_init(&xfull[s], 1);
-      mbar_init(&xempty[s], 1);
+      mbar_init(&xempty[s], 8);
     }
     for (int s = 0; s < NQ; ++s) {
       mbar_init(&qfull[s], 1);
-      mbar_init(&qempty[s], 8 * Cfg::kTeams);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full[b], Cfg::kTeams);   // one commit per MMA warp
-      mbar_init(&tmem_empty[b], 128);
+      mbar_init(&qempty[s], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (dbg && threadIdx.x == 0) dbg_row[1] = tcq_timer();
 
   // this CTA's contiguous range of the linearised (n-tile, k-step pair) sequence
@@ -653,184 +571,142 @@ __global__ void __launch_bounds__(TcqCfg<BT>::kThreads, 1)
   const long long T = (long long)p.n_tiles * KP;
   const int t_begin = (int)(T * (long long)blockIdx.x / (long long)gridDim.x);
   const int t_end = (int)(T * (long long)(blockIdx.x + 1) / (long long)gridDim.x);
-  constexpr int kQWarp = 6 + 8 * Cfg::kTeams;
+  constexpr int kQWarp = 16, kXWarp = 17;
   // groups of constants per packed stage: G = 64 -> one per k-step; G >= 128 (or one group per row) -> one per pair
   const int ng = p.g_shift == 6 ? 2 : 1;
 
   if (warp == kQWarp) {
     // ================================================================= Q-TMA: packed weights + group constants
     // (the whole warp walks the loop, one elected lane issues: uniform operands, no per-instruction retry loops)
-    {
-      const bool leader = elect_one();
-      const uint32_t NW = (uint32_t)p.N >> 3;
-      const uint32_t tx = (uint32_t)Cfg::kQTileBytes + (uint32_t)ng * 320u;
-      const int pf_ahead = p.ksplit;   // (field reused by this kernel: L2 prefetch distance in pairs)
-      int qs = 0;
-      uint32_t qph = 0;
-      for (int t = t_begin; t < t_end;) {
-        const int nt = t / KP, d0 = t - nt * KP;
-        const int d1 = (KP - d0 < t_end - t) ? KP : d0 + (t_end - t);
-        for (int d = d0; d < d1; ++d) {
-          mbar_wait(&qempty[qs], qph ^ 1);
-          uint8_t* dst = q_base + (size_t)qs * Cfg::kQStageBytes;
-          const uint32_t g = (uint32_t)(d * Cfg::kQRows) >> p.g_shift;
-          if (leader) {
-            // optional HBM -> L2 prefetch of the pair pf_ahead positions further down this CTA's range (knob 22)
-            if (pf_ahead > 0) {
-              const int tp = t + (d - d0) + pf_ahead;
-              if (tp < t_end) {
-                const int ntp = tp / KP;
-                tma_prefetch_l2_2d(&tmq, ntp * 16, (tp - ntp * KP) * Cfg::kQRows);
-              }
-            }
-            mbar_arrive_expect_tx(&qfull[qs], tx);
-            tma_load_2d(dst, &tmq, &qfull[qs], nt * 16, d * Cfg::kQRows);
-            for (int h = 0; h < ng; ++h) {
-              bulk_load_1d(dst + Cfg::kQTileBytes + h * 256, p.scales + (size_t)(g + h) * p.N + (size_t)nt * kTileN, 256,
-                           &qfull[qs]);
-              bulk_load_1d(dst + Cfg::kQTileBytes + 512 + h * 64, p.qzeros + (size_t)(g + h) * NW + (size_t)nt * 16, 64,
-                           &qfull[qs]);
+    const bool leader = elect_one();
+    const uint32_t NW = (uint32_t)p.N >> 3;
+    const uint32_t tx = (uint32_t)Cfg::kQTileBytes + (uint32_t)ng * 320u;
+    const int pf_ahead = p.ksplit;   // (field reused by this kernel: L2 prefetch distance in pairs)
+    int qs = 0;
+    uint32_t qph = 0;
+    for (int t = t_begin; t < t_end;) {
+      const int nt = t / KP, d0 = t - nt * KP;
+      const int d1 = (KP - d0 < t_end - t) ? KP : d0 + (t_end - t);
+      for (int d = d0; d < d1; ++d) {
+        mbar_wait(&qempty[qs], qph ^ 1);
+        uint8_t* dst = q_base + (size_t)qs * Cfg::kQStageBytes;
+        const uint32_t g = (uint32_t)(d * Cfg::kQRows) >> p.g_shift;
+        if (leader) {
+          // optional HBM -> L2 prefetch of the pair pf_ahead positions further down this CTA's range (knob 22)
+          if (pf_ahead > 0) {
+            const int tp = t + (d - d0) + pf_ahead;
+            if (tp < t_end) {
+              const int ntp = tp / KP;
+              tma_prefetch_l2_2d(&tmq, ntp * 16, (tp - ntp * KP) * Cfg::kQRows);
             }
           }
-          __syncwarp();
-          if (++qs == NQ) { qs = 0; qph ^= 1; }
-        }
-        t += d1 - d0;
-      }
-    }
-  } else if (warp == 0) {
-    // ================================================================= X-TMA: activation tiles, own ring (the tiles
-    // come from L2 with ~1 us of latency: tying them to the A stages made that latency the k-step time)
-    {
-      const bool leader = elect_one();
-      pdl_wait();  // the activations are the predecessor's output
-      int xs = 0;
-      uint32_t xph = 0;
-      for (int t = t_begin; t < t_end;) {
-        const int nt = t / KP, d0 = t - nt * KP;
-        const int d1 = (KP - d0 < t_end - t) ? KP : d0 + (t_end - t);
-        for (int s = 2 * d0; s < 2 * d1; ++s) {
-          mbar_wait(&xempty[xs], xph ^ 1);
-          if (leader) {
-            mbar_arrive_expect_tx(&xfull[xs], Cfg::kXStageBytes);
-            tma_load_2d(x_base + (size_t)xs * Cfg::kXStageBytes, &tmx, &xfull[xs], s * kBK, 0);
+          mbar_arrive_expect_tx(&qfull[qs], tx);
+          tma_load_2d(dst, &tmq, &qfull[qs], nt * 16, d * Cfg::kQRows);
+          for (int h = 0; h < ng; ++h) {
+            bulk_load_1d(dst + Cfg::kQTileBytes + h * 256, p.scales + (size_t)(g + h) * p.N + (size_t)nt * kTileN, 256,
+                         &qfull[qs]);
+            bulk_load_1d(dst + Cfg::kQTileBytes + 512 + h * 64, p.qzeros + (size_t)(g + h) * NW + (size_t)nt * 16, 64,
+                         &qfull[qs]);
           }
-          __syncwarp();
-          if (++xs == NX) { xs = 0; xph ^= 1; }
         }
-        t += d1 - d0;
-      }
-    }
-  } else if (warp == 1 || warp == kQWarp + 1) {
-    // ================================================================= MMA issuers (warp 1: team 0, last warp: team 1)
-    // The WHOLE warp walks the loop (waits, stage bookkeeping, descriptors) and one elected lane issues: everything the
-    // tcgen05 instructions consume is then warp-uniform for the compiler (uniform registers).  Under `if (lane == 0)`
-    // the same operands are divergent values, and every UTCHMMA / UTCBAR came wrapped in an ELECT + 5 x R2UR + retry
-    // loop: ~130 instructions and ~700 clk per k-step on ONE thread - the k-step time of the first version (ncu source
-    // page: the producers' top stall was the wait for the MMA's stage release).
-    // MMA warp w serves team w: k-step w of every pair (A stages w, w + 2; X stages w, w + 2, ...), accumulator w.
-    {
-      constexpr uint32_t idesc = umma_idesc_f16(kTileN, BT, 1, 0);
-      const int mw = warp == 1 ? 0 : 1;
-      const bool leader = elect_one();
-      const int mma_per_step = (p.dbg & 8) ? 0 : ((p.dbg & 16) ? 1 : kBK / 16);
-      const uint32_t a_base_s = smem_u32(a_base), x_base_s = smem_u32(x_base);
-      const uint64_t da0 = umma_smem_desc(a_base_s, 8192, 1024);   // MN-major SW128; start address in bits [0, 14)
-      const uint64_t db0 = umma_smem_desc(x_base_s, 16, 1024);     // K-major SW128
-      int stage = mw, xs = mw;
-      uint32_t phase = 0, xph = 0;
-      int it = 0;
-      for (int t = t_begin; t < t_end; ++it) {
-        const int nt = t / KP, d0 = t - nt * KP;
-        const int d1 = (KP - d0 < t_end - t) ? KP : d0 + (t_end - t);
-        const int buf = it & 1;
-        const uint32_t use = (uint32_t)(it >> 1) & 1u;
-        mbar_wait(&tmem_empty[buf], use ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)((buf * Cfg::kTeams + mw) * Cfg::kAccCols);
-        for (int d = d0; d < d1; ++d) {
-          mbar_wait(&xfull[xs], xph);
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          // descriptors advance by adding (byte offset >> 4) to the start-address field (no carry: smem < 256 KB)
-          const uint64_t da = da0 + (uint64_t)((uint32_t)(stage * kAStageBytes) >> 4);
-          const uint64_t db = db0 + (uint64_t)((uint32_t)(xs * Cfg::kXStageBytes) >> 4);
-          if (leader) {
-#pragma unroll
-            for (int k16 = 0; k16 < kBK / 16; ++k16)
-              if (k16 < mma_per_step)   // (4 unless a timing experiment is on: knob 20)
-                umma_f16_ss(d_tmem, da + (uint64_t)(k16 * (2048 >> 4)), db + (uint64_t)(k16 * (32 >> 4)), idesc,
-                            (d > d0 || k16 > 0) ? 1u : 0u);
-            umma_commit(&empty[stage]);
-            umma_commit(&xempty[xs]);
-          }
-          __syncwarp();
-          stage += Cfg::kTeams;
-          if (stage >= NS) { stage -= NS; phase ^= 1; }
-          xs += Cfg::kTeams;
-          if (xs >= NX) { xs -= NX; xph ^= 1; }
-        }
-        if (leader) umma_commit(&tmem_full[buf]);
         __syncwarp();
-        t += d1 - d0;
+        if (++qs == NQ) { qs = 0; qph ^= 1; }
       }
-      if (dbg && leader && mw == 0) { dbg_row[4] = tcq_timer(); dbg_row[7] = (unsigned long long)it; }
+      t += d1 - d0;
     }
-  } else if (warp < 6) {
-    // ================================================================= epilogue (4 warps)
-    const int et = threadIdx.x - 64;  // 0..127
-    const int q4 = warp & 3;          // TMEM lane quadrant this warp may read
-    pdl_wait();                       // outputs / workspace may alias memory the predecessor still uses
+  } else if (warp == kXWarp) {
+    // ================================================================= X-TMA: activation tiles, own ring
+    const bool leader = elect_one();
+    pdl_wait();  // the activations are the predecessor's output
+    int xs = 0;
+    uint32_t xph = 0;
+    for (int t = t_begin; t < t_end;) {
+      const int nt = t / KP, d0 = t - nt * KP;
+      const int d1 = (KP - d0 < t_end - t) ? KP : d0 + (t_end - t);
+      for (int s = 2 * d0; s < 2 * d1; ++s) {
+        mbar_wait(&xempty[xs], xph ^ 1);
+        if (leader) {
+          mbar_arrive_expect_tx(&xfull[xs], Cfg::kXStageBytes);
+          tma_load_2d(x_base + (size_t)xs * Cfg::kXStageBytes, &tmx, &xfull[xs], s * kBK, 0);
+        }
+        __syncwarp();
+        if (++xs == NX) { xs = 0; xph ^= 1; }
+      }
+      t += d1 - d0;
+    }
+  } else if (warp < 8) {
+    // ================================================================= consumers: wgmma + epilogue (2 warpgroups)
+    const int wg = warp >> 2;
+    const int et = threadIdx.x;  // 0..255
+    const uint32_t a_s = smem_u32(a_base) + (uint32_t)wg * kAHalfBytes;
+    const uint32_t x_s = smem_u32(x_base);
+    pdl_wait();  // outputs / workspace may alias memory the predecessor still uses
+    int stage = 0, xs = 0;
+    uint32_t phase = 0, xph = 0;
     int it = 0;
     for (int t = t_begin; t < t_end; ++it) {
       const int nt = t / KP, d0 = t - nt * KP;
       const int d1 = (KP - d0 < t_end - t) ? KP : d0 + (t_end - t);
       const bool whole = (d0 == 0 && d1 == KP);
-      const int buf = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(&tmem_full[buf], use);
-      tc_fence_after();
-      const int n = nt * kTileN + q4 * 32 + lane;   // N % 128 == 0: always in range
-      const float bias_v = p.bias != nullptr ? __half2float(p.bias[n]) : 0.f;
-      const uint32_t tbuf = tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(buf * Cfg::kTeams * Cfg::kAccCols);
-#pragma unroll 1
-      for (int c0 = 0; c0 < BT; c0 += 16) {
-        // the two teams' accumulators of 16 tokens, added in a fixed order
-        uint32_t v[16], w[16];
-        tmem_ld_32x16(tbuf + (uint32_t)c0, v);
-        tmem_ld_32x16(tbuf + (uint32_t)(Cfg::kAccCols + c0), w);
-        tmem_ld_wait();
-        if (c0 < p.M) {
+      float acc[BT / 2];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int m = c0 + j;
-            if (m < p.M) {
-              const float f = __uint_as_float(v[j]) + __uint_as_float(w[j]);
-              if (whole)
-                p.y[(int64_t)m * p.N + n] = __float2half_rn(f + bias_v);
-              else
-                red_add_f32(&p.acc_ws[(int64_t)m * p.N + n], f);
-            }
-          }
+      for (int i = 0; i < BT / 2; ++i) acc[i] = 0.f;
+      int prev = -1, prev_x = -1;
+      for (int s = 2 * d0; s < 2 * d1; ++s) {
+        mbar_wait(&xfull[xs], xph);
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        tc_mma_stage<BT, true>(acc, a_s + (uint32_t)stage * kAStageBytes, x_s + (uint32_t)xs * Cfg::kXStageBytes);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) {
+          mbar_arrive(&empty[prev]);
+          mbar_arrive(&xempty[prev_x]);
+        }
+        prev = stage;
+        prev_x = xs;
+        if (++stage == NS) { stage = 0; phase ^= 1; }
+        if (++xs == NX) { xs = 0; xph ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) {
+        mbar_arrive(&empty[prev]);
+        mbar_arrive(&xempty[prev_x]);
+      }
+      if (dbg && et == 0) dbg_row[5] = tcq_timer();
+
+      // accumulator element i of this thread: feature n_a (+8 when i & 2), token m_a + 8 (i / 4) + (i & 1)
+      const int n_a = nt * kTileN + wg * 64 + (warp & 3) * 16 + (lane >> 2);   // N % 128 == 0: always in range
+      const int m_a = 2 * (lane & 3);
+      const float bias_a = p.bias != nullptr ? __half2float(p.bias[n_a]) : 0.f;
+      const float bias_b = p.bias != nullptr ? __half2float(p.bias[n_a + 8]) : 0.f;
+#pragma unroll
+      for (int i = 0; i < BT / 2; ++i) {
+        const int n = n_a + ((i & 2) ? 8 : 0);
+        const int m = m_a + 8 * (i >> 2) + (i & 1);
+        if (m < p.M) {
+          if (whole)
+            p.y[(int64_t)m * p.N + n] = __float2half_rn(acc[i] + ((i & 2) ? bias_b : bias_a));
+          else
+            red_add_f32(&p.acc_ws[(int64_t)m * p.N + n], acc[i]);
         }
       }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[buf]);
-      if (dbg && et == 0) dbg_row[5] = tcq_timer();
       if (!whole) {
         // relaxed REDs -> CTA-scope barrier -> one acq_rel ticket (release is cumulative over what the barrier ordered)
-        named_bar_sync(1, 128);
+        named_bar_sync(1, 256);
         if (et == 0) {
-          const int prev = atom_add_acq_rel(&p.tickets[nt], d1 - d0);
-          *s_flag = (prev + (d1 - d0) == KP);
+          const int prev_t = atom_add_acq_rel(&p.tickets[nt], d1 - d0);
+          *s_flag = (prev_t + (d1 - d0) == KP);
         }
-        named_bar_sync(1, 128);
+        named_bar_sync(1, 256);
         const bool last = *s_flag != 0;
-        named_bar_sync(1, 128);  // everyone has read the flag before a later segment rewrites it
+        named_bar_sync(1, 256);  // everyone has read the flag before a later segment rewrites it
         if (last) {
-          // all loads of a batch of 16 tokens are in flight before the first store (one L2 round trip per batch, not
-          // one per token: the first version spent 0.45 us per token here)
-          for (int m0 = 0; m0 < p.M; m0 += 16) {
+          // thread et finalises feature (et % 128) for its half of every 32-token batch; all loads of a batch of 16
+          // tokens are in flight before the first store (one L2 round trip per batch, not one per token)
+          const int n = nt * kTileN + (et & 127);
+          const float bias_v = p.bias != nullptr ? __half2float(p.bias[n]) : 0.f;
+          for (int m0 = 16 * (et >> 7); m0 < p.M; m0 += 32) {
             float f[16];
 #pragma unroll
             for (int j = 0; j < 16; ++j)
@@ -848,68 +724,49 @@ __global__ void __launch_bounds__(TcqCfg<BT>::kThreads, 1)
       }
       t += d1 - d0;
     }
-    if (dbg && et == 0) dbg_row[6] = tcq_timer();
+    if (dbg && et == 0) { dbg_row[4] = tcq_timer(); dbg_row[6] = dbg_row[4]; dbg_row[7] = (unsigned long long)it; }
   } else {
-    // ================================================================= dequant producers (2 teams x 8 warps)
-    // Team t owns k-step t of every packed stage (rows 64 t ..): A stages t, t + 2.  The two teams' [wait, LDS, dequant,
-    // STS, proxy fence, arrive] chains overlap.
-    const int pt = threadIdx.x - 192;
-    const int team = pt >> 8;
-    const int dt = pt & 255;  // 0..255 within the team
+    // ================================================================= dequant producers (8 warps)
+    // Each packed stage holds two k-steps: rows 0..63 go to one A stage, rows 64..127 to the next.  Both halves' words
+    // are read from shared memory before the first store, so the LDS latency overlaps the first half's dequantisation.
+    const int dt = threadIdx.x - 256;  // 0..255
     const uint32_t a_base_s = smem_u32(a_base);
     const uint32_t q_base_s = smem_u32(q_base);
     const uint32_t c = dt & 15, rb = dt >> 4;
-    const uint32_t q_off = ((uint32_t)team * kBK + rb) * 64u + c * 4u;    // rows 64 team + rb + 16 j of word column c
-    const uint32_t gh = ng == 2 ? (uint32_t)team : 0u;                      // which group of constants of the stage
-    const uint32_t sc_off = Cfg::kQTileBytes + gh * 256u + c * 16u;         // 8 scales of word column c
-    const uint32_t z_off = Cfg::kQTileBytes + 512u + gh * 64u + c * 4u;     // its 8 zero-points
     using L = GemmLayoutLoaderT<1>;
-    auto fetch = [&](L& r, int qs) {
-      const uint32_t qa = q_base_s + (uint32_t)qs * Cfg::kQStageBytes;
+    auto fetch = [&](L& r, uint32_t qa, uint32_t h) {
+      const uint32_t q_off = (h * kBK + rb) * 64u + c * 4u;                        // rows 64 h + rb + 16 j, word column c
+      const uint32_t gh = ng == 2 ? h : 0u;                                       // which group of constants
 #pragma unroll
       for (int j = 0; j < 4; ++j) r.q[j] = lds_u1(qa + q_off + (uint32_t)j * 1024u);
-      r.sc[0] = lds_u4(qa + sc_off);
-      r.zq[0] = lds_u1(qa + z_off);
+      r.sc[0] = lds_u4(qa + Cfg::kQTileBytes + gh * 256u + c * 16u);              // 8 scales of word column c
+      r.zq[0] = lds_u1(qa + Cfg::kQTileBytes + 512u + gh * 64u + c * 4u);         // its 8 zero-points
     };
     const int npairs = t_end - t_begin;
-    L cur, nxt;
-    cur.init();
-    nxt.init();
-    int qs = 0, stage = team;
+    int qs = 0, stage = 0;
     uint32_t qph = 0, phase = 0;
-    if (npairs > 0) {
-      mbar_wait(&qfull[0], 0);
-      if (dbg && pt == 0) dbg_row[2] = tcq_timer();
-      fetch(cur, 0);
-    }
     for (int i = 0; i < npairs; ++i) {
-      const int qs_n = (qs + 1 == NQ) ? 0 : qs + 1;
-      const uint32_t qph_n = (qs + 1 == NQ) ? (qph ^ 1) : qph;
-      if (i + 1 < npairs) {     // the next stage's packed words: in flight while this step is dequantised
-        mbar_wait(&qfull[qs_n], qph_n);
-        fetch(nxt, qs_n);
+      mbar_wait(&qfull[qs], qph);
+      if (dbg && dt == 0 && i == 0) dbg_row[2] = tcq_timer();
+      const uint32_t qa = q_base_s + (uint32_t)qs * Cfg::kQStageBytes;
+      L hw[2];
+      fetch(hw[0], qa, 0u);
+      fetch(hw[1], qa, 1u);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mbar_wait(&empty[stage], phase ^ 1);
+        if (!(p.dbg & 2)) hw[h].store(p, 0, 0, dt, a_base_s + (uint32_t)stage * kAStageBytes);   // (knob 20)
+        if (!(p.dbg & 4)) fence_proxy_async_smem();   // every writer: generic-proxy stores -> visible to the tensor core
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&full[stage]);
+          if (h == 1) mbar_arrive(&qempty[qs]);   // after the stores that consumed the stage's words (data dependence)
+        }
+        if (++stage == NS) { stage = 0; phase ^= 1; }
       }
-      mbar_wait(&empty[stage], phase ^ 1);
-      if (!(p.dbg & 2)) cur.store(p, 0, 0, dt, a_base_s + (uint32_t)stage * kAStageBytes);   // (timing experiment: knob 20)
-      if (!(p.dbg & 4)) fence_proxy_async_smem();   // every writer: generic-proxy stores -> visible to the tensor core
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&full[stage]);
-        mbar_arrive(&qempty[qs]);  // after the stores that consumed the stage's words (data dependence)
-      }
-      stage += Cfg::kTeams;
-      if (stage >= NS) { stage -= NS; phase ^= 1; }
-      cur = nxt;
-      qs = qs_n;
-      qph = qph_n;
+      if (++qs == NQ) { qs = 0; qph ^= 1; }
     }
-    if (dbg && pt == 0) dbg_row[3] = tcq_timer();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
+    if (dbg && dt == 0) dbg_row[3] = tcq_timer();
   }
 }
 
@@ -1010,7 +867,7 @@ static cudaError_t launch_tc(const CUtensorMap& tm, const CUtensorMap& tmq, cons
   }
   const int n_work = p.n_tiles * p.m_tiles * p.ksplit;
   const int grid = n_work < sm_count() ? n_work : sm_count();
-  return launch_kernel(kern, dim3(grid), dim3(tc_threads<LAYOUT>()), Cfg::kSmemBytes, st, tm, tmq, p);
+  return launch_kernel(kern, dim3(grid), dim3(kTcThreads), Cfg::kSmemBytes, st, tm, tmq, p);
 }
 
 template <int LAYOUT>
@@ -1019,8 +876,7 @@ static cudaError_t dispatch_bt(int BT, const CUtensorMap& tm, const CUtensorMap&
   switch (BT) {
     case 32: return launch_tc<32, LAYOUT>(tm, tmq, p, st);
     case 64: return launch_tc<64, LAYOUT>(tm, tmq, p, st);
-    case 128: return launch_tc<128, LAYOUT>(tm, tmq, p, st);
-    default: return launch_tc<256, LAYOUT>(tm, tmq, p, st);
+    default: return launch_tc<128, LAYOUT>(tm, tmq, p, st);
   }
 }
 
@@ -1038,15 +894,14 @@ int gemm_tcq_grid(int n_tiles, int KP, int M, int sms, int mode) {
     long long g = 0;
     if (n_tiles <= sms) {
       // every tile is cut into ks ranges (boundaries b * KP / ks never cross a tile since the grid is a multiple of
-      // n_tiles); ks = 1 stores whole tiles directly.  Measured better than the balanced cut at every M <= 128 on the
-      // shapes with N / 128 <= 148 (profiles/r02_tcq_sweep.json).
+      // n_tiles); ks = 1 stores whole tiles directly: no fp32 reduction at all.
       int ks = sms / n_tiles;
       if (ks > KP / 2) ks = KP / 2;
       if (ks < 1) ks = 1;
       g = (long long)n_tiles * ks;
     } else if (mode == 2 || M >= 64) {
       // more tiles than SMs: whole tiles per CTA when they divide evenly (224 tiles -> 112 CTAs x 2); below 64 tokens
-      // the balanced cut wins there (all 148 SMs stream, the split-K traffic is small)
+      // the balanced cut (every SM streams, the split-K traffic is small) is kept
       const int tpc = (n_tiles + sms - 1) / sms;
       if (n_tiles % tpc == 0) g = n_tiles / tpc;
     }
@@ -1098,7 +953,7 @@ cudaError_t gemm_tc(const GemmArgs& a, int layout, float* acc_ws, int* tickets, 
   const bool g_pow2 = (a.G & (a.G - 1)) == 0;
   if (!g_pow2 && a.G != a.K) return cudaErrorNotSupported;  // AWQ group sizes: 32 / 64 / 128 / whole row
   if ((reinterpret_cast<uintptr_t>(a.x) & 15) != 0 || (a.ldx % 8) != 0) return cudaErrorMisalignedAddress;
-  const int BT = a.M <= 32 ? 32 : (a.M <= 64 ? 64 : (a.M <= 128 ? 128 : 256));
+  const int BT = a.M <= 32 ? 32 : (a.M <= 64 ? 64 : 128);
   TcParams p;
   p.qweight = a.qweight;
   p.scales = reinterpret_cast<const __half*>(a.scales);
@@ -1122,7 +977,7 @@ cudaError_t gemm_tc(const GemmArgs& a, int layout, float* acc_ws, int* tickets, 
     p.m_tiles = 1;
     p.ksplit = knob(22);   // small-M kernel: L2 prefetch distance in k-step pairs (0 = off)
     p.has_tmq = 1;
-    p.dbg = (knob(3) == 9 ? 1 : 0) | ((knob(20) & 15) << 1);   // knob 20: timing experiments (results invalid)
+    p.dbg = (knob(3) == 9 ? 1 : 0) | ((knob(20) & 3) << 1);   // knob 20: producer timing experiments (results invalid)
     cudaError_t eq = make_x_tmap(a.x, a.ldx, a.M, a.K, BQ, &tmxq);
     if (eq == cudaSuccess)
       eq = make_tmap_2d(a.qweight, 1, (uint64_t)(a.N / 8), (uint64_t)a.K, (uint64_t)(a.N / 8) * 4, 16, 2 * kBK, &tmwq, false);
@@ -1146,9 +1001,9 @@ cudaError_t gemm_tc(const GemmArgs& a, int layout, float* acc_ws, int* tickets, 
     if (ksplit < 1) ksplit = 1;
     while (ksplit > 1 && KS / ksplit < 4) --ksplit;  // at least 4 k-steps per slice
   }
-  // Above 64 tokens the reduction is no longer free: ~0.15 us per token (M * 128 fp32 REDs per CTA, M / 16 L2 round trips
-  // for the finaliser) against ~0.5 us per k-step saved on the critical path (profiles/r02_m_sweep_final.json: 14336 x
-  // 4096 at M = 256 114 -> 66 us with 4 slices, 4096 x 4096 45 -> 47 us) - split only when it pays.
+  // Above 64 tokens the reduction is no longer free (M * 128 fp32 REDs per CTA, M / 16 L2 round trips for the
+  // finaliser) against the k-steps it takes off the critical path - split only when it pays.  The cost model (0.15 per
+  // token vs 0.5 per k-step saved) was carried over from the kernel's earlier tuning and not re-measured on H100.
   if (a.M > 64 && ksplit > 1 && (float)(KS - KS / ksplit) * 0.5f < 0.15f * (float)a.M) ksplit = 1;
   const int forced = knob(1);
   if (forced > 0 && a.M <= 2 * kMaxSplitM && acc_ws != nullptr && tickets != nullptr) ksplit = forced > KS ? KS : forced;

@@ -1,11 +1,11 @@
 // CUDA-core GEMV path (M <= 8 tokens) for the three AWQ layouts.  HBM-bound: the job of these kernels
 // is to stream the packed int4 weights once, with 128-bit coalesced loads and enough bytes in flight
-// to cover DRAM latency, and to keep the ALU cost per weight below the issue budget that 6.5+ TB/s
-// leaves (about 46 weights / clock / SM on a 148-SM B200).
+// to cover DRAM latency, and to keep the ALU cost per weight below the issue budget the HBM rate leaves
+// (about 3.35 TB/s / 132 SMs / ~1.8 GHz = 28 weights / clock / SM on an H100 SXM).
 //
 // Arithmetic (all layouts): the 4-bit code q is used directly as an fp16 *subnormal* bit pattern
 // (q * 2^-24, or q * 2^-20 for the nibbles that sit 4 bits higher), multiplied with the fp16 activation
-// and accumulated in fp32 by FHFMA (fma.rn.f32.f16: exact product, one fp32 rounding) - one ALU op per
+// and accumulated in fp32 (fhfma: exact product, one fp32 rounding) - one FMA per
 // weight plus 5/8 op of LOP3/SHF unpack.  Zero-point and scale are applied once per (group, column):
 //     y[n] += s[g,n] * ( 2^24 * sum_k x[k] q[k,n]  -  z[g,n] * sum_k x[k] )
 // The cross-thread / cross-CTA (split-K) reduction is fp32; the result is rounded to fp16 once.
@@ -26,8 +26,8 @@ constexpr float kScaleB = 1048576.0f;   // 2^20: code read through mask 0x00f000
 
 // ======================================================================= GEMM layout [K, N/8]
 // v2: the dot products run on the tensor pipe through mma.sync.m16n8k16 with REGISTER-resident fragments.
-// Why: measured on B200, FHFMA issues at ~16 lanes/clk/SM (quarter rate), which caps a CUDA-core fp32
-// GEMV at ~1.7 TB/s (26% of HBM peak); feeding the same registers to HMMA costs 0.75 ALU op per weight.
+// Why: a CUDA-core fp32 GEMV spends at least one FMA (plus the operand conversions) per weight, more than the issue
+// budget above; feeding the same registers to HMMA costs 0.75 ALU op per weight.
 //
 // Fragment construction without a transpose: one AWQ word = 8 columns of ONE k, low half-word = even
 // columns, high half-word = odd columns.  For two consecutive rows (k, k+1) of the same word column
@@ -253,6 +253,8 @@ static cudaError_t launch_gemv_gemm_layout(const GemmArgs& a, float* acc_ws, int
 }
 
 // Rows per warp: the largest of {128, 64, 32} that divides G and still leaves >= 2 CTAs per SM.
+static int v3_sm_count();   // device SM count (defined with the persistent GEMV below)
+
 static int pick_rw(int K, int N, int G) {
   const int forced = knob(0);
   if (forced == 32 || forced == 64 || forced == 128) return (G % forced == 0) ? forced : 32;
@@ -260,13 +262,13 @@ static int pick_rw(int K, int N, int G) {
   for (int rw = 128; rw > 32; rw >>= 1) {
     if (G % rw != 0) continue;
     const int kc = kGvWarps * rw;
-    if ((int64_t)colblk * ((K + kc - 1) / kc) >= 2 * 148) return rw;
+    if ((int64_t)colblk * ((K + kc - 1) / kc) >= 2 * v3_sm_count()) return rw;
   }
   return 32;
 }
 
 // N % 32 == 0, G % 32 == 0 (every AWQ checkpoint: G in {32, 64, 128, K}) and 8-byte aligned activation rows
-// take the tensor-pipe GEMV; other shapes are routed to the tcgen05 kernel by the C-ABI layer.
+// take the tensor-pipe GEMV; other shapes are routed to the wgmma kernel by the C-ABI layer.
 bool gemv_gemm_layout_supported(const GemmArgs& a) {
   return (a.N % 32) == 0 && (a.G % 32) == 0 && (reinterpret_cast<uintptr_t>(a.qweight) % 16) == 0 && a.M <= 8 &&
          (a.ldx % 4) == 0 && (reinterpret_cast<uintptr_t>(a.x) % 8) == 0;
@@ -290,9 +292,9 @@ cudaError_t gemv_gemm_layout(const GemmArgs& a, float* acc_ws, int* tickets, cud
 }  // namespace b200awq
 
 // ======================================================================= GEMM layout, persistent TMA-ring GEMV
-// v3/v4.  What the register-staged kernel above taught (ncu, B200): with loads staged in REGISTERS a CTA
+// v3/v4.  What the register-staged kernel above taught: with loads staged in REGISTERS a CTA
 // keeps ~50 KB per SM in flight and every short-lived CTA pays its own chain of dependent latencies
-// (DRAM -> MMA -> fold constants -> atomics -> fence -> ticket): DRAM sat at 9-29 % busy.  A first
+// (DRAM -> MMA -> fold constants -> atomics -> fence -> ticket) and leaves DRAM mostly idle.  A first
 // ring-buffer version with four warps sharing each 16-row block spent 2/3 of its instructions on
 // per-block flush / fold / barriers.  This version:
 //   * ONE persistent CTA per SM; a producer warp streams 8 KB weight tiles (64 rows x 256 columns, TMA 2-D,
@@ -351,7 +353,7 @@ __global__ void __launch_bounds__(kV3Threads, 1)
     // before the wait - not even to decide that the job is padding (a CTA that exits without waiting would also let the
     // grid "complete" early and break the chain for the successor).  The expert's weights depend on the routing, so
     // unlike the dense GEMV there is nothing to prefetch ahead of the wait.  (Found by bench.py's Mixtral leg: with
-    // knob 4 the step ran in 1.8 ms instead of 3.3 ms - jobs saw stale tables and returned as padding.)
+    // knob 4 the step ran far too fast - jobs saw stale tables and returned as padding.)
     pdl_wait();
     const int job = blockIdx.y;
     if (job * 8 >= *moe.num_post_pad) return;
@@ -413,9 +415,8 @@ __global__ void __launch_bounds__(kV3Threads, 1)
       const int w = lane;
       const int a = t0 + (int)((int64_t)ntile * w / kV3Warps);
       const int bnd = t0 + (int)((int64_t)ntile * (w + 1) / kV3Warps);
-      // Optional HBM -> L2 prefetch kL2Ahead tiles ahead of the shared-memory ring (knob 8).  Measured r1 (ring
-      // sweep in profiles/): no gain - 19.5 us without vs 20.7 us with it on 4096x28672 - the 24-stage ring already
-      // saturates what the consumers can drain, extra requests only lengthen the queues.  Default: off.
+      // Optional HBM -> L2 prefetch kL2Ahead tiles ahead of the shared-memory ring (knob 8): the deep ring already
+      // keeps the consumers fed, extra requests only lengthen the queues.  Default: off.
       const int kL2Ahead = l2_ahead > 0 ? SPW + l2_ahead : 0;  // 0: no L2 prefetch
       int cbp = a / TPC, ktp = a - cbp * TPC;      // prefetch cursor (no per-tile divisions)
       auto pf_one = [&]() {
@@ -649,9 +650,8 @@ static int v3_sm_count() {
 }
 
 // Successor table: decode calls the same linears in the same order every token; remember, per weight
-// tensor, which weight tensor was used next, and let the kernel prefetch it into L2.  Measured on B200 (r1):
-// 478.6 vs 498.7 tok/s decode with / without it - HBM is not idle enough in the kernel tails for the extra
-// L2 traffic to pay, so it is OFF by default (knob 6 = 1 enables it for experiments).
+// tensor, which weight tensor was used next, and let the kernel prefetch it into L2.  HBM is not idle enough in the
+// kernel tails for the extra L2 traffic to pay, so it is OFF by default (knob 6 = 1 enables it for experiments).
 struct NextW {
   const void* ptr;
   long long bytes;
@@ -710,9 +710,9 @@ static cudaError_t launch_v3(const GemmArgs& a, float* acc_ws, int* tickets, cud
                        reinterpret_cast<const __half*>(a.scales), a.qzeros, reinterpret_cast<const __half*>(a.bias),
                        reinterpret_cast<__half*>(a.y), acc_ws, tickets, a.M, a.K, a.N, a.G, g_shift,
                        reinterpret_cast<const uint8_t*>(nx.ptr), nx.bytes, knob(3) == 1 ? 1 : 0, knob(8) > 0 ? knob(8) - 1 : 0,
-                       // packed epilogue at M = 1 only: there it saves the ticket and read-back round trips (4096 x 4096:
-                       // 8.75 -> 7.18 us); for M >= 2 the returning 64-bit atomics cost more than they save on the
-                       // larger shapes (4096 x 14336, M = 8: 32 -> 49 us), so those keep fp32 REDs + tickets.
+                       // packed epilogue at M = 1 only: there it saves the ticket and read-back round trips; for M >= 2
+                       // the returning 64-bit atomics (M per column) cost more than they save, so those keep fp32 REDs +
+                       // tickets (a choice carried over from the earlier tuning, not re-measured on H100).
                        // knob 18 = 1: ticket epilogue everywhere
                        V3Moe{}, (MT == 1 && a.K / kV3TileRows < 256 && knob(18) == 0) ? 1 : 0);
 }
@@ -768,8 +768,8 @@ bool gemv_v3_supported(const GemmArgs& a) {
 cudaError_t gemv_v3(const GemmArgs& a, float* acc_ws, int* tickets, cudaStream_t st) {
   constexpr size_t kMaxSmem = 227 * 1024;
   if (a.M <= 1) {
-    // knob 7 = 1: stage the activations in shared memory (2 ring stages per warp instead of 3).  Measured r1:
-    // 477 vs 498 tok/s - the x loads were not the stall, the third stage is worth more.
+    // knob 7 = 1: stage the activations in shared memory (2 ring stages per warp instead of 3; off by default: the x
+    // loads were not the stall, the third stage is worth more - carried over, not re-measured on H100).
     if (knob(7) != 0 && V3Smem<1, 2>::bytes + (size_t)(a.K + 8) * 2 <= kMaxSmem) return launch_v3<1, 2, true>(a, acc_ws, tickets, st);
     if (knob(9) == 1) return launch_v3<1, 1, false>(a, acc_ws, tickets, st);
     if (knob(9) == 2) return launch_v3<1, 2, false>(a, acc_ws, tickets, st);

@@ -276,8 +276,8 @@ __device__ __forceinline__ void v3_fold(const uint8_t* sa, float* my_red, float*
 
 // As v3_fold, but the folded column sums stay in REGISTERS: lane l owns word-column l = 8 columns x MT tokens
 // (ycol[m][j]).  The per-warp column accumulators in shared memory cost 8 KB x MT per CTA - with MT = 8 that left room
-// for ONE ring stage per warp and the M = 8 GEMV ran 2.2x slower than M = 1 (19.9 vs 8.8 us on 4096 x 4096,
-// profiles/r02_m_sweep.json); in registers every MT gets at least two stages.
+// for ONE ring stage per warp and the M = 8 GEMV ran about twice as slow as M = 1; in registers every MT gets at
+// least two stages.
 template <int MT>
 __device__ __forceinline__ void v3_fold_reg(const uint8_t* sa, float* my_red, float (&ycol)[MT][8], int lane, int g, int tig,
                                             const float (&acc)[4][4][4], const float (&xs_acc)[4]) {

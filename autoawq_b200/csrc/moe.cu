@@ -11,7 +11,7 @@
 // (half a 16-slot block: one expert) ride through mma.sync.m16n8k16 as the n = 8 dimension, exactly like the M <= 8
 // GEMV (gemv.cu): one CTA = 256 output columns x 8 slots, streaming the expert's K rows in chunks of 512 with
 // register-staged 128-bit loads.  HBM-bound at decode (each active expert's weights are read once per half-block);
-// a tcgen05 grouped GEMM for prefill-sized token counts is the next step.
+// a tensor-core grouped GEMM for prefill-sized token counts is the next step.
 #include "common.cuh"
 #include "gemv_tile.cuh"
 #include "kernels.h"

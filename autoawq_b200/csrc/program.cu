@@ -1,9 +1,8 @@
 // Decode program: the whole chain of M = 1 operator calls of a decode step (RMSNorm -> W4A16 linear -> ... ->
 // SiLU*mul -> linear) recorded once and executed by ONE persistent kernel launch.
 //
-// Why (measured, B200, profiles/r01_gemv_v3_phase_timeline.log): a stand-alone GEMV launch spends ~5 us of its
-// 7-20 us outside the weight stream - launch + ring fill (the first tile lands after ~5 us of loaded HBM latency),
-// the split-K tail, the ticket round trip - and HBM idles through every one of those gaps, 128 times per decode
+// Why: a stand-alone GEMV launch spends microseconds outside the weight stream - launch + ring fill (the first tile
+// lands after the loaded HBM latency), the split-K tail, the ticket round trip - and HBM idles through every one of those gaps, 128 times per decode
 // step.  The packed weights never depend on the activations, so here the producer warp of every CTA walks the
 // WHOLE op list and keeps its shared-memory ring full across op boundaries: while the consumers of op i reduce,
 // publish and wait for the grid-wide completion of op i, the tiles of op i+1 are already landing.
@@ -22,8 +21,8 @@
 //   * duty warp: off the critical path, stores this CTA's slice of every op's fp16 output (and of the SiLU*mul
 //     output), so every tensor of the per-op path holds the same values after a run, and recycles the four rotating
 //     rows (staged[] / zeroed[] counters, see program_kernel).
-//   History (profiles/r01_program_l2ahead_sweep.md, DESIGN.md 3.5): tickets + last-arriver finalisation: ~10 us per
-//   op boundary, 529 tok/s; fp32 row + one release/acquire counter per op: ~8 us, 652 tok/s; packed rows: 734-744.
+//   History (DESIGN.md 3.5): tickets + last-arriver finalisation per op boundary, then an fp32 row + one
+//   release/acquire counter per op, then the packed rows (fewest dependent L2 round trips per boundary).
 //
 // Reference call sequence this replaces: awq/modules/fused/block.py:117-170 (norm -> qkv -> ... -> o -> norm ->
 // mlp) with awq/modules/fused/mlp.py:41-55 (gate/up GEMM, silu*mul, down GEMM), each a separate awq_ext call.
@@ -116,8 +115,8 @@ __device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long
   asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 // Polling load: STRONG (relaxed at gpu scope), not a weak load with a cache hint - the rows are polled without any
-// acquire in front, and a weak ld.cg may keep returning a stale copy from the near L2 partition for ever (seen on
-// B200: the duty warps spun on complete rows).
+// acquire in front, and a weak ld.cg may keep returning a stale copy from the near L2 partition for ever (the duty
+// warps were once seen spinning on complete rows).
 __device__ __forceinline__ ulonglong2 ldcg_u64x2(const unsigned long long* p) {
   ulonglong2 r;
   asm volatile("ld.relaxed.gpu.global.v2.u64 {%0,%1}, [%2];" : "=l"(r.x), "=l"(r.y) : "l"(p) : "memory");
@@ -309,9 +308,10 @@ __global__ void __launch_bounds__(kProgThreads, 1)
         const int a = t0 + (int)((int64_t)ntile * w / kV3Warps);
         const int bnd = t0 + (int)((int64_t)ntile * (w + 1) / kV3Warps);
         int cb = a / TPC, kt = a - cb * TPC;
-        // gate (knob 10): hold the next op's loads back until this CTA's sums of the previous op are on their way
-        // (measured +9 %: the REDs do not queue behind a fresh burst of bulk loads; the ring refills while the
-        // consumers poll and stage)
+        // gate (knob 10): hold the next op's loads back until this CTA's sums of the previous op are on their way, so the
+        // REDs do not queue behind a fresh burst of bulk loads; the ring refills while the consumers poll and stage.
+        // On an H100 (400 W) it makes no measurable difference (2.07 vs 2.05 ms per Llama-3-8B step with / without,
+        // inside the run-to-run spread); it is kept as the default.
         if (gate && op > 0) prog_wait_smem(pub_op, op, kWGate, op);
         for (int t = a; t < bnd; ++t) {
           const int stage = w * SPW + stage_i;
@@ -721,12 +721,15 @@ bool stream_format_supported(int K, int N, int G, int mode) {
   if (mode == 1 && ((N / 2) % 8) != 0) return false;
   return mode == 0 || mode == 1;
 }
+static int prog_sm_count();   // device SM count (defined below)
+
 cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N, int G,
                         int mode, cudaStream_t st) {
   if (!stream_format_supported(K, N, G, mode)) return cudaErrorNotSupported;
   const int UK = G < 128 ? G : 128;
   const int64_t total = (int64_t)(N / 16) * (K / UK) * ((UK / 16) * 32 + 12);
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int cap = prog_sm_count() * 16;
+  const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
   stream_pack_kernel<<<blocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros,
                                              static_cast<uint8_t*>(out), K, N, G, mode);
   return cudaGetLastError();
@@ -840,8 +843,6 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     e = cudaFuncSetAttribute(stream_program_kernel<8, 4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(stream_program_kernel<12, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(stream_program_kernel<16, 2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     cudaFree(pr->d_stream);
@@ -1081,10 +1082,11 @@ cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st) {
   cudaError_t e = program_abort_clear(st);
   if (e != cudaSuccess) return e;
   if (p->stream) {
-    // knob 9: consumer warps of the stream kernel: 8 (4 ring stages each, 4 units in flight; the default: measured
-    // best, 1.50 / 1.59 / 1.73 ms per Llama-3-8B step with 8 / 12 / 16), 12 (3 stages, 2 units) or 16 (2 stages, 2 units)
-    const int nw = knob(9) == 12 ? 12 : (knob(9) == 16 ? 16 : 8);
-    const int spw = nw == 8 ? 4 : (nw == 12 ? 3 : 2);
+    // knob 9: consumer warps of the stream kernel: 8 (4 ring stages each, 4 units in flight; the default) or 12 (3 stages,
+    // 2 units).  No 16-warp variant: 17 warps put 5 on one of the SM's four register-file partitions, which caps a thread
+    // at 96 registers on sm_90 and spills the unit loop.
+    const int nw = knob(9) == 12 ? 12 : 8;
+    const int spw = nw == 8 ? 4 : 3;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(prog_sm_count());
     cfg.blockDim = dim3(32 + nw * 32);
@@ -1097,17 +1099,14 @@ cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st) {
     cfg.numAttrs = 1;
     const SpOp* sops = p->d_sp_ops;
     const uint32_t* cta = p->d_cta;
-    // knob 8: HBM -> L2 prefetch window per producer lane in KB (<= 0 = off, the default: it helps only when the weight
-    // stream is the bottleneck - 1041 -> 895 us without the unit math - and costs 1-6 % with it)
+    // knob 8: HBM -> L2 prefetch window per producer lane in KB (<= 0 = off, the default: it can only help when the
+    // weight stream is the bottleneck, which the unit math is not; not re-measured on H100)
     const int l2_ahead = knob(8) <= 0 ? 0 : knob(8) * 1024;
     // knob 10: ops ahead of the consumers' staging for which shared-memory loads may already be issued (0 = ungated,
     // the default; n > 0: at most n - 1 ops ahead, 1 = strictly gated)
     const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
     if (nw == 8)
       return cudaLaunchKernelEx(&cfg, stream_program_kernel<8, 4, 4>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                                p->d_state, knob(3), l2_ahead, gate_ahead);
-    if (nw == 16)
-      return cudaLaunchKernelEx(&cfg, stream_program_kernel<16, 2, 2>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
                                 p->d_state, knob(3), l2_ahead, gate_ahead);
     return cudaLaunchKernelEx(&cfg, stream_program_kernel<12, 3, 2>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
                               p->d_state, knob(3), l2_ahead, gate_ahead);

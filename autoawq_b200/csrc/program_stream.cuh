@@ -3,11 +3,10 @@
 // a post-load re-layout is awq/modules/linear/exllama.py:66-79) so that the grid-wide hand-off between two
 // dependent linears shrinks to "store, poll".
 //
-// Why (round-1 measurements, profiles/r01_program_phase_timeline.log): with the checkpoint's GEMM layout
-// [K, N/8] a DRAM-efficient tile is >= 128 bytes = 256 columns wide, so N = 4096 has only 16 column blocks for 148
-// CTAs: split-K with a fan-in of ~9 CTAs per column block is forced, and its cost - ~110 k 64-bit REDs per op into
-// L2, every CTA polling 64-bit sums, a reclamation protocol for the accumulator rows - was ~6 us per op boundary
-// against ~4 us of weight streaming.  In the stream format ANY partition is contiguous in memory, so the work is
+// Why: with the checkpoint's GEMM layout [K, N/8] a DRAM-efficient tile is >= 128 bytes = 256 columns wide, so
+// N = 4096 has only 16 column blocks for 132 CTAs: split-K with a fan-in of ~8 CTAs per column block is forced, and its
+// cost - ~100 k 64-bit REDs per op into L2, every CTA polling 64-bit sums, a reclamation protocol for the accumulator
+// rows - is comparable to the op's own weight streaming.  In the stream format ANY partition is contiguous in memory, so the work is
 // cut OUTPUT-STATIONARY: a CTA owns whole 16-column sets (all of K), its 8 consumer warps split the CTA's units
 // (set, 128 rows of K) evenly, partial sums meet in shared memory, and the CTA publishes FINISHED fp16 outputs:
 //   * no cross-CTA reduction, no atomics, no fixed-point packing, nothing to zero or reclaim, no duty warp;
@@ -159,10 +158,9 @@ __global__ void __launch_bounds__(256)
 //   raw sums:  S = sum_k x_k (1024 + c q)   (mma.sync on the raw codes, two accumulator chains: even / odd fragments)
 //   fold:      s (S - (1024 + c z) X) / c   with X = sum_k x_k of the unit   (csrc/gemv_tile.cuh:v3_fold)
 // NU units in flight per call (sp_units<F, NU>): a single unit is one long dependency chain (LDS -> unpack -> 4
-// chained HMMA -> fold, ~250 cycles) and a warp has nothing else to overlap it with - measured: unit-at-a-time the
-// kernel was bound by exactly that latency at 4.5 TB/s (tools/stream_experiments.py: 759 us per step without the
-// math, 1510 with), while the tensor pipe itself sustains 0.33 HMMA/clk/SM = 12.5 TB/s of int4 weights
-// (tools/hmma_rate.cu).  Four units interleaved give eight independent chains per warp.
+// chained HMMA -> fold, a few hundred cycles) and a warp has nothing else to overlap it with: unit-at-a-time the
+// kernel is bound by that latency, not by the tensor pipe.  Four units interleaved give eight independent chains per
+// warp.
 template <int F, int NUQ>
 __device__ __forceinline__ void sp_units(const uint8_t* __restrict__ st, int UB, const uint32_t* __restrict__ xs,
                                          const float* __restrict__ xsum, const int (&ju)[NUQ], int lane, bool xl,
@@ -355,7 +353,7 @@ __global__ void __launch_bounds__(32 + NW * 32, 1)
       fetch(1, nxt);
       // HBM -> L2 prefetch cursor, running ahead of the ring by at most `l2_ahead` bytes per lane: while the
       // consumers hand activations from op to op the ring is full and HBM would idle; with the next chunks already in
-      // L2 the ring refills at L2 speed afterwards (the weights of ~1.5 ops fit: 148 x 8 lanes x l2_ahead)
+      // L2 the ring refills at L2 speed afterwards (SM count x 8 lanes x l2_ahead bytes)
       Run pcur, pnxt;
       int pop = 0;
       fetch(0, pcur);
@@ -378,7 +376,7 @@ __global__ void __launch_bounds__(32 + NW * 32, 1)
         bool issued = false;
         // Gate: shared-memory loads of an op start only once this CTA has staged that op's activations (+ gate_ahead
         // ops).  A deep ring of bulk loads is also a deep queue on the SM's return path: every poll of the hand-off
-        // waited behind ~100 KB of weight tiles (measured: 1.3 us per L2 round trip against 0.13 us unloaded).  While
+        // waits behind ~100 KB of weight tiles, several times its unloaded L2 round trip.  While
         // the consumers hand over, the stream continues into L2 (prefetch cursor below), not into this SM.
         if (active && (gate_ahead >= (1 << 20) || op <= ld_acquire_cta_smem(staged_op) + gate_ahead)) {
           const int stage = w * SPW + stage_i;
@@ -487,7 +485,7 @@ __global__ void __launch_bounds__(32 + NW * 32, 1)
           if (ok && (lane & (seg - 1)) == 0) xsum[c >> uk_shift] = sx;
         };
         // passes are taken in batches of 4: every load of a batch is in flight before the first tag is looked at
-        // (a poll is an L2 round trip of ~1 us under load; K = 14336 has 7 passes)
+        // (a poll is a loaded L2 round trip; K = 14336 has 7 passes)
         // (the first kSpStageWarps warps stage; the others wait at the barriers)
         const int cb_first = cw < kSpStageWarps ? cw * 256 : K;
         for (int cb0 = cb_first; cb0 < K; cb0 += 4 * kSpStagePass) {      // warp-uniform trip counts

@@ -1,12 +1,12 @@
-"""Host-side mirror of the reference's quantised-linear modules on the B200 kernels.
+"""Host-side mirror of the reference's quantised-linear modules on this repository's kernels.
 
 Same class names, constructor arguments, buffer names / shapes / dtypes, `from_linear` signature and
 forward semantics as awq/modules/linear/{gemm.py:116-298, gemv.py:27-197, gemv_fast.py:68-208}, so the
 parity tests read like tests of the reference and a checkpoint's state-dict loads unchanged.  The
 reference's own (unmodified) classes work on top of `awq_ext` / `awq_v2_ext` too - that is the real
-drop-in point; these mirrors exist because /root/reference does not travel to the GPU box, and because
+drop-in point; these mirrors exist because the reference package need not be installed where the kernels run, and because
 they skip the reference's "dequantise the whole matrix then cuBLAS" detour for >= 1024 tokens
-(gemm.py:48-54): one fused tcgen05 kernel covers every M.
+(gemm.py:48-54): one fused wgmma kernel covers every M.
 """
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
 """Column / row sharding of packed AWQ tensors across the GPUs of one box (SURVEY.md 8e).
 
 The reference has no tensor parallelism (multi-GPU = accelerate layer placement, awq/models/base.py:527-535);
-BASELINE config 5 (Llama-3-70B on 8 x B200) needs it.  A linear is independent per output column and
+BASELINE config 5 (Llama-3-70B on 8 x H100) needs it.  A linear is independent per output column and
 additive over K, and the packed formats slice cleanly:
 
   column-parallel (split N; qkv / gate / up):  GEMM layout  qweight[:, n0/8:n1/8], qzeros[:, n0/8:n1/8],
@@ -112,7 +112,7 @@ def all_reduce_sum(y: torch.Tensor, group=None) -> torch.Tensor:
 
 
 class TensorParallelMLP:
-    """gate|up (column-parallel, fused) -> SiLU*mul -> down (row-parallel) -> all-reduce, on the B200 kernels.
+    """gate|up (column-parallel, fused) -> SiLU*mul -> down (row-parallel) -> all-reduce, on this repository's kernels.
     Per-rank weights are the slices above; used by the 70B-shape tensor-parallel bench leg (bench.py `tp70b`) and
     the tests.  gate / up are split on the boundaries of down's K split (its group size), so the activation width
     of a rank always equals its number of down rows, also when (I / G) % world != 0."""

@@ -1,4 +1,4 @@
-/* b200awq.h - C ABI of the B200 (sm_100a) AWQ W4A16 linear path.
+/* b200awq.h - C ABI of the H100 (sm_90a) AWQ W4A16 linear path.
  *
  * This is the drop-in boundary: a plain C shared library (libb200awq.so) whose entry points are what a
  * replacement for the reference's `awq_ext` / `awq_v2_ext` pybind modules binds.  No torch types: device
@@ -44,7 +44,7 @@ enum {
   B200AWQ_EUNSUPPORTED = 2,/* shape outside the implemented envelope (e.g. K % 64 != 0 on the tensor-core path) */
   B200AWQ_EWORKSPACE = 3,  /* workspace missing or too small */
   B200AWQ_ECUDA = 4,       /* a CUDA runtime / driver call failed */
-  B200AWQ_EARCH = 5        /* device is not sm_100 */
+  B200AWQ_EARCH = 5        /* device is not sm_90 */
 };
 
 int b200awq_abi_version(void);
@@ -65,7 +65,7 @@ int b200awq_dequantize_gemm(const int32_t* qweight, const void* scales, const in
 
 /* Y[M, N] f16 = X[M, K] f16 . deq(W) (+ bias[N] f16 if non-null), GEMM layout.  ldx = row pitch of X in
  * elements (>= K).  M <= 4 runs the persistent tensor-core GEMV (M <= 8 where the small-M kernel does not apply),
- * 5 <= M <= 128 the small-M tcgen05 kernel with TMA-staged packed weights, larger M the tcgen05 GEMM. */
+ * 5 <= M <= 128 the small-M wgmma kernel with TMA-staged packed weights, larger M the wgmma GEMM. */
 int b200awq_gemm_forward(const void* x, int64_t ldx, const int32_t* qweight, const void* scales,
                          const int32_t* qzeros, const void* bias, void* y, int M, int K, int N, int group_size,
                          void* workspace, size_t workspace_bytes, b200awq_stream_t stream);
@@ -129,7 +129,8 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *   key 0: GEMV rows per warp override: 32 / 64 / 128 (0 = heuristic)
  *   key 1: tensor-core path split-K override (0 = heuristic)
  *   key 2: M threshold at or below which the GEMV kernels are used (default 8; the GEMM-layout entry point lowers it to 4
- *          wherever the small-M tensor-core kernel of key 19 applies: it is faster from 5 tokens on)
+ *          wherever the small-M tensor-core kernel of key 19 applies: over the Llama-3-8B linears it is faster from 5
+ *          tokens on, measured on H100)
  *   key 3: 1 = the persistent GEMV records per-CTA phase timestamps (read with b200awq_debug_read);
  *          2 = the decode-program kernel records per-op phase timestamps of its first 8 CTAs / 32 ops
  *          (b200awq_debug_read then returns [op][cta][8] uint64 ns: op begin, previous op complete, activations
@@ -137,7 +138,7 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *          3 = b200awq_debug_read returns the decode-program kernel's abort record instead: int32 [0..3] = {code, op,
  *          CTA, aborted} of the first wait that exceeded 0.5 s (every spin loop of that kernel gives up rather than
  *          hang the GPU), then per CTA 10 ints = (code << 16 | op) of the wait each warp abandoned;
- *          4 = the decode-program kernel does not recycle its accumulator rows (inspection with tools/program_debug.py)
+ *          4 = the decode-program kernel does not recycle its accumulator rows (inspection of the rows after a run)
  *          9 = the small-M tensor-core kernel (9 <= M <= 128, GEMM layout) records per-CTA phase timestamps
  *          (b200awq_debug_read returns [cta][8] uint64 ns: entry, setup done, first packed stage landed, producers
  *          done, MMA issuer done, last accumulator drained, epilogue done, number of segments)
@@ -146,17 +147,20 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *   key 5: 1 = disable the persistent TMA-ring GEMV (use the register-staged GEMV for every M <= 8 shape)
  *   key 6: 1 = enable the learned next-weight L2 prefetch (the M <= 8 path remembers which weight tensor
  *          followed which in the call sequence and prefetches the successor's packed weights into L2 at the
- *          tail of each kernel); default 0 - it measured slightly slower on B200
+ *          tail of each kernel); default 0
  *   key 7: 1 = stage the activations in shared memory in the persistent GEMV (M <= 2); default 0
  *   key 8: persistent GEMV L2-prefetch distance + 1 in tiles (0 / 1 = off, the default)
  *   key 9: persistent GEMV ring stages per consumer warp for M = 1 (1 / 2; 0 = default 3); the decode-program
- *          kernel uses 1 stage per warp when this is 1 (default 2)
+ *          kernel uses 1 stage per warp when this is 1 (default 2); the stream decode program runs 12 consumer warps
+ *          when this is 12 (default 8; any other value, 16 included, means 8: a 16-warp CTA spills on sm_90)
  *   key 10: decode program: 2 = do NOT hold the next op's weight loads back until the CTA has pushed its sums of
- *           the previous op (default: hold them back, +9 % measured)
+ *           the previous op (default: hold them back; no measurable difference on H100); the stream decode program
+ *           reads it as its gate: 0 = ungated (the default: 1.93 vs 1.98 ms per Llama-3-8B step with 2 = gated one op
+ *           ahead, H100 at 400 W), n > 0 = loads at most n - 1 ops ahead of the staging
  *   key 11: decode program: 2 = no back-off in the duty warp's polls (default: 400 ns sleep between attempts)
  *   key 12: 2 = grouped_gemm_forward always uses the register-staged grouped kernel
  *   key 13: decode program (read at b200awq_program_create): minimum tiles per participating CTA; ops with fewer
- *           tiles per CTA are shared by fewer CTAs (0 = every CTA takes part in every op, the default: measured best)
+ *           tiles per CTA are shared by fewer CTAs (0 = every CTA takes part in every op, the default)
  *   key 18: 1 = the persistent GEMV uses round 1's split-K epilogue (fp32 REDs, tickets, read-back) also at M = 1,
  *           instead of the packed one (one returning 64-bit atomic per element; bit-reproducible)
  *   key 17: 1 = b200awq_comm_all_reduce uses the flag protocol (push, fence, flag, wait, reduce) instead of the default
@@ -167,8 +171,8 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *   key 19: 1 = never use the small-M kernel with TMA-staged packed weights (gemm_tcq_kernel; default: every GEMM-layout
  *           call with 5 <= M <= 128 (M above key 2's threshold), G >= 64, K % 128 == 0, N % 128 == 0 runs it)
  *   key 20: small-M kernel timing experiments (outputs are WRONG while set): bit 0 = producers skip the dequantisation and
- *           the shared-memory stores, bit 1 = producers skip the generic->async proxy fence, bit 2 = no MMA is
- *           issued (commits only), bit 3 = one MMA per k-step instead of four
+ *           the shared-memory stores, bit 1 = producers skip the generic->async proxy fence (the MMA loop itself has
+ *           no experiment switch: a runtime condition around wgmma would change its code)
  *   key 21: small-M kernel work cut: 0 = tile-aligned ranges when N / 128 <= SM count (or from 64 tokens on), balanced
  *           (n-tile, k-step pair) ranges otherwise; 1 = always balanced; 2 = tile-aligned whenever possible
  *   key 22: small-M kernel: HBM -> L2 prefetch distance in k-step pairs ahead of the shared-memory ring (0 = off, default)

@@ -8,7 +8,7 @@ This file is a numpy restatement of the reference's algorithm for the hot path
 CUDA library is missing instead of falling back to this code.
 
 Parity pinning: every function below is checked against outputs of the real
-reference (imported from /root/reference in the build container) by
+reference (imported from an upstream checkout, oracle/reference.py) by
 ``tests/golden/make_golden.py``; the resulting vectors are committed under
 ``tests/golden/*.npz`` and re-checked by ``tests/test_oracle_golden.py`` on every
 run.  The one known-answer recipe the reference's own tests hold for this path
@@ -17,7 +17,7 @@ N=1792, g=128, dequant allclose rtol=1e-4) is mirrored in those fixtures.
 GEMM/GEMV *outputs* are unpinned by the reference (no test, SURVEY.md section 8c); for
 them the oracle is the fp64 contraction of the bit-exact dequantised weights.
 
-Reference map (file:line under /root/reference):
+Reference map (file:line in the reference checkout):
   AWQ_ORDER / AWQ_REVERSE_ORDER ........ awq/utils/packing_utils.py:4-5
   unpack_gemm, dequantize_gemm ......... awq/utils/packing_utils.py:8-43,87-102
   pack_gemm ............................ awq/modules/linear/gemm.py:194-249

@@ -6,7 +6,7 @@ What the reference executes on a CPU box (no awq_ext, no Triton, no IPEX):
 WQLinearMMFunction.forward's naive branch, awq/modules/linear/gemm.py:71-77 (identical to
 WQLinear_IPEX's fallback, awq/modules/linear/gemm_ipex.py:105-107): dequantize_gemm
 (awq/utils/packing_utils.py:87-102) followed by torch.matmul in fp16, on every call.
-/root/reference does not exist on the GPU box, hence this port; its dequant is checked bit-for-bit
+The reference checkout is not available where the GPU runs, hence this port; its dequant is checked bit-for-bit
 against the numpy oracle (tests/test_oracle_golden.py::test_torch_port_matches_oracle).
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE (oracle): numpy restatement of the B200 *stream format* - the one-time re-layout of a
+"""TEST INFRASTRUCTURE (oracle): numpy restatement of the *stream format* - the one-time re-layout of a
 GEMM-layout AWQ linear (awq/modules/linear/gemm.py:135-158: qweight [K, N/8] i32, qzeros [K/G, N/8] i32, scales
 [K/G, N] f16) that the decode-program kernel streams (autoawq_b200/csrc/program_stream.cuh; the reference's
 precedent for a post-load re-layout is awq/modules/linear/exllama.py:66-79).  Only tests may import this.

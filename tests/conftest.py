@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -36,7 +36,7 @@ def golden_dir():
 
 @pytest.fixture(autouse=True, scope="session")
 def _program_watchdog_for_sanitizer_runs():
-    """B200AWQ_WATCHDOG_S=<seconds> (tools/sanitize.sh): lengthen the decode-program kernels' spin watchdog
+    """B200AWQ_WATCHDOG_S=<seconds> (runs under compute-sanitizer): lengthen the decode-program kernels' spin watchdog
     (knob 16) - under compute-sanitizer a healthy wait takes longer than the default 0.5 s."""
     secs = os.environ.get("B200AWQ_WATCHDOG_S")
     if secs:

@@ -1,6 +1,6 @@
 """Generate the golden fixtures in this directory FROM THE REAL REFERENCE.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Run where an upstream checkout of the reference exists (AWQ_REFERENCE_DIR, see oracle/reference.py):
 
     python tests/golden/make_golden.py
 
@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
+REF = os.environ.get("AWQ_REFERENCE_DIR", "/root/reference")
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))  # repo root, for oracle.*
 
 warnings.filterwarnings("ignore")

@@ -1,6 +1,6 @@
 """The driver's contract for `bench.py --impl reference` (the reference's CPU path on the host cores), checked on the CPU
 box: ONE JSON line with the keys the driver reads, the CPU-baseline description, zero-copy e2e, and the workload named in
-`config`.  (The B200 arm needs a GPU; its line is checked by the driver and recorded under profiles/.)"""
+`config`.  (The GPU arm needs a GPU; its line is checked on the H100.)"""
 import json
 import os
 import subprocess

@@ -6,7 +6,7 @@ Bars: integer unpack + dequantisation: BIT-EXACT.  Forward outputs (fp16), again
 y64 = X . W16 of the bit-exact dequantised fp16 weights:
     |y - y64| <= 2^-10 * |y64|  +  wr * (|X| . |W16|)  +  1e-6
   * 2^-10 |y64|: the single rounding of the result to fp16 (2^-11) with a factor 2 of slack;
-  * wr = 2^-16 on the tcgen05 path (its A operand IS W16, bit-exact; only fp32 accumulation order differs);
+  * wr = 2^-16 on the wgmma path (its A operand IS W16, bit-exact; only fp32 accumulation order differs);
   * wr = 2^-11 on the M <= 8 GEMV path: it applies scale / zero-point per group in fp32 instead of rounding
     every weight to fp16 first - closer to the real-number value (q - z) * s than the reference, and at most
     one fp16 rounding PER WEIGHT away from it, which is exactly what 2^-11 (|X| . |W16|) bounds.
@@ -190,11 +190,11 @@ def test_workspace_is_self_cleaning(ext):
     y0 = e.linear_forward("gemm", *args)
     x16 = np.random.default_rng(2).standard_normal((24, 4096)).astype(np.float16)
     e.linear_forward("gemm", _t(x16), *args[1:])
-    # split-K of the tcgen05 GEMM above 128 tokens (4 tiles x 64 k-steps: 16 slices pay at 160 tokens)
+    # split-K of the wgmma GEMM above 128 tokens (4 tiles x 64 k-steps: 16 slices pay at 160 tokens)
     x200 = np.random.default_rng(3).standard_normal((160, 4096)).astype(np.float16)
     w = O.dequantize_gemm(c["qweight"], c["qzeros"], c["scales"], 128)
     y200 = e.linear_forward("gemm", _t(x200), *args[1:]).cpu().numpy()
-    _close(y200, O.gemm_f64(x200, w), _budget(x200, w), WR_TC, "split-K tcgen05 GEMM, M = 160")
+    _close(y200, O.gemm_f64(x200, w), _budget(x200, w), WR_TC, "split-K wgmma GEMM, M = 160")
     torch.cuda.synchronize()
     for ws in e._WS.values():
         assert int(ws.view(torch.int32).ne(0).sum()) == 0
@@ -385,7 +385,7 @@ def test_persistent_gemv_is_bit_reproducible(ext):
     """Round 2: the M = 1 GEMV adds its split-K partials as 64-bit fixed-point words with ONE returning atomic per
     element (csrc/gemv_tile.cuh): integer addition does not depend on the arrival order of the CTAs, so repeated calls
     agree bit for bit (round 1's fp32 REDs did not), and the workspace is all-zero afterwards.  (M >= 2 keeps the fp32
-    REDs: measured faster there.)"""
+    REDs.)"""
     from autoawq_b200 import ext as e
 
     for (K, N, M) in [(4096, 4096, 1), (4096, 6144, 1), (14336, 4096, 1), (4096, 28672, 1)]:

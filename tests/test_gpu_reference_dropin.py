@@ -1,13 +1,13 @@
-"""The drop-in, exercised for real: the UNMODIFIED reference package (tests/_refload.py: baseline/_ref, installed by
+"""The drop-in, exercised for real: the UNMODIFIED reference package (tests/_refload.py: oracle/_ref, copied by
 `__graft_entry__.build()`) imported with this repo's `awq_ext` / `awq_v2_ext` on the path, so that the reference's
 own module classes - WQLinear_GEMM / GEMV / GEMVFast (awq/modules/linear/*.py), WQLinearMMFunction incl. backward
 (gemm.py:24-114), FasterTransformerRMSNorm (fused/norm.py:19-38), fuse_qkv (utils/fused_utils.py:45-142),
 apply_moe_weights (fused/moe.py:45-89) and the loader `from_quantized` / `_load_quantized_modules`
-(models/base.py:409-570,634-685) - run on the B200 kernels.  Results are compared with the CPU oracle (fp64
+(models/base.py:409-570,634-685) - run on this repository's kernels.  Results are compared with the CPU oracle (fp64
 contraction of the bit-exact dequantised weights), not with this repo's mirrors.
 
-Skipped (loudly) when no copy of the reference is reachable; on the GPU box `baseline/_ref` travels with the
-snapshot.
+Skipped (loudly) when no copy of the reference is reachable: `oracle/_ref` is made by `build()` where an upstream
+checkout exists and travels with the built tree.
 """
 import json
 import os
@@ -49,8 +49,8 @@ def _close(y, ref64, budget, wr, what=""):
 def ref():
     awq = _refload.load_reference(shim=True)
     if awq is None:
-        pytest.skip("no copy of the reference reachable (baseline/_ref missing: run __graft_entry__.build() in the "
-                    "build container before shipping)")
+        pytest.skip("no copy of the reference reachable (oracle/_ref missing: run __graft_entry__.build() where "
+                    "an upstream checkout exists)")
     import awq.modules.linear.gemm as G
     import awq.modules.linear.gemv as V
     import awq.modules.linear.gemv_fast as F

@@ -3,7 +3,7 @@
   Llama-3-8B (config 2/3):       qkv 4096x6144, o 4096x4096, gate|up 4096x28672, down 14336x4096
   Llama-3-70B / 8 ranks (cfg 5): qkv 8192x1280, o 1024x8192, gate|up 8192x7168,  down 3584x8192
 
-x M in {1, 2, 4, 8, 16, 64, 300} (GEMV kernels, the small-batch kernel, the tcgen05 kernel) in all three
+x M in {1, 2, 4, 8, 16, 64, 300} (GEMV kernels, the small-batch kernel, the wgmma kernel) in all three
 checkpoint layouts (GEMM / GEMV / GEMVFast), through the awq_ext / awq_v2_ext operator surface.  The oracle is
 the fp64 contraction of the bit-exact dequantised weights, evaluated on a strided sample of output columns
 (every 61st + the edges: the full product at M = 300 on 4096x28672 would be 70 GFLOP of fp64 per case; each

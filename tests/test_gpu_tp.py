@@ -1,5 +1,5 @@
 """2-GPU check of the column -> row sharded MLP with the NCCL all-reduce (skipped with fewer than 2 GPUs).
-Compares the tensor-parallel result on the B200 kernels with the unsharded oracle contraction."""
+Compares the tensor-parallel result on this repository's kernels with the unsharded oracle contraction."""
 import os
 import socket
 

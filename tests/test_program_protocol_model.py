@@ -134,7 +134,7 @@ def test_protocol_random_schedules(seed):
 
 def test_protocol_catches_the_lane0_bug():
     """Publishing staged[i] before the warp's other lanes finished polling lets another CTA zero the row under them:
-    they then wait for ever (what tools/program_stuck.py showed on the GPU)."""
+    they then wait for ever (what the kernel's abort record showed on the GPU)."""
     hit = 0
     for seed in range(40):
         try:

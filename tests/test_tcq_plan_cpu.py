@@ -13,7 +13,7 @@ SHAPES = [(4096, 4096), (4096, 6144), (4096, 14336), (4096, 28672), (14336, 4096
           (8192, 7168), (3584, 8192), (512, 256), (1152, 384), (2048, 640), (128, 128), (4096, 128)]
 
 
-def _plan(M, K, N, sms=148, mode=0, G=128):
+def _plan(M, K, N, sms=132, mode=0, G=128):
     g, kp = ctypes.c_int(0), ctypes.c_int(0)
     rc = lib.b200awq_tcq_plan(M, K, N, G, sms, mode, ctypes.byref(g), ctypes.byref(kp))
     return rc, g.value, kp.value
@@ -39,7 +39,7 @@ def test_plan_covers_every_pair_once(K, N, M, mode):
     assert rc == 0 and KP == K // 128
     n_tiles = N // 128
     T = n_tiles * KP
-    assert 1 <= grid <= 148
+    assert 1 <= grid <= 132
     seen = [[0] * KP for _ in range(n_tiles)]
     tickets = [0] * n_tiles
     for b in range(grid):
@@ -53,10 +53,10 @@ def test_plan_covers_every_pair_once(K, N, M, mode):
                 seen[nt][d] += 1
             if not (d0 == 0 and d1 == KP):      # partial segment: split-K ticket
                 tickets[nt] += d1 - d0
-        if mode == 2 or (mode == 0 and (n_tiles <= 148 or M >= 64)):
-            if n_tiles <= 148 or n_tiles % -(-n_tiles // 148) == 0:
+        if mode == 2 or (mode == 0 and (n_tiles <= 132 or M >= 64)):
+            if n_tiles <= 132 or n_tiles % -(-n_tiles // 132) == 0:
                 assert len({nt for nt, _, _ in segs}) == len(segs), "one segment per tile"
-                if n_tiles <= 148:
+                if n_tiles <= 132:
                     assert len(segs) == 1, "tile-aligned cut: a range never straddles a tile"
     assert all(c == 1 for row in seen for c in row)
     assert all(t in (0, KP) for t in tickets), "partial segments of a tile complete exactly K / 128"
@@ -68,14 +68,14 @@ def test_plan_envelope_and_errors():
     assert _plan(16, 4096, 4096 + 64)[0] != 0      # N % 128
     assert _plan(16, 4096, 4096, G=32)[0] != 0     # G < 64
     assert _plan(16, 4096, 4096, G=64)[0] == 0
-    assert lib.b200awq_tcq_plan(16, 4096, 4096, 128, 148, 0, None, None) != 0
+    assert lib.b200awq_tcq_plan(16, 4096, 4096, 128, 132, 0, None, None) != 0
 
 
 def test_plan_examples_from_design():
-    """The cuts DESIGN 3.3b quotes: 112 whole tiles for 4096 x 14336, 4 ranges per tile for 4096 x 4096, balanced 148
+    """The cuts DESIGN 3.3b quotes: 112 whole tiles for 4096 x 14336, 4 ranges per tile for 4096 x 4096, balanced 132
     below 64 tokens and 112 x 2 tiles from 64 tokens on 4096 x 28672."""
     assert _plan(16, 4096, 14336)[1] == 112
     assert _plan(16, 4096, 4096)[1] == 128
-    assert _plan(16, 4096, 28672)[1] == 148
+    assert _plan(16, 4096, 28672)[1] == 132
     assert _plan(64, 4096, 28672)[1] == 112
-    assert _plan(16, 4096, 6144)[1] == 144
+    assert _plan(16, 4096, 6144)[1] == 96

@@ -1,14 +1,16 @@
 """Executable model of the small-M tensor-core kernel's pipeline protocol (csrc/gemm_tc.cu: gemm_tcq_kernel), run on
-the CPU.  The kernel's six kinds of warps talk through mbarrier rings only - packed stages (Q-TMA -> both producer
-teams), A stages (team t -> MMA warp t), activation stages (X-TMA -> MMA warps), two TMEM accumulator buffers (MMA warps
--> epilogue) - and every ring index / phase-parity expression of the device code is restated here verbatim.  Random
-interleavings of the roles (and of the asynchronous agents: TMA landings, tensor-core execution and its commits) check
+the CPU.  The kernel's four kinds of warps talk through mbarrier rings only - packed stages (Q-TMA -> the producer
+warps), A stages (producers -> the consumer warpgroups), activation stages (X-TMA -> consumers) - and each of the two
+consumer warpgroups (independent roles, one arrival per warp) releases a stage only after the wgmma group that read it
+has retired (`wgmma.wait_group 1` after issuing the next group, `wait_group 0` at the end of a segment).  Every ring index / phase-parity expression of the device code is
+restated here verbatim.  Random interleavings of the roles (and of the asynchronous agents: TMA landings, tensor-core
+execution) check
 
   * liveness: every role finishes (no lost wake-up, no wait on a parity that never comes);
   * safety: a stage is never overwritten before its last reader has read it, and every reader sees exactly the step it
-    expects (packed stage d -> both teams, A stage of k-step s -> the MMA of k-step s, X stage likewise), also across ring
-    wrap-arounds, several segments per CTA (TMEM buffer recycling) and one-pair ranges;
-  * the accumulators the epilogue drains hold exactly the k-steps of the segment, once each.
+    expects (packed stage d -> both k-steps of the pair, A stage of k-step s -> the MMA of k-step s, X stage likewise),
+    also across ring wrap-arounds, several segments per CTA and one-pair ranges;
+  * the accumulators the epilogue reads hold exactly the k-steps of the segment, once each.
 
 The model knows nothing about CUDA: it pins the index arithmetic, which is where such kernels break.  (The real
 kernel's own tests are tests/test_gpu_parity.py::test_small_m_*.)"""
@@ -35,22 +37,20 @@ class Mbar:
 
 
 class Sim:
-    def __init__(self, NS, NX, NQ, ranges, KP, seed):
+    def __init__(self, NS, NX, NQ, ranges, KP, seed, empty_count=8):
         self.NS, self.NX, self.NQ, self.KP = NS, NX, NQ, KP
         self.t_begin, self.t_end = ranges
         self.rng = random.Random(seed)
-        self.full = [Mbar(8) for _ in range(NS)]          # 8 producer warps of one team (modelled as 1 agent x 8 arrivals)
-        self.empty = [Mbar(1) for _ in range(NS)]
+        self.full = [Mbar(8) for _ in range(NS)]          # 8 producer warps (modelled as 1 agent x 8 arrivals)
+        self.empty = [Mbar(empty_count) for _ in range(NS)]   # 8 consumer warps: 4 per warpgroup
         self.xfull = [Mbar(2) for _ in range(NX)]         # expect_tx arrival + "bytes landed"
-        self.xempty = [Mbar(1) for _ in range(NX)]
+        self.xempty = [Mbar(empty_count) for _ in range(NX)]
         self.qfull = [Mbar(2) for _ in range(NQ)]
-        self.qempty = [Mbar(16) for _ in range(NQ)]       # both teams
-        self.tmem_full = [Mbar(2) for _ in range(2)]      # one commit per MMA warp
-        self.tmem_empty = [Mbar(128) for _ in range(2)]
+        self.qempty = [Mbar(8) for _ in range(NQ)]
         self.q_data = [None] * NQ                          # content tags: what a stage currently holds
         self.a_data = [None] * NS
         self.x_data = [None] * NX
-        self.acc = [[[] for _ in range(2)] for _ in range(2)]   # [buf][team] -> accumulated k-steps
+        self.acc = [[], []]                                # per consumer warpgroup: k-steps of its retired MMAs
         self.async_ops = []                                # pending asynchronous actions (TMA landings, MMA execution)
         self.drained = []                                  # (segment, steps) seen by the epilogue
 
@@ -88,71 +88,71 @@ class Sim:
                 if xs == self.NX:
                     xs, xph = 0, xph ^ 1
 
-    def producer(self, team):
-        steps = [(nt, d) for nt, d0, d1 in self.segments() for d in range(d0, d1)]
-        npairs = len(steps)
-        qs, stage, qph, phase = 0, team, 0, 0
-        cur = None
-        if npairs > 0:
-            yield lambda: self.qfull[0].passed(0)
-            cur = self.q_data[0]
-        for i in range(npairs):
-            qs_n = 0 if qs + 1 == self.NQ else qs + 1
-            qph_n = qph ^ 1 if qs + 1 == self.NQ else qph
-            nxt = None
-            if i + 1 < npairs:
-                yield lambda qs_n=qs_n, qph_n=qph_n: self.qfull[qs_n].passed(qph_n)
-                nxt = self.q_data[qs_n]                                    # fetch: LDS of the next stage
-            yield lambda stage=stage, phase=phase: self.empty[stage].passed(phase ^ 1)
-            assert cur == steps[i], f"team {team}: packed stage holds {cur}, expected {steps[i]}"
-            nt, d = steps[i]
-            self.a_data[stage] = (nt, 2 * d + team)                       # dequantised tile of k-step 2 d + team
-            for _ in range(8):
-                self.full[stage].arrive()
-                self.qempty[qs].arrive()
-            stage += 2
-            if stage >= self.NS:
-                stage, phase = stage - self.NS, phase ^ 1
-            cur, qs, qph = nxt, qs_n, qph_n
-
-    def mma(self, mw):
-        stage, xs, phase, xph = mw, mw, 0, 0
-        for it, (nt, d0, d1) in enumerate(self.segments()):
-            buf, use = it & 1, (it >> 1) & 1
-            yield lambda buf=buf, use=use: self.tmem_empty[buf].passed(use ^ 1)
+    def producer(self):
+        qs, stage, qph, phase = 0, 0, 0, 0
+        for nt, d0, d1 in self.segments():
             for d in range(d0, d1):
+                yield lambda qs=qs, qph=qph: self.qfull[qs].passed(qph)
+                got = self.q_data[qs]                                      # fetch: LDS of both halves of the stage
+                assert got == (nt, d), f"packed stage {qs} holds {got}, expected {(nt, d)}"
+                for h in range(2):
+                    yield lambda stage=stage, phase=phase: self.empty[stage].passed(phase ^ 1)
+                    self.a_data[stage] = (nt, 2 * d + h)                   # dequantised tile of k-step 2 d + h
+                    for _ in range(8):
+                        self.full[stage].arrive()
+                        if h == 1:
+                            self.qempty[qs].arrive()
+                    stage += 1
+                    if stage == self.NS:
+                        stage, phase = 0, phase ^ 1
+                qs += 1
+                if qs == self.NQ:
+                    qs, qph = 0, qph ^ 1
+
+    def pending_mma(self, wg):
+        return sum(1 for op in self.async_ops if op[0] == "mma" and op[1] == wg)
+
+    def consumer(self, wg):
+        """Consumer warpgroup wg (4 warps, one arrival each): its own wgmma groups, its own half of every A stage."""
+        stage, xs, phase, xph = 0, 0, 0, 0
+        for it, (nt, d0, d1) in enumerate(self.segments()):
+            self.acc[wg] = []
+            prev = None
+            for s in range(2 * d0, 2 * d1):
                 yield lambda xs=xs, xph=xph: self.xfull[xs].passed(xph)
                 yield lambda stage=stage, phase=phase: self.full[stage].passed(phase)
-                # issue: the tensor core reads the operands LATER (asynchronously), then the commits arrive
-                self.async_ops.append(("mma", mw, buf, stage, xs, (nt, 2 * d + mw), d == d0))
-                stage += 2
-                if stage >= self.NS:
-                    stage, phase = stage - self.NS, phase ^ 1
-                xs += 2
-                if xs >= self.NX:
-                    xs, xph = xs - self.NX, xph ^ 1
-            self.async_ops.append(("commit_acc", mw, buf))
-
-    def epilogue(self):
-        for it, (nt, d0, d1) in enumerate(self.segments()):
-            buf, use = it & 1, (it >> 1) & 1
-            yield lambda buf=buf, use=use: self.tmem_full[buf].passed(use)
-            got = sorted(self.acc[buf][0] + self.acc[buf][1])
+                # issue + commit: the tensor core reads the operands LATER (asynchronously)
+                self.async_ops.append(("mma", wg, stage, xs, (nt, s)))
+                yield lambda: self.pending_mma(wg) <= 1                   # wgmma.wait_group 1
+                if prev is not None:
+                    for _ in range(4):
+                        self.empty[prev[0]].arrive()
+                        self.xempty[prev[1]].arrive()
+                prev = (stage, xs)
+                stage += 1
+                if stage == self.NS:
+                    stage, phase = 0, phase ^ 1
+                xs += 1
+                if xs == self.NX:
+                    xs, xph = 0, xph ^ 1
+            yield lambda: self.pending_mma(wg) == 0                       # wgmma.wait_group 0
+            if prev is not None:
+                for _ in range(4):
+                    self.empty[prev[0]].arrive()
+                    self.xempty[prev[1]].arrive()
             want = [(nt, s) for s in range(2 * d0, 2 * d1)]
-            assert got == want, f"segment {it}: accumulators hold {got}, expected {want}"
-            self.drained.append((it, got))
-            for _ in range(128):
-                self.tmem_empty[buf].arrive()
+            assert sorted(self.acc[wg]) == want, f"segment {it}, warpgroup {wg}: accumulators hold {self.acc[wg]}"
+            self.drained.append((it, wg, list(self.acc[wg])))
 
-    # ---- asynchronous agents: per-queue FIFO order (TMA per ring, tensor core per issuing warp), random across queues
+    # ---- asynchronous agents: the tensor core executes each warpgroup's MMAs in issue order (the two warpgroups
+    # independently); TMA landings of one ring may complete in any order relative to other rings - pick any op that is
+    # first of its (kind, ring or warpgroup) queue
     def step_async(self):
         if not self.async_ops:
             return False
-        # the tensor core executes one warp's MMAs / commits in issue order; TMA landings of one ring may complete in
-        # any order relative to other rings - pick any op that is first of its (kind, owner) queue
         firsts, seen = [], set()
         for i, op in enumerate(self.async_ops):
-            key = ("tc", op[1]) if op[0] in ("mma", "commit_acc") else (op[0], op[1])
+            key = (op[0], op[1])
             if key not in seen:
                 seen.add(key)
                 firsts.append(i)
@@ -165,23 +165,15 @@ class Sim:
             _, xs, tag = op
             self.x_data[xs] = tag
             self.xfull[xs].arrive()
-        elif op[0] == "mma":
-            _, mw, buf, stage, xs, want, first = op
-            assert self.a_data[stage] == want, f"MMA {mw}: A stage {stage} holds {self.a_data[stage]}, expected {want}"
-            assert self.x_data[xs] == want, f"MMA {mw}: X stage {xs} holds {self.x_data[xs]}, expected {want}"
-            if first:
-                self.acc[buf][mw] = []
-            self.acc[buf][mw].append(want)
-            self.empty[stage].arrive()        # tcgen05.commit -> empty[stage], xempty[xs]
-            self.xempty[xs].arrive()
         else:
-            _, mw, buf = op
-            self.tmem_full[buf].arrive()
+            _, wg, stage, xs, want = op
+            assert self.a_data[stage] == want, f"MMA {wg}: A stage {stage} holds {self.a_data[stage]}, expected {want}"
+            assert self.x_data[xs] == want, f"MMA {wg}: X stage {xs} holds {self.x_data[xs]}, expected {want}"
+            self.acc[wg].append(want)
         return True
 
     def run(self):
-        roles = {"q": self.q_tma(), "x": self.x_tma(), "p0": self.producer(0), "p1": self.producer(1),
-                 "m0": self.mma(0), "m1": self.mma(1), "e": self.epilogue()}
+        roles = {"q": self.q_tma(), "x": self.x_tma(), "p": self.producer(), "c0": self.consumer(0), "c1": self.consumer(1)}
         waiting = {}
         for name, gen in list(roles.items()):
             try:
@@ -207,7 +199,7 @@ class Sim:
             assert idle < 3, f"deadlock: {sorted(roles)} blocked, {len(self.async_ops)} async ops pending"
         while self.step_async():
             pass
-        assert len(self.drained) == len(self.segments())
+        assert len(self.drained) == 2 * len(self.segments())
 
 
 CONFIGS = [
@@ -231,14 +223,26 @@ def test_model_detects_a_missing_release():
     """The model is not vacuous: without the producers' wait for `empty` an A stage is overwritten before its MMA ran."""
 
     class Broken(Sim):
-        def producer(self, team):
-            for cond in Sim.producer(self, team):
+        def producer(self):
+            for cond in Sim.producer(self):
                 yield cond if "empty" not in cond.__code__.co_names else (lambda: True)
 
     caught = 0
     for seed in range(20):
         try:
             Broken(2, 16, 14, (0, 64), 32, seed).run()
+        except AssertionError:
+            caught += 1
+    assert caught > 0
+
+
+def test_model_detects_a_barrier_count_of_one_warpgroup():
+    """With `empty` / `xempty` initialised for one warpgroup's 4 arrivals instead of both warpgroups' 8, the faster
+    warpgroup frees a stage the other one may still be reading."""
+    caught = 0
+    for seed in range(40):
+        try:
+            Sim(2, 2, 3, (0, 64), 32, seed, empty_count=4).run()
         except AssertionError:
             caught += 1
     assert caught > 0
