@@ -77,6 +77,8 @@ SIGNATURES = {
     "b200awq_comm_error": (_c_int, [_c_void_p]),
     "b200awq_comm_destroy": (_c_int, [_c_void_p]),
     "b200awq_program_create": (_c_int, [ctypes.POINTER(Op), _c_int, ctypes.POINTER(_c_void_p)]),
+    "b200awq_program_create_batched": (_c_int, [ctypes.POINTER(Op), _c_int, _c_int, ctypes.POINTER(_c_void_p)]),
+    "b200awq_program_tokens": (_c_int, [_c_void_p]),
     "b200awq_program_num_ops": (_c_int, [_c_void_p]),
     "b200awq_program_kind": (_c_int, [_c_void_p]),
     "b200awq_stream_bytes": (_c_size_t, [_c_int, _c_int, _c_int]),

@@ -206,20 +206,29 @@ int b200awq_silu_and_mul(const void* gate_up, void* out, int rows, int d, b200aw
 }
 
 
-int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t* out) {
+int b200awq_program_create_batched(const b200awq_op_t* ops, int n_ops, int max_tokens, b200awq_program_t* out) {
   if (out == nullptr) return B200AWQ_EINVAL;
   *out = nullptr;
+  if (max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
   Program* p = nullptr;
   cudaError_t ce = cudaSuccess;
-  const int rc = program_create(ops, n_ops, &p, &ce);
+  const int rc = program_create(ops, n_ops, max_tokens, &p, &ce);
   if (rc == B200AWQ_ECUDA) return fold(ce);
   if (rc != B200AWQ_OK) return rc;
   *out = reinterpret_cast<b200awq_program_t>(p);
   return B200AWQ_OK;
 }
 
+int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t* out) {
+  return b200awq_program_create_batched(ops, n_ops, 1, out);
+}
+
 int b200awq_program_num_ops(b200awq_program_t prog) {
   return prog == nullptr ? 0 : program_num_ops(reinterpret_cast<Program*>(prog));
+}
+
+int b200awq_program_tokens(b200awq_program_t prog) {
+  return prog == nullptr ? 0 : program_m(reinterpret_cast<Program*>(prog));
 }
 
 int b200awq_program_kind(b200awq_program_t prog) {

@@ -59,6 +59,7 @@ struct __align__(128) ProgOp {
   int n_part;             // CTAs that share this op's tiles (the first n_part; 0 = all): small ops use fewer, so that
                           // fewer CTAs add into each column block (knob 13 = minimum tiles per participating CTA)
   const int32_t* qw_src;  // the checkpoint-format qweight (host-side use: the stream variant re-lays it out)
+  int src_ld;             // row pitch of src in elements (host-side use: the batched stream variant, M > 1)
 };
 static_assert(sizeof(ProgOp) == 256, "ProgOp layout");
 
@@ -230,6 +231,7 @@ __device__ __forceinline__ void prog_wait_row_clean(volatile int* red_ok, const 
 
 }  // namespace b200awq
 #include "program_stream.cuh"
+#include "program_batch.cuh"
 namespace b200awq {
 
 constexpr int kProgThreads = kV3Threads + 32;   // producer warp + 8 consumer warps + duty warp
@@ -708,6 +710,8 @@ struct Program {
   int* d_state = nullptr;
   int row_stride = 0;
   size_t stream_bytes = 0;
+  // batched stream variant (M > 1, program_batch.cuh): ring stages per warp, sets per CTA, units along K (smem sizes)
+  int sb_spw = 0, sb_lmax = 0, sb_nu_max = 0;
 };
 
 size_t stream_format_bytes(int K, int N, int G) {
@@ -735,9 +739,10 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
   return cudaGetLastError();
 }
 
-// Builds the stream variant from the folded op table.  Returns false when the sequence is outside its envelope
-// (the caller then tries the split-K kernel).  *err != cudaSuccess reports a CUDA failure.
-static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, cudaError_t* err) {
+// Builds the stream variant from the folded op table, for M token rows (M > 1: the batched kernel of
+// program_batch.cuh).  Returns false when the sequence is outside its envelope (the caller then tries the split-K
+// kernel, M = 1 only).  *err != cudaSuccess reports a CUDA failure.
+static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
@@ -758,20 +763,32 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       }
     }
   size_t wbytes = 0, max_cols = 0;
-  int max_K = 0;
+  int max_K = 0, lmax = 0, nu_max = 0;
   std::vector<size_t> woff(n);
   for (int i = 0; i < n; ++i) {
     const ProgOp& p = table[i];
     if (!stream_format_supported(p.K, p.N, p.G, mode[i])) return false;
     const int UK = p.G < 128 ? p.G : 128;
     if (p.K / UK > kSpXsumMax) return false;
-    if ((p.N / 16 + grid - 1) / grid > kSpLMax) return false;
+    if (M == 1 && (p.N / 16 + grid - 1) / grid > kSpLMax) return false;
+    lmax = std::max(lmax, (p.N / 16 + grid - 1) / grid);
+    nu_max = std::max(nu_max, p.K / UK);
     woff[i] = wbytes;
     wbytes += (stream_format_bytes(p.K, p.N, p.G) + 255) & ~(size_t)255;
     max_cols = std::max(max_cols, (size_t)(mode[i] ? p.N / 2 : p.N));
     max_K = std::max(max_K, p.K);
   }
-  if (sp_fixed_smem(12, 3) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;   // (the largest configuration)
+  if (M == 1) {
+    if (sp_fixed_smem(12, 3) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;   // (the largest configuration)
+  } else {
+    // the batched kernel: the deepest ring (<= 4 stages per warp) that leaves room for M rows of activations
+    int spw = kSbMaxStages;
+    while (spw > 0 && sb_fixed_smem(spw, lmax, sb_mt(M), nu_max) + (size_t)max_K * sb_mt(M) * 2 > (size_t)227 * 1024) --spw;
+    if (spw == 0) return false;
+    pr->sb_spw = spw;
+    pr->sb_lmax = lmax;
+    pr->sb_nu_max = nu_max;
+  }
   for (int i = 0; i < n; ++i) {
     const ProgOp& p = table[i];
     SpOp& o = ops[i];
@@ -809,11 +826,14 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
         if (mode[j] == 1 || i - j >= kSpRows) return false;   // raw gate|up columns of a fused producer / row recycled
         const uintptr_t y0 = reinterpret_cast<uintptr_t>(table[j].y), s0 = reinterpret_cast<uintptr_t>(p.src);
         if (s0 < y0 || s0 + (size_t)p.K * 2 > y0 + (size_t)table[j].N * 2 || ((s0 - y0) & 7) != 0) return false;
+        if (M > 1 && p.src_ld != table[j].N) return false;   // row m of the source must be row m of the producer
         o.src_op = j;
         o.src_off = static_cast<int>((s0 - y0) / 2);
       } else {
         o.src = p.src;
         if ((reinterpret_cast<uintptr_t>(p.src) & 7) != 0) return false;
+        if (M > 1 && ((reinterpret_cast<uintptr_t>(p.src) & 15) != 0 || (p.src_ld % 8) != 0)) return false;
+        o.ldx = p.src_ld;
       }
     }
   }
@@ -827,9 +847,10 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   cudaError_t e = cudaMalloc(&pr->d_stream, wbytes);
   if (e == cudaSuccess) e = cudaMalloc(&pr->d_sp_ops, (size_t)n * sizeof(SpOp));
   if (e == cudaSuccess) e = cudaMalloc(&pr->d_cta, cta.size() * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&pr->d_rows, (size_t)kSpRows * pr->row_stride * sizeof(uint32_t));
+  const size_t row_bytes = (size_t)kSpRows * M * pr->row_stride * sizeof(uint32_t);   // M hand-off rows per op
+  if (e == cudaSuccess) e = cudaMalloc(&pr->d_rows, row_bytes);
   if (e == cudaSuccess) e = cudaMalloc(&pr->d_state, 2 * sizeof(int));
-  if (e == cudaSuccess) e = cudaMemset(pr->d_rows, 0, (size_t)kSpRows * pr->row_stride * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMemset(pr->d_rows, 0, row_bytes);
   if (e == cudaSuccess) e = cudaMemset(pr->d_state, 0, 2 * sizeof(int));
   for (int i = 0; i < n && e == cudaSuccess; ++i) {
     ops[i].wstream = pr->d_stream + woff[i];
@@ -843,6 +864,13 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     e = cudaFuncSetAttribute(stream_program_kernel<8, 4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(stream_program_kernel<12, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  if (e == cudaSuccess && M > 1) {
+    e = cudaFuncSetAttribute(stream_batch_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  }
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     cudaFree(pr->d_stream);
@@ -860,7 +888,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   }
   pr->stream = true;
   pr->stream_bytes = wbytes;
-  pr->xs_bytes = (size_t)max_K * 2;
+  pr->xs_bytes = (size_t)max_K * (M == 1 ? 1 : sb_mt(M)) * 2;   // M = 1: one row (stream_program_kernel)
   return true;
 }
 
@@ -889,10 +917,11 @@ static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
 //     overlap with the previous op's output is rejected; outputs older than that are ordinary global reads;
 //   * a linear must not write (y) what it reads (src) or what its own prologue publishes (xout);
 //   * a buffer that a pending glue record depends on must not be overwritten before the record's last use.
-int program_create(const b200awq_op_t* ops, int n, Program** out, cudaError_t* cuda_err) {
+// Every op has the same M <= max_tokens rows (M > 1: the batched stream kernel only); extents below cover all M rows.
+int program_create(const b200awq_op_t* ops, int n, int max_tokens, Program** out, cudaError_t* cuda_err) {
   *cuda_err = cudaSuccess;
   *out = nullptr;
-  if (ops == nullptr || n <= 0) return B200AWQ_EINVAL;
+  if (ops == nullptr || n <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
   std::vector<ProgOp> table;
   struct Glue {
     int kind;
@@ -912,22 +941,23 @@ int program_create(const b200awq_op_t* ops, int n, Program** out, cudaError_t* c
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
     if (op.M != M) return B200AWQ_EUNSUPPORTED;
+    auto rows_bytes = [&](int width) { return (size_t)(M > 0 ? M : 1) * width * 2; };   // M contiguous fp16 rows
     if (op.kind == B200AWQ_OP_RMSNORM || op.kind == B200AWQ_OP_SILU_AND_MUL) {
       if (op.x == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
       if (op.kind == B200AWQ_OP_RMSNORM && op.weight == nullptr) return B200AWQ_EINVAL;
       if ((op.K % 8) != 0 || !aligned16(op.x) || !aligned16(op.y) || (op.weight != nullptr && !aligned16(op.weight)))
         return B200AWQ_EUNSUPPORTED;
-      const size_t in_bytes = (size_t)(op.kind == B200AWQ_OP_SILU_AND_MUL ? 2 : 1) * op.K * 2;
-      if (overlaps(op.y, (size_t)op.K * 2, op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;  // in-place glue op
+      const size_t in_bytes = (size_t)M * (op.kind == B200AWQ_OP_SILU_AND_MUL ? 2 : 1) * op.K * 2;
+      if (overlaps(op.y, rows_bytes(op.K), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;  // in-place glue op
       for (Glue& gl : glues)
-        if (gl.live && (overlaps(gl.out, (size_t)gl.width * 2, op.y, (size_t)op.K * 2) ||
-                        overlaps(gl.src, (size_t)(gl.kind == kProSilu ? 2 : 1) * gl.width * 2, op.y, (size_t)op.K * 2))) {
+        if (gl.live && (overlaps(gl.out, rows_bytes(gl.width), op.y, rows_bytes(op.K)) ||
+                        overlaps(gl.src, rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width), op.y, rows_bytes(op.K)))) {
           if (!gl.used) return B200AWQ_EUNSUPPORTED;
           gl.live = false;
         }
       // its input must not be a buffer only CTA 0 publishes
       for (const Glue& gl : glues)
-        if (overlaps(gl.out, (size_t)gl.width * 2, op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
+        if (overlaps(gl.out, rows_bytes(gl.width), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
       glues.push_back(Glue{op.kind == B200AWQ_OP_RMSNORM ? kProRmsnorm : kProSilu, op.x, op.weight, op.y, op.K, op.eps,
                            false, true});
       continue;
@@ -938,9 +968,10 @@ int program_create(const b200awq_op_t* ops, int n, Program** out, cudaError_t* c
       return B200AWQ_EINVAL;
     GemmArgs a{op.x, op.ldx, static_cast<const int32_t*>(op.qweight), op.scales, static_cast<const int32_t*>(op.qzeros),
                op.bias, op.y, op.M, op.K, op.N, op.group_size};
-    if (M != 1) return B200AWQ_EUNSUPPORTED;
-    // envelope of the split-K kernel (the stream variant has its own, checked in stream_build)
-    if (!gemv_v3_supported(a) || (op.N / kV3TileCols) * (op.K / kV3TileRows) < grid ||   // every CTA owns tiles
+    if (M < 1 || M > max_tokens) return B200AWQ_EUNSUPPORTED;
+    if (M > 1 && op.ldx < op.K) return B200AWQ_EINVAL;
+    // envelope of the split-K kernel, M = 1 only (the stream variant has its own, checked in stream_build)
+    if (M > 1 || !gemv_v3_supported(a) || (op.N / kV3TileCols) * (op.K / kV3TileRows) < grid ||   // every CTA owns tiles
         op.K / kV3TileRows >= 256)                                                       // tiles per column fit the packed word
       v3_ok = false;
     ProgOp p;
@@ -982,43 +1013,48 @@ int program_create(const b200awq_op_t* ops, int n, Program** out, cudaError_t* c
       p.norm_w = static_cast<const __half*>(hit->w);
       p.xout = hit->used ? nullptr : static_cast<__half*>(hit->out);   // published once, by its first consumer
       p.eps = hit->eps;
+      p.src_ld = (hit->kind == kProSilu ? 2 : 1) * op.K;   // glue buffers are contiguous rows
       hit->used = true;
+      if (M > 1 && op.ldx != op.K) return B200AWQ_EUNSUPPORTED;
     } else {
       p.prologue = kProCopy;
       p.src = static_cast<const __half*>(op.x);
+      p.src_ld = M > 1 ? static_cast<int>(op.ldx) : op.K;
       if (!aligned16(op.x)) return B200AWQ_EUNSUPPORTED;
       for (const Glue& gl : glues)   // reading a buffer only CTA 0 publishes (a dead or mismatching record)
-        if (overlaps(gl.out, (size_t)gl.width * 2, op.x, (size_t)op.K * 2)) return B200AWQ_EUNSUPPORTED;
+        if (overlaps(gl.out, rows_bytes(gl.width), op.x, ((size_t)(M - 1) * p.src_ld + op.K) * 2)) return B200AWQ_EUNSUPPORTED;
     }
-    const size_t src_bytes = (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K * 2;
-    if (overlaps(p.y, (size_t)op.N * 2, p.src, src_bytes)) return B200AWQ_EUNSUPPORTED;
-    if (p.xout != nullptr && overlaps(p.xout, (size_t)op.K * 2, p.y, (size_t)op.N * 2)) return B200AWQ_EUNSUPPORTED;
+    // the source's M rows (row pitch src_ld), this op's output (M rows of N)
+    const size_t src_bytes = ((size_t)(M - 1) * p.src_ld + (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K) * 2;
+    const size_t y_bytes = rows_bytes(op.N);
+    if (overlaps(p.y, y_bytes, p.src, src_bytes)) return B200AWQ_EUNSUPPORTED;
+    if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), p.y, y_bytes)) return B200AWQ_EUNSUPPORTED;
     if (!table.empty()) {
       // the previous op's fp16 output reaches memory only while THIS op stages its activations: a source inside it
       // is taken from the previous op's fp32 accumulators instead (same values), anything else touching it is a race
       const ProgOp& pv = table.back();
       const uintptr_t y0 = reinterpret_cast<uintptr_t>(pv.y), s0 = reinterpret_cast<uintptr_t>(p.src);
-      if (s0 >= y0 && s0 + src_bytes <= y0 + (size_t)pv.N * 2) {
+      if (s0 >= y0 && s0 + src_bytes <= y0 + rows_bytes(pv.N)) {
         if (((s0 - y0) & 15) != 0) return B200AWQ_EUNSUPPORTED;
         p.src_prev = 1;
         p.src_off = static_cast<int>((s0 - y0) / 2);
-      } else if (overlaps(pv.y, (size_t)pv.N * 2, p.src, src_bytes)) {
+      } else if (overlaps(pv.y, rows_bytes(pv.N), p.src, src_bytes)) {
         return B200AWQ_EUNSUPPORTED;
       } else {
         // a source written by an older op of this program: wait for that op's duty-warp stores
         for (int j = static_cast<int>(table.size()) - 2; j >= 0; --j)
-          if (overlaps(table[j].y, (size_t)table[j].N * 2, p.src, src_bytes)) {
+          if (overlaps(table[j].y, rows_bytes(table[j].N), p.src, src_bytes)) {
             p.ext_dep = j;
             break;
           }
       }
-      if (p.xout != nullptr && overlaps(p.xout, (size_t)op.K * 2, pv.y, (size_t)pv.N * 2)) return B200AWQ_EUNSUPPORTED;
+      if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), pv.y, rows_bytes(pv.N))) return B200AWQ_EUNSUPPORTED;
     }
     // writing y over something a live glue record still needs ends that record
     for (Glue& gl : glues)
       if (gl.live && &gl != hit &&
-          (overlaps(gl.out, (size_t)gl.width * 2, p.y, (size_t)op.N * 2) ||
-           overlaps(gl.src, (size_t)(gl.kind == kProSilu ? 2 : 1) * gl.width * 2, p.y, (size_t)op.N * 2))) {
+          (overlaps(gl.out, rows_bytes(gl.width), p.y, y_bytes) ||
+           overlaps(gl.src, rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width), p.y, y_bytes))) {
         if (!gl.used) return B200AWQ_EUNSUPPORTED;
         gl.live = false;
       }
@@ -1036,7 +1072,7 @@ int program_create(const b200awq_op_t* ops, int n, Program** out, cudaError_t* c
   pr->max_N = max_N;
   cudaError_t e = cudaGetDevice(&pr->device);
   // first choice: the stream variant (one-time re-layout, output-stationary partition); knob 14 = 1 skips it
-  if (e == cudaSuccess && knob(14) != 1 && stream_build(pr, table, grid, &e)) {
+  if (e == cudaSuccess && knob(14) != 1 && stream_build(pr, table, grid, M, &e)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -1081,6 +1117,24 @@ cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st) {
   // staged[] and zeroed[] counters (see program_kernel)
   cudaError_t e = program_abort_clear(st);
   if (e != cudaSuccess) return e;
+  if (p->stream && p->M > 1) {
+    // batched stream variant: 8 consumer warps, the ring depth chosen at creation, MT = the smallest of 2 / 4 / 8 >= M
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(prog_sm_count());
+    cfg.blockDim = dim3(32 + kSbWarps * 32);
+    cfg.dynamicSmemBytes = sb_fixed_smem(p->sb_spw, p->sb_lmax, sb_mt(p->M), p->sb_nu_max) + p->xs_bytes;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: the hand-off polls are grid-wide waits
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const SpOp* sops = p->d_sp_ops;
+    const uint32_t* cta = p->d_cta;
+    auto kern = sb_mt(p->M) == 2 ? stream_batch_kernel<2> : (sb_mt(p->M) == 4 ? stream_batch_kernel<4> : stream_batch_kernel<8>);
+    return cudaLaunchKernelEx(&cfg, kern, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
+                              p->sb_lmax, p->sb_nu_max, knob(3));
+  }
   if (p->stream) {
     // knob 9: consumer warps of the stream kernel: 8 (4 ring stages each, 4 units in flight; the default) or 12 (3 stages,
     // 2 units).  No 16-warp variant: 17 warps put 5 on one of the SM's four register-file partitions, which caps a thread

@@ -49,7 +49,8 @@ struct __align__(128) SpOp {
   int prologue;                // kProCopy / kProRmsnorm
   int src_op, src_off;         // >= 0: the source is op src_op's published row, from column src_off
   float eps;
-  int pad_[4];
+  int ldx;                     // row pitch (elements) of `src` when a batched program stages several rows
+  int pad_[3];
 };
 static_assert(sizeof(SpOp) == 128, "SpOp layout");
 

@@ -15,6 +15,10 @@ a `DecodeProgram` once, and `run()` replays it every token:
 
 If the sequence does not fit the fused kernel (M != 1, unsupported shape, aliasing) `build()` keeps the op list and
 `run()` issues the per-op entry points instead - still the CUDA path, `prog.fused` tells which.
+
+A fused block built for batch size B (every call has B rows) is fused when the program is created with
+`DecodeProgram(max_tokens=B)`, B <= 8: one persistent kernel then runs all B tokens (csrc/program_batch.cuh), each
+bit-identical to an M = 1 program on that token's row.  Without it, M > 1 replays the per-op kernels as before.
 """
 from __future__ import annotations
 
@@ -27,7 +31,10 @@ from ._cabi import B200AwqError, Op, check, lib
 
 
 class DecodeProgram:
-    def __init__(self):
+    def __init__(self, max_tokens: int = 1):
+        if not 1 <= int(max_tokens) <= 8:
+            raise B200AwqError("b200awq: max_tokens must be in 1..8")
+        self.max_tokens = int(max_tokens)  # > 1: build() may fuse a sequence recorded with up to this many rows per op
         self._ops: list = []          # (kind, dict of tensors / scalars)
         self._keep: list = []         # every tensor named by an op stays alive with the program
         self._handle = None
@@ -109,13 +116,17 @@ class DecodeProgram:
         return arr
 
     def _create(self, arr, kind_knob: int):
-        """b200awq_program_create under knob 14 = kind_knob; returns a handle or None (sequence outside that kernel)."""
+        """b200awq_program_create (b200awq_program_create_batched when max_tokens > 1) under knob 14 = kind_knob;
+        returns a handle or None (sequence outside that kernel)."""
         prev = lib.b200awq_get_knob(14)
         lib.b200awq_set_knob(14, kind_knob)
         try:
             handle = ctypes.c_void_p()
             with ext._DeviceGuard(self._dev):
-                code = lib.b200awq_program_create(arr, len(self._ops), ctypes.byref(handle))
+                if self.max_tokens > 1:
+                    code = lib.b200awq_program_create_batched(arr, len(self._ops), self.max_tokens, ctypes.byref(handle))
+                else:
+                    code = lib.b200awq_program_create(arr, len(self._ops), ctypes.byref(handle))
         finally:
             lib.b200awq_set_knob(14, prev)
         if code == _cabi.EUNSUPPORTED:
@@ -147,7 +158,8 @@ class DecodeProgram:
         layout (csrc/program.cu).  With `calibrate` (default) and knob 14 = 0, both are created when the sequence fits
         both, each is timed on the device (a load-time step, like the re-layout itself; the recorded buffers are
         overwritten by those runs exactly as `run()` would), and the faster one is kept - `calibration` holds the two
-        times.  Knob 14 = 1 / 2 forces the split-K / stream kernel."""
+        times.  Knob 14 = 1 / 2 forces the split-K / stream kernel.  A sequence with M > 1 rows per op (max_tokens >= M)
+        has only the batched stream kernel: nothing to calibrate."""
         self._no_more()
         if not self._ops:
             raise B200AwqError("b200awq: empty program")
@@ -180,6 +192,15 @@ class DecodeProgram:
         if self._handle is None:
             return "per-op"
         return "stream" if lib.b200awq_program_kind(self._handle) == 2 else "splitk"
+
+    @property
+    def tokens(self) -> int:
+        """Token rows per run (M of the recorded ops; 0 before anything was recorded)."""
+        if self._handle is not None:
+            return lib.b200awq_program_tokens(self._handle)
+        for kind, o in self._ops:
+            return o["M"] if kind == "linear" else o["rows"]
+        return 0
 
     @property
     def kernel_ops(self) -> int:

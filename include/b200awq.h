@@ -222,6 +222,19 @@ typedef struct b200awq_op {
 typedef struct b200awq_program* b200awq_program_t;
 
 int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t* out);
+/* Batched decode programs: the same op list recorded with M token rows per op (a fused block built for batch size M:
+ * RMSNorm / SiLU*mul over M contiguous rows, linears with M rows at pitch ldx), 1 <= max_tokens <= 8 (else
+ * B200AWQ_EINVAL).  Every op must have the same M <= max_tokens, else B200AWQ_EUNSUPPORTED.  M = 1 behaves exactly like
+ * b200awq_program_create.  M > 1 is always the stream variant (kind 2; the split-K kernel is M = 1 only, so knob 14 = 1
+ * returns B200AWQ_EUNSUPPORTED): one persistent kernel stages the M rows and uses M token columns of its MMAs, so
+ * every token is bit-identical to an M = 1 stream program run on that row alone.  A linear that reads a previous op's
+ * output must read it at that op's row pitch (ldx == N of the producer; a column offset is fine); an external source
+ * needs 16-byte aligned rows and ldx % 8 == 0.  The activations of M rows of the longest K must fit shared memory
+ * next to the weight ring: Llama-3-8B shapes (K up to 14336) fuse up to M = 4.  The program owns its hand-off rows
+ * (4 x M rows of the widest output): the caller's workspace is the one of b200awq_program_run below. */
+int b200awq_program_create_batched(const b200awq_op_t* ops, int n_ops, int max_tokens, b200awq_program_t* out);
+/* token rows per run (M of the recorded ops); 0 for a null handle */
+int b200awq_program_tokens(b200awq_program_t prog);
 /* 0: null handle; 1: split-K kernel on the checkpoint layout (round 1); 2: stream variant - at creation every
  * linear of the program was re-laid-out once into the stream format (below), the kernel partitions the work
  * output-stationary and hands activations from op to op as tagged fp16 words (csrc/program_stream.cuh).  Creation
