@@ -31,7 +31,23 @@ class Op(ctypes.Structure):
     ]
 
 
-OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL = 1, 2, 3
+class Moe(ctypes.Structure):
+    """b200awq_moe_t (include/b200awq.h): the descriptor a SPARSE_MOE op's `weight` points at."""
+
+    _fields_ = [
+        ("E", ctypes.c_int32), ("top_k", ctypes.c_int32), ("renormalize", ctypes.c_int32),
+        ("group_size", ctypes.c_int32), ("H", ctypes.c_int32), ("I", ctypes.c_int32), ("block_size", ctypes.c_int32),
+        ("sorted_len", ctypes.c_int32), ("gate_weight", ctypes.c_void_p),
+        ("w1_qweight", ctypes.c_void_p), ("w1_scales", ctypes.c_void_p), ("w1_qzeros", ctypes.c_void_p),
+        ("w2_qweight", ctypes.c_void_p), ("w2_scales", ctypes.c_void_p), ("w2_qzeros", ctypes.c_void_p),
+        ("logits", ctypes.c_void_p), ("topk_weights", ctypes.c_void_p), ("topk_ids", ctypes.c_void_p),
+        ("token_expert_indices", ctypes.c_void_p), ("sorted_ids", ctypes.c_void_p), ("expert_ids", ctypes.c_void_p),
+        ("num_tokens_post_pad", ctypes.c_void_p), ("gate_up", ctypes.c_void_p), ("act", ctypes.c_void_p),
+        ("down", ctypes.c_void_p),
+    ]
+
+
+OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE = 1, 2, 3, 4
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -79,6 +95,7 @@ SIGNATURES = {
     "b200awq_program_create": (_c_int, [ctypes.POINTER(Op), _c_int, ctypes.POINTER(_c_void_p)]),
     "b200awq_program_create_batched": (_c_int, [ctypes.POINTER(Op), _c_int, _c_int, ctypes.POINTER(_c_void_p)]),
     "b200awq_program_tokens": (_c_int, [_c_void_p]),
+    "b200awq_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_program_num_ops": (_c_int, [_c_void_p]),
     "b200awq_program_kind": (_c_int, [_c_void_p]),
     "b200awq_stream_bytes": (_c_size_t, [_c_int, _c_int, _c_int]),

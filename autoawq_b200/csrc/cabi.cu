@@ -223,6 +223,10 @@ int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t
   return b200awq_program_create_batched(ops, n_ops, 1, out);
 }
 
+int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8) {
+  return moe_plan(E, top_k, H, I, group_size, sm_count, out8);
+}
+
 int b200awq_program_num_ops(b200awq_program_t prog) {
   return prog == nullptr ? 0 : program_num_ops(reinterpret_cast<Program*>(prog));
 }

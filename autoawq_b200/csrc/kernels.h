@@ -87,6 +87,7 @@ int program_create(const struct ::b200awq_op* ops, int n, int max_tokens, Progra
 int program_max_n(const Program* p);
 int program_m(const Program* p);
 int program_num_ops(const Program* p);
+int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8);   // host only (b200awq_moe_plan)
 cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st);
 int program_is_stream(const Program* p);
 size_t program_stream_bytes(const Program* p);

@@ -198,7 +198,7 @@ struct ProgWatch {
   }
 };
 enum { kWStaged = 1, kWExtDep = 2, kWEmpty = 3, kWFull = 4, kWGate = 5, kWRedOk = 6, kWStagedOp = 7, kWDutyY = 8,
-       kWDutySilu = 9, kWCopy = 10, kWSilu = 11, kWNorm = 12 };
+       kWDutySilu = 9, kWCopy = 10, kWSilu = 11, kWNorm = 12, kWRoute = 13 /* producer: a MoE block's routing */ };
 __device__ __forceinline__ void prog_wait(const int* cnt, int target, int code, int op) {
   ProgWatch wd;
   while (ld_acquire_s32(cnt) < target)
@@ -712,7 +712,43 @@ struct Program {
   size_t stream_bytes = 0;
   // batched stream variant (M > 1, program_batch.cuh): ring stages per warp, sets per CTA, units along K (smem sizes)
   int sb_spw = 0, sb_lmax = 0, sb_nu_max = 0;
+  // sparse-MoE blocks (stream_moe_kernel): their descriptors
+  SpMoe* d_moe = nullptr;
+  int n_moe = 0;
 };
+
+// One SPARSE_MOE op as the folding sees it: two table entries (gate|up, down) and the recorded descriptor
+struct MoeFold {
+  int kind = 0;        // 0: plain linear, 1: gate|up of block `mi`, 2: its down
+  int mi = -1;
+};
+
+// Envelope and partition of a sparse-MoE block in an M = 1 stream program (host only, see b200awq_moe_plan)
+int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
+  if (E <= 0 || topk <= 0 || topk > E || H <= 0 || I <= 0 || G <= 0 || grid <= 0 || out8 == nullptr)
+    return B200AWQ_EINVAL;
+  if (E > kSpMoeEMax || topk > kSpMoeKMax) return B200AWQ_EUNSUPPORTED;
+  if (!stream_format_supported(H, 2 * I, G, 1) || !stream_format_supported(I, H, G, 0)) return B200AWQ_EUNSUPPORTED;
+  const int UK = G < 128 ? G : 128;
+  const int sets_a = topk * (2 * I / 16), nu_a = H / UK;
+  const int nu_b1 = I / UK, sets_b = H / 16;
+  const int lmax_a = (sets_a + grid - 1) / grid;
+  const int lmax_b = (sets_b + grid - 1) / grid * topk;     // partial rows: (set, slot)
+  if (H / UK > kSpXsumMax || topk * nu_b1 > kSpXsumMax) return B200AWQ_EUNSUPPORTED;
+  if (lmax_a > kSpLMax || lmax_b > kSpLMax) return B200AWQ_EUNSUPPORTED;
+  const int kmax = H > topk * I ? H : topk * I;
+  const size_t smem = sp_fixed_smem(8, 4, true) + (size_t)kmax * 2;
+  if (smem > (size_t)227 * 1024) return B200AWQ_EUNSUPPORTED;
+  out8[0] = 2;                         // kernel ops
+  out8[1] = sets_a;                    // gate|up: 16-column sets (top_k slots x 2I / 16)
+  out8[2] = (2 * I / 16) * nu_a;       // gate|up: units per slot segment
+  out8[3] = lmax_a;                    // gate|up: most sets one CTA owns
+  out8[4] = topk * nu_b1;              // down: units per set (K' = top_k * I)
+  out8[5] = nu_b1;                     // down: units per slot segment
+  out8[6] = lmax_b;                    // down: most (set, slot) partial rows one CTA keeps
+  out8[7] = (int)smem;                 // dynamic shared memory of the kernel for this block alone
+  return B200AWQ_OK;
+}
 
 size_t stream_format_bytes(int K, int N, int G) {
   if (K <= 0 || N <= 0 || G <= 0) return 0;
@@ -742,10 +778,20 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
 // Builds the stream variant from the folded op table, for M token rows (M > 1: the batched kernel of
 // program_batch.cuh).  Returns false when the sequence is outside its envelope (the caller then tries the split-K
 // kernel, M = 1 only).  *err != cudaSuccess reports a CUDA failure.
-static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err) {
+// Sparse-MoE blocks (`fold[i].kind` != 0, M = 1 only): the gate|up entry is a mode-1 op over top_k slots of 2I
+// columns, the down entry reads its published row (K' = top_k I); both stream E per-expert slices packed back to back.
+static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
+                         const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
+  const bool has_moe = !moes.empty();
+  if (has_moe && M != 1) return false;
+  std::vector<int> plan_a(moes.size() * 8);
+  for (size_t b = 0; b < moes.size(); ++b) {
+    const b200awq_moe_t& m = moes[b];
+    if (moe_plan(m.E, m.top_k, m.H, m.I, m.group_size, grid, &plan_a[b * 8]) != B200AWQ_OK) return false;
+  }
   // creation is a load-time step (not capturable): whatever produced the checkpoint tensors on any stream is done
   // before the re-layout reads them
   if ((*err = cudaDeviceSynchronize()) != cudaSuccess) return false;
@@ -762,23 +808,41 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
         mode[i - 1] = 1;
       }
     }
+  auto moe_kind = [&](int i) { return fold.empty() ? 0 : fold[i].kind; };
+  // bytes of one expert's slice of a MoE entry's stream copy (256-byte aligned)
+  auto expert_bytes = [&](int i) {
+    const b200awq_moe_t& m = moes[fold[i].mi];
+    const size_t b = moe_kind(i) == 1 ? stream_format_bytes(m.H, 2 * m.I, m.group_size)
+                                      : stream_format_bytes(m.I, m.H, m.group_size);
+    return (b + 255) & ~(size_t)255;
+  };
+  for (int i = 0; i < n; ++i)
+    if (moe_kind(i) == 1) mode[i] = 1;
   size_t wbytes = 0, max_cols = 0;
   int max_K = 0, lmax = 0, nu_max = 0;
   std::vector<size_t> woff(n);
   for (int i = 0; i < n; ++i) {
     const ProgOp& p = table[i];
-    if (!stream_format_supported(p.K, p.N, p.G, mode[i])) return false;
-    const int UK = p.G < 128 ? p.G : 128;
-    if (p.K / UK > kSpXsumMax) return false;
-    if (M == 1 && (p.N / 16 + grid - 1) / grid > kSpLMax) return false;
-    lmax = std::max(lmax, (p.N / 16 + grid - 1) / grid);
-    nu_max = std::max(nu_max, p.K / UK);
-    woff[i] = wbytes;
-    wbytes += (stream_format_bytes(p.K, p.N, p.G) + 255) & ~(size_t)255;
+    if (moe_kind(i) != 0) {   // envelope checked by moe_plan (per-expert shapes, sets and partial rows per CTA)
+      woff[i] = wbytes;
+      wbytes += (size_t)moes[fold[i].mi].E * expert_bytes(i);
+    } else {
+      if (!stream_format_supported(p.K, p.N, p.G, mode[i])) return false;
+      const int UK = p.G < 128 ? p.G : 128;
+      if (p.K / UK > kSpXsumMax) return false;
+      if (M == 1 && (p.N / 16 + grid - 1) / grid > kSpLMax) return false;
+      lmax = std::max(lmax, (p.N / 16 + grid - 1) / grid);
+      nu_max = std::max(nu_max, p.K / UK);
+      woff[i] = wbytes;
+      wbytes += (stream_format_bytes(p.K, p.N, p.G) + 255) & ~(size_t)255;
+    }
     max_cols = std::max(max_cols, (size_t)(mode[i] ? p.N / 2 : p.N));
     max_K = std::max(max_K, p.K);
   }
-  if (M == 1) {
+  if (M == 1 && has_moe) {
+    // the MoE kernel runs 8 consumer warps with 4 ring stages each, behind the routing area
+    if (sp_fixed_smem(8, 4, true) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
+  } else if (M == 1) {
     if (sp_fixed_smem(12, 3) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;   // (the largest configuration)
   } else {
     // the batched kernel: the deepest ring (<= 4 stages per warp) that leaves room for M rows of activations
@@ -836,6 +900,20 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
         o.ldx = p.src_ld;
       }
     }
+    if (moe_kind(i) != 0) {
+      o.moe = moe_kind(i);
+      o.moe_i = fold[i].mi;
+      if (o.moe == 2) {
+        // the down entry stages the gate|up entry's published SiLU*mul row (top_k x I words, slot-major); the recorded
+        // activation tensor is written as a side effect of that entry
+        if (i == 0 || moe_kind(i - 1) != 1 || fold[i - 1].mi != fold[i].mi) return false;
+        o.prologue = kProCopy;
+        o.src = nullptr;
+        o.src_op = i - 1;
+        o.src_off = 0;
+        ops[i - 1].act_out = const_cast<__half*>(p.src);
+      }
+    }
   }
   // CTA partition: whole 16-column sets, as even as the set count allows
   std::vector<uint32_t> cta((size_t)n * (grid + 1));
@@ -855,8 +933,52 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   for (int i = 0; i < n && e == cudaSuccess; ++i) {
     ops[i].wstream = pr->d_stream + woff[i];
     ops[i].cta_begin = pr->d_cta + (size_t)i * (grid + 1);
+    if (moe_kind(i) != 0) {
+      // one stream copy per expert slice of the stacked tensors ([E, K, N/8], [E, K/G, N], [E, K/G, N/8])
+      const b200awq_moe_t& m = moes[fold[i].mi];
+      const int K = moe_kind(i) == 1 ? m.H : m.I, N = moe_kind(i) == 1 ? 2 * m.I : m.H, G = m.group_size;
+      const int32_t* qw = static_cast<const int32_t*>(table[i].qw_src);
+      for (int x = 0; x < m.E && e == cudaSuccess; ++x)
+        e = stream_pack(qw + (size_t)x * K * (N / 8), table[i].scales + (size_t)x * (K / G) * N,
+                        table[i].qzeros + (size_t)x * (K / G) * (N / 8), pr->d_stream + woff[i] + (size_t)x * expert_bytes(i),
+                        K, N, G, mode[i], nullptr);
+      continue;
+    }
     e = stream_pack(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K, table[i].N,
                     table[i].G, mode[i], nullptr);
+  }
+  if (e == cudaSuccess && has_moe) {
+    std::vector<SpMoe> md(moes.size());
+    for (size_t b = 0; b < moes.size(); ++b) {
+      const b200awq_moe_t& m = moes[b];
+      SpMoe& d = md[b];
+      std::memset(&d, 0, sizeof(d));
+      d.gate_w = static_cast<const __half*>(m.gate_weight);
+      d.logits = static_cast<__half*>(m.logits);
+      d.topk_w = m.topk_weights;
+      d.topk_ids = m.topk_ids;
+      d.tok_idx = m.token_expert_indices;
+      d.sorted_ids = m.sorted_ids;
+      d.expert_ids = m.expert_ids;
+      d.npost = m.num_tokens_post_pad;
+      d.down = static_cast<__half*>(m.down);
+      d.E = m.E;
+      d.topk = m.top_k;
+      d.renorm = m.renormalize != 0;
+      d.block_size = m.block_size;
+      d.sorted_len = m.sorted_len;
+      d.seg_a = plan_a[b * 8 + 2];
+      d.seg_b = plan_a[b * 8 + 5];
+      d.I = m.I;
+      for (int i = 0; i < n; ++i)
+        if (moe_kind(i) != 0 && fold[i].mi == (int)b) (moe_kind(i) == 1 ? d.eb_a : d.eb_b) = (long long)expert_bytes(i);
+    }
+    e = cudaMalloc(&pr->d_moe, md.size() * sizeof(SpMoe));
+    if (e == cudaSuccess) e = cudaMemcpy(pr->d_moe, md.data(), md.size() * sizeof(SpMoe), cudaMemcpyHostToDevice);
+    pr->n_moe = static_cast<int>(md.size());
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)(227 * 1024));
   }
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_sp_ops, ops.data(), (size_t)n * sizeof(SpOp), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_cta, cta.data(), cta.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
@@ -878,11 +1000,14 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     cudaFree(pr->d_cta);
     cudaFree(pr->d_rows);
     cudaFree(pr->d_state);
+    cudaFree(pr->d_moe);
     pr->d_stream = nullptr;
     pr->d_sp_ops = nullptr;
     pr->d_cta = nullptr;
     pr->d_rows = nullptr;
     pr->d_state = nullptr;
+    pr->d_moe = nullptr;
+    pr->n_moe = 0;
     *err = e;
     return false;
   }
@@ -918,10 +1043,67 @@ static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
 //   * a linear must not write (y) what it reads (src) or what its own prologue publishes (xout);
 //   * a buffer that a pending glue record depends on must not be overwritten before the record's last use.
 // Every op has the same M <= max_tokens rows (M > 1: the batched stream kernel only); extents below cover all M rows.
-int program_create(const b200awq_op_t* ops, int n, int max_tokens, Program** out, cudaError_t* cuda_err) {
+int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program** out, cudaError_t* cuda_err) {
   *cuda_err = cudaSuccess;
   *out = nullptr;
-  if (ops == nullptr || n <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
+  if (ops_in == nullptr || n_in <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
+  // A SPARSE_MOE op folds as two linears: gate|up (x [H] -> the recorded gate_up [top_k, 2I], N = top_k 2I) and down
+  // (the recorded activations [top_k, I] -> y [H], K = top_k I); the hazard rules below then see every buffer they touch.
+  // Only the stream kernel runs them (M = 1; stream_build checks the envelope); otherwise the caller replays per op.
+  std::vector<b200awq_op_t> xops;
+  std::vector<MoeFold> xfold;
+  std::vector<b200awq_moe_t> moes;
+  for (int i = 0; i < n_in; ++i) {
+    const b200awq_op_t& op = ops_in[i];
+    if (op.kind != B200AWQ_OP_SPARSE_MOE) {
+      xops.push_back(op);
+      xfold.push_back(MoeFold{});
+      continue;
+    }
+    const b200awq_moe_t* m = static_cast<const b200awq_moe_t*>(op.weight);
+    if (m == nullptr || op.x == nullptr || op.y == nullptr || m->gate_weight == nullptr || m->w1_qweight == nullptr ||
+        m->w1_scales == nullptr || m->w1_qzeros == nullptr || m->w2_qweight == nullptr || m->w2_scales == nullptr ||
+        m->w2_qzeros == nullptr || m->logits == nullptr || m->topk_weights == nullptr || m->topk_ids == nullptr ||
+        m->token_expert_indices == nullptr || m->sorted_ids == nullptr || m->expert_ids == nullptr ||
+        m->num_tokens_post_pad == nullptr || m->gate_up == nullptr || m->act == nullptr || m->down == nullptr)
+      return B200AWQ_EINVAL;
+    if (m->E <= 0 || m->top_k <= 0 || m->top_k > m->E || m->H <= 0 || m->H != op.K || m->I <= 0 || m->group_size <= 0 ||
+        (m->H % m->group_size) != 0 || (m->I % m->group_size) != 0 || m->block_size <= 0 ||
+        m->sorted_len < m->top_k * op.M + m->E * (m->block_size - 1))
+      return B200AWQ_EINVAL;
+    if (op.M != 1) return B200AWQ_EUNSUPPORTED;
+    const int mi = static_cast<int>(moes.size());
+    moes.push_back(*m);
+    b200awq_op_t a;
+    std::memset(&a, 0, sizeof(a));
+    a.kind = B200AWQ_OP_LINEAR_GEMM;
+    a.M = op.M;
+    a.group_size = m->group_size;
+    b200awq_op_t b = a;
+    a.K = m->H;
+    a.N = m->top_k * 2 * m->I;
+    a.ldx = a.K;
+    a.x = op.x;
+    a.qweight = m->w1_qweight;
+    a.scales = m->w1_scales;
+    a.qzeros = m->w1_qzeros;
+    a.y = m->gate_up;
+    b.K = m->top_k * m->I;
+    b.N = m->H;
+    b.ldx = b.K;
+    b.x = m->act;
+    b.qweight = m->w2_qweight;
+    b.scales = m->w2_scales;
+    b.qzeros = m->w2_qzeros;
+    b.y = op.y;
+    xops.push_back(a);
+    xfold.push_back(MoeFold{1, mi});
+    xops.push_back(b);
+    xfold.push_back(MoeFold{2, mi});
+  }
+  const b200awq_op_t* ops = xops.data();
+  const int n = static_cast<int>(xops.size());
+  std::vector<MoeFold> fold;     // per table entry
   std::vector<ProgOp> table;
   struct Glue {
     int kind;
@@ -936,7 +1118,7 @@ int program_create(const b200awq_op_t* ops, int n, int max_tokens, Program** out
   std::vector<Glue> glues;
   const int grid = prog_sm_count();
   int max_K = 0, max_N = 0, M = -1;
-  bool v3_ok = true;
+  bool v3_ok = moes.empty();     // the split-K kernel has no MoE support
   for (int i = 0; i < n; ++i) {
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
@@ -1061,6 +1243,7 @@ int program_create(const b200awq_op_t* ops, int n, int max_tokens, Program** out
     max_K = op.K > max_K ? op.K : max_K;
     max_N = op.N > max_N ? op.N : max_N;
     table.push_back(p);
+    fold.push_back(xfold[i]);
   }
   for (const Glue& gl : glues)
     if (!gl.used) return B200AWQ_EUNSUPPORTED;   // a glue op nobody consumes would never run
@@ -1072,7 +1255,7 @@ int program_create(const b200awq_op_t* ops, int n, int max_tokens, Program** out
   pr->max_N = max_N;
   cudaError_t e = cudaGetDevice(&pr->device);
   // first choice: the stream variant (one-time re-layout, output-stationary partition); knob 14 = 1 skips it
-  if (e == cudaSuccess && knob(14) != 1 && stream_build(pr, table, grid, M, &e)) {
+  if (e == cudaSuccess && knob(14) != 1 && stream_build(pr, table, grid, M, &e, fold, moes)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -1159,11 +1342,20 @@ cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st) {
     // knob 10: ops ahead of the consumers' staging for which shared-memory loads may already be issued (0 = ungated,
     // the default; n > 0: at most n - 1 ops ahead, 1 = strictly gated)
     const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
+    const SpMoe* no_moe = nullptr;
+    if (p->n_moe > 0) {
+      // programs with sparse-MoE blocks: the MOE instantiation, always 8 consumer warps x 4 ring stages
+      cfg.blockDim = dim3(32 + 8 * 32);
+      cfg.dynamicSmemBytes = sp_fixed_smem(8, 4, true) + p->xs_bytes;
+      const SpMoe* md = p->d_moe;
+      return cudaLaunchKernelEx(&cfg, stream_moe_kernel, sops, cta, p->n_ops, p->d_rows,
+                                p->row_stride, p->d_state, knob(3), l2_ahead, gate_ahead, md);
+    }
     if (nw == 8)
       return cudaLaunchKernelEx(&cfg, stream_program_kernel<8, 4, 4>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                                p->d_state, knob(3), l2_ahead, gate_ahead);
+                                p->d_state, knob(3), l2_ahead, gate_ahead, no_moe);
     return cudaLaunchKernelEx(&cfg, stream_program_kernel<12, 3, 2>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                              p->d_state, knob(3), l2_ahead, gate_ahead);
+                              p->d_state, knob(3), l2_ahead, gate_ahead, no_moe);
   }
   e = cudaMemsetAsync(p->d_done, 0, (size_t)2 * (p->n_ops + 1) * sizeof(int), st);
   if (e != cudaSuccess) return e;
@@ -1200,6 +1392,7 @@ void program_destroy(Program* p) {
   cudaFree(p->d_cta);
   cudaFree(p->d_rows);
   cudaFree(p->d_state);
+  cudaFree(p->d_moe);
   delete p;
 }
 

@@ -50,13 +50,42 @@ struct __align__(128) SpOp {
   int src_op, src_off;         // >= 0: the source is op src_op's published row, from column src_off
   float eps;
   int ldx;                     // row pitch (elements) of `src` when a batched program stages several rows
-  int pad_[3];
+  int moe;                     // MoE kernel only: 0 plain op, 1 a MoE block's gate|up (routing prologue), 2 its down
+  int moe_i;                   // index of the block's SpMoe
+  int pad_[1];
 };
 static_assert(sizeof(SpOp) == 128, "SpOp layout");
 
-__host__ __device__ constexpr size_t sp_fixed_smem(int nw, int spw) {
+// Sparse-MoE block (stream_moe_kernel): one block = two kernel ops.
+//   gate|up (moe = 1): K = H, N = top_k * 2I: the top_k selected experts' gate|up linears side by side, slot-major
+//     (set s of the op = set s % (I / 8) of slot s / (I / 8)'s expert, mode 1: publishes top_k x I SiLU*mul words);
+//   down (moe = 2): K = top_k * I (the published row unchanged), N = H: unit j of a set reads slot j / (I / UK)'s
+//     expert; every CTA keeps one partial row per (set, slot) and publishes sum_k fp16(w_k * slot_k) directly.
+// A unit u of either op lives in segment q = u / seg (seg = units per slot: (I / 8) * (H / UK) for gate|up, I / UK
+// for down): slot q % top_k, unit (q / top_k) * seg + u % seg of the expert's stream copy.  A bulk copy never crosses
+// a segment (the consumers cut their chunks the same way).
+constexpr int kSpMoeEMax = 64;                    // experts
+constexpr int kSpMoeKMax = 8;                     // top_k
+constexpr int kSpMoeSmem = 512;                   // logits [64] f32, weights [8] f32, ids [8] i32, routed op
+struct SpMoe {
+  const __half* gate_w;        // router weight [E, H] fp16
+  __half* logits;              // [E] fp16 (what nn.Linear returns)
+  float* topk_w;               // [top_k] (renormalised when renorm)
+  int* topk_ids;               // [top_k]
+  int* tok_idx;                // [top_k] token_expert_indices (k * M + m = k)
+  int* sorted_ids;             // [sorted_len] moe_align_block_size outputs
+  int* expert_ids;
+  int* npost;
+  __half* down;                // [top_k, H] per-slot down outputs x routing weight
+  long long eb_a, eb_b;        // bytes per expert slice of the gate|up / down stream copies
+  int E, topk, renorm, block_size, sorted_len;
+  int seg_a, seg_b, I;
+};
+
+// (moe: the MoE kernel's routing area, SpMoeSmem, follows the fixed part)
+__host__ __device__ constexpr size_t sp_fixed_smem(int nw, int spw, bool moe = false) {
   return (size_t)nw * spw * kSpStageBytes + (size_t)kSpLMax * nw * 16 * 4 + (size_t)kSpXsumMax * 4 +
-         (size_t)2 * nw * spw * 8 + 2 * 128 + 256;
+         (size_t)2 * nw * spw * 8 + 2 * 128 + 256 + (moe ? kSpMoeSmem : 0);
 }
 static_assert(sp_fixed_smem(8, 4) % 16 == 0 && sp_fixed_smem(12, 3) % 16 == 0 && sp_fixed_smem(16, 2) % 16 == 0,
               "xs must stay 16-byte aligned");
@@ -243,7 +272,8 @@ __device__ __forceinline__ void sp_chunk(const uint8_t* __restrict__ st, int UB,
 
 // debug stamps (knob 3 = 2), per op and CTA (first 8 CTAs, first 32 ops):
 // [0] op begin, [1] source row complete (poll over), [2] activations staged, [3] warp 0's first chunk landed,
-// [4] warp 0 finished its units, [5] all warps finished, [6] outputs published, [7] unused
+// [4] warp 0 finished its units, [5] all warps finished, [6] outputs published, [7] routing published (the gate|up op
+// of a MoE block; 0 for other ops)
 // knob 3 = 8: per-WARP stamps of the first 8 CTAs / 16 ops: g_sp_dbg[op][cta][warp][slot], slots: 0 op begin, 1 own
 // polls done, 2 staged (past the barrier), 3 first chunk landed, 4 own units done, 5 past the post-loop barrier,
 // 6 own finish stores issued.  (A timer read right after bar.sync captures the ARRIVAL: the barrier blocks at the next
@@ -280,434 +310,45 @@ __device__ __forceinline__ void cp_async_4(void* smem_dst, const void* gsrc) {
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-template <int NW, int SPW, int GR>
+// MOE kernel: the routing area in shared memory, right behind the fixed part
+struct SpMoeSmem {
+  float* m_logit;      // [64] widened fp16 logits
+  float* m_w;          // [8] routing weights
+  int* m_ids;          // [8] expert of each slot
+  int* routed_op;      // last gate|up op whose routing is in m_w / m_ids (release / acquire at CTA scope)
+};
+__device__ __forceinline__ SpMoeSmem sp_moe_smem(uint8_t* area) {
+  SpMoeSmem s;
+  s.m_logit = reinterpret_cast<float*>(area);
+  s.m_w = s.m_logit + kSpMoeEMax;
+  s.m_ids = reinterpret_cast<int*>(s.m_w + kSpMoeKMax);
+  s.routed_op = s.m_ids + kSpMoeKMax;
+  return s;
+}
+
+// The kernel body is program_stream_body.inc: stream_program_kernel<NW, SPW, GR> (MOE = false; `moe` unused) and
+// stream_moe_kernel (programs with sparse-MoE blocks, SpMoe above) include it.  Every MoE-only step sits behind
+// `if constexpr (MOE)`: stream_program_kernel is the plain kernel, instruction for instruction.
+// (MOE is only ever false here; it is a template parameter rather than a local constant because a local constant,
+// unlike the parameter, changes the register assignment ptxas makes for this kernel)
+template <int NW, int SPW, int GR, bool MOE = false>
 __global__ void __launch_bounds__(32 + NW * 32, 1)
     stream_program_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
                           uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
-                          int gate_ahead) {
-  extern __shared__ __align__(1024) uint8_t sp_smem[];
-  uint8_t* ring = sp_smem;
-  float* part = reinterpret_cast<float*>(sp_smem + (size_t)(NW * SPW) * kSpStageBytes);   // [LMax][8 warps][16]
-  float* xsum = part + kSpLMax * NW * 16;                                           // [K / UK]
-  uint64_t* full = reinterpret_cast<uint64_t*>(xsum + kSpXsumMax);
-  uint64_t* empty = full + (NW * SPW);
-  SpOp* sdesc = reinterpret_cast<SpOp*>(empty + (NW * SPW));      // [2] op descriptors, prefetched one op ahead
-  int* misc = reinterpret_cast<int*>(sdesc + 2);
-  float* wsum = reinterpret_cast<float*>(misc);        // [8]
-  int* wfirst = misc + 8;                              // [NW] first local set each warp touched (-1: none)
-  int* wlast = misc + 8 + NW;                    // [NW]
-  uint32_t* scta = reinterpret_cast<uint32_t*>(misc + 8 + 2 * NW);   // [2][2] this CTA's unit range (with sdesc)
-  int* staged_op = misc + 12 + 2 * NW;                 // last op this CTA staged (release / acquire at CTA scope)
-  static_assert((13 + 2 * NW) * 4 <= 256, "misc area");
-  uint32_t* xs = reinterpret_cast<uint32_t*>(sp_smem + sp_fixed_smem(NW, SPW));   // activations in B-fragment order
+                          int gate_ahead, const SpMoe* __restrict__ moe) {
+#include "program_stream_body.inc"
+}
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nblk = gridDim.x, bid = blockIdx.x;
-  const int base = state[0];     // tag base of this run (advanced by the last CTA to leave, see the end)
-
-  if (tid == 0) {
-    for (int s = 0; s < (NW * SPW); ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    fence_mbar_init();
-    *staged_op = -1;
-  }
-  if (warp == 1) {   // op 0's descriptor
-    reinterpret_cast<uint32_t*>(sdesc)[lane] = reinterpret_cast<const uint32_t*>(ops)[lane];
-    if (lane < 2) scta[lane] = cta_all[bid + lane];
-  }
-  __syncthreads();
-
-  if (warp == 0) {
-    // ============================================================ producer: the weight stream of ALL ops
-    // Lane w feeds consumer warp w's private ring.  The eight lanes run ONE converged loop and probe their
-    // "slot free" barriers with the non-blocking mbarrier.test_wait: with a blocking try_wait per lane (round 1, and
-    // the first version of this kernel) a lane waiting for a slot that frees up late suspended the whole warp, so
-    // slots that were free long ago were refilled microseconds late and the ring ran dry at every op boundary.
-    // Descriptor fields of the next op are fetched one op ahead into registers (global loads, off the critical path).
-    {
-      const int w = lane < NW ? lane : 0;
-      bool active = lane < NW;
-      struct Run {
-        uint32_t u, ub;
-        int UB, ups;
-        const uint8_t* src;
-      };
-      auto fetch = [&](int op, Run& r) {
-        r.u = r.ub = 0;
-        r.UB = r.ups = 1;
-        r.src = nullptr;
-        if (op < n_ops && lane < NW) {
-          const uint32_t u0 = cta_all[(size_t)op * (nblk + 1) + bid], u1 = cta_all[(size_t)op * (nblk + 1) + bid + 1];
-          const uint32_t nu = u1 - u0;
-          r.u = u0 + (uint32_t)((uint64_t)nu * w / NW);
-          r.ub = u0 + (uint32_t)((uint64_t)nu * (w + 1) / NW);
-          r.UB = ops[op].unit_bytes;
-          r.ups = ops[op].ups;
-          r.src = ops[op].wstream;
-        }
-      };
-      Run cur, nxt;
-      int op = 0;
-      fetch(0, cur);
-      fetch(1, nxt);
-      // HBM -> L2 prefetch cursor, running ahead of the ring by at most `l2_ahead` bytes per lane: while the
-      // consumers hand activations from op to op the ring is full and HBM would idle; with the next chunks already in
-      // L2 the ring refills at L2 speed afterwards (SM count x 8 lanes x l2_ahead bytes)
-      Run pcur, pnxt;
-      int pop = 0;
-      fetch(0, pcur);
-      fetch(1, pnxt);
-      bool pactive = lane < NW && l2_ahead > 0;
-      int ahead = 0;                               // bytes prefetched beyond the ring's load cursor
-      int stage_i = 0;
-      uint32_t ph = 0;
-      ProgWatch wd;
-      for (;;) {
-        while (active && cur.u >= cur.ub) {        // this lane's run of the op is requested: next op
-          if (++op >= n_ops) {
-            active = false;
-            break;
-          }
-          cur = nxt;
-          fetch(op + 1, nxt);
-        }
-        if (!__any_sync(0xffffffffu, active)) break;
-        bool issued = false;
-        // Gate: shared-memory loads of an op start only once this CTA has staged that op's activations (+ gate_ahead
-        // ops).  A deep ring of bulk loads is also a deep queue on the SM's return path: every poll of the hand-off
-        // waits behind ~100 KB of weight tiles, several times its unloaded L2 round trip.  While
-        // the consumers hand over, the stream continues into L2 (prefetch cursor below), not into this SM.
-        if (active && (gate_ahead >= (1 << 20) || op <= ld_acquire_cta_smem(staged_op) + gate_ahead)) {
-          const int stage = w * SPW + stage_i;
-          if (mbar_test_wait(&empty[stage], ph ^ 1)) {
-            const int n = (int)(cur.ub - cur.u) < cur.ups ? (int)(cur.ub - cur.u) : cur.ups;
-            mbar_arrive_expect_tx(&full[stage], (uint32_t)(n * cur.UB));
-            bulk_load_1d(ring + (size_t)stage * kSpStageBytes, cur.src + (size_t)cur.u * cur.UB, (uint32_t)(n * cur.UB),
-                         &full[stage]);
-            cur.u += (uint32_t)cur.ups;
-            ahead -= n * cur.UB;
-            if (++stage_i == SPW) { stage_i = 0; ph ^= 1; }
-            issued = true;
-          }
-        }
-        if (!__any_sync(0xffffffffu, issued)) {
-          // nothing to load: prefetch one more chunk into L2 if the window allows, else leave the issue slots alone
-          bool pf = false;
-          if (pactive) {
-            if (ahead < 0) {                       // the ring overtook the prefetch cursor: catch up
-              pop = op;
-              pcur = cur;
-              pnxt = nxt;
-              ahead = 0;
-            }
-            while (pactive && pcur.u >= pcur.ub) {
-              if (++pop >= n_ops) {
-                pactive = false;
-                break;
-              }
-              pcur = pnxt;
-              fetch(pop + 1, pnxt);
-            }
-            if (pactive && ahead < l2_ahead) {
-              const int n = (int)(pcur.ub - pcur.u) < pcur.ups ? (int)(pcur.ub - pcur.u) : pcur.ups;
-              // (chunks still inside the ring window were loaded already: prefetching them again is harmless)
-              bulk_prefetch_l2(pcur.src + (size_t)pcur.u * pcur.UB, (uint32_t)(n * pcur.UB));
-              pcur.u += (uint32_t)pcur.ups;
-              ahead += n * pcur.UB;
-              pf = true;
-            }
-          }
-          if (!__any_sync(0xffffffffu, pf)) {
-            if (__any_sync(0xffffffffu, wd.tick(kWEmpty, op))) break;   // watchdog (warp-uniform): never hang the GPU
-            __nanosleep(32);
-          }
-        }
-      }
-    }
-  } else {
-    // ================================================================ consumers
-    const int cw = warp - 1;
-    const int ct = tid - 32;
-    const int g = lane >> 2, tig = lane & 3;
-    const bool xl = g == 0;       // M = 1: token 0 is column n = 0 of the MMA's B operand, supplied by the g = 0 lanes
-    int stage_i = 0;
-    uint32_t ph = 0;
-
-    for (int op = 0; op < n_ops; ++op) {
-      const SpOp* o = sdesc + (op & 1);                            // shared memory (prefetched during op - 1)
-      const int K = o->K, N = o->N, NU = o->NU, F = o->F, UB = o->unit_bytes, ups = o->ups, mode = o->mode;
-      const uint32_t u0 = scta[(op & 1) * 2], u1 = scta[(op & 1) * 2 + 1];
-      const uint32_t nu = u1 - u0;
-      const uint32_t ua = u0 + (uint32_t)((uint64_t)nu * cw / NW), ub = u0 + (uint32_t)((uint64_t)nu * (cw + 1) / NW);
-      const int set0 = (int)(u0 / NU);                            // first set of the CTA
-      const __half* bias = o->bias;
-      __half* y = o->y;
-      __half* act_out = o->act_out;
-      SP_STAMP(0);
-      SP_WSTAMP(0);
-
-      // ---- stage the activations (whole row, every CTA): poll the producer's published row / read global memory,
-      //      apply the recorded RMSNorm, write them in B-fragment order and keep the per-unit sums sum_k x_k.
-      //      Thread t takes 8 consecutive k per pass (k = 2048 pass + 8 t) and sums squares in the order of
-      //      aux.cu's rmsnorm_kernel, so the norm reproduces the stand-alone kernel bit for bit.
-      {
-        const int uk_shift = o->uk_shift;
-        const int seg = (1 << uk_shift) >> 3;                      // lanes per unit (each lane holds 8 consecutive k)
-        const bool from_row = o->src_op >= 0;
-        const uint32_t* row = from_row ? rows + (size_t)(o->src_op % kSpRows) * row_stride + o->src_off : nullptr;
-        const uint32_t want = from_row ? sp_tag(base, o->src_op) : 0u;
-        const __half* src = o->src;
-        const bool norm = o->prologue == kProRmsnorm;
-        const __half* nw = o->norm_w;
-        float ss = 0.f;
-        // the norm weights of the first batch of passes depend on nothing: in flight before the polls
-        uint4 nwv[4];
-        if (norm) {
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            const int c = cw * 256 + b * kSpStagePass + lane * 8;
-            if (cw < kSpStageWarps && c < K) nwv[b] = __ldg(reinterpret_cast<const uint4*>(nw + c));
-          }
-        }
-        // fragment order: k = 16 ks + j -> word ks * 8 + ((j & 7) >> 1) * 2 + (j >> 3)   (a word = the pair (j, j + 1))
-        auto frag_ptr = [&](int c) { return xs + (c >> 4) * 8 + ((c >> 3) & 1); };   // + 2 * pair index
-        auto unit_sums = [&](int c, bool ok, const uint32_t (&h)[4]) {
-          float sx = 0.f;
-          if (ok) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 f = __half22float2(u32_as_h2(h[q]));
-              sx += f.x + f.y;
-            }
-          }
-          for (int d = 1; d < seg; d <<= 1) sx += __shfl_xor_sync(0xffffffffu, sx, d);
-          if (ok && (lane & (seg - 1)) == 0) xsum[c >> uk_shift] = sx;
-        };
-        // passes are taken in batches of 4: every load of a batch is in flight before the first tag is looked at
-        // (a poll is a loaded L2 round trip; K = 14336 has 7 passes)
-        // (the first kSpStageWarps warps stage; the others wait at the barriers)
-        const int cb_first = cw < kSpStageWarps ? cw * 256 : K;
-        for (int cb0 = cb_first; cb0 < K; cb0 += 4 * kSpStagePass) {      // warp-uniform trip counts
-          uint4 v0[4], v1[4];
-          if (from_row) {
-#pragma unroll
-            for (int b = 0; b < 4; ++b) {
-              const int c = cb0 + b * kSpStagePass + lane * 8;
-              if (c < K) {
-                v0[b] = ld_relaxed_u4(row + c);
-                v1[b] = ld_relaxed_u4(row + c + 4);
-              }
-            }
-          }
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            const int cb = cb0 + b * kSpStagePass;
-            if (cb >= K) break;                                          // warp-uniform
-            const int c = cb + lane * 8;
-            const bool ok = c < K;
-            uint32_t h[4] = {0u, 0u, 0u, 0u};                            // the eight fp16 values as four pairs
-            if (ok) {
-              if (from_row) {
-                ProgWatch wd;
-                for (;;) {
-                  const uint4 a = v0[b], d = v1[b];
-                  if ((a.x >> 16) == want && (a.y >> 16) == want && (a.z >> 16) == want && (a.w >> 16) == want &&
-                      (d.x >> 16) == want && (d.y >> 16) == want && (d.z >> 16) == want && (d.w >> 16) == want)
-                    break;
-                  if (dbg == 6 || dbg == 7) break; // experiment: do not wait for the producers (results are garbage)
-                  if (wd.tick(kWCopy, op)) break;
-                  v0[b] = ld_relaxed_u4(row + c);
-                  v1[b] = ld_relaxed_u4(row + c + 4);
-                }
-                h[0] = (v0[b].x & 0xffffu) | (v0[b].y << 16);
-                h[1] = (v0[b].z & 0xffffu) | (v0[b].w << 16);
-                h[2] = (v1[b].x & 0xffffu) | (v1[b].y << 16);
-                h[3] = (v1[b].z & 0xffffu) | (v1[b].w << 16);
-              } else {
-                const uint4 v = ldg_stream_u4(src + c);
-                h[0] = v.x; h[1] = v.y; h[2] = v.z; h[3] = v.w;
-              }
-              uint32_t* dst = frag_ptr(c);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                dst[2 * q] = h[q];
-                const float2 f = __half22float2(u32_as_h2(h[q]));
-                ss += f.x * f.x + f.y * f.y;
-              }
-            }
-            if (!norm) unit_sums(c, ok, h);
-          }
-        }
-        SP_STAMP(1);
-        SP_WSTAMP(1);
-        if (norm) {
-          ss = prog_warp_sum(ss);
-          if (lane == 0 && cw < kSpStageWarps) wsum[cw] = ss;
-          named_bar_sync_gv(1, (NW * 32));
-          float tot = 0.f;
-#pragma unroll
-          for (int i = 0; i < kSpStageWarps; ++i) tot += wsum[i];
-          const float rs = rsqrtf(tot / static_cast<float>(K) + o->eps);
-          __half* xout = o->xout;
-          int xlo = 0, xhi = 0;
-          if (xout != nullptr) {       // this CTA's share of the norm's recorded output buffer
-            const int u8 = K >> 3;
-            xlo = (int)((int64_t)u8 * bid / nblk) << 3;
-            xhi = (int)((int64_t)u8 * (bid + 1) / nblk) << 3;
-          }
-          for (int cb0 = cb_first; cb0 < K; cb0 += 4 * kSpStagePass) {   // the thread's own chunks again
-#pragma unroll
-            for (int b = 0; b < 4; ++b) {
-              const int cb = cb0 + b * kSpStagePass;
-              if (cb >= K) break;
-              const int c = cb + lane * 8;
-              const bool ok = c < K;
-              uint32_t h[4] = {0u, 0u, 0u, 0u};
-              if (ok) {
-                uint32_t* dst = frag_ptr(c);
-                const uint4 wv = cb0 == cb_first ? nwv[b] : __ldg(reinterpret_cast<const uint4*>(nw + c));
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 a = __half22float2(u32_as_h2(dst[2 * q]));
-                  const float2 wq = __half22float2(u32_as_h2((&wv.x)[q]));
-                  // arithmetic of aux.cu's rmsnorm_kernel: fp16(x * rs * w)
-                  h[q] = h2_as_u32(__halves2half2(__float2half_rn(a.x * rs * wq.x), __float2half_rn(a.y * rs * wq.y)));
-                  dst[2 * q] = h[q];
-                }
-                if (c >= xlo && c < xhi) *reinterpret_cast<uint4*>(xout + c) = make_uint4(h[0], h[1], h[2], h[3]);
-              }
-              unit_sums(c, ok, h);
-            }
-          }
-        }
-        named_bar_sync_gv(1, (NW * 32));
-      }
-      if (ct == 0) st_release_cta_smem(staged_op, op);      // releases the producer's loads of this op (see the gate)
-      SP_STAMP(2);
-      SP_TOUCH_SMEM();
-      SP_WSTAMP(2);
-      // every warp is past op - 1's finish phase (it read sdesc[(op - 1) & 1]): fetch op + 1's descriptor into that
-      // slot, asynchronously - it lands during this op's unit loop
-      if (cw == 0 && op + 1 < n_ops) {
-        SpOp* dn = sdesc + ((op + 1) & 1);
-        if (lane < 8) cp_async_16(reinterpret_cast<uint8_t*>(dn) + lane * 16, reinterpret_cast<const uint8_t*>(ops + op + 1) + lane * 16);
-        else if (lane < 10)
-          cp_async_4(scta + ((op + 1) & 1) * 2 + (lane - 8), cta_all + (size_t)(op + 1) * (nblk + 1) + bid + (lane - 8));
-      }
-
-      // ---- this warp's run of units
-      {
-        int s_cur = (int)(ua / NU), j = (int)(ua - (uint32_t)s_cur * NU);
-        float ylo = 0.f, yhi = 0.f;
-        int first_ls = -1, last_ls = -1;
-        auto flush = [&]() {
-          const int ls = s_cur - set0;
-          if (tig == 0) {
-            float* p = part + ((size_t)ls * NW + cw) * 16;
-            p[g] = ylo;
-            p[g + 8] = yhi;
-          }
-          if (first_ls < 0) first_ls = ls;
-          last_ls = ls;
-          ylo = yhi = 0.f;
-        };
-        for (uint32_t u = ua; u < ub; u += ups) {
-          const int n = (int)(ub - u) < ups ? (int)(ub - u) : ups;
-          const int stage = cw * SPW + stage_i;
-          prog_mbar_wait(&full[stage], ph, kWFull, op);
-          if (u == ua) {
-            SP_STAMP(3);
-            SP_WSTAMP(3);
-          }
-          const uint8_t* st = ring + (size_t)stage * kSpStageBytes;
-          if (dbg != 5 && dbg != 7) {      // (5 / 7: experiment without the unit math)
-            auto apply = [&](float t_lo, float t_hi) {
-              ylo += t_lo;
-              yhi += t_hi;
-              if (++j == NU) {
-                flush();
-                j = 0;
-                ++s_cur;
-              }
-            };
-            const int j0 = j;
-            if (F == 8) sp_chunk<8, GR>(st, UB, n, xs, xsum, j0, NU, lane, xl, apply);
-            else if (F == 4) sp_chunk<4, GR>(st, UB, n, xs, xsum, j0, NU, lane, xl, apply);
-            else sp_chunk<2, GR>(st, UB, n, xs, xsum, j0, NU, lane, xl, apply);
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[stage]);
-          if (++stage_i == SPW) { stage_i = 0; ph ^= 1; }
-        }
-        if (j != 0 && ua < ub) flush();     // the run ended inside a set
-        if (lane == 0) {                    // (written by every warp for every op: nothing to reset)
-          wfirst[cw] = first_ls;
-          wlast[cw] = last_ls;
-        }
-      }
-      SP_STAMP(4);
-      SP_WSTAMP(4);
-      if (cw == 0) cp_async_wait_all();     // op + 1's descriptor has landed (issued a whole unit loop ago)
-      named_bar_sync_gv(1, (NW * 32));
-      SP_STAMP(5);
-      SP_TOUCH_SMEM();
-      SP_WSTAMP(5);
-
-      // ---- finish: sum the warps' partial sums in a fixed order, publish (fp16 | tag) and the per-op-path tensors
-      {
-        const int nsets = nu == 0 ? 0 : (int)((u1 - 1) / NU) - set0 + 1;
-        const uint32_t tagw = sp_tag(base, op) << 16;
-        uint32_t* out_row = rows + (size_t)(op % kSpRows) * row_stride;
-        for (int t = ct; t < nsets * 8; t += (NW * 32)) {
-          const int ls = t >> 3, gg = t & 7;
-          float lo = 0.f, hi = 0.f;
-#pragma unroll
-          for (int w = 0; w < NW; ++w) {
-            if (wfirst[w] >= 0 && wfirst[w] <= ls && ls <= wlast[w]) {
-              const float* p = part + ((size_t)ls * NW + w) * 16;
-              lo += p[gg];
-              hi += p[gg + 8];
-            }
-          }
-          int clo, chi;
-          sp_cols(mode, N, set0 + ls, gg, clo, chi);
-          if (bias != nullptr) {
-            lo += __half2float(bias[clo]);
-            hi += __half2float(bias[chi]);
-          }
-          const __half hlo = __float2half_rn(lo), hhi = __float2half_rn(hi);
-          if (mode == 0) {
-            st_relaxed_u32(out_row + clo, tagw | __half_as_ushort(hlo));
-            st_relaxed_u32(out_row + chi, tagw | __half_as_ushort(hhi));
-          } else {
-            // fused SiLU*mul with the arithmetic of aux.cu's silu_mul_kernel
-            const float gf = __half2float(hlo), uf = __half2float(hhi);
-            const __half a = __float2half_rn(gf / (1.f + __expf(-gf)) * uf);
-            st_relaxed_u32(out_row + clo, tagw | __half_as_ushort(a));
-            if (act_out != nullptr) act_out[clo] = a;
-          }
-          y[clo] = hlo;      // the per-op path's tensors: nobody inside the kernel reads them
-          y[chi] = hhi;
-        }
-      }
-      SP_STAMP(6);
-      SP_WSTAMP(6);
-      // (the next op's staging barriers separate these reads of part[] / wfirst[] from the next writes; the
-      // descriptor slot this op used is overwritten only after the next op's staging barrier)
-    }
-  }
-
-  // ---- the last CTA to leave advances the tag base for the next run (every CTA read it before doing anything)
-  __syncthreads();
-  if (tid == 0) {
-    __threadfence();
-    if (atomicAdd(&state[1], 1) == nblk - 1) {
-      state[1] = 0;
-      state[0] = (base + n_ops) % 65535;
-    }
-  }
+// programs with sparse-MoE blocks: 8 consumer warps, 4 ring stages each
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_moe_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                      uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
+                      int gate_ahead, const SpMoe* __restrict__ moe) {
+  constexpr int NW = 8, SPW = 4, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();   // nothing is read before the predecessor is done, should it ever be launched with PDL (a no-op under
+                // the cooperative launch of program_run)
+#include "program_stream_body.inc"
 }
 
 }  // namespace b200awq

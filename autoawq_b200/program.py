@@ -19,6 +19,10 @@ If the sequence does not fit the fused kernel (M != 1, unsupported shape, aliasi
 A fused block built for batch size B (every call has B rows) is fused when the program is created with
 `DecodeProgram(max_tokens=B)`, B <= 8: one persistent kernel then runs all B tokens (csrc/program_batch.cuh), each
 bit-identical to an M = 1 program on that token's row.  Without it, M > 1 replays the per-op kernels as before.
+
+`sparse_moe(x, gate_weight, w1, w2, top_k)` records a whole Mixtral sparse-MoE block (FusedSparseMoeBlock.forward);
+at M = 1 the stream kernel runs it as two kernel ops with the routing computed inside (DESIGN.md 3.5d), otherwise
+`run()` replays apply_moe_weights' sequence through ext.  `moe_buffers(i)` returns the block's routing and intermediates.
 """
 from __future__ import annotations
 
@@ -96,6 +100,98 @@ class DecodeProgram:
         self._max_n = max(self._max_n, N)
         return y.reshape(x.shape[:-1] + (N,))
 
+    @staticmethod
+    def _stacked(w, name):
+        if hasattr(w, "qweight"):
+            return w.qweight, w.scales, w.qzeros
+        if isinstance(w, (tuple, list)) and len(w) == 3:
+            return tuple(w)
+        raise B200AwqError(f"b200awq: {name} must have .qweight/.scales/.qzeros or be a 3-tuple")
+
+    def sparse_moe(self, x, gate_weight, w1, w2, top_k, renormalize=True):
+        """FusedSparseMoeBlock.forward (awq/modules/fused/moe.py:26-89) on the normed rows x [.., H]: router matmul,
+        topk_softmax, optional renormalisation, moe_alig_block_size, grouped gate|up, SiLU*mul, grouped down x routing
+        weight, sum over the slots.  gate_weight: the router's nn.Linear weight [E, H] fp16 (no bias); w1 / w2: the
+        stacked GEMM-layout experts of awq/models/mixtral.py:129-151 ([E, H, 2I/8] / [E, I, H/8] qweight).  Returns
+        out [M, H] fp16; the routing and the intermediate tensors are the program's (moe_buffers)."""
+        self._no_more()
+        self._dev_of(x)
+        q1, s1, z1 = self._stacked(w1, "w1")
+        q2, s2, z2 = self._stacked(w2, "w2")
+        for t, dt, n in ((q1, torch.int32, "w1.qweight"), (s1, torch.float16, "w1.scales"), (z1, torch.int32, "w1.qzeros"),
+                         (q2, torch.int32, "w2.qweight"), (s2, torch.float16, "w2.scales"), (z2, torch.int32, "w2.qzeros")):
+            ext._require_cuda(t)
+            if t.dim() != 3 or t.dtype != dt or not t.is_contiguous():
+                raise B200AwqError(f"b200awq: {n} must be a contiguous stacked [E, ..] {dt} tensor")
+        E, H, I = q1.shape[0], q1.shape[1], q1.shape[2] * 4
+        G = H // s1.shape[1]
+        top_k = int(top_k)
+        if gate_weight.dtype != torch.float16 or tuple(gate_weight.shape) != (E, H) or not gate_weight.is_contiguous():
+            raise B200AwqError(f"b200awq: gate_weight must be a contiguous [E={E}, H={H}] float16 tensor")
+        if tuple(q2.shape) != (E, I, H // 8) or I // s2.shape[1] != G or not 1 <= top_k <= E:
+            raise B200AwqError("b200awq: w1 / w2 / top_k do not describe one sparse-MoE block")
+        if x.dtype != torch.float16 or x.shape[-1] != H or not x.is_contiguous():
+            raise B200AwqError(f"b200awq: sparse_moe expects contiguous float16 rows [.., {H}]")
+        M = x.numel() // H
+        dev, f16, i32 = x.device, torch.float16, torch.int32
+        block = 16                                      # moe_align_block_size's block at moe.py:54-56
+        b = dict(logits=torch.empty((M, E), dtype=f16, device=dev),
+                 topk_weights=torch.empty((M, top_k), dtype=torch.float32, device=dev),
+                 topk_ids=torch.empty((M, top_k), dtype=i32, device=dev),
+                 token_expert_indices=torch.empty((M, top_k), dtype=i32, device=dev),
+                 sorted_ids=torch.empty((M * top_k + E * (block - 1),), dtype=i32, device=dev),
+                 expert_ids=torch.empty((M * top_k + E,), dtype=i32, device=dev),
+                 num_tokens_post_pad=torch.empty((1,), dtype=i32, device=dev),
+                 gate_up=torch.empty((M, top_k, 2 * I), dtype=f16, device=dev),
+                 act=torch.empty((M, top_k, I), dtype=f16, device=dev),
+                 down=torch.empty((M, top_k, H), dtype=f16, device=dev))
+        out = torch.empty((M, H), dtype=f16, device=dev)
+        raw_w = torch.empty((M, top_k), dtype=torch.float32, device=dev)    # topk_softmax's output (replay)
+        d = _cabi.Moe()
+        d.E, d.top_k, d.renormalize, d.group_size, d.H, d.I = E, top_k, 1 if renormalize else 0, G, H, I
+        d.block_size, d.sorted_len = block, b["sorted_ids"].numel()
+        d.gate_weight = gate_weight.data_ptr()
+        d.w1_qweight, d.w1_scales, d.w1_qzeros = q1.data_ptr(), s1.data_ptr(), z1.data_ptr()
+        d.w2_qweight, d.w2_scales, d.w2_qzeros = q2.data_ptr(), s2.data_ptr(), z2.data_ptr()
+        for k, t in b.items():
+            setattr(d, k, t.data_ptr())
+        x2 = x.reshape(M, H)
+        self._ops.append(("moe", dict(x=x2, gate_weight=gate_weight, w1=(q1, s1, z1), w2=(q2, s2, z2), top_k=top_k,
+                                      renormalize=bool(renormalize), E=E, H=H, I=I, M=M, out=out, raw_w=raw_w,
+                                      buffers=b, desc=d)))
+        self._keep += [x, x2, gate_weight, q1, s1, z1, q2, s2, z2, out, raw_w] + list(b.values())
+        return out.reshape(x.shape)
+
+    def moe_buffers(self, i: int = 0) -> dict:
+        """The tensors the i-th recorded sparse_moe op owns (read-only views): logits [M, E] f16, topk_weights [M, top_k]
+        f32 (after the renormalisation), topk_ids / token_expert_indices [M, top_k] i32, sorted_ids / expert_ids /
+        num_tokens_post_pad (moe_alig_block_size), gate_up [M, top_k, 2I], act [M, top_k, I], down [M, top_k, H] (per-slot
+        down outputs x routing weight) and out [M, H].  A run overwrites them; the program reads none of them, so writing
+        into them changes nothing but what the caller reads back."""
+        o = [o for kind, o in self._ops if kind == "moe"][i]
+        return dict(o["buffers"], out=o["out"])
+
+    @staticmethod
+    def _moe_replay(o) -> None:
+        """apply_moe_weights' sequence (awq/modules/fused/moe.py:45-89) through ext, into the op's own buffers."""
+        b, M, H = o["buffers"], o["M"], o["H"]
+        torch.matmul(o["x"], o["gate_weight"].t(), out=b["logits"])
+        ext.topk_softmax(o["raw_w"], b["topk_ids"], b["token_expert_indices"], b["logits"].float())
+        if o["renormalize"]:
+            torch.div(o["raw_w"], o["raw_w"].sum(dim=-1, keepdim=True), out=b["topk_weights"])
+        else:
+            b["topk_weights"].copy_(o["raw_w"])
+        b["sorted_ids"].fill_(b["topk_ids"].numel())
+        ext.moe_alig_block_size(b["topk_ids"], o["E"], 16, b["sorted_ids"], b["expert_ids"], b["num_tokens_post_pad"])
+        gu = ext.grouped_gemm_forward(o["x"].view(M, 1, H), *o["w1"], b["topk_weights"], b["sorted_ids"], b["expert_ids"],
+                                      b["num_tokens_post_pad"], False, 8)
+        b["gate_up"].copy_(gu)
+        ext.silu_and_mul(b["act"], b["gate_up"])
+        dn = ext.grouped_gemm_forward(b["act"], *o["w2"], b["topk_weights"], b["sorted_ids"], b["expert_ids"],
+                                      b["num_tokens_post_pad"], True, 8)
+        b["down"].copy_(dn)
+        torch.sum(b["down"], dim=1, out=o["out"])
+
     # ------------------------------------------------------------------ build / run
     def _c_ops(self):
         arr = (Op * len(self._ops))()
@@ -107,6 +203,9 @@ class DecodeProgram:
             elif kind == "silu":
                 c.kind, c.M, c.K = _cabi.OP_SILU_AND_MUL, o["rows"], o["d"]
                 c.x, c.y = o["gate_up"].data_ptr(), o["out"].data_ptr()
+            elif kind == "moe":
+                c.kind, c.M, c.K, c.N = _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
+                c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
             else:
                 c.kind, c.M, c.K, c.N, c.group_size, c.ldx = _cabi.OP_LINEAR_GEMM, o["M"], o["K"], o["N"], o["G"], o["ldx"]
                 c.x, c.qweight, c.scales, c.qzeros = (o["x"].data_ptr(), o["qweight"].data_ptr(), o["scales"].data_ptr(),
@@ -199,17 +298,18 @@ class DecodeProgram:
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
-            return o["M"] if kind == "linear" else o["rows"]
+            return o["M"] if kind in ("linear", "moe") else o["rows"]
         return 0
 
     @property
     def kernel_ops(self) -> int:
+        """Ops of the fused kernel: one per linear, two per sparse_moe (gate|up with the routing, down); 0 per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
     def launches_per_run(self) -> int:
-        """Kernels of this library launched by one run()."""
-        return 1 if self.fused else len(self._ops)
+        """Kernels of this library launched by one run() (a per-op sparse_moe issues 6)."""
+        return 1 if self.fused else sum(6 if kind == "moe" else 1 for kind, _ in self._ops)
 
     def run(self) -> None:
         if not self._built:
@@ -227,6 +327,8 @@ class DecodeProgram:
                 ext.layernorm_forward_cuda(o["x"], o["weight"], o["out"], o["eps"])
             elif kind == "silu":
                 ext.silu_and_mul(o["out"], o["gate_up"])
+            elif kind == "moe":
+                self._moe_replay(o)
             else:
                 ext.linear_forward("gemm", o["x"], o["qweight"], o["scales"], o["qzeros"], o["G"], o["bias"], out=o["y"])
 

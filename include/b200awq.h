@@ -202,8 +202,27 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  * kernel's ordering cannot honour); the caller then issues the ops one by one.  Pointers are captured, not
  * copied: the tensors must stay alive and in place for the life of the program.  Create / destroy allocate and
  * copy (not capturable); run only enqueues a memset + one kernel on `stream` (capturable).  A program is not
- * re-entrant: one run in flight at a time. */
-enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3 };
+ * re-entrant: one run in flight at a time.
+ *
+ *   SPARSE_MOE    : a whole sparse-MoE block (awq/modules/fused/moe.py:26-89, FusedSparseMoeBlock.forward):
+ *                   x = normed input row [H], y = output [H], K = H, weight = a b200awq_moe_t descriptor; the op's
+ *                   result is sum_k fp16(w_k * down_k(silu_mul(gate_up_k(x)))) over the top_k routed experts.
+ *     Folding: two kernel ops.  (1) gate|up with a routing prologue: every CTA computes the router logits (fp32 dots,
+ *     rounded to fp16 like nn.Linear), softmax and top-k with topk_softmax's arithmetic (ties: lower expert) and the
+ *     optional fp32 renormalisation from its staged row, then streams the top_k selected experts' gate|up slices with
+ *     SiLU*mul fused (top_k x I activation words, slot-major).  (2) down with K' = top_k I: unit j of a set reads slot
+ *     j / (I / 128)'s expert; each slot's fp32 sum is multiplied by its routing weight and rounded to fp16 (as
+ *     grouped_gemm_forward(mul_weights) does), the slots are summed in fp32 in slot order and rounded once (torch.sum).
+ *     After a run every buffer of the descriptor holds what the per-op sequence (gate matmul, topk_softmax,
+ *     renormalisation, moe_alig_block_size, grouped_gemm_forward, silu_and_mul, grouped_gemm_forward(mul_weights),
+ *     sum) would leave there; routing tensors for M = 1.
+ *     Envelope (else B200AWQ_EUNSUPPORTED, the caller replays per op): M = 1, the stream kernel (knob 14 != 1),
+ *     E <= 64, top_k <= 8, the per-expert shapes in the stream format, at most 32 16-column sets of the gate|up op and
+ *     32 (set, slot) partial rows of the down op per CTA, and the activations of the longest K (top_k I for down) in
+ *     shared memory next to the 8-warp x 4-stage weight ring (b200awq_moe_plan below says which).
+ *     Memory: the program keeps a stream-format copy of every expert of both stacked tensors (about the size of the
+ *     packed checkpoint again: ~24 GB for Mixtral-8x7B's 32 layers). */
+enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -218,6 +237,40 @@ typedef struct b200awq_op {
   const void* weight;
   void* y;
 } b200awq_op_t;
+
+/* SPARSE_MOE descriptor (b200awq_op_t.weight points at it; the program copies it at creation, the tensors it names
+ * are captured by address).  Stacked GEMM-layout experts as awq/models/mixtral.py:129-151 builds them. */
+typedef struct b200awq_moe {
+  int32_t E, top_k, renormalize, group_size;
+  int32_t H, I;                 /* hidden size, expert intermediate size */
+  int32_t block_size;           /* moe_alig_block_size block (16 at the reference's call site) */
+  int32_t sorted_len;           /* entries of sorted_ids: >= top_k * M + E * (block_size - 1) */
+  const void* gate_weight;      /* router nn.Linear weight [E, H] f16, no bias */
+  const int32_t* w1_qweight;    /* gate|up [E, H, 2I/8] */
+  const void* w1_scales;        /* [E, H/G, 2I] f16 */
+  const int32_t* w1_qzeros;     /* [E, H/G, 2I/8] */
+  const int32_t* w2_qweight;    /* down [E, I, H/8] */
+  const void* w2_scales;        /* [E, I/G, H] f16 */
+  const int32_t* w2_qzeros;     /* [E, I/G, H/8] */
+  /* outputs, as the per-op sequence leaves them (M = 1) */
+  void* logits;                 /* [E] f16 */
+  float* topk_weights;          /* [top_k] f32, after the renormalisation */
+  int32_t* topk_ids;            /* [top_k] */
+  int32_t* token_expert_indices;/* [top_k] */
+  int32_t* sorted_ids;          /* [sorted_len] (entries past the padded runs = top_k) */
+  int32_t* expert_ids;          /* [>= top_k + E] */
+  int32_t* num_tokens_post_pad; /* [1] */
+  void* gate_up;                /* [top_k, 2I] f16 */
+  void* act;                    /* [top_k, I] f16 */
+  void* down;                   /* [top_k, H] f16: per-slot down outputs x routing weight */
+} b200awq_moe_t;
+
+/* Host-side plan of one SPARSE_MOE block in an M = 1 stream program on a device with `sm_count` SMs (no GPU needed).
+ * out8 = {kernel ops (2), gate|up 16-column sets (top_k 2I / 16), gate|up units per slot segment, most gate|up sets one
+ * CTA owns, down units per set (top_k I / min(G, 128)), down units per slot segment, most (set, slot) partial rows one
+ * CTA keeps in the down op, dynamic shared memory of the kernel for this block alone}.  B200AWQ_EUNSUPPORTED outside the
+ * envelope above, B200AWQ_EINVAL for bad arguments. */
+int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8);
 
 typedef struct b200awq_program* b200awq_program_t;
 
@@ -240,7 +293,7 @@ int b200awq_program_tokens(b200awq_program_t prog);
  * output-stationary and hands activations from op to op as tagged fp16 words (csrc/program_stream.cuh).  Creation
  * prefers 2 and falls back to 1 (shapes / aliasing outside its envelope; knob 14 = 1 forces 1, 2 forbids 1). */
 int b200awq_program_kind(b200awq_program_t prog);
-/* number of fused kernel ops (= linear ops) of the program; 0 for a null handle */
+/* number of fused kernel ops (= linear ops, two per SPARSE_MOE op) of the program; 0 for a null handle */
 int b200awq_program_num_ops(b200awq_program_t prog);
 /* workspace: b200awq_workspace_bytes(8, K, max N over the program's linears rounded up to 8): four rows of 64-bit
  * packed split-K sums; zero-initialised and left all-zero like the per-op workspace (the same buffer may serve both) */
