@@ -47,7 +47,7 @@ class Moe(ctypes.Structure):
     ]
 
 
-OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE = 1, 2, 3, 4
+OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD = 1, 2, 3, 4, 5
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -95,6 +95,7 @@ SIGNATURES = {
     "b200awq_program_create": (_c_int, [ctypes.POINTER(Op), _c_int, ctypes.POINTER(_c_void_p)]),
     "b200awq_program_create_batched": (_c_int, [ctypes.POINTER(Op), _c_int, _c_int, ctypes.POINTER(_c_void_p)]),
     "b200awq_program_tokens": (_c_int, [_c_void_p]),
+    "b200awq_program_plan": (_c_int, [ctypes.POINTER(Op), _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_program_num_ops": (_c_int, [_c_void_p]),
     "b200awq_program_kind": (_c_int, [_c_void_p]),

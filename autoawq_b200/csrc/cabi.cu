@@ -223,6 +223,18 @@ int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t
   return b200awq_program_create_batched(ops, n_ops, 1, out);
 }
 
+int b200awq_program_plan(const b200awq_op_t* ops, int n_ops, int max_tokens, int sm_count, int residual_window,
+                         int* kernel_ops) {
+  if (kernel_ops == nullptr || sm_count <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
+  *kernel_ops = 0;
+  Program* p = nullptr;
+  cudaError_t ce = cudaSuccess;
+  ProgramPlan plan{sm_count, residual_window, 0};
+  const int rc = program_create(ops, n_ops, max_tokens, &p, &ce, &plan);
+  if (rc == B200AWQ_OK) *kernel_ops = plan.kernel_ops;
+  return rc;
+}
+
 int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8) {
   return moe_plan(E, top_k, H, I, group_size, sm_count, out8);
 }

@@ -83,7 +83,12 @@ cudaError_t gemm_tcq_debug_read(void* dst, size_t bytes);   // phase timestamps 
 
 // decode program (program.cu)
 struct Program;
-int program_create(const struct ::b200awq_op* ops, int n, int max_tokens, Program** out, cudaError_t* cuda_err);
+// plan (b200awq_program_plan): fold only, for `grid` SMs and a residual window (<= 0: the library's); no CUDA call
+struct ProgramPlan {
+  int grid, window, kernel_ops;
+};
+int program_create(const struct ::b200awq_op* ops, int n, int max_tokens, Program** out, cudaError_t* cuda_err,
+                   ProgramPlan* plan = nullptr);
 int program_max_n(const Program* p);
 int program_m(const Program* p);
 int program_num_ops(const Program* p);

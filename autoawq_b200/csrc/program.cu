@@ -198,7 +198,8 @@ struct ProgWatch {
   }
 };
 enum { kWStaged = 1, kWExtDep = 2, kWEmpty = 3, kWFull = 4, kWGate = 5, kWRedOk = 6, kWStagedOp = 7, kWDutyY = 8,
-       kWDutySilu = 9, kWCopy = 10, kWSilu = 11, kWNorm = 12, kWRoute = 13 /* producer: a MoE block's routing */ };
+       kWDutySilu = 9, kWCopy = 10, kWSilu = 11, kWNorm = 12, kWRoute = 13 /* producer: a MoE block's routing */,
+       kWResidual = 14 /* finish: the tagged row of a residual add's source op */ };
 __device__ __forceinline__ void prog_wait(const int* cnt, int target, int code, int op) {
   ProgWatch wd;
   while (ld_acquire_s32(cnt) < target)
@@ -715,6 +716,16 @@ struct Program {
   // sparse-MoE blocks (stream_moe_kernel): their descriptors
   SpMoe* d_moe = nullptr;
   int n_moe = 0;
+  // residual adds (stream_residual_kernel / stream_batch_residual_kernel): one SpRes per kernel op, null without adds
+  SpRes* d_res = nullptr;
+};
+
+// An ADD folded into table entry i (program_create): the entry's y is swapped for the ADD's output (what its row
+// publishes, so the hazard rules resolve later readers to the row); raw_y is the linear's own output, still stored
+struct ResFold {
+  const void* raw_y = nullptr;   // null: no ADD folded into this entry
+  const void* ext = nullptr;     // external residual (no op of the program writes it)
+  int op = -1;                   // >= 0: the residual is that older entry's published row
 };
 
 // One SPARSE_MOE op as the folding sees it: two table entries (gate|up, down) and the recorded descriptor
@@ -781,7 +792,8 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
 // Sparse-MoE blocks (`fold[i].kind` != 0, M = 1 only): the gate|up entry is a mode-1 op over top_k slots of 2I
 // columns, the down entry reads its published row (K' = top_k I); both stream E per-expert slices packed back to back.
 static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
-                         const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes) {
+                         const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes,
+                         const std::vector<ResFold>& res) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
@@ -818,6 +830,13 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   };
   for (int i = 0; i < n; ++i)
     if (moe_kind(i) == 1) mode[i] = 1;
+  // residual adds: the producer and an in-program residual must publish plain columns (a mode-1 row holds SiLU*mul)
+  bool has_res = false;
+  for (int i = 0; i < n && !res.empty(); ++i)
+    if (res[i].raw_y != nullptr) {
+      if (mode[i] == 1 || (res[i].op >= 0 && mode[res[i].op] == 1)) return false;
+      has_res = true;
+    }
   size_t wbytes = 0, max_cols = 0;
   int max_K = 0, lmax = 0, nu_max = 0;
   std::vector<size_t> woff(n);
@@ -839,8 +858,8 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     max_cols = std::max(max_cols, (size_t)(mode[i] ? p.N / 2 : p.N));
     max_K = std::max(max_K, p.K);
   }
-  if (M == 1 && has_moe) {
-    // the MoE kernel runs 8 consumer warps with 4 ring stages each, behind the routing area
+  if (M == 1 && (has_moe || has_res)) {
+    // the MoE / residual kernel runs 8 consumer warps with 4 ring stages each, behind the routing area
     if (sp_fixed_smem(8, 4, true) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
   } else if (M == 1) {
     if (sp_fixed_smem(12, 3) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;   // (the largest configuration)
@@ -858,7 +877,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     SpOp& o = ops[i];
     std::memset(&o, 0, sizeof(o));
     o.bias = p.bias;
-    o.y = p.y;
+    o.y = (!res.empty() && res[i].raw_y != nullptr) ? static_cast<__half*>(const_cast<void*>(res[i].raw_y)) : p.y;
     o.K = p.K;
     o.N = p.N;
     const int UK = p.G < 128 ? p.G : 128;
@@ -980,6 +999,27 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       e = cudaFuncSetAttribute(stream_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)(227 * 1024));
   }
+  if (e == cudaSuccess && has_res) {
+    std::vector<SpRes> rd(n);
+    for (int i = 0; i < n; ++i) {
+      std::memset(&rd[i], 0, sizeof(SpRes));
+      rd[i].op = -1;
+      if (res[i].raw_y == nullptr) continue;
+      rd[i].out = table[i].y;                       // the ADD's output (the entry's y was swapped for it)
+      rd[i].op = res[i].op;
+      rd[i].ext = static_cast<const __half*>(res[i].ext);
+    }
+    e = cudaMalloc(&pr->d_res, (size_t)n * sizeof(SpRes));
+    if (e == cudaSuccess) e = cudaMemcpy(pr->d_res, rd.data(), (size_t)n * sizeof(SpRes), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_residual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_residual_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_residual_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_residual_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  }
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_sp_ops, ops.data(), (size_t)n * sizeof(SpOp), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_cta, cta.data(), cta.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
   if (e == cudaSuccess)
@@ -1001,6 +1041,8 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     cudaFree(pr->d_rows);
     cudaFree(pr->d_state);
     cudaFree(pr->d_moe);
+    cudaFree(pr->d_res);
+    pr->d_res = nullptr;
     pr->d_stream = nullptr;
     pr->d_sp_ops = nullptr;
     pr->d_cta = nullptr;
@@ -1043,7 +1085,8 @@ static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
 //   * a linear must not write (y) what it reads (src) or what its own prologue publishes (xout);
 //   * a buffer that a pending glue record depends on must not be overwritten before the record's last use.
 // Every op has the same M <= max_tokens rows (M > 1: the batched stream kernel only); extents below cover all M rows.
-int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program** out, cudaError_t* cuda_err) {
+int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program** out, cudaError_t* cuda_err,
+                   ProgramPlan* plan) {
   *cuda_err = cudaSuccess;
   *out = nullptr;
   if (ops_in == nullptr || n_in <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
@@ -1116,14 +1159,70 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     bool live;
   };
   std::vector<Glue> glues;
-  const int grid = prog_sm_count();
+  // plan: the folding alone, for `plan->grid` SMs and residual window `plan->window`, without any CUDA call
+  const int grid = plan != nullptr ? plan->grid : prog_sm_count();
+  const int res_window = plan != nullptr && plan->window > 0 ? plan->window : kSpResWindow;
+  std::vector<int> stage_row;    // per table entry: the op whose WHOLE published row its staging waits for, or -1
   int max_K = 0, max_N = 0, M = -1;
   bool v3_ok = moes.empty();     // the split-K kernel has no MoE support
+  std::vector<ResFold> res;      // per table entry: the ADD folded into it, if any
+  std::vector<std::pair<const void*, size_t>> ext_res;   // external residuals: no op of the program may write them
   for (int i = 0; i < n; ++i) {
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
     if (op.M != M) return B200AWQ_EUNSUPPORTED;
     auto rows_bytes = [&](int width) { return (size_t)(M > 0 ? M : 1) * width * 2; };   // M contiguous fp16 rows
+    // a read of a linear's raw output after an ADD was folded into it: its row carries the sum, not y
+    auto reads_raw_y = [&](const void* p, size_t bytes) {
+      for (size_t j = 0; j < table.size(); ++j)
+        if (res[j].raw_y != nullptr && overlaps(res[j].raw_y, rows_bytes(table[j].N), p, bytes)) return true;
+      return false;
+    };
+    if (op.kind == B200AWQ_OP_ADD) {
+      // y = x + weight, folded into the epilogue of the op recorded just before it (a linear / a MoE block's down)
+      if (op.x == nullptr || op.weight == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
+      if ((op.K % 8) != 0 || !aligned16(op.x) || !aligned16(op.weight) || !aligned16(op.y)) return B200AWQ_EUNSUPPORTED;
+      const size_t bytes = rows_bytes(op.K);
+      if (overlaps(op.y, bytes, op.x, bytes) || overlaps(op.y, bytes, op.weight, bytes)) return B200AWQ_EUNSUPPORTED;
+      if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty()) return B200AWQ_EUNSUPPORTED;
+      ProgOp& pv = table.back();
+      const void* r;                 // the residual: the operand that is not the producer's whole output
+      if (op.x == pv.y) r = op.weight;
+      else if (op.weight == pv.y) r = op.x;
+      else return B200AWQ_EUNSUPPORTED;  // neither operand is the producer's output (both external)
+      if (op.K != pv.N || overlaps(r, bytes, pv.y, bytes)) return B200AWQ_EUNSUPPORTED;
+      ResFold rf;
+      rf.raw_y = pv.y;
+      // in-program residual: the newest op that wrote any of it must have published exactly it, kSpResWindow ops back
+      for (int j = static_cast<int>(table.size()) - 2; j >= 0 && rf.op < 0; --j) {
+        const bool hit = overlaps(table[j].y, rows_bytes(table[j].N), r, bytes) ||
+                         (res[j].raw_y != nullptr && overlaps(res[j].raw_y, rows_bytes(table[j].N), r, bytes));
+        if (!hit) continue;
+        if (r != table[j].y || table[j].N != op.K) return B200AWQ_EUNSUPPORTED;
+        if (static_cast<int>(table.size()) - 1 - j > res_window) return B200AWQ_EUNSUPPORTED;
+        rf.op = j;
+      }
+      for (const Glue& gl : glues)   // a glue output is written by CTA slices, never published as a row
+        if (overlaps(gl.out, rows_bytes(gl.width), r, bytes)) return B200AWQ_EUNSUPPORTED;
+      if (rf.op < 0) {
+        rf.ext = r;
+        ext_res.emplace_back(r, bytes);
+      }
+      // the output must not overlap what the producer reads (other CTAs may still be staging it) or publishes
+      const size_t pv_src = ((size_t)(M - 1) * pv.src_ld + (size_t)(pv.prologue == kProSilu ? 2 : 1) * pv.K) * 2;
+      if (overlaps(op.y, bytes, pv.src, pv_src) || (pv.xout != nullptr && overlaps(op.y, bytes, pv.xout, rows_bytes(pv.K))))
+        return B200AWQ_EUNSUPPORTED;
+      for (Glue& gl : glues)         // writing the output over something a live glue record still needs ends that record
+        if (gl.live && (overlaps(gl.out, rows_bytes(gl.width), op.y, bytes) ||
+                        overlaps(gl.src, rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width), op.y, bytes))) {
+          if (!gl.used) return B200AWQ_EUNSUPPORTED;
+          gl.live = false;
+        }
+      pv.y = static_cast<__half*>(op.y);   // the producer's row now publishes the sum
+      res.back() = rf;
+      v3_ok = false;                 // the split-K kernel has no residual support
+      continue;
+    }
     if (op.kind == B200AWQ_OP_RMSNORM || op.kind == B200AWQ_OP_SILU_AND_MUL) {
       if (op.x == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
       if (op.kind == B200AWQ_OP_RMSNORM && op.weight == nullptr) return B200AWQ_EINVAL;
@@ -1137,6 +1236,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
           if (!gl.used) return B200AWQ_EUNSUPPORTED;
           gl.live = false;
         }
+      if (reads_raw_y(op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
       // its input must not be a buffer only CTA 0 publishes
       for (const Glue& gl : glues)
         if (overlaps(gl.out, rows_bytes(gl.width), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
@@ -1160,7 +1260,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     std::memset(&p, 0, sizeof(p));
     p.ext_dep = -1;
     p.qw_src = a.qweight;
-    if (v3_ok) {
+    if (v3_ok && plan == nullptr) {
       cudaError_t e = make_tmap_2d(a.qweight, /*int32*/ 1, (uint64_t)(a.N / 8), (uint64_t)a.K, (uint64_t)(a.N / 8) * 4, 32,
                                    kV3TileRows, &p.tmw);
       if (e != cudaSuccess) {
@@ -1209,7 +1309,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     // the source's M rows (row pitch src_ld), this op's output (M rows of N)
     const size_t src_bytes = ((size_t)(M - 1) * p.src_ld + (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K) * 2;
     const size_t y_bytes = rows_bytes(op.N);
-    if (overlaps(p.y, y_bytes, p.src, src_bytes)) return B200AWQ_EUNSUPPORTED;
+    if (overlaps(p.y, y_bytes, p.src, src_bytes) || reads_raw_y(p.src, src_bytes)) return B200AWQ_EUNSUPPORTED;
     if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), p.y, y_bytes)) return B200AWQ_EUNSUPPORTED;
     if (!table.empty()) {
       // the previous op's fp16 output reaches memory only while THIS op stages its activations: a source inside it
@@ -1242,12 +1342,64 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       }
     max_K = op.K > max_K ? op.K : max_K;
     max_N = op.N > max_N ? op.N : max_N;
+    {
+      // a staging wait on the whole row of op s waits for every CTA that owns columns of s
+      const int s = p.src_prev ? static_cast<int>(table.size()) - 1 : p.ext_dep;
+      const size_t width = (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K;
+      stage_row.push_back(s >= 0 && p.src == table[s].y && width == (size_t)table[s].N ? s : -1);
+    }
     table.push_back(p);
     fold.push_back(xfold[i]);
+    res.emplace_back();
   }
   for (const Glue& gl : glues)
     if (!gl.used) return B200AWQ_EUNSUPPORTED;   // a glue op nobody consumes would never run
   if (table.empty()) return B200AWQ_EUNSUPPORTED;
+  const int nt = static_cast<int>(table.size());
+  for (const auto& er : ext_res) {
+    // an external residual is read at the finish of its op, any time during the run: nothing of the program may write it
+    for (int j = 0; j < nt; ++j)
+      if (overlaps(table[j].y, (size_t)M * table[j].N * 2, er.first, er.second) ||
+          (res[j].raw_y != nullptr && overlaps(res[j].raw_y, (size_t)M * table[j].N * 2, er.first, er.second)))
+        return B200AWQ_EUNSUPPORTED;
+    for (const Glue& gl : glues)
+      if (overlaps(gl.out, (size_t)M * gl.width * 2, er.first, er.second)) return B200AWQ_EUNSUPPORTED;
+    for (const b200awq_moe_t& m : moes)
+      if (overlaps(m.gate_up, (size_t)m.top_k * 2 * m.I * 2, er.first, er.second) ||
+          overlaps(m.act, (size_t)m.top_k * m.I * 2, er.first, er.second) ||
+          overlaps(m.down, (size_t)m.top_k * m.H * 2, er.first, er.second) ||
+          overlaps(m.logits, (size_t)m.E * 2, er.first, er.second) ||
+          overlaps(m.topk_weights, (size_t)m.top_k * M * 4, er.first, er.second) ||
+          overlaps(m.topk_ids, (size_t)m.top_k * M * 4, er.first, er.second) ||
+          overlaps(m.token_expert_indices, (size_t)m.top_k * M * 4, er.first, er.second) ||
+          overlaps(m.sorted_ids, (size_t)m.sorted_len * 4, er.first, er.second) ||
+          overlaps(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4, er.first, er.second) ||
+          overlaps(m.num_tokens_post_pad, 4, er.first, er.second))
+        return B200AWQ_EUNSUPPORTED;
+  }
+  for (int i = 0; i < nt; ++i) {
+    // An in-program residual (row j % 4) is read in op i's finish, by the CTA that published those columns in op j (same
+    // width, same partition).  Ops j + 4, j + 8, ... publish into that row again.  Op i itself (i = j + 4) only rewrites
+    // the words each thread has just read; the next one after i, op k, may overwrite them only once every CTA has
+    // finished op i: some op in (i, k] must stage the WHOLE row of an op >= i that every CTA owns columns of (a wait on a
+    // slice of a row, or on a narrow op, waits for a few CTAs only).  tests/test_stream_residual_model.py replays random
+    // programs through this rule (b200awq_program_plan).
+    const int j = res[i].op;
+    if (j < 0) continue;
+    int k = j + kSpRows;
+    while (k <= i) k += kSpRows;
+    if (k >= nt) continue;
+    int reach = -1;
+    for (int m = i + 1; m <= k; ++m) {
+      const int s = stage_row[m];
+      if (s >= 0 && table[s].N / 16 >= grid) reach = std::max(reach, s);
+    }
+    if (reach < i) return B200AWQ_EUNSUPPORTED;
+  }
+  if (plan != nullptr) {
+    plan->kernel_ops = nt;
+    return B200AWQ_OK;
+  }
 
   Program* pr = new Program();
   pr->n_ops = static_cast<int>(table.size());
@@ -1255,7 +1407,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   pr->max_N = max_N;
   cudaError_t e = cudaGetDevice(&pr->device);
   // first choice: the stream variant (one-time re-layout, output-stationary partition); knob 14 = 1 skips it
-  if (e == cudaSuccess && knob(14) != 1 && stream_build(pr, table, grid, M, &e, fold, moes)) {
+  if (e == cudaSuccess && knob(14) != 1 && stream_build(pr, table, grid, M, &e, fold, moes, res)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -1314,6 +1466,13 @@ cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st) {
     cfg.numAttrs = 1;
     const SpOp* sops = p->d_sp_ops;
     const uint32_t* cta = p->d_cta;
+    if (p->d_res != nullptr) {   // residual adds: the same kernel with the residual steps in its finish
+      auto rk = sb_mt(p->M) == 2 ? stream_batch_residual_kernel<2>
+                                 : (sb_mt(p->M) == 4 ? stream_batch_residual_kernel<4> : stream_batch_residual_kernel<8>);
+      const SpRes* rd = p->d_res;
+      return cudaLaunchKernelEx(&cfg, rk, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
+                                p->sb_lmax, p->sb_nu_max, knob(3), rd);
+    }
     auto kern = sb_mt(p->M) == 2 ? stream_batch_kernel<2> : (sb_mt(p->M) == 4 ? stream_batch_kernel<4> : stream_batch_kernel<8>);
     return cudaLaunchKernelEx(&cfg, kern, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
                               p->sb_lmax, p->sb_nu_max, knob(3));
@@ -1343,6 +1502,15 @@ cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st) {
     // the default; n > 0: at most n - 1 ops ahead, 1 = strictly gated)
     const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
     const SpMoe* no_moe = nullptr;
+    if (p->d_res != nullptr) {
+      // programs with residual adds (with or without sparse-MoE blocks): always 8 consumer warps x 4 ring stages
+      cfg.blockDim = dim3(32 + 8 * 32);
+      cfg.dynamicSmemBytes = sp_fixed_smem(8, 4, true) + p->xs_bytes;
+      const SpMoe* md = p->d_moe;
+      const SpRes* rd = p->d_res;
+      return cudaLaunchKernelEx(&cfg, stream_residual_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
+                                knob(3), l2_ahead, gate_ahead, md, rd);
+    }
     if (p->n_moe > 0) {
       // programs with sparse-MoE blocks: the MOE instantiation, always 8 consumer warps x 4 ring stages
       cfg.blockDim = dim3(32 + 8 * 32);
@@ -1393,6 +1561,7 @@ void program_destroy(Program* p) {
   cudaFree(p->d_rows);
   cudaFree(p->d_state);
   cudaFree(p->d_moe);
+  cudaFree(p->d_res);
   delete p;
 }
 

@@ -132,369 +132,24 @@ __global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
     stream_batch_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
                         uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int M, int spw, int lmax,
                         int nu_max, int dbg) {
-  constexpr int NW = kSbWarps, GR = kSbGR;
-  extern __shared__ __align__(1024) uint8_t sb_smem[];
-  const int NS = NW * spw;
-  uint8_t* ring = sb_smem;
-  float* part = reinterpret_cast<float*>(sb_smem + (size_t)NS * kSpStageBytes);   // [lmax][8 warps][MT][16]
-  float* xsum = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(part) + sb_part_bytes(lmax, MT));   // [NU][MT]
-  uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(xsum) + sb_xsum_bytes(nu_max, MT));
-  uint64_t* empty = full + NS;
-  SpOp* sdesc = reinterpret_cast<SpOp*>(empty + NS);        // [2] op descriptors, prefetched one op ahead
-  int* misc = reinterpret_cast<int*>(sdesc + 2);
-  float* wsum = reinterpret_cast<float*>(misc);             // [MT][8] per-warp sums of squares of every row
-  int* wfirst = misc + 64;                                  // [NW] first local set each warp touched (-1: none)
-  int* wlast = misc + 64 + NW;                              // [NW]
-  uint32_t* scta = reinterpret_cast<uint32_t*>(misc + 64 + 2 * NW);   // [2][2] this CTA's unit range
-  int* staged_op = misc + 68 + 2 * NW;
-  static_assert((69 + 2 * NW) * 4 <= 512 && MT <= 8, "misc area");
-  uint32_t* xs = reinterpret_cast<uint32_t*>(sb_smem + sb_fixed_smem(spw, lmax, MT, nu_max));   // [K / 16][MT][8 words]
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nblk = gridDim.x, bid = blockIdx.x;
-  // a cooperative launch never carries the PDL attribute (then this is a no-op); the tag state below is written by
-  // the previous run of this program
+  // a cooperative launch never carries the PDL attribute (then this is a no-op); the tag state the body reads first is
+  // written by the previous run of this program
   pdl_wait();
-  const int base = state[0];
+#include "program_batch_body.inc"
+}
 
-  if (tid == 0) {
-    for (int s = 0; s < NS; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    fence_mbar_init();
-    *staged_op = -1;
-  }
-  if (warp == 1) {
-    reinterpret_cast<uint32_t*>(sdesc)[lane] = reinterpret_cast<const uint32_t*>(ops)[lane];
-    if (lane < 2) scta[lane] = cta_all[bid + lane];
-  }
-  __syncthreads();
-
-  if (warp == 0) {
-    // ============================================================ producer: the weight stream of ALL ops
-    // as in stream_program_kernel (ungated, no L2 prefetch cursor: the defaults there)
-    const int w = lane < NW ? lane : 0;
-    bool active = lane < NW;
-    struct Run {
-      uint32_t u, ub;
-      int UB, ups;
-      const uint8_t* src;
-    };
-    auto fetch = [&](int op, Run& r) {
-      r.u = r.ub = 0;
-      r.UB = r.ups = 1;
-      r.src = nullptr;
-      if (op < n_ops && lane < NW) {
-        const uint32_t u0 = cta_all[(size_t)op * (nblk + 1) + bid], u1 = cta_all[(size_t)op * (nblk + 1) + bid + 1];
-        const uint32_t nu = u1 - u0;
-        r.u = u0 + (uint32_t)((uint64_t)nu * w / NW);
-        r.ub = u0 + (uint32_t)((uint64_t)nu * (w + 1) / NW);
-        r.UB = ops[op].unit_bytes;
-        r.ups = ops[op].ups;
-        r.src = ops[op].wstream;
-      }
-    };
-    Run cur, nxt;
-    int op = 0;
-    fetch(0, cur);
-    fetch(1, nxt);
-    int stage_i = 0;
-    uint32_t ph = 0;
-    ProgWatch wd;
-    for (;;) {
-      while (active && cur.u >= cur.ub) {
-        if (++op >= n_ops) {
-          active = false;
-          break;
-        }
-        cur = nxt;
-        fetch(op + 1, nxt);
-      }
-      if (!__any_sync(0xffffffffu, active)) break;
-      bool issued = false;
-      if (active) {
-        const int stage = w * spw + stage_i;
-        if (mbar_test_wait(&empty[stage], ph ^ 1)) {
-          const int n = (int)(cur.ub - cur.u) < cur.ups ? (int)(cur.ub - cur.u) : cur.ups;
-          mbar_arrive_expect_tx(&full[stage], (uint32_t)(n * cur.UB));
-          bulk_load_1d(ring + (size_t)stage * kSpStageBytes, cur.src + (size_t)cur.u * cur.UB, (uint32_t)(n * cur.UB),
-                       &full[stage]);
-          cur.u += (uint32_t)cur.ups;
-          if (++stage_i == spw) { stage_i = 0; ph ^= 1; }
-          issued = true;
-        }
-      }
-      if (!__any_sync(0xffffffffu, issued)) {
-        if (__any_sync(0xffffffffu, wd.tick(kWEmpty, op))) break;   // watchdog (warp-uniform): never hang the GPU
-        __nanosleep(32);
-      }
-    }
-  } else {
-    // ================================================================ consumers
-    const int cw = warp - 1;
-    const int ct = tid - 32;
-    const int g = lane >> 2, tig = lane & 3;
-    const int m0 = 2 * tig, m1 = 2 * tig + 1;   // tokens of this lane's accumulators (d0 / d2 and d1 / d3)
-    int stage_i = 0;
-    uint32_t ph = 0;
-
-    for (int op = 0; op < n_ops; ++op) {
-      const SpOp* o = sdesc + (op & 1);
-      const int K = o->K, N = o->N, NU = o->NU, F = o->F, UB = o->unit_bytes, ups = o->ups, mode = o->mode;
-      const uint32_t u0 = scta[(op & 1) * 2], u1 = scta[(op & 1) * 2 + 1];
-      const uint32_t nu = u1 - u0;
-      const uint32_t ua = u0 + (uint32_t)((uint64_t)nu * cw / NW), ub = u0 + (uint32_t)((uint64_t)nu * (cw + 1) / NW);
-      const int set0 = (int)(u0 / NU);
-      const __half* bias = o->bias;
-      __half* y = o->y;
-      __half* act_out = o->act_out;
-      SP_STAMP(0);
-
-      // ---- stage M rows: per row exactly the M = 1 staging (thread t: 8 consecutive k per pass, k = 2048 pass + 8 t;
-      //      sums of squares in the order of aux.cu's rmsnorm_kernel).  The (row, pass) items are taken in batches of
-      //      4 so that four loads are in flight before the first tag is looked at.
-      {
-        const int uk_shift = o->uk_shift;
-        const int seg = (1 << uk_shift) >> 3;
-        const bool from_row = o->src_op >= 0;
-        const uint32_t* row0 = from_row ? rows + (size_t)(o->src_op % kSpRows) * M * row_stride + o->src_off : nullptr;
-        const uint32_t want = from_row ? sp_tag(base, o->src_op) : 0u;
-        const __half* src = o->src;
-        const int64_t ldx = o->ldx;
-        const bool norm = o->prologue == kProRmsnorm;
-        const __half* nw = o->norm_w;
-        const int cb_first = cw * 256;
-        const int P = cb_first < K ? (K - cb_first + kSpStagePass - 1) / kSpStagePass : 0;   // passes per row
-        const int items = P * M;
-        auto frag_ptr = [&](int c, int m) { return xs + ((size_t)(c >> 4) * MT + m) * 8 + ((c >> 3) & 1); };
-        auto unit_sums = [&](int c, int m, bool ok, const uint32_t (&h)[4]) {
-          float sx = 0.f;
-          if (ok) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 f = __half22float2(u32_as_h2(h[q]));
-              sx += f.x + f.y;
-            }
-          }
-          for (int d = 1; d < seg; d <<= 1) sx += __shfl_xor_sync(0xffffffffu, sx, d);
-          if (ok && (lane & (seg - 1)) == 0) xsum[(c >> uk_shift) * MT + m] = sx;
-        };
-        float ss = 0.f;
-        for (int q0 = 0; q0 < items; q0 += 4) {       // warp-uniform trip counts
-          uint4 v0[4], v1[4];
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            const int q = q0 + b, m = q / (P > 0 ? P : 1), c = cb_first + (q - m * P) * kSpStagePass + lane * 8;
-            if (q < items && c < K) {
-              if (from_row) {
-                v0[b] = ld_relaxed_u4(row0 + (size_t)m * row_stride + c);
-                v1[b] = ld_relaxed_u4(row0 + (size_t)m * row_stride + c + 4);
-              } else {
-                v0[b] = ldg_stream_u4(src + m * ldx + c);
-              }
-            }
-          }
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            const int q = q0 + b;
-            if (q >= items) break;                                       // warp-uniform
-            const int m = q / P, p = q - m * P;
-            const int c = cb_first + p * kSpStagePass + lane * 8;
-            const bool ok = c < K;
-            uint32_t h[4] = {0u, 0u, 0u, 0u};
-            if (ok) {
-              if (from_row) {
-                const uint32_t* row = row0 + (size_t)m * row_stride;
-                ProgWatch wd;
-                for (;;) {
-                  const uint4 a = v0[b], d = v1[b];
-                  if ((a.x >> 16) == want && (a.y >> 16) == want && (a.z >> 16) == want && (a.w >> 16) == want &&
-                      (d.x >> 16) == want && (d.y >> 16) == want && (d.z >> 16) == want && (d.w >> 16) == want)
-                    break;
-                  if (wd.tick(kWCopy, op)) break;
-                  v0[b] = ld_relaxed_u4(row + c);
-                  v1[b] = ld_relaxed_u4(row + c + 4);
-                }
-                h[0] = (v0[b].x & 0xffffu) | (v0[b].y << 16);
-                h[1] = (v0[b].z & 0xffffu) | (v0[b].w << 16);
-                h[2] = (v1[b].x & 0xffffu) | (v1[b].y << 16);
-                h[3] = (v1[b].z & 0xffffu) | (v1[b].w << 16);
-              } else {
-                h[0] = v0[b].x; h[1] = v0[b].y; h[2] = v0[b].z; h[3] = v0[b].w;
-              }
-              uint32_t* dst = frag_ptr(c, m);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                dst[2 * k] = h[k];
-                const float2 f = __half22float2(u32_as_h2(h[k]));
-                ss += f.x * f.x + f.y * f.y;
-              }
-            }
-            if (!norm) unit_sums(c, m, ok, h);
-            if (p == P - 1) {                                            // row m done: this warp's sum of squares
-              if (norm) {
-                const float sw = prog_warp_sum(ss);
-                if (lane == 0) wsum[m * 8 + cw] = sw;
-              }
-              ss = 0.f;
-            }
-          }
-        }
-        if (cb_first >= K && norm && lane == 0)                          // a warp without k of its own
-          for (int m = 0; m < M; ++m) wsum[m * 8 + cw] = 0.f;
-        SP_STAMP(1);
-        if (norm) {
-          named_bar_sync_gv(1, NW * 32);
-          __half* xout = o->xout;
-          int xlo = 0, xhi = 0;
-          if (xout != nullptr) {
-            const int u8 = K >> 3;
-            xlo = (int)((int64_t)u8 * bid / nblk) << 3;
-            xhi = (int)((int64_t)u8 * (bid + 1) / nblk) << 3;
-          }
-          for (int q = 0; q < items; ++q) {
-            const int m = q / P, p = q - m * P;
-            const int c = cb_first + p * kSpStagePass + lane * 8;
-            const bool ok = c < K;
-            float tot = 0.f;
-#pragma unroll
-            for (int i = 0; i < kSpStageWarps; ++i) tot += wsum[m * 8 + i];
-            const float rs = rsqrtf(tot / static_cast<float>(K) + o->eps);
-            uint32_t h[4] = {0u, 0u, 0u, 0u};
-            if (ok) {
-              uint32_t* dst = frag_ptr(c, m);
-              const uint4 wv = __ldg(reinterpret_cast<const uint4*>(nw + c));
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const float2 a = __half22float2(u32_as_h2(dst[2 * k]));
-                const float2 wk = __half22float2(u32_as_h2((&wv.x)[k]));
-                h[k] = h2_as_u32(__halves2half2(__float2half_rn(a.x * rs * wk.x), __float2half_rn(a.y * rs * wk.y)));
-                dst[2 * k] = h[k];
-              }
-              if (c >= xlo && c < xhi)
-                *reinterpret_cast<uint4*>(xout + (size_t)m * K + c) = make_uint4(h[0], h[1], h[2], h[3]);
-            }
-            unit_sums(c, m, ok, h);
-          }
-        }
-        named_bar_sync_gv(1, NW * 32);
-      }
-      if (ct == 0) st_release_cta_smem(staged_op, op);
-      SP_STAMP(2);
-      if (cw == 0 && op + 1 < n_ops) {
-        SpOp* dn = sdesc + ((op + 1) & 1);
-        if (lane < 8) cp_async_16(reinterpret_cast<uint8_t*>(dn) + lane * 16, reinterpret_cast<const uint8_t*>(ops + op + 1) + lane * 16);
-        else if (lane < 10)
-          cp_async_4(scta + ((op + 1) & 1) * 2 + (lane - 8), cta_all + (size_t)(op + 1) * (nblk + 1) + bid + (lane - 8));
-      }
-
-      // ---- this warp's run of units: the split and fold order of the M = 1 kernel, two tokens per lane
-      {
-        int s_cur = (int)(ua / NU), j = (int)(ua - (uint32_t)s_cur * NU);
-        float ylo0 = 0.f, yhi0 = 0.f, ylo1 = 0.f, yhi1 = 0.f;
-        int first_ls = -1, last_ls = -1;
-        auto flush = [&]() {
-          const int ls = s_cur - set0;
-          float* p = part + ((size_t)ls * NW + cw) * MT * 16;
-          if (m0 < M) {
-            p[m0 * 16 + g] = ylo0;
-            p[m0 * 16 + g + 8] = yhi0;
-          }
-          if (m1 < M) {
-            p[m1 * 16 + g] = ylo1;
-            p[m1 * 16 + g + 8] = yhi1;
-          }
-          if (first_ls < 0) first_ls = ls;
-          last_ls = ls;
-          ylo0 = yhi0 = ylo1 = yhi1 = 0.f;
-        };
-        for (uint32_t u = ua; u < ub; u += ups) {
-          const int n = (int)(ub - u) < ups ? (int)(ub - u) : ups;
-          const int stage = cw * spw + stage_i;
-          prog_mbar_wait(&full[stage], ph, kWFull, op);
-          if (u == ua) SP_STAMP(3);
-          const uint8_t* st = ring + (size_t)stage * kSpStageBytes;
-          auto apply = [&](const float (&t_lo)[2], const float (&t_hi)[2]) {
-            ylo0 += t_lo[0];
-            yhi0 += t_hi[0];
-            ylo1 += t_lo[1];
-            yhi1 += t_hi[1];
-            if (++j == NU) {
-              flush();
-              j = 0;
-              ++s_cur;
-            }
-          };
-          const int j0 = j;
-          if (F == 8) sb_chunk<8, GR, MT>(st, UB, n, xs, xsum, j0, NU, lane, M, apply);
-          else if (F == 4) sb_chunk<4, GR, MT>(st, UB, n, xs, xsum, j0, NU, lane, M, apply);
-          else sb_chunk<2, GR, MT>(st, UB, n, xs, xsum, j0, NU, lane, M, apply);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[stage]);
-          if (++stage_i == spw) { stage_i = 0; ph ^= 1; }
-        }
-        if (j != 0 && ua < ub) flush();
-        if (lane == 0) {
-          wfirst[cw] = first_ls;
-          wlast[cw] = last_ls;
-        }
-      }
-      SP_STAMP(4);
-      if (cw == 0) cp_async_wait_all();
-      named_bar_sync_gv(1, NW * 32);
-      SP_STAMP(5);
-
-      // ---- finish: per token, the warps' partial sums in a fixed order, publish (fp16 | tag) into the token's row
-      {
-        const int nsets = nu == 0 ? 0 : (int)((u1 - 1) / NU) - set0 + 1;
-        const uint32_t tagw = sp_tag(base, op) << 16;
-        uint32_t* out_rows = rows + (size_t)(op % kSpRows) * M * row_stride;
-        const int per_set = 8 * M;
-        for (int t = ct; t < nsets * per_set; t += NW * 32) {
-          const int ls = t / per_set, r = t - ls * per_set, m = r >> 3, gg = r & 7;
-          float lo = 0.f, hi = 0.f;
-#pragma unroll
-          for (int w = 0; w < NW; ++w) {
-            if (wfirst[w] >= 0 && wfirst[w] <= ls && ls <= wlast[w]) {
-              const float* p = part + (((size_t)ls * NW + w) * MT + m) * 16;
-              lo += p[gg];
-              hi += p[gg + 8];
-            }
-          }
-          int clo, chi;
-          sp_cols(mode, N, set0 + ls, gg, clo, chi);
-          if (bias != nullptr) {
-            lo += __half2float(bias[clo]);
-            hi += __half2float(bias[chi]);
-          }
-          const __half hlo = __float2half_rn(lo), hhi = __float2half_rn(hi);
-          uint32_t* out_row = out_rows + (size_t)m * row_stride;
-          if (mode == 0) {
-            st_relaxed_u32(out_row + clo, tagw | __half_as_ushort(hlo));
-            st_relaxed_u32(out_row + chi, tagw | __half_as_ushort(hhi));
-          } else {
-            const float gf = __half2float(hlo), uf = __half2float(hhi);
-            const __half a = __float2half_rn(gf / (1.f + __expf(-gf)) * uf);
-            st_relaxed_u32(out_row + clo, tagw | __half_as_ushort(a));
-            if (act_out != nullptr) act_out[(size_t)m * (N >> 1) + clo] = a;
-          }
-          y[(size_t)m * N + clo] = hlo;
-          y[(size_t)m * N + chi] = hhi;
-        }
-      }
-      SP_STAMP(6);
-    }
-  }
-
-  __syncthreads();
-  if (tid == 0) {
-    __threadfence();
-    if (atomicAdd(&state[1], 1) == nblk - 1) {
-      state[1] = 0;
-      state[0] = (base + n_ops) % 65535;
-    }
-  }
+// batched programs with residual adds (SpRes, program_stream.cuh): the same body plus the residual steps of the finish
+template <int MT>
+__global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
+    stream_batch_residual_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                                 uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int M, int spw,
+                                 int lmax, int nu_max, int dbg, const SpRes* __restrict__ res) {
+  // a cooperative launch never carries the PDL attribute (then this is a no-op); the tag state the body reads first is
+  // written by the previous run of this program
+  pdl_wait();
+#define SP_RESIDUAL 1
+#include "program_batch_body.inc"
+#undef SP_RESIDUAL
 }
 
 }  // namespace b200awq

@@ -108,6 +108,41 @@ __device__ __forceinline__ int ld_acquire_cta_smem(const int* p) {
 }
 __device__ __forceinline__ uint32_t sp_tag(int base, int op) { return (uint32_t)((base + op) % 65535 + 1); }
 
+// Residual add folded into an op's finish (B200AWQ_OP_ADD; stream_residual_kernel / stream_batch_residual_kernel): one
+// entry per kernel op in a side table (SpOp has no room left).  out == null: the op has no residual.  Otherwise the op
+// publishes fp16(fp16(sum [+ bias]) + residual) into its hand-off row and stores it to `out`, and still stores the raw
+// fp16(sum [+ bias]) to its y.  The residual of column c, token row m is ext[m N + c] (a buffer no op of the program
+// writes: ready at launch) when op < 0, else the tagged word of op `op`'s published row (kSpResWindow ops back at most).
+constexpr int kSpResWindow = 4;                   // largest producer - residual distance in kernel ops (program_create;
+                                                  // tests/test_stream_residual_model.py derives it)
+struct SpRes {
+  const __half* ext;
+  __half* out;
+  int op;
+  int pad_;
+};
+__device__ __forceinline__ uint32_t ld_relaxed_u32(const void* p) {
+  uint32_t r;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");
+  return r;
+}
+// the residual of column c (token row m of M) for op `op`: external, or polled from the source op's tagged row
+__device__ __forceinline__ float sp_residual(const SpRes& r, const uint32_t* rows, int row_stride, int M, int m, int N,
+                                             int c, int base, int op) {
+  if (r.op < 0) return __half2float(r.ext[(size_t)m * N + c]);
+  const uint32_t* p = rows + ((size_t)(r.op % kSpRows) * M + m) * row_stride + c;
+  const uint32_t want = sp_tag(base, r.op);
+  uint32_t v = ld_relaxed_u32(p);
+  if ((v >> 16) != want) {
+    ProgWatch wd;
+    do {
+      if (wd.tick(kWResidual, op)) break;
+      v = ld_relaxed_u32(p);
+    } while ((v >> 16) != want);
+  }
+  return __half2float(__ushort_as_half((unsigned short)(v & 0xffffu)));
+}
+
 // set -> original columns (oracle/stream_format.py:set_columns)
 __device__ __forceinline__ void sp_cols(int mode, int N, int s, int g, int& lo, int& hi) {
   if (mode == 0) {
@@ -349,6 +384,20 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
   pdl_wait();   // nothing is read before the predecessor is done, should it ever be launched with PDL (a no-op under
                 // the cooperative launch of program_run)
 #include "program_stream_body.inc"
+}
+
+// M = 1 programs with residual adds (SpRes above), with or without sparse-MoE blocks: the MoE instantiation plus the
+// residual steps of the finish, which only SP_RESIDUAL compiles in (the kernels above do not see them at all)
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_residual_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                           uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
+                           int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res) {
+  constexpr int NW = 8, SPW = 4, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#include "program_stream_body.inc"
+#undef SP_RESIDUAL
 }
 
 }  // namespace b200awq

@@ -23,6 +23,11 @@ bit-identical to an M = 1 program on that token's row.  Without it, M > 1 replay
 `sparse_moe(x, gate_weight, w1, w2, top_k)` records a whole Mixtral sparse-MoE block (FusedSparseMoeBlock.forward);
 at M = 1 the stream kernel runs it as two kernel ops with the routing computed inside (DESIGN.md 3.5d), otherwise
 `run()` replays apply_moe_weights' sequence through ext.  `moe_buffers(i)` returns the block's routing and intermediates.
+
+`add(a, b)` records the decoder block's residual add (`h = hidden_states + attn_output`, awq/modules/fused/block.py:
+50-52,117-118).  It adds no kernel op: it folds into the epilogue of the linear (or sparse_moe) recorded just before it,
+so a layer splits only at attention - [o + h_in -> h, norm2(h), gate|up, silu, down + h -> out, norm1'(out), qkv'] is one
+program (DESIGN.md 3.5e).  Outside the folding rule `run()` replays per op, with `torch.add` for the adds.
 """
 from __future__ import annotations
 
@@ -99,6 +104,28 @@ class DecodeProgram:
         self._keep += [x, x2, qweight, scales, qzeros, y] + ([bias] if bias is not None else [])
         self._max_n = max(self._max_n, N)
         return y.reshape(x.shape[:-1] + (N,))
+
+    def add(self, a, b, out=None):
+        """out = a + b (fp16, torch's rounding).  `out` is allocated like gemm_forward_cuda's y when not given and
+        returned.  Fused when one operand is the whole output of the linear / sparse_moe recorded just before and the
+        other is a buffer nothing in the program writes, or the output of an op at most four kernel ops back (DESIGN.md
+        3.5e states the rule for the rows such a residual is read from)."""
+        self._no_more()
+        self._dev_of(a)
+        for t in (a, b) + ((out,) if out is not None else ()):
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+            if t.dtype != torch.float16 or not t.is_contiguous():
+                raise B200AwqError("b200awq: add expects contiguous float16 tensors")
+        if a.shape != b.shape or (out is not None and out.shape != a.shape):
+            raise B200AwqError(f"b200awq: add expects equal shapes, got {tuple(a.shape)} and {tuple(b.shape)}")
+        K = a.shape[-1]
+        M = a.numel() // K
+        if out is None:
+            out = torch.empty((M, K), dtype=torch.float16, device=a.device).reshape(a.shape)
+        self._ops.append(("add", dict(a=a, b=b, out=out, M=M, K=K)))
+        self._keep += [a, b, out]
+        return out
 
     @staticmethod
     def _stacked(w, name):
@@ -203,6 +230,9 @@ class DecodeProgram:
             elif kind == "silu":
                 c.kind, c.M, c.K = _cabi.OP_SILU_AND_MUL, o["rows"], o["d"]
                 c.x, c.y = o["gate_up"].data_ptr(), o["out"].data_ptr()
+            elif kind == "add":
+                c.kind, c.M, c.K = _cabi.OP_ADD, o["M"], o["K"]
+                c.x, c.weight, c.y = o["a"].data_ptr(), o["b"].data_ptr(), o["out"].data_ptr()
             elif kind == "moe":
                 c.kind, c.M, c.K, c.N = _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
@@ -298,17 +328,19 @@ class DecodeProgram:
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
-            return o["M"] if kind in ("linear", "moe") else o["rows"]
+            return o["M"] if kind in ("linear", "moe", "add") else o["rows"]
         return 0
 
     @property
     def kernel_ops(self) -> int:
-        """Ops of the fused kernel: one per linear, two per sparse_moe (gate|up with the routing, down); 0 per-op."""
+        """Ops of the fused kernel: one per linear, two per sparse_moe (gate|up with the routing, down), none per add
+        (it folds into its producer's epilogue); 0 per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
     def launches_per_run(self) -> int:
-        """Kernels of this library launched by one run() (a per-op sparse_moe issues 6)."""
+        """Kernels launched by one run(): 1 when fused (adds included); per op, one per recorded call, 6 per
+        sparse_moe, and one torch.add launch per add."""
         return 1 if self.fused else sum(6 if kind == "moe" else 1 for kind, _ in self._ops)
 
     def run(self) -> None:
@@ -329,6 +361,8 @@ class DecodeProgram:
                 ext.silu_and_mul(o["out"], o["gate_up"])
             elif kind == "moe":
                 self._moe_replay(o)
+            elif kind == "add":
+                torch.add(o["a"], o["b"], out=o["out"])
             else:
                 ext.linear_forward("gemm", o["x"], o["qweight"], o["scales"], o["qzeros"], o["G"], o["bias"], out=o["y"])
 

@@ -221,8 +221,26 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     32 (set, slot) partial rows of the down op per CTA, and the activations of the longest K (top_k I for down) in
  *     shared memory next to the 8-warp x 4-stage weight ring (b200awq_moe_plan below says which).
  *     Memory: the program keeps a stream-format copy of every expert of both stacked tensors (about the size of the
- *     packed checkpoint again: ~24 GB for Mixtral-8x7B's 32 layers). */
-enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4 };
+ *     packed checkpoint again: ~24 GB for Mixtral-8x7B's 32 layers).
+ *
+ *   ADD           : the decoder block's residual add (awq/modules/fused/block.py:50-52,117-118): y[M, K] = x + weight,
+ *                   elementwise fp16 with torch's rounding, fp16(float(x) + float(weight)); x, weight, y = M contiguous
+ *                   rows of K (null: B200AWQ_EINVAL; K % 8 != 0 or a pointer not 16-byte aligned: B200AWQ_EUNSUPPORTED).
+ *     Folding: an ADD adds no kernel op.  It folds into the epilogue of the kernel op that produced one operand, which
+ *     must be the op recorded immediately before it (a linear, or the down op of a SPARSE_MOE) and whose whole output
+ *     (all M rows x N, N = K) that operand is.  The other operand, the residual, is either a buffer no op of the program
+ *     writes, or the output of an older op j of the program at most 4 kernel ops back (its published row).  Ops j + 4,
+ *     j + 8, ... publish into that row again; for the first of them after the producer i, k, some op in (i, k] must
+ *     stage the whole published row of an op >= i that has at least 16 columns per SM, so that no CTA can overwrite a
+ *     residual word before every CTA has read it (tests/test_stream_residual_model.py; b200awq_program_plan below).  The producer's
+ *     hand-off row then carries the sum: later ops that read the ADD's output read the sum, and a later op that reads
+ *     the producer's raw output is rejected.  Both the producer's y and the ADD's y are stored.  Everything else is
+ *     B200AWQ_EUNSUPPORTED and the caller replays per op: an ADD after a glue op or another ADD, after a gate|up whose
+ *     output only SiLU*mul reads, with both operands external, in place, with a residual out of the window or one the
+ *     program overwrites.  Only the stream kernels run it (M = 1: 8 consumer warps x 4 stages, knob 9 ignored; M > 1: the
+ *     batched kernel); the split-K kernel does not, so knob 14 = 1 gives B200AWQ_EUNSUPPORTED. */
+enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
+       B200AWQ_OP_ADD = 5 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -275,6 +293,13 @@ int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_coun
 typedef struct b200awq_program* b200awq_program_t;
 
 int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t* out);
+/* Host-side plan (no GPU, no CUDA call): the folding rules of b200awq_program_create_batched alone, for a device with
+ * `sm_count` SMs and an in-program residual window of `residual_window` kernel ops (<= 0: the library's, 4).  B200AWQ_OK
+ * with *kernel_ops = the fused kernel ops when the sequence folds (create may still replay per op: the stream kernels'
+ * shape and shared-memory envelope are checked at creation), B200AWQ_EUNSUPPORTED / B200AWQ_EINVAL as create returns
+ * them for the folding. */
+int b200awq_program_plan(const b200awq_op_t* ops, int n_ops, int max_tokens, int sm_count, int residual_window,
+                         int* kernel_ops);
 /* Batched decode programs: the same op list recorded with M token rows per op (a fused block built for batch size M:
  * RMSNorm / SiLU*mul over M contiguous rows, linears with M rows at pitch ldx), 1 <= max_tokens <= 8 (else
  * B200AWQ_EINVAL).  Every op must have the same M <= max_tokens, else B200AWQ_EUNSUPPORTED.  M = 1 behaves exactly like
