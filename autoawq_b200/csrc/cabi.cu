@@ -248,7 +248,7 @@ int b200awq_program_tokens(b200awq_program_t prog) {
 }
 
 int b200awq_program_kind(b200awq_program_t prog) {
-  return prog == nullptr ? 0 : (program_is_stream(reinterpret_cast<Program*>(prog)) ? 2 : 1);
+  return prog == nullptr ? 0 : 2;
 }
 
 size_t b200awq_stream_bytes(int K, int N, int group_size) {
@@ -266,13 +266,10 @@ int b200awq_stream_pack(const int32_t* qweight, const void* scales, const int32_
 
 int b200awq_program_run(b200awq_program_t prog, void* workspace, size_t workspace_bytes, b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_program_run");
+  (void)workspace;   // the program owns its hand-off rows
+  (void)workspace_bytes;
   if (prog == nullptr) return B200AWQ_EINVAL;
-  Program* p = reinterpret_cast<Program*>(prog);
-  if (program_is_stream(p)) return fold(program_run(p, nullptr, static_cast<cudaStream_t>(stream)));   // owns its rows
-  Ws ws;
-  // four rows of 64-bit packed sums (= 8 floats per column), max-N columns rounded up to 8, rotate through the ops
-  if (!carve(workspace, workspace_bytes, 8, (program_max_n(p) + 7) & ~7, &ws)) return B200AWQ_EWORKSPACE;
-  return fold(program_run(p, ws.acc, static_cast<cudaStream_t>(stream)));
+  return fold(program_run(reinterpret_cast<Program*>(prog), static_cast<cudaStream_t>(stream)));
 }
 
 int b200awq_program_destroy(b200awq_program_t prog) {

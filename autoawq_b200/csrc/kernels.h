@@ -89,12 +89,10 @@ struct ProgramPlan {
 };
 int program_create(const struct ::b200awq_op* ops, int n, int max_tokens, Program** out, cudaError_t* cuda_err,
                    ProgramPlan* plan = nullptr);
-int program_max_n(const Program* p);
 int program_m(const Program* p);
 int program_num_ops(const Program* p);
 int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8);   // host only (b200awq_moe_plan)
-cudaError_t program_run(Program* p, float* acc_ws, cudaStream_t st);
-int program_is_stream(const Program* p);
+cudaError_t program_run(Program* p, cudaStream_t st);
 size_t program_stream_bytes(const Program* p);
 // stream format (program_stream.cuh; oracle/stream_format.py): one-time re-layout of a GEMM-layout linear
 size_t stream_format_bytes(int K, int N, int G);

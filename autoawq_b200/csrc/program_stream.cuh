@@ -1,4 +1,4 @@
-// Decode program, stream variant: the persistent kernel of program.cu re-built around a ONE-TIME RE-LAYOUT of the
+// Decode program kernel (program.cu is its host side): a persistent kernel built around a ONE-TIME RE-LAYOUT of the
 // packed weights (the "stream format", restated in numpy in oracle/stream_format.py; the reference's precedent for
 // a post-load re-layout is awq/modules/linear/exllama.py:66-79) so that the grid-wide hand-off between two
 // dependent linears shrinks to "store, poll".

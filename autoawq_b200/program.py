@@ -48,9 +48,8 @@ class DecodeProgram:
         self._keep: list = []         # every tensor named by an op stays alive with the program
         self._handle = None
         self._built = False
-        self._max_n = 0
         self._dev = None
-        self.calibration = None       # {"stream_ms", "splitk_ms"} when build() timed both kernels
+        self.calibration = None       # kept for callers that record it: there is one kernel, nothing is calibrated
 
     # ------------------------------------------------------------------ recording (awq_ext call names)
     def _dev_of(self, t: torch.Tensor):
@@ -102,7 +101,6 @@ class DecodeProgram:
         self._ops.append(("linear", dict(x=x2, qweight=qweight, scales=scales, qzeros=qzeros, bias=bias, y=y, M=M, K=K,
                                          N=N, G=G, ldx=x2.stride(0) if M > 1 else K)))
         self._keep += [x, x2, qweight, scales, qzeros, y] + ([bias] if bias is not None else [])
-        self._max_n = max(self._max_n, N)
         return y.reshape(x.shape[:-1] + (N,))
 
     def add(self, a, b, out=None):
@@ -244,69 +242,24 @@ class DecodeProgram:
                 c.y = o["y"].data_ptr()
         return arr
 
-    def _create(self, arr, kind_knob: int):
-        """b200awq_program_create (b200awq_program_create_batched when max_tokens > 1) under knob 14 = kind_knob;
-        returns a handle or None (sequence outside that kernel)."""
-        prev = lib.b200awq_get_knob(14)
-        lib.b200awq_set_knob(14, kind_knob)
-        try:
-            handle = ctypes.c_void_p()
-            with ext._DeviceGuard(self._dev):
-                if self.max_tokens > 1:
-                    code = lib.b200awq_program_create_batched(arr, len(self._ops), self.max_tokens, ctypes.byref(handle))
-                else:
-                    code = lib.b200awq_program_create(arr, len(self._ops), ctypes.byref(handle))
-        finally:
-            lib.b200awq_set_knob(14, prev)
-        if code == _cabi.EUNSUPPORTED:
-            return None
-        check(code, "b200awq_program_create")
-        return handle
-
-    def _time(self, handle, runs: int = 5) -> float:
-        """Median device time (ms) of one run of `handle` on the current stream (load-time calibration)."""
-        dev = self._dev
-        with ext._DeviceGuard(dev):
-            st = ext._stream(dev)
-            ws = ext._workspace(dev, st, lib.b200awq_workspace_bytes(8, 0, (self._max_n + 7) & ~7))
-            ts = []
-            for i in range(runs + 2):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                check(lib.b200awq_program_run(handle, ws.data_ptr(), ws.numel(), st), "b200awq_program_run")
-                e1.record()
-                e1.synchronize()
-                if i >= 2:
-                    ts.append(e0.elapsed_time(e1))
-        ts.sort()
-        return ts[len(ts) // 2]
-
-    def build(self, calibrate: bool = True) -> "DecodeProgram":
-        """Fold the recorded calls into a fused program.  Two kernels can run it: the stream variant (one-time
-        re-layout of the weights, output-stationary, csrc/program_stream.cuh) and the split-K kernel on the checkpoint
-        layout (csrc/program.cu).  With `calibrate` (default) and knob 14 = 0, both are created when the sequence fits
-        both, each is timed on the device (a load-time step, like the re-layout itself; the recorded buffers are
-        overwritten by those runs exactly as `run()` would), and the faster one is kept - `calibration` holds the two
-        times.  Knob 14 = 1 / 2 forces the split-K / stream kernel.  A sequence with M > 1 rows per op (max_tokens >= M)
-        has only the batched stream kernel: nothing to calibrate."""
+    def build(self) -> "DecodeProgram":
+        """Fold the recorded calls into a fused program: one-time re-layout of the weights into the stream format and
+        the output-stationary kernel (csrc/program_stream.cuh; csrc/program_batch.cuh for M > 1 rows per op,
+        max_tokens >= M).  A sequence outside the kernel's envelope, or any sequence under knob 14 = 1, keeps the op
+        list: `run()` then replays it per op."""
         self._no_more()
         if not self._ops:
             raise B200AwqError("b200awq: empty program")
         arr = self._c_ops()
-        self.calibration = None
-        forced = lib.b200awq_get_knob(14)
-        if forced in (1, 2) or not calibrate:
-            self._handle = self._create(arr, forced)
-        else:
-            hs, hk = self._create(arr, 2), self._create(arr, 1)
-            if hs is not None and hk is not None:
-                ts, tk = self._time(hs), self._time(hk)
-                self.calibration = {"stream_ms": round(ts, 4), "splitk_ms": round(tk, 4)}
-                keep, drop = (hs, hk) if ts <= tk else (hk, hs)
-                lib.b200awq_program_destroy(drop)
-                self._handle = keep
+        handle = ctypes.c_void_p()
+        with ext._DeviceGuard(self._dev):
+            if self.max_tokens > 1:
+                code = lib.b200awq_program_create_batched(arr, len(self._ops), self.max_tokens, ctypes.byref(handle))
             else:
-                self._handle = hs if hs is not None else hk      # None: per-op replay (still the CUDA path)
+                code = lib.b200awq_program_create(arr, len(self._ops), ctypes.byref(handle))
+        if code != _cabi.EUNSUPPORTED:
+            check(code, "b200awq_program_create")
+            self._handle = handle         # otherwise None: per-op replay (still the CUDA path)
         self._built = True
         return self
 
@@ -316,11 +269,8 @@ class DecodeProgram:
 
     @property
     def kind(self) -> str:
-        """"stream" (re-laid-out weights, output-stationary kernel), "splitk" (round-1 kernel on the checkpoint
-        layout) or "per-op"."""
-        if self._handle is None:
-            return "per-op"
-        return "stream" if lib.b200awq_program_kind(self._handle) == 2 else "splitk"
+        """"stream" (re-laid-out weights, output-stationary kernel) or "per-op"."""
+        return "per-op" if self._handle is None else "stream"
 
     @property
     def tokens(self) -> int:
@@ -349,9 +299,7 @@ class DecodeProgram:
         dev = self._dev
         if self._handle is not None:
             with ext._DeviceGuard(dev):
-                st = ext._stream(dev)
-                ws = ext._workspace(dev, st, lib.b200awq_workspace_bytes(8, 0, (self._max_n + 7) & ~7))
-                code = lib.b200awq_program_run(self._handle, ws.data_ptr(), ws.numel(), st)
+                code = lib.b200awq_program_run(self._handle, None, 0, ext._stream(dev))
             check(code, "b200awq_program_run")
             return
         for kind, o in self._ops:

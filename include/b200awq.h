@@ -133,12 +133,11 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *          tokens on, measured on H100)
  *   key 3: 1 = the persistent GEMV records per-CTA phase timestamps (read with b200awq_debug_read);
  *          2 = the decode-program kernel records per-op phase timestamps of its first 8 CTAs / 32 ops
- *          (b200awq_debug_read then returns [op][cta][8] uint64 ns: op begin, previous op complete, activations
- *          staged, first tile landed, warp 0 done, all warps done, partial sums pushed, next op's loads released);
+ *          (b200awq_debug_read then returns [op][cta][8] uint64 ns: op begin, source row complete, activations
+ *          staged, first chunk landed, warp 0 done, all warps done, outputs published, routing published);
  *          3 = b200awq_debug_read returns the decode-program kernel's abort record instead: int32 [0..3] = {code, op,
  *          CTA, aborted} of the first wait that exceeded 0.5 s (every spin loop of that kernel gives up rather than
  *          hang the GPU), then per CTA 10 ints = (code << 16 | op) of the wait each warp abandoned;
- *          4 = the decode-program kernel does not recycle its accumulator rows (inspection of the rows after a run)
  *          9 = the small-M tensor-core kernel (9 <= M <= 128, GEMM layout) records per-CTA phase timestamps
  *          (b200awq_debug_read returns [cta][8] uint64 ns: entry, setup done, first packed stage landed, producers
  *          done, MMA issuer done, last accumulator drained, epilogue done, number of segments)
@@ -150,17 +149,12 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *          tail of each kernel); default 0
  *   key 7: 1 = stage the activations in shared memory in the persistent GEMV (M <= 2); default 0
  *   key 8: persistent GEMV L2-prefetch distance + 1 in tiles (0 / 1 = off, the default)
- *   key 9: persistent GEMV ring stages per consumer warp for M = 1 (1 / 2; 0 = default 3); the decode-program
- *          kernel uses 1 stage per warp when this is 1 (default 2); the stream decode program runs 12 consumer warps
- *          when this is 12 (default 8; any other value, 16 included, means 8: a 16-warp CTA spills on sm_90)
- *   key 10: decode program: 2 = do NOT hold the next op's weight loads back until the CTA has pushed its sums of
- *           the previous op (default: hold them back; no measurable difference on H100); the stream decode program
- *           reads it as its gate: 0 = ungated (the default: 1.93 vs 1.98 ms per Llama-3-8B step with 2 = gated one op
- *           ahead, H100 at 400 W), n > 0 = loads at most n - 1 ops ahead of the staging
- *   key 11: decode program: 2 = no back-off in the duty warp's polls (default: 400 ns sleep between attempts)
+ *   key 9: persistent GEMV ring stages per consumer warp for M = 1 (1 / 2; 0 = default 3); the M = 1 decode program
+ *          runs 12 consumer warps when this is 12 (default 8; any other value, 16 included, means 8: a 16-warp CTA
+ *          spills on sm_90)
+ *   key 10: decode program gate: 0 = ungated (the default: 1.93 vs 1.98 ms per Llama-3-8B step with 2 = gated one op
+ *           ahead, H100 at 400 W), n > 0 = weight loads at most n - 1 ops ahead of the staging
  *   key 12: 2 = grouped_gemm_forward always uses the register-staged grouped kernel
- *   key 13: decode program (read at b200awq_program_create): minimum tiles per participating CTA; ops with fewer
- *           tiles per CTA are shared by fewer CTAs (0 = every CTA takes part in every op, the default)
  *   key 18: 1 = the persistent GEMV uses round 1's split-K epilogue (fp32 REDs, tickets, read-back) also at M = 1,
  *           instead of the packed one (one returning 64-bit atomic per element; bit-reproducible)
  *   key 17: 1 = b200awq_comm_all_reduce uses the flag protocol (push, fence, flag, wait, reduce) instead of the default
@@ -176,8 +170,9 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *   key 21: small-M kernel work cut: 0 = tile-aligned ranges when N / 128 <= SM count (or from 64 tokens on), balanced
  *           (n-tile, k-step pair) ranges otherwise; 1 = always balanced; 2 = tile-aligned whenever possible
  *   key 22: small-M kernel: HBM -> L2 prefetch distance in k-step pairs ahead of the shared-memory ring (0 = off, default)
- *   key 14: decode program kind (read at b200awq_program_create): 0 = stream variant when the sequence fits it,
- *           else the split-K kernel; 1 = split-K kernel only; 2 = stream variant only
+ *   key 14: decode programs (read at b200awq_program_create): 1 = do not fuse: create returns B200AWQ_EUNSUPPORTED for
+ *           any sequence that folds (folding errors are still reported as such) and the caller replays per op, the
+ *           reference the fused kernels are held to; any other value = fuse when the sequence fits the kernels
  */
 int b200awq_set_knob(int key, int value);
 int b200awq_get_knob(int key);
@@ -198,9 +193,9 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *   SILU_AND_MUL  : x = gate|up [2K], y = output [K]                             (K = d)
  *   LINEAR_GEMM   : as b200awq_gemm_forward (GEMM layout)
  * b200awq_program_create returns B200AWQ_EUNSUPPORTED when the sequence does not fit the fused kernel (M != 1,
- * a shape outside the persistent GEMV's envelope, a glue op whose output no later linear reads, aliasing the
- * kernel's ordering cannot honour); the caller then issues the ops one by one.  Pointers are captured, not
- * copied: the tensors must stay alive and in place for the life of the program.  Create / destroy allocate and
+ * a shape outside the stream format's or the kernel's envelope, a glue op whose output no later linear reads,
+ * aliasing the kernel's ordering cannot honour); the caller then issues the ops one by one.  Pointers are captured,
+ * not copied: the tensors must stay alive and in place for the life of the program.  Create / destroy allocate and
  * copy (not capturable); run only enqueues a memset + one kernel on `stream` (capturable).  A program is not
  * re-entrant: one run in flight at a time.
  *
@@ -216,10 +211,10 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     After a run every buffer of the descriptor holds what the per-op sequence (gate matmul, topk_softmax,
  *     renormalisation, moe_alig_block_size, grouped_gemm_forward, silu_and_mul, grouped_gemm_forward(mul_weights),
  *     sum) would leave there; routing tensors for M = 1.
- *     Envelope (else B200AWQ_EUNSUPPORTED, the caller replays per op): M = 1, the stream kernel (knob 14 != 1),
- *     E <= 64, top_k <= 8, the per-expert shapes in the stream format, at most 32 16-column sets of the gate|up op and
- *     32 (set, slot) partial rows of the down op per CTA, and the activations of the longest K (top_k I for down) in
- *     shared memory next to the 8-warp x 4-stage weight ring (b200awq_moe_plan below says which).
+ *     Envelope (else B200AWQ_EUNSUPPORTED, the caller replays per op): M = 1, knob 14 != 1, E <= 64, top_k <= 8, the
+ *     per-expert shapes in the stream format, at most 32 16-column sets of the gate|up op and 32 (set, slot) partial
+ *     rows of the down op per CTA, and the activations of the longest K (top_k I for down) in shared memory next to the
+ *     8-warp x 4-stage weight ring (b200awq_moe_plan below says which).
  *     Memory: the program keeps a stream-format copy of every expert of both stacked tensors (about the size of the
  *     packed checkpoint again: ~24 GB for Mixtral-8x7B's 32 layers).
  *
@@ -237,8 +232,7 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     the producer's raw output is rejected.  Both the producer's y and the ADD's y are stored.  Everything else is
  *     B200AWQ_EUNSUPPORTED and the caller replays per op: an ADD after a glue op or another ADD, after a gate|up whose
  *     output only SiLU*mul reads, with both operands external, in place, with a residual out of the window or one the
- *     program overwrites.  Only the stream kernels run it (M = 1: 8 consumer warps x 4 stages, knob 9 ignored; M > 1: the
- *     batched kernel); the split-K kernel does not, so knob 14 = 1 gives B200AWQ_EUNSUPPORTED. */
+ *     program overwrites.  M = 1 runs 8 consumer warps x 4 stages (knob 9 ignored); M > 1 the batched kernel. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5 };
 
@@ -303,25 +297,23 @@ int b200awq_program_plan(const b200awq_op_t* ops, int n_ops, int max_tokens, int
 /* Batched decode programs: the same op list recorded with M token rows per op (a fused block built for batch size M:
  * RMSNorm / SiLU*mul over M contiguous rows, linears with M rows at pitch ldx), 1 <= max_tokens <= 8 (else
  * B200AWQ_EINVAL).  Every op must have the same M <= max_tokens, else B200AWQ_EUNSUPPORTED.  M = 1 behaves exactly like
- * b200awq_program_create.  M > 1 is always the stream variant (kind 2; the split-K kernel is M = 1 only, so knob 14 = 1
- * returns B200AWQ_EUNSUPPORTED): one persistent kernel stages the M rows and uses M token columns of its MMAs, so
+ * b200awq_program_create.  One persistent kernel stages the M rows and uses M token columns of its MMAs, so
  * every token is bit-identical to an M = 1 stream program run on that row alone.  A linear that reads a previous op's
  * output must read it at that op's row pitch (ldx == N of the producer; a column offset is fine); an external source
  * needs 16-byte aligned rows and ldx % 8 == 0.  The activations of M rows of the longest K must fit shared memory
  * next to the weight ring: Llama-3-8B shapes (K up to 14336) fuse up to M = 4.  The program owns its hand-off rows
- * (4 x M rows of the widest output): the caller's workspace is the one of b200awq_program_run below. */
+ * (4 x M rows of the widest output). */
 int b200awq_program_create_batched(const b200awq_op_t* ops, int n_ops, int max_tokens, b200awq_program_t* out);
 /* token rows per run (M of the recorded ops); 0 for a null handle */
 int b200awq_program_tokens(b200awq_program_t prog);
-/* 0: null handle; 1: split-K kernel on the checkpoint layout (round 1); 2: stream variant - at creation every
- * linear of the program was re-laid-out once into the stream format (below), the kernel partitions the work
- * output-stationary and hands activations from op to op as tagged fp16 words (csrc/program_stream.cuh).  Creation
- * prefers 2 and falls back to 1 (shapes / aliasing outside its envelope; knob 14 = 1 forces 1, 2 forbids 1). */
+/* 0: null handle; 2: a program - at creation every linear of the program was re-laid-out once into the stream format
+ * (below), the kernel partitions the work output-stationary and hands activations from op to op as tagged fp16 words
+ * (csrc/program_stream.cuh).  1 (the split-K kernel on the checkpoint layout of earlier versions) is no longer
+ * returned. */
 int b200awq_program_kind(b200awq_program_t prog);
 /* number of fused kernel ops (= linear ops, two per SPARSE_MOE op) of the program; 0 for a null handle */
 int b200awq_program_num_ops(b200awq_program_t prog);
-/* workspace: b200awq_workspace_bytes(8, K, max N over the program's linears rounded up to 8): four rows of 64-bit
- * packed split-K sums; zero-initialised and left all-zero like the per-op workspace (the same buffer may serve both) */
+/* workspace / workspace_bytes: accepted and ignored (null is fine); the program owns its hand-off rows */
 int b200awq_program_run(b200awq_program_t prog, void* workspace, size_t workspace_bytes, b200awq_stream_t stream);
 int b200awq_program_destroy(b200awq_program_t prog);
 

@@ -107,13 +107,10 @@ def small_blocks():
     return [Block(2048, 4096, 3072, 128, seed=s) for s in (1, 2)]
 
 
-@pytest.fixture(params=["stream", "splitk"])
+@pytest.fixture(params=["stream"])
 def kind(request, api):
-    """Both program kernels: the stream variant (one-time re-layout, csrc/program_stream.cuh; the default) and the
-    split-K kernel on the checkpoint layout (csrc/program.cu; knob 14 = 1)."""
-    api.set_knob(14, 2 if request.param == "stream" else 1)
-    yield request.param
-    api.set_knob(14, 0)
+    """The kind a fused program reports: the stream kernel (one-time re-layout, csrc/program_stream.cuh)."""
+    return request.param
 
 
 def _h0(hidden, M, seed=0):
@@ -171,9 +168,9 @@ def test_program_replays_and_leaves_scratch_clean(api, small_blocks, kind):
 
 
 def test_program_is_bit_reproducible(api, kind):
-    """The split-K sums travel as integers (csrc/program.cu, packed hand-off): the result does not depend on the order
-    in which CTAs arrive, so two runs on the same input must agree bit for bit - at the Llama-3-8B shapes, where
-    every column block has ~10 contributors."""
+    """Every output is summed in a fixed order by the CTA that owns it (output-stationary, csrc/program_stream.cuh):
+    the result does not depend on the order in which CTAs arrive, so two runs on the same input must agree bit for
+    bit - at the Llama-3-8B shapes."""
     from autoawq_b200.program import DecodeProgram
 
     blocks = [Block(4096, 14336, 6144, 128, seed=21)]
@@ -266,8 +263,8 @@ def test_program_llama8b_layer_shapes(api, kind):
 
 def test_program_bias_group64_and_older_source(api, kind):
     """Paths the Llama chain does not touch: linears with a bias (added before the fp16 rounding, as the per-op path
-    does), group size 64, and a linear whose source is the output of an op OLDER than its predecessor (read back from
-    global memory after that op's duty-warp stores, `ext_dep`)."""
+    does), group size 64, and a linear whose source is the output of an op OLDER than its predecessor (read from that
+    op's published row, `ext_dep`)."""
     from autoawq_b200.program import DecodeProgram
 
     H, G = 2048, 64

@@ -56,7 +56,7 @@ def test_batched_program_matches_oracle(api, small_blocks, M):
 @gpu
 @pytest.mark.parametrize("M", [3, 8])
 def test_batched_tokens_bit_identical_to_single_token_programs(api, small_blocks, M):
-    """Token m of a batched run equals an M = 1 stream program (knob 14 = 2, 8 consumer warps) on row m alone."""
+    """Token m of a batched run equals an M = 1 stream program (8 consumer warps) on row m alone."""
     import torch
 
     from autoawq_b200.program import DecodeProgram
@@ -209,7 +209,7 @@ def test_batched_general_groups_and_column_slice(api):
 
 @gpu
 def test_batched_envelope(api, small_blocks):
-    """M > max_tokens, mixed M across ops and knob 14 = 1 (split-K only, M = 1) replay per op - still correct."""
+    """M > max_tokens, mixed M across ops and knob 14 = 1 (do not fuse) replay per op - still correct."""
     import torch
 
     from autoawq_b200.program import DecodeProgram

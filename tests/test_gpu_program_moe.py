@@ -147,7 +147,7 @@ def test_moe_program_matches_oracle_and_per_op(case, renormalize):
     bufs = prog.moe_buffers(0)
     _check_block(moe, xn, bufs, renormalize, f"fused {case}")
     fused = {n: t.clone() for n, t in bufs.items()}
-    # the per-op replay of the same recording (knob 14 = 1: the split-K kernel has no MoE support)
+    # the per-op replay of the same recording (knob 14 = 1: do not fuse)
     ref, xn_r, out_r = _build(moe, h, renormalize, kind_knob=1)
     assert not ref.fused and ref.kernel_ops == 0
     ref.run()

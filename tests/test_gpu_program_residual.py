@@ -133,7 +133,7 @@ def test_segment_fuses_and_matches_oracle_and_unfused_programs(G):
     fused = {k: t.clone() for k, t in bufs.items()}
     _, ref = _unfused_reference(b, attn, h_in)
     _assert_same(fused, ref, "fused vs unfused programs + torch.add")
-    # the per-op replay (knob 14 = 1: the split-K kernel has no residual support) issues torch.add: the same values
+    # the per-op replay (knob 14 = 1: do not fuse) issues torch.add: the same values
     rp, rbufs = _fused(b, attn, h_in, knob={14: 1})
     assert not rp.fused and rp.kernel_ops == 0
     rp.run()

@@ -8,7 +8,7 @@ import re
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "autoawq_b200", "csrc")
 # launched with <<<>>> or the cooperative attribute only (plain stream order), never with the PDL attribute
-EXEMPT = {"stream_pack_kernel", "oneshot_allreduce_kernel", "ll_allreduce_kernel", "program_kernel", "stream_program_kernel"}
+EXEMPT = {"stream_pack_kernel", "oneshot_allreduce_kernel", "ll_allreduce_kernel", "stream_program_kernel"}
 
 
 def _kernels(path):

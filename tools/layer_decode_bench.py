@@ -118,7 +118,7 @@ def main():
         p3.silu_and_mul(b["act"], b["gu"])
         b["down"] = p3.gemm_forward_cuda(b["act"], *w["down"], 8)
         for p in (p1, p2, p3):
-            p.build(calibrate=False)
+            p.build()
             assert p.fused, "(b): a program did not fuse"
         plan_b.append((p1, p2, p3))
 
@@ -140,7 +140,7 @@ def main():
     p0 = DecodeProgram()
     p0.layernorm_forward_cuda(Bc[0]["h"], norm1[0], Bc[0]["xn"], EPS)
     Bc[0]["qkv"] = p0.gemm_forward_cuda(Bc[0]["xn"], *rep.w[0]["qkv"], 8)
-    p0.build(calibrate=False)
+    p0.build()
     assert p0.fused, "(c): the first program did not fuse"
     plan_c = [p0]
     for l in range(L):
@@ -157,7 +157,7 @@ def main():
             nb = Bc[l + 1]
             p.layernorm_forward_cuda(nb["h"], norm1[l + 1], nb["xn"], EPS)
             nb["qkv"] = p.gemm_forward_cuda(nb["xn"], *rep.w[l + 1]["qkv"], 8)
-        p.build(calibrate=False)
+        p.build()
         assert p.fused and p.kernel_ops == (4 if l + 1 < L else 3), "(c): a segment did not fuse"
         plan_c.append(p)
 
