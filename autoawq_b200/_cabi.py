@@ -47,7 +47,18 @@ class Moe(ctypes.Structure):
     ]
 
 
-OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD = 1, 2, 3, 4, 5
+class Rope(ctypes.Structure):
+    """b200awq_rope_t (include/b200awq.h): the descriptor of b200awq_rope_kv and of a ROPE_KV op's `weight`."""
+
+    _fields_ = [
+        ("n_heads", ctypes.c_int32), ("n_kv_heads", ctypes.c_int32), ("head_dim", ctypes.c_int32),
+        ("cache_len", ctypes.c_int32), ("freqs_len", ctypes.c_int32), ("pad_", ctypes.c_int32),
+        ("cache_batch_stride", ctypes.c_int64), ("pos", ctypes.c_void_p), ("freqs", ctypes.c_void_p),
+        ("q_out", ctypes.c_void_p), ("k_cache", ctypes.c_void_p), ("v_cache", ctypes.c_void_p),
+    ]
+
+
+OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV = 1, 2, 3, 4, 5, 6
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -74,6 +85,7 @@ SIGNATURES = {
     ),
     "b200awq_rmsnorm": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_float, _c_void_p]),
     "b200awq_silu_and_mul": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_void_p]),
+    "b200awq_rope_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Rope), _c_int, _c_void_p]),
     "b200awq_set_knob": (_c_int, [_c_int, _c_int]),
     "b200awq_get_knob": (_c_int, [_c_int]),
     "b200awq_debug_read": (_c_int, [_c_void_p, _c_size_t]),
@@ -101,6 +113,8 @@ SIGNATURES = {
     "b200awq_program_kind": (_c_int, [_c_void_p]),
     "b200awq_stream_bytes": (_c_size_t, [_c_int, _c_int, _c_int]),
     "b200awq_stream_pack": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
+    "b200awq_stream_pack_rotary": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int,
+                                            _c_void_p]),
     "b200awq_program_run": (_c_int, [_c_void_p, _c_void_p, _c_size_t, _c_void_p]),
     "b200awq_program_destroy": (_c_int, [_c_void_p]),
 }

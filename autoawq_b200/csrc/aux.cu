@@ -1,9 +1,11 @@
 // Glue kernels the reference's fused modules call through awq_ext (SURVEY.md 8f #1, #2):
 //   rmsnorm       <- awq_ext.layernorm_forward_cuda   (awq/modules/fused/norm.py:33-36)
 //   silu_and_mul  <- awq_ext.silu_and_mul             (awq/modules/fused/moe.py:76)
+//   rope_kv       <- RoPE.forward + WindowedCache.update_kv (awq/modules/fused/attn.py:53-86,243-267)
 // fp16 in/out, fp32 math.  Bandwidth-trivial (KBs per decode step); kept simple.
 #include "common.cuh"
 #include "kernels.h"
+#include "rope.cuh"
 
 namespace b200awq {
 
@@ -63,6 +65,38 @@ __global__ void __launch_bounds__(256)
   const float g = __half2float(gu[(int64_t)r * 2 * d + j]);
   const float u = __half2float(gu[(int64_t)r * 2 * d + d + j]);
   out[i] = __float2half_rn(g / (1.f + __expf(-g)) * u);
+}
+
+// one thread per (token row, head, pair); rope.cuh has the arithmetic
+__global__ void __launch_bounds__(256)
+    rope_kv_kernel(const __half* __restrict__ qkv, int64_t ldqkv, b200awq_rope_t r, int M) {
+  pdl_trigger();
+  pdl_wait();
+  const int pos = rope_pos(r);
+  const int half = r.head_dim >> 1, heads = r.n_heads + 2 * r.n_kv_heads;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pos < 0 || i >= (int64_t)M * heads * half) return;
+  const int m = static_cast<int>(i / ((int64_t)heads * half));
+  const int p = static_cast<int>(i - (int64_t)m * heads * half), h = p / half, c = h * r.head_dim + (p - h * half);
+  const __half* row = qkv + m * ldqkv;
+  rope_pair(r, pos, m, c, row[c], row[c + half]);
+}
+
+int rope_validate(const b200awq_rope_t* r, int64_t ldqkv) {
+  if (r == nullptr || r->pos == nullptr || r->freqs == nullptr || r->q_out == nullptr || r->k_cache == nullptr ||
+      r->v_cache == nullptr)
+    return B200AWQ_EINVAL;
+  if (r->n_heads <= 0 || r->n_kv_heads <= 0 || r->head_dim <= 0 || (r->head_dim % 2) != 0 || r->cache_len <= 0 ||
+      r->freqs_len <= 0 || r->cache_batch_stride < (int64_t)r->cache_len * r->n_kv_heads * r->head_dim ||
+      ldqkv < (int64_t)(r->n_heads + 2 * r->n_kv_heads) * r->head_dim)
+    return B200AWQ_EINVAL;
+  return B200AWQ_OK;
+}
+
+cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t& r, int M, cudaStream_t st) {
+  const int64_t n = (int64_t)M * (r.n_heads + 2 * r.n_kv_heads) * (r.head_dim / 2);
+  return launch_kernel(rope_kv_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
+                       reinterpret_cast<const __half*>(qkv), ldqkv, r, M);
 }
 
 cudaError_t rmsnorm(const void* x, const void* w, void* out, int rows, int hidden, float eps, cudaStream_t st) {

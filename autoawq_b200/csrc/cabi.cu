@@ -205,6 +205,15 @@ int b200awq_silu_and_mul(const void* gate_up, void* out, int rows, int d, b200aw
   return fold(silu_and_mul(gate_up, out, rows, d, static_cast<cudaStream_t>(stream)));
 }
 
+int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_rope_kv");
+  if (qkv == nullptr || M < 0) return B200AWQ_EINVAL;
+  const int v = rope_validate(rope, ldqkv);
+  if (v != B200AWQ_OK) return v;
+  if (M == 0) return B200AWQ_OK;
+  return fold(rope_kv(qkv, ldqkv, *rope, M, static_cast<cudaStream_t>(stream)));
+}
+
 
 int b200awq_program_create_batched(const b200awq_op_t* ops, int n_ops, int max_tokens, b200awq_program_t* out) {
   if (out == nullptr) return B200AWQ_EINVAL;
@@ -262,6 +271,17 @@ int b200awq_stream_pack(const int32_t* qweight, const void* scales, const int32_
   if (!shape_ok(1, K, N, group_size)) return B200AWQ_EINVAL;
   if (!stream_format_supported(K, N, group_size, mode)) return B200AWQ_EUNSUPPORTED;
   return fold(stream_pack(qweight, scales, qzeros, out, K, N, group_size, mode, static_cast<cudaStream_t>(stream)));
+}
+
+int b200awq_stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K,
+                               int N, int group_size, int head_dim, b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_stream_pack_rotary");
+  if (!qweight || !scales || !qzeros || !out || head_dim <= 0) return B200AWQ_EINVAL;
+  if (!shape_ok(1, K, N, group_size)) return B200AWQ_EINVAL;
+  if (!stream_format_supported(K, N, group_size, 0) || (head_dim % 16) != 0 || (N % head_dim) != 0)
+    return B200AWQ_EUNSUPPORTED;
+  return fold(stream_pack_rotary(qweight, scales, qzeros, out, K, N, group_size, head_dim,
+                                 static_cast<cudaStream_t>(stream)));
 }
 
 int b200awq_program_run(b200awq_program_t prog, void* workspace, size_t workspace_bytes, b200awq_stream_t stream) {

@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 struct b200awq_op;
+struct b200awq_rope;
 
 namespace b200awq {
 
@@ -136,5 +137,10 @@ void comm_destroy(Comm* c);
 
 cudaError_t rmsnorm(const void* x, const void* w, void* out, int rows, int hidden, float eps, cudaStream_t st);
 cudaError_t silu_and_mul(const void* gate_up, void* out, int rows, int d, cudaStream_t st);
+// B200AWQ_OK, or the code b200awq_rope_kv returns for a bad descriptor / qkv pitch (host only)
+int rope_validate(const struct ::b200awq_rope* r, int64_t ldqkv);
+cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_rope& r, int M, cudaStream_t st);
+cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
+                               int G, int head_dim, cudaStream_t st);
 
 }  // namespace b200awq

@@ -25,6 +25,7 @@
 #include "common.cuh"
 #include "gemv_tile.cuh"
 #include "kernels.h"
+#include "rope.cuh"
 
 namespace b200awq {
 
@@ -153,6 +154,9 @@ struct Program {
   int n_moe = 0;
   // residual adds (stream_residual_kernel / stream_batch_residual_kernel): one SpRes per kernel op, null without adds
   SpRes* d_res = nullptr;
+  // ROPE_KV ops (stream_rope_kernel / stream_batch_rope_kernel): one SpRope per kernel op, null without them (d_res is
+  // then allocated too, empty where there is no add: the rope kernels are the residual kernels plus the rope steps)
+  SpRope* d_rope = nullptr;
 };
 
 // An ADD folded into table entry i (program_create): the entry's y is swapped for the ADD's output (what its row
@@ -209,6 +213,19 @@ bool stream_format_supported(int K, int N, int G, int mode) {
 }
 static int prog_sm_count();   // device SM count (defined below)
 
+cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
+                               int G, int head_dim, cudaStream_t st) {
+  if (!stream_format_supported(K, N, G, 0) || head_dim <= 0 || (head_dim % 16) != 0 || (N % head_dim) != 0)
+    return cudaErrorNotSupported;
+  const int UK = G < 128 ? G : 128;
+  const int64_t total = (int64_t)(N / 16) * (K / UK) * ((UK / 16) * 32 + 12);
+  const int cap = prog_sm_count() * 16;
+  const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
+  stream_pack_rotary_kernel<<<blocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros,
+                                                    static_cast<uint8_t*>(out), K, N, G, head_dim);
+  return cudaGetLastError();
+}
+
 cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N, int G,
                         int mode, cudaStream_t st) {
   if (!stream_format_supported(K, N, G, mode)) return cudaErrorNotSupported;
@@ -226,9 +243,10 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
 // failure.
 // Sparse-MoE blocks (`fold[i].kind` != 0, M = 1 only): the gate|up entry is a mode-1 op over top_k slots of 2I
 // columns, the down entry reads its published row (K' = top_k I); both stream E per-expert slices packed back to back.
+// ROPE_KV ops (`ropes[i].head_dim` != 0): entry i is packed in mode 2 and its finish rotates / appends (SpRope).
 static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
                          const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes,
-                         const std::vector<ResFold>& res) {
+                         const std::vector<ResFold>& res, const std::vector<b200awq_rope_t>& ropes) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
@@ -265,6 +283,13 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   };
   for (int i = 0; i < n; ++i)
     if (moe_kind(i) == 1) mode[i] = 1;
+  bool has_rope = false;
+  for (int i = 0; i < n && !ropes.empty(); ++i)
+    if (ropes[i].head_dim != 0) {
+      if (mode[i] != 0) return false;   // (program_create rejects a gate|up producer already)
+      mode[i] = 2;
+      has_rope = true;
+    }
   // residual adds: the producer and an in-program residual must publish plain columns (a mode-1 row holds SiLU*mul)
   bool has_res = false;
   for (int i = 0; i < n && !res.empty(); ++i)
@@ -281,7 +306,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       woff[i] = wbytes;
       wbytes += (size_t)moes[fold[i].mi].E * expert_bytes(i);
     } else {
-      if (!stream_format_supported(p.K, p.N, p.G, mode[i])) return false;
+      if (!stream_format_supported(p.K, p.N, p.G, mode[i] == 2 ? 0 : mode[i])) return false;
       const int UK = p.G < 128 ? p.G : 128;
       if (p.K / UK > kSpXsumMax) return false;
       if (M == 1 && (p.N / 16 + grid - 1) / grid > kSpLMax) return false;
@@ -290,10 +315,10 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       woff[i] = wbytes;
       wbytes += (stream_format_bytes(p.K, p.N, p.G) + 255) & ~(size_t)255;
     }
-    max_cols = std::max(max_cols, (size_t)(mode[i] ? p.N / 2 : p.N));
+    max_cols = std::max(max_cols, (size_t)(mode[i] == 1 ? p.N / 2 : p.N));
     max_K = std::max(max_K, p.K);
   }
-  if (M == 1 && (has_moe || has_res)) {
+  if (M == 1 && (has_moe || has_res || has_rope)) {
     // the MoE / residual kernel runs 8 consumer warps with 4 ring stages each, behind the routing area
     if (sp_fixed_smem(8, 4, true) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
   } else if (M == 1) {
@@ -398,8 +423,12 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
                         K, N, G, mode[i], nullptr);
       continue;
     }
-    e = stream_pack(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K, table[i].N,
-                    table[i].G, mode[i], nullptr);
+    if (mode[i] == 2)
+      e = stream_pack_rotary(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K,
+                             table[i].N, table[i].G, ropes[i].head_dim, nullptr);
+    else
+      e = stream_pack(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K, table[i].N,
+                      table[i].G, mode[i], nullptr);
   }
   if (e == cudaSuccess && has_moe) {
     std::vector<SpMoe> md(moes.size());
@@ -434,12 +463,12 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       e = cudaFuncSetAttribute(stream_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)(227 * 1024));
   }
-  if (e == cudaSuccess && has_res) {
+  if (e == cudaSuccess && (has_res || has_rope)) {
     std::vector<SpRes> rd(n);
     for (int i = 0; i < n; ++i) {
       std::memset(&rd[i], 0, sizeof(SpRes));
       rd[i].op = -1;
-      if (res[i].raw_y == nullptr) continue;
+      if (res.empty() || res[i].raw_y == nullptr) continue;
       rd[i].out = table[i].y;                       // the ADD's output (the entry's y was swapped for it)
       rd[i].op = res[i].op;
       rd[i].ext = static_cast<const __half*>(res[i].ext);
@@ -454,6 +483,20 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       e = cudaFuncSetAttribute(stream_batch_residual_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(stream_batch_residual_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  }
+  if (e == cudaSuccess && has_rope) {
+    std::vector<SpRope> rp(n);
+    for (int i = 0; i < n; ++i) rp[i].r = ropes[i];
+    e = cudaMalloc(&pr->d_rope, (size_t)n * sizeof(SpRope));
+    if (e == cudaSuccess) e = cudaMemcpy(pr->d_rope, rp.data(), (size_t)n * sizeof(SpRope), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_rope_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_rope_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_rope_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_rope_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   }
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_sp_ops, ops.data(), (size_t)n * sizeof(SpOp), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_cta, cta.data(), cta.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
@@ -477,7 +520,9 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     cudaFree(pr->d_state);
     cudaFree(pr->d_moe);
     cudaFree(pr->d_res);
+    cudaFree(pr->d_rope);
     pr->d_res = nullptr;
+    pr->d_rope = nullptr;
     pr->d_stream = nullptr;
     pr->d_sp_ops = nullptr;
     pr->d_cta = nullptr;
@@ -601,6 +646,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   int M = -1;
   std::vector<ResFold> res;     // per table entry: the ADD folded into it, if any
   std::vector<std::pair<const void*, size_t>> ext_res;   // external residuals: no op of the program may write them
+  std::vector<b200awq_rope_t> ropes;   // per table entry: the ROPE_KV folded into it (head_dim == 0: none)
+  std::vector<int> rope_ops;           // table entries that carry one
   for (int i = 0; i < n; ++i) {
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
@@ -612,6 +659,23 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         if (res[j].raw_y != nullptr && overlaps(res[j].raw_y, rows_bytes(table[j].N), p, bytes)) return true;
       return false;
     };
+    if (op.kind == B200AWQ_OP_ROPE_KV) {
+      // RoPE + cache append, folded into the finish of the linear recorded just before it (whose whole output is qkv)
+      const b200awq_rope_t* r = static_cast<const b200awq_rope_t*>(op.weight);
+      if (op.x == nullptr) return B200AWQ_EINVAL;
+      const int v = rope_validate(r, M > 1 ? op.ldx : INT64_MAX);   // (one row: no pitch; N is checked below)
+      if (v != B200AWQ_OK) return v;
+      const int D = r->head_dim;
+      if (op.N != (r->n_heads + 2 * r->n_kv_heads) * D || (D % 16) != 0) return B200AWQ_EUNSUPPORTED;
+      // (an ADD or a glue op in between: the op before is not a linear; a SPARSE_MOE's entries are not plain linears)
+      if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty() || fold.back().kind != 0)
+        return B200AWQ_EUNSUPPORTED;
+      const ProgOp& pv = table.back();
+      if (op.x != pv.y || op.N != pv.N || (M > 1 && op.ldx != op.N)) return B200AWQ_EUNSUPPORTED;
+      ropes.back() = *r;
+      rope_ops.push_back(static_cast<int>(table.size()) - 1);
+      continue;
+    }
     if (op.kind == B200AWQ_OP_ADD) {
       // y = x + weight, folded into the epilogue of the op recorded just before it (a linear / a MoE block's down)
       if (op.x == nullptr || op.weight == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
@@ -757,6 +821,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     table.push_back(p);
     fold.push_back(xfold[i]);
     res.emplace_back();
+    ropes.emplace_back();
+    std::memset(&ropes.back(), 0, sizeof(b200awq_rope_t));
   }
   for (const Glue& gl : glues)
     if (!gl.used) return B200AWQ_EUNSUPPORTED;   // a glue op nobody consumes would never run
@@ -781,6 +847,55 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
           overlaps(m.sorted_ids, (size_t)m.sorted_len * 4, er.first, er.second) ||
           overlaps(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4, er.first, er.second) ||
           overlaps(m.num_tokens_post_pad, 4, er.first, er.second))
+        return B200AWQ_EUNSUPPORTED;
+  }
+  // ROPE_KV: the rotated q and the appended cache rows are written in a finish, while other CTAs run later ops.  No
+  // other op of the program may read or write them, nor write the position / frequency table the finish reads; the
+  // producer must not be a gate|up whose product a SiLU*mul reads (its row would hold silu(gate) * up).
+  for (int ri : rope_ops) {
+    const b200awq_rope_t& r = ropes[ri];
+    const size_t cache = ((size_t)(M - 1) * r.cache_batch_stride + (size_t)r.cache_len * r.n_kv_heads * r.head_dim) * 2;
+    const std::pair<const void*, size_t> outs[3] = {{r.q_out, (size_t)M * r.n_heads * r.head_dim * 2},
+                                                    {r.k_cache, cache}, {r.v_cache, cache}};
+    const std::pair<const void*, size_t> ins[2] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * r.head_dim * 4}};
+    auto hits_out = [&](const void* p, size_t b) {
+      for (const auto& o : outs)
+        if (overlaps(o.first, o.second, p, b)) return true;
+      return false;
+    };
+    auto hits_any = [&](const void* p, size_t b) {
+      return hits_out(p, b) || overlaps(ins[0].first, ins[0].second, p, b) || overlaps(ins[1].first, ins[1].second, p, b);
+    };
+    if (overlaps(outs[0].first, outs[0].second, outs[1].first, outs[1].second) ||
+        overlaps(outs[0].first, outs[0].second, outs[2].first, outs[2].second) ||
+        overlaps(outs[1].first, outs[1].second, outs[2].first, outs[2].second))
+      return B200AWQ_EUNSUPPORTED;
+    for (int j = 0; j < nt; ++j) {
+      const size_t src_bytes = ((size_t)(M - 1) * table[j].src_ld + (size_t)(table[j].prologue == kProSilu ? 2 : 1) * table[j].K) * 2;
+      if (hits_any(table[j].y, (size_t)M * table[j].N * 2) ||
+          (res[j].raw_y != nullptr && hits_any(res[j].raw_y, (size_t)M * table[j].N * 2)) ||
+          (table[j].src != nullptr && hits_out(table[j].src, src_bytes)) ||
+          (res[j].ext != nullptr && hits_out(res[j].ext, (size_t)M * table[j].N * 2)))
+        return B200AWQ_EUNSUPPORTED;
+      if (table[j].prologue == kProSilu && overlaps(table[j].src, src_bytes, table[ri].y, (size_t)M * table[ri].N * 2))
+        return B200AWQ_EUNSUPPORTED;   // a SiLU*mul of the qkv output: the producer would be a mode-1 gate|up
+      if (j != ri && ropes[j].head_dim != 0) {   // another ROPE_KV: its outputs are writes, its inputs reads
+        const b200awq_rope_t& o = ropes[j];
+        const size_t oc = ((size_t)(M - 1) * o.cache_batch_stride + (size_t)o.cache_len * o.n_kv_heads * o.head_dim) * 2;
+        if (hits_any(o.q_out, (size_t)M * o.n_heads * o.head_dim * 2) || hits_any(o.k_cache, oc) || hits_any(o.v_cache, oc))
+          return B200AWQ_EUNSUPPORTED;
+      }
+    }
+    for (const Glue& gl : glues)
+      if (hits_any(gl.out, (size_t)M * gl.width * 2) || hits_out(gl.src, (size_t)M * (gl.kind == kProSilu ? 2 : 1) * gl.width * 2))
+        return B200AWQ_EUNSUPPORTED;
+    for (const b200awq_moe_t& m : moes)
+      if (hits_any(m.gate_up, (size_t)m.top_k * 2 * m.I * 2) || hits_any(m.act, (size_t)m.top_k * m.I * 2) ||
+          hits_any(m.down, (size_t)m.top_k * m.H * 2) || hits_any(m.logits, (size_t)m.E * 2) ||
+          hits_any(m.topk_weights, (size_t)m.top_k * M * 4) || hits_any(m.topk_ids, (size_t)m.top_k * M * 4) ||
+          hits_any(m.token_expert_indices, (size_t)m.top_k * M * 4) || hits_any(m.sorted_ids, (size_t)m.sorted_len * 4) ||
+          hits_any(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4) || hits_any(m.num_tokens_post_pad, 4) ||
+          hits_out(m.gate_weight, (size_t)m.E * m.H * 2))
         return B200AWQ_EUNSUPPORTED;
   }
   for (int i = 0; i < nt; ++i) {
@@ -813,7 +928,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   pr->n_ops = nt;
   pr->M = M;
   cudaError_t e = cudaGetDevice(&pr->device);
-  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res)) {
+  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -847,6 +962,14 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     cfg.numAttrs = 1;
     const SpOp* sops = p->d_sp_ops;
     const uint32_t* cta = p->d_cta;
+    if (p->d_rope != nullptr) {  // a ROPE_KV op: the residual kernel plus the rope steps of a mode-2 finish
+      auto qk = sb_mt(p->M) == 2 ? stream_batch_rope_kernel<2>
+                                 : (sb_mt(p->M) == 4 ? stream_batch_rope_kernel<4> : stream_batch_rope_kernel<8>);
+      const SpRes* rd = p->d_res;
+      const SpRope* qd = p->d_rope;
+      return cudaLaunchKernelEx(&cfg, qk, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
+                                p->sb_lmax, p->sb_nu_max, knob(3), rd, qd);
+    }
     if (p->d_res != nullptr) {   // residual adds: the same kernel with the residual steps in its finish
       auto rk = sb_mt(p->M) == 2 ? stream_batch_residual_kernel<2>
                                  : (sb_mt(p->M) == 4 ? stream_batch_residual_kernel<4> : stream_batch_residual_kernel<8>);
@@ -882,6 +1005,16 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
   // the default; n > 0: at most n - 1 ops ahead, 1 = strictly gated)
   const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
   const SpMoe* no_moe = nullptr;
+  if (p->d_rope != nullptr) {
+    // programs with a ROPE_KV op (with or without adds / sparse-MoE blocks): 8 consumer warps x 4 ring stages
+    cfg.blockDim = dim3(32 + 8 * 32);
+    cfg.dynamicSmemBytes = sp_fixed_smem(8, 4, true) + p->xs_bytes;
+    const SpMoe* md = p->d_moe;
+    const SpRes* rd = p->d_res;
+    const SpRope* qd = p->d_rope;
+    return cudaLaunchKernelEx(&cfg, stream_rope_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
+                              knob(3), l2_ahead, gate_ahead, md, rd, qd);
+  }
   if (p->d_res != nullptr) {
     // programs with residual adds (with or without sparse-MoE blocks): always 8 consumer warps x 4 ring stages
     cfg.blockDim = dim3(32 + 8 * 32);
@@ -915,6 +1048,7 @@ void program_destroy(Program* p) {
   cudaFree(p->d_state);
   cudaFree(p->d_moe);
   cudaFree(p->d_res);
+  cudaFree(p->d_rope);
   delete p;
 }
 

@@ -152,4 +152,20 @@ __global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
 #undef SP_RESIDUAL
 }
 
+// batched programs with a ROPE_KV op (SpRope, program_stream.cuh): the residual kernel plus RoPE + cache append in a
+// mode-2 finish (token row m writes cache batch m)
+template <int MT>
+__global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
+    stream_batch_rope_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                             uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int M, int spw,
+                             int lmax, int nu_max, int dbg, const SpRes* __restrict__ res,
+                             const SpRope* __restrict__ rope) {
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#include "program_batch_body.inc"
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
 }  // namespace b200awq

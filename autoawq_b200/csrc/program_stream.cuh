@@ -143,6 +143,13 @@ __device__ __forceinline__ float sp_residual(const SpRes& r, const uint32_t* row
   return __half2float(__ushort_as_half((unsigned short)(v & 0xffffu)));
 }
 
+// ROPE_KV folded into a qkv linear's finish (stream_rope_kernel / stream_batch_rope_kernel): one entry per kernel op in a
+// side table, like SpRes.  The op is packed in mode 2 (sp_cols_rot, head_dim = r.head_dim); r.head_dim == 0 on every
+// other op.  The descriptor is the recorded b200awq_rope_t (rope.cuh does the arithmetic).
+struct SpRope {
+  b200awq_rope_t r;
+};
+
 // set -> original columns (oracle/stream_format.py:set_columns)
 __device__ __forceinline__ void sp_cols(int mode, int N, int s, int g, int& lo, int& hi) {
   if (mode == 0) {
@@ -154,11 +161,21 @@ __device__ __forceinline__ void sp_cols(int mode, int N, int s, int g, int& lo, 
   }
 }
 
+// mode 2 (a qkv linear whose ROPE_KV folds into its finish): set s of head h = s / (D / 16) holds the RoPE pairs
+// lo = h D + 8 t + g, hi = lo + D / 2 (t = s % (D / 16)), so one lane finishes both columns of a rotation
+__device__ __forceinline__ void sp_cols_rot(int D, int s, int g, int& lo, int& hi) {
+  const int per_head = D >> 4, h = s / per_head, t = s - h * per_head;
+  lo = h * D + 8 * t + g;
+  hi = lo + (D >> 1);
+}
+
 // ------------------------------------------------------------------------------------------ re-layout kernel
-// One thread per output word / per group-constant slot; run once per linear at program creation.
-__global__ void __launch_bounds__(256)
-    stream_pack_kernel(const int32_t* __restrict__ qweight, const __half* __restrict__ scales,
-                       const int32_t* __restrict__ qzeros, uint8_t* __restrict__ out, int K, int N, int G, int mode) {
+// One thread per output word / per group-constant slot; run once per linear at program creation.  cols(s, g, lo, hi)
+// maps set s, lane group g to its two original columns.
+template <typename Cols>
+__device__ __forceinline__ void sp_pack(const int32_t* __restrict__ qweight, const __half* __restrict__ scales,
+                                        const int32_t* __restrict__ qzeros, uint8_t* __restrict__ out, int K, int N,
+                                        int G, Cols cols) {
   const int UK = G < 128 ? G : 128, F = UK >> 4, NU = K / UK, UB = F * 128 + kSpAux;
   const int NW = N >> 3;
   const int wpu = F * 32 + 12;   // 32-bit slots per unit: fragment words + 8 scale pairs + 2 zero words + 2 pad
@@ -185,7 +202,7 @@ __global__ void __launch_bounds__(256)
       }
       const int g = lane >> 2, tig = lane & 3;
       int lo, hi;
-      sp_cols(mode, N, s, g, lo, hi);
+      cols(s, g, lo, hi);
       const int k0 = j * UK + 16 * f + 2 * tig;
       const uint32_t w = nib(k0, lo) | nib(k0, hi) << 4 | nib(k0 + 8, lo) << 8 | nib(k0 + 8, hi) << 12 |
                          nib(k0 + 1, lo) << 16 | nib(k0 + 1, hi) << 20 | nib(k0 + 9, lo) << 24 | nib(k0 + 9, hi) << 28;
@@ -196,14 +213,14 @@ __global__ void __launch_bounds__(256)
       uint32_t v = 0;
       if (a < 8) {
         int lo, hi;
-        sp_cols(mode, N, s, a, lo, hi);
+        cols(s, a, lo, hi);
         const __half sl = scales[(int64_t)grp * N + lo], sh = scales[(int64_t)grp * N + hi];
         v = (uint32_t)__half_as_ushort(sl) | (uint32_t)__half_as_ushort(sh) << 16;
       } else if (a < 10) {
         for (int b = 0; b < 4; ++b) {
           const int g = (a - 8) * 4 + b;
           int lo, hi;
-          sp_cols(mode, N, s, g, lo, hi);
+          cols(s, g, lo, hi);
           auto znib = [&](int col) -> uint32_t {
             const uint32_t w = (uint32_t)qzeros[(int64_t)grp * NW + (col >> 3)];
             const int jj = col & 7;
@@ -215,6 +232,21 @@ __global__ void __launch_bounds__(256)
       reinterpret_cast<uint32_t*>(ub + F * 128)[a] = v;
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+    stream_pack_kernel(const int32_t* __restrict__ qweight, const __half* __restrict__ scales,
+                       const int32_t* __restrict__ qzeros, uint8_t* __restrict__ out, int K, int N, int G, int mode) {
+  sp_pack(qweight, scales, qzeros, out, K, N, G,
+          [=](int s, int g, int& lo, int& hi) { sp_cols(mode, N, s, g, lo, hi); });
+}
+__global__ void __launch_bounds__(256)
+    stream_pack_rotary_kernel(const int32_t* __restrict__ qweight, const __half* __restrict__ scales,
+                              const int32_t* __restrict__ qzeros, uint8_t* __restrict__ out, int K, int N, int G,
+                              int head_dim) {
+  pdl_wait();   // (launched without the PDL attribute: a no-op, kept so the kernel stays safe under one)
+  sp_pack(qweight, scales, qzeros, out, K, N, G,
+          [=](int s, int g, int& lo, int& hi) { sp_cols_rot(head_dim, s, g, lo, hi); });
 }
 
 // ------------------------------------------------------------------------------------------ the kernel
@@ -397,6 +429,23 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
   pdl_wait();
 #define SP_RESIDUAL 1
 #include "program_stream_body.inc"
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with a ROPE_KV op (SpRope above), with or without residual adds and sparse-MoE blocks: the residual
+// kernel plus the rotation / cache stores of a mode-2 finish, which only SP_ROPE compiles in
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_rope_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                       uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
+                       int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                       const SpRope* __restrict__ rope) {
+  constexpr int NW = 8, SPW = 4, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#include "program_stream_body.inc"
+#undef SP_ROPE
 #undef SP_RESIDUAL
 }
 

@@ -17,7 +17,8 @@ __all__ = [
     "gemm_forward_cuda", "dequantize_weights_cuda", "gemv_forward_cuda", "gemmv2_forward_cuda",
     "gemv_forward_cuda_decode", "gemm_forward_cuda_prefill", "layernorm_forward_cuda", "silu_and_mul",
     "topk_softmax", "moe_alig_block_size", "grouped_gemm_forward",
-    "linear_forward", "stream_pack", "set_knob", "get_knob", "B200AwqError",
+    "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "set_knob", "get_knob",
+    "B200AwqError",
 ]
 
 _WS: dict = {}
@@ -238,6 +239,65 @@ def silu_and_mul(out, gate_up):
     check(code, "b200awq_silu_and_mul")
 
 
+def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out):
+    """Checks the tensors of one RoPE + KV-cache append and returns (b200awq_rope_t, qkv as [M, N], M).
+
+    qkv [.., (H + 2 KV) D] f16 (rows at a unit stride, any row pitch); freqs: the fp32 [S_f, D/2, 2] real view of
+    RoPE.freqs_cis (awq/modules/fused/attn.py:29-43) or the complex64 [S_f, D/2] table itself; pos: a device int32
+    tensor of one element; k_cache / v_cache: WindowedCache's contiguous-row f16 [B >= M, S, KV, D] (cache.py:5-31);
+    q_out: contiguous f16 with M H D elements.  n_kv_heads = 0 means n_heads, as WindowedCache sizes it."""
+    _require_cuda(qkv, freqs, pos, k_cache, v_cache, q_out)
+    H = int(n_heads)
+    KV = int(n_kv_heads) or H
+    if freqs.dtype == torch.complex64:
+        freqs = torch.view_as_real(freqs)
+    if freqs.dtype != torch.float32 or freqs.dim() != 3 or freqs.shape[-1] != 2 or not freqs.is_contiguous():
+        raise B200AwqError("b200awq: freqs must be RoPE.freqs_cis (complex64 [S, D/2]) or its contiguous real view")
+    D = 2 * freqs.shape[1]
+    N = (H + 2 * KV) * D
+    if qkv.dtype != torch.float16 or qkv.shape[-1] != N:
+        raise B200AwqError(f"b200awq: qkv must be float16 [.., (n_heads + 2 n_kv_heads) head_dim = {N}]")
+    q2 = qkv.reshape(-1, N)
+    if q2.stride(-1) != 1:
+        raise B200AwqError("b200awq: qkv rows must have a unit stride")
+    M = q2.shape[0]
+    for name, c in (("k_cache", k_cache), ("v_cache", v_cache)):
+        if c.dtype != torch.float16 or c.dim() != 4 or tuple(c.shape[2:]) != (KV, D) or c.shape[0] < M:
+            raise B200AwqError(f"b200awq: {name} must be float16 [B >= {M}, S, {KV}, {D}]")
+        if c.stride(3) != 1 or c.stride(2) != D or c.stride(1) != KV * D:
+            raise B200AwqError(f"b200awq: {name} must have contiguous [S, KV, D] entries")
+    if k_cache.shape[1] != v_cache.shape[1] or k_cache.stride(0) != v_cache.stride(0):
+        raise B200AwqError("b200awq: k_cache and v_cache must have the same shape and strides")
+    if pos.dtype != torch.int32 or pos.numel() != 1:
+        raise B200AwqError("b200awq: pos must be a device int32 tensor with one element")
+    if q_out.dtype != torch.float16 or not q_out.is_contiguous() or q_out.numel() != M * H * D:
+        raise B200AwqError(f"b200awq: q_out must be a contiguous float16 tensor of {M} x {H} x {D} elements")
+    r = _cabi.Rope()
+    r.n_heads, r.n_kv_heads, r.head_dim = H, KV, D
+    r.cache_len, r.freqs_len = k_cache.shape[1], freqs.shape[0]
+    r.cache_batch_stride = k_cache.stride(0)
+    r.pos, r.freqs, r.q_out = pos.data_ptr(), freqs.data_ptr(), q_out.data_ptr()
+    r.k_cache, r.v_cache = k_cache.data_ptr(), v_cache.data_ptr()
+    return r, q2, M
+
+
+def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None):
+    """RoPE.forward on q and k of the fused qkv output and WindowedCache.update_kv of k and v at position *pos
+    (awq/modules/fused/attn.py:243-267): writes q_out [M, H, D] and the row `pos` of cache batch entries 0..M-1, nothing
+    else (nothing at all when pos is outside the cache or the frequency table).  pos is read on the device: a captured
+    CUDA graph replays at the position stored there.  Returns q_out (allocated when not given)."""
+    H = int(n_heads)
+    D = (freqs_cis.shape[1] if freqs_cis.dtype == torch.complex64 else freqs_cis.shape[-2]) * 2
+    if q_out is None:
+        M = qkv.numel() // qkv.shape[-1] if qkv.shape[-1] else 0
+        q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
+    r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out)
+    with _DeviceGuard(qkv.device):
+        code = lib.b200awq_rope_kv(q2.data_ptr(), q2.stride(0) if M > 1 else q2.shape[1], r, M, _stream(qkv.device))
+    check(code, f"b200awq_rope_kv(M={M}, H={H}, KV={r.n_kv_heads}, D={D})")
+    return q_out
+
+
 # ------------------------------------------------------------------------------------ MoE (awq_ext surface)
 def topk_softmax(topk_weights, topk_ids, token_expert_indicies, gating_output):
     """awq_ext.topk_softmax (fused/moe.py:162-167): fills the three output tensors [M, topk] from gating_output
@@ -351,6 +411,26 @@ def stream_pack(qweight, scales, qzeros, mode: int = 0) -> torch.Tensor:
         code = lib.b200awq_stream_pack(qweight.data_ptr(), scales.data_ptr(), qzeros.data_ptr(), out.data_ptr(), K, N, G,
                                        int(mode), _stream(qweight.device))
     check(code, f"b200awq_stream_pack(K={K}, N={N}, G={G}, mode={mode})")
+    return out
+
+
+def stream_pack_rotary(qweight, scales, qzeros, head_dim: int) -> torch.Tensor:
+    """The stream format in mode 2 (include/b200awq.h): RoPE's column pairs (i, i + D/2) of every head share a lane.
+    What a decode program packs a qkv linear into when a ROPE_KV op folds into its finish."""
+    _require_cuda(qweight, scales, qzeros)
+    _check_w(qweight, torch.int32, "qweight")
+    _check_w(scales, torch.float16, "scales")
+    _check_w(qzeros, torch.int32, "qzeros")
+    K, N = qweight.shape[0], qweight.shape[1] * 8
+    G = K // scales.shape[0]
+    nbytes = lib.b200awq_stream_bytes(K, N, G)
+    if nbytes == 0:
+        raise B200AwqError(f"b200awq: no stream format for K={K}, N={N}, G={G}")
+    out = torch.empty(nbytes, dtype=torch.uint8, device=qweight.device)
+    with _DeviceGuard(qweight.device):
+        code = lib.b200awq_stream_pack_rotary(qweight.data_ptr(), scales.data_ptr(), qzeros.data_ptr(), out.data_ptr(),
+                                              K, N, G, int(head_dim), _stream(qweight.device))
+    check(code, f"b200awq_stream_pack_rotary(K={K}, N={N}, G={G}, head_dim={head_dim})")
     return out
 
 

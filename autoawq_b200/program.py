@@ -28,6 +28,12 @@ at M = 1 the stream kernel runs it as two kernel ops with the routing computed i
 50-52,117-118).  It adds no kernel op: it folds into the epilogue of the linear (or sparse_moe) recorded just before it,
 so a layer splits only at attention - [o + h_in -> h, norm2(h), gate|up, silu, down + h -> out, norm1'(out), qkv'] is one
 program (DESIGN.md 3.5e).  Outside the folding rule `run()` replays per op, with `torch.add` for the adds.
+
+`rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads)` records the start of the attention block
+(RoPE.forward on q and k, WindowedCache.update_kv of k and v: awq/modules/fused/attn.py:243-267).  It adds no kernel
+op either: it folds into the finish of the qkv linear recorded just before it, so the segment ends with q rotated and
+the cache row written, and attention reads them directly (DESIGN.md 3.5f).  `pos` is a device int32 tensor: advance it
+in place between runs (or graph replays).
 """
 from __future__ import annotations
 
@@ -124,6 +130,35 @@ class DecodeProgram:
         self._ops.append(("add", dict(a=a, b=b, out=out, M=M, K=K)))
         self._keep += [a, b, out]
         return out
+
+    def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None):
+        """RoPE.forward(xq, xk, start_pos = *pos, seqlen = 1) + cache.update_kv(xv, xk) on the fused qkv output (q heads,
+        then k heads, then v heads, as get_attention_shapes slices it): writes q_out [M, H, D] (allocated when not given,
+        and returned) and row *pos of k_cache / v_cache batch entries 0..M-1, nothing when *pos is outside the cache or
+        freqs_cis.  freqs_cis: the RoPE module's complex64 [S_f, D/2] table (any rope_theta / scaling it was built with
+        applies as is).  Partial rotary, q_norm / k_norm and ALiBi are not this op: the caller keeps those steps."""
+        self._no_more()
+        self._dev_of(qkv)
+        H = int(n_heads)
+        if freqs_cis.dtype == torch.complex64:
+            freqs_cis = torch.view_as_real(freqs_cis)
+        if freqs_cis.dtype != torch.float32 or freqs_cis.dim() != 3:
+            raise B200AwqError("b200awq: freqs_cis must be RoPE.freqs_cis (complex64 [S, D/2]) or its real view")
+        D = 2 * freqs_cis.shape[1]
+        M = qkv.numel() // qkv.shape[-1] if qkv.shape[-1] else 0
+        if q_out is None:
+            q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
+        for t in (freqs_cis, pos, k_cache, v_cache, q_out):
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+        desc, q2, M = ext.rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out)
+        if q2.data_ptr() != qkv.data_ptr():
+            raise B200AwqError("b200awq: rope_kv_cache records qkv by address: pass its rows as they are")
+        self._ops.append(("rope", dict(qkv=q2, freqs=freqs_cis, pos=pos, k_cache=k_cache, v_cache=v_cache, q_out=q_out,
+                                       H=H, KV=desc.n_kv_heads, M=M, N=q2.shape[1],
+                                       ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc)))
+        self._keep += [qkv, q2, freqs_cis, pos, k_cache, v_cache, q_out]
+        return q_out
 
     @staticmethod
     def _stacked(w, name):
@@ -234,6 +269,9 @@ class DecodeProgram:
             elif kind == "moe":
                 c.kind, c.M, c.K, c.N = _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
+            elif kind == "rope":
+                c.kind, c.M, c.N, c.ldx = _cabi.OP_ROPE_KV, o["M"], o["N"], o["ldx"]
+                c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["desc"])
             else:
                 c.kind, c.M, c.K, c.N, c.group_size, c.ldx = _cabi.OP_LINEAR_GEMM, o["M"], o["K"], o["N"], o["G"], o["ldx"]
                 c.x, c.qweight, c.scales, c.qzeros = (o["x"].data_ptr(), o["qweight"].data_ptr(), o["scales"].data_ptr(),
@@ -278,19 +316,19 @@ class DecodeProgram:
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
-            return o["M"] if kind in ("linear", "moe", "add") else o["rows"]
+            return o["M"] if kind in ("linear", "moe", "add", "rope") else o["rows"]
         return 0
 
     @property
     def kernel_ops(self) -> int:
-        """Ops of the fused kernel: one per linear, two per sparse_moe (gate|up with the routing, down), none per add
-        (it folds into its producer's epilogue); 0 per-op."""
+        """Ops of the fused kernel: one per linear, two per sparse_moe (gate|up with the routing, down), none per add or
+        rope_kv_cache (they fold into their producer's epilogue); 0 per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
     def launches_per_run(self) -> int:
-        """Kernels launched by one run(): 1 when fused (adds included); per op, one per recorded call, 6 per
-        sparse_moe, and one torch.add launch per add."""
+        """Kernels launched by one run(): 1 when fused (adds and rope_kv_cache included); per op, one per recorded
+        call, 6 per sparse_moe, one torch.add launch per add and one b200awq_rope_kv launch per rope_kv_cache."""
         return 1 if self.fused else sum(6 if kind == "moe" else 1 for kind, _ in self._ops)
 
     def run(self) -> None:
@@ -311,6 +349,10 @@ class DecodeProgram:
                 self._moe_replay(o)
             elif kind == "add":
                 torch.add(o["a"], o["b"], out=o["out"])
+            elif kind == "rope":
+                with ext._DeviceGuard(dev):
+                    code = lib.b200awq_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["M"], ext._stream(dev))
+                check(code, "b200awq_rope_kv")
             else:
                 ext.linear_forward("gemm", o["x"], o["qweight"], o["scales"], o["qzeros"], o["G"], o["bias"], out=o["y"])
 

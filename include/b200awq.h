@@ -18,6 +18,7 @@
  *                                   awq_v2_ext.gemm_forward_cuda_prefill  awq/modules/linear/gemv_fast.py:203-205
  *   b200awq_rmsnorm .............. awq_ext.layernorm_forward_cuda   awq/modules/fused/norm.py:33-36
  *   b200awq_silu_and_mul ......... awq_ext.silu_and_mul             awq/modules/fused/moe.py:76
+ *   b200awq_rope_kv .............. RoPE.forward + WindowedCache.update_kv   awq/modules/fused/attn.py:53-86,243-267
  *
  * Tensor layouts (SURVEY.md Appendix A):
  *   GEMM  : qweight [K, N/8] i32 (AWQ interleave), qzeros [K/G, N/8] i32, scales [K/G, N] f16
@@ -232,9 +233,21 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     the producer's raw output is rejected.  Both the producer's y and the ADD's y are stored.  Everything else is
  *     B200AWQ_EUNSUPPORTED and the caller replays per op: an ADD after a glue op or another ADD, after a gate|up whose
  *     output only SiLU*mul reads, with both operands external, in place, with a residual out of the window or one the
- *     program overwrites.  M = 1 runs 8 consumer warps x 4 stages (knob 9 ignored); M > 1 the batched kernel. */
+ *     program overwrites.  M = 1 runs 8 consumer warps x 4 stages (knob 9 ignored); M > 1 the batched kernel.
+ *
+ *   ROPE_KV       : the start of the attention block (awq/modules/fused/attn.py:243-267): rotate q and k of the fused
+ *                   qkv output with RoPE.forward and write k and v into the WindowedCache row update_kv writes.
+ *                   x = qkv [M, (H + 2 KV) D] f16 at row pitch ldx, weight = a b200awq_rope_t descriptor (below), M, and
+ *                   N = (H + 2 KV) D.  As b200awq_rope_kv.
+ *     Folding: a ROPE_KV adds no kernel op.  It folds into the finish of the linear recorded immediately before it, whose
+ *     whole output must be its qkv: that linear is re-laid-out in stream mode 2 (rotary pairs, below), so the thread that
+ *     finishes column i of a head also holds column i + D/2 and rotates the pair in registers.  The linear's y and
+ *     published row keep the raw qkv values.  B200AWQ_EUNSUPPORTED (the caller replays per op) when the op before it is
+ *     not a plain linear (a glue op, an ADD, a gate|up whose product SiLU*mul reads, a SPARSE_MOE) or already carries an
+ *     ADD, when N != (H + 2 KV) D or D % 16 != 0, or when any other op of the program reads or writes q_out or the
+ *     caches. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
-       B200AWQ_OP_ADD = 5 };
+       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -283,6 +296,31 @@ typedef struct b200awq_moe {
  * CTA keeps in the down op, dynamic shared memory of the kernel for this block alone}.  B200AWQ_EUNSUPPORTED outside the
  * envelope above, B200AWQ_EINVAL for bad arguments. */
 int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8);
+
+/* RoPE + KV-cache append of one decode step (awq/modules/fused/attn.py:53-86 RoPE.forward, cache.py:41-46
+ * WindowedCache.update_kv).  For token row m < M, head h < H + 2 KV and pair i < D/2, with a = qkv[m, h D + i],
+ * b = qkv[m, h D + D/2 + i], (c, s) = freqs[pos, i]:
+ *   q head (h < H):   q_out[m, h, i] = fp16(fma(a, c, -(b s))), q_out[m, h, i + D/2] = fp16(fma(b, c, a s))
+ *   k head:           the same rotation into k_cache[m, pos, h - H, .]
+ *   v head:           a, b unrotated into v_cache[m, pos, h - H - KV, .]
+ * (the fp32 complex product of RoPE.forward with the FMA contraction torch's CUDA kernel uses, then .type_as(fp16);
+ * torch's loops for some shapes round a few elements differently, within one fp16 ulp of this).
+ * Nothing else is written; when *pos is outside [0, min(cache_len, freqs_len)) nothing at all.  The kernel reads *pos
+ * on the device, so a captured CUDA graph replays at whatever position the caller stored there. */
+typedef struct b200awq_rope {
+  int32_t n_heads, n_kv_heads, head_dim; /* H, KV, D (D % 2 == 0) */
+  int32_t cache_len;                     /* S: positions of the cache */
+  int32_t freqs_len;                     /* S_f: rows of freqs */
+  int32_t pad_;
+  int64_t cache_batch_stride;            /* elements between two batch entries of k_cache / v_cache (>= S KV D) */
+  const int32_t* pos;                    /* device int32[1]: the position written (start_pos) */
+  const float* freqs;                    /* [S_f, D/2, 2] f32 (cos, sin): torch.view_as_real(RoPE.freqs_cis) */
+  void* q_out;                           /* [M, H, D] f16 */
+  void* k_cache;                         /* [B >= M, S, KV, D] f16 */
+  void* v_cache;                         /* [B >= M, S, KV, D] f16 */
+} b200awq_rope_t;
+/* ldqkv: row pitch of qkv in elements (>= (H + 2 KV) D).  `rope` is a host pointer, read at the call. */
+int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream);
 
 typedef struct b200awq_program* b200awq_program_t;
 
@@ -343,11 +381,16 @@ int b200awq_comm_destroy(b200awq_comm_t comm);
  * in sets of 16, K in units of min(G, 128) rows; a unit is contiguous (fragments in mma.m16n8k16 A-operand order +
  * the unit's scales / zeros), the buffer is set-major, so any partition of the work is a contiguous byte range.
  * mode 0: set s = columns 16 s .. 16 s + 15; mode 1 (a fused gate|up linear): gate column j and up column j share
- * a lane, so SiLU*mul happens in the producer.  Requires N % 16 == 0, K % 128 == 0, G in {32, 64} or G % 128 == 0.
- * b200awq_stream_bytes returns 0 for unsupported shapes. */
+ * a lane, so SiLU*mul happens in the producer; mode 2 (a qkv linear followed by ROPE_KV, b200awq_stream_pack_rotary):
+ * set s of head h = s / (D / 16) pairs column h D + 8 t + g with h D + D/2 + 8 t + g (t = s % (D / 16)), so RoPE's
+ * rotation partners share a lane (requires D % 16 == 0 and N % D == 0).  Requires N % 16 == 0, K % 128 == 0, G in
+ * {32, 64} or G % 128 == 0.  b200awq_stream_bytes returns 0 for unsupported shapes; the byte count is the same for
+ * every mode. */
 size_t b200awq_stream_bytes(int K, int N, int group_size);
 int b200awq_stream_pack(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
                         int group_size, int mode, b200awq_stream_t stream);
+int b200awq_stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K,
+                               int N, int group_size, int head_dim, b200awq_stream_t stream);
 
 #ifdef __cplusplus
 }
