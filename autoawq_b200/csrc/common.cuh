@@ -240,6 +240,29 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
       ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// L2 cache policies (createpolicy) for the .L2::cache_hint forms below: evict_first for data that is dead once it has
+// been read, evict_last for data that must stay in L2 until it is read
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void bulk_prefetch_l2_hint(const void* gsrc, uint32_t bytes, uint64_t policy) {
+  asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(gsrc), "r"(bytes), "l"(policy)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_load_1d_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar,
+                                                  uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+      ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
 
 // -------------------------------------------------------------------------------------- wgmma
 // Warpgroup MMA (sm_90a): four consecutive warps, aligned to a multiple of four, issue one D[64 x N] (+)= A[64 x 16] .

@@ -149,6 +149,10 @@ struct Program {
   size_t stream_bytes = 0;
   // batched stream variant (M > 1, program_batch.cuh): ring stages per warp, sets per CTA, units along K (smem sizes)
   int sb_spw = 0, sb_lmax = 0, sb_nu_max = 0;
+  // M = 1 stream kernels (program_stream.cuh): ring stages per warp with 8 / 12 consumer warps (sp_pick_spw); the
+  // device's L2 size (the run-ahead window, knob 8)
+  int sp_spw8 = 0, sp_spw12 = 0;
+  int l2_bytes = 0;
   // sparse-MoE blocks (stream_moe_kernel): their descriptors
   SpMoe* d_moe = nullptr;
   int n_moe = 0;
@@ -187,7 +191,7 @@ int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
   if (H / UK > kSpXsumMax || topk * nu_b1 > kSpXsumMax) return B200AWQ_EUNSUPPORTED;
   if (lmax_a > kSpLMax || lmax_b > kSpLMax) return B200AWQ_EUNSUPPORTED;
   const int kmax = H > topk * I ? H : topk * I;
-  const size_t smem = sp_fixed_smem(8, 4, true) + (size_t)kmax * 2;
+  const size_t smem = sp_fixed_smem(8, 4, true) + (size_t)kmax * 2;   // (at the minimum ring depth)
   if (smem > (size_t)227 * 1024) return B200AWQ_EUNSUPPORTED;
   out8[0] = 2;                         // kernel ops
   out8[1] = sets_a;                    // gate|up: 16-column sets (top_k slots x 2I / 16)
@@ -212,6 +216,15 @@ bool stream_format_supported(int K, int N, int G, int mode) {
   return mode == 0 || mode == 1;
 }
 static int prog_sm_count();   // device SM count (defined below)
+
+// The deepest ring (stages per consumer warp, at most kSpMaxStages) of an M = 1 stream kernel with nw consumer warps
+// that fits 227 KB next to the program's activations (xs_bytes).  A program stream_build accepts gets at least 4 stages
+// at 8 warps and 3 at 12.
+static int sp_pick_spw(int nw, bool moe, size_t xs_bytes) {
+  int spw = kSpMaxStages;
+  while (spw > 1 && sp_fixed_smem(nw, spw, moe) + xs_bytes > (size_t)227 * 1024) --spw;
+  return spw;
+}
 
 cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
                                int G, int head_dim, cudaStream_t st) {
@@ -318,11 +331,14 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     max_cols = std::max(max_cols, (size_t)(mode[i] == 1 ? p.N / 2 : p.N));
     max_K = std::max(max_K, p.K);
   }
-  if (M == 1 && (has_moe || has_res || has_rope)) {
-    // the MoE / residual kernel runs 8 consumer warps with 4 ring stages each, behind the routing area
-    if (sp_fixed_smem(8, 4, true) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
-  } else if (M == 1) {
-    if (sp_fixed_smem(12, 3) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;   // (the largest configuration)
+  if (M == 1) {
+    // the envelope: a ring of 4 stages at 8 warps (the MoE / residual / rope kernels, behind the routing area) or 3 at
+    // 12 must fit; the program then runs the deepest ring its activations leave room for
+    const bool moe_k = has_moe || has_res || has_rope;
+    if (moe_k && sp_fixed_smem(8, 4, true) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
+    if (!moe_k && sp_fixed_smem(12, 3, false) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
+    pr->sp_spw8 = sp_pick_spw(8, moe_k, (size_t)max_K * 2);
+    pr->sp_spw12 = moe_k ? 0 : sp_pick_spw(12, false, (size_t)max_K * 2);
   } else {
     // the batched kernel: the deepest ring (<= 4 stages per warp) that leaves room for M rows of activations
     int spw = kSbMaxStages;
@@ -501,9 +517,10 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_sp_ops, ops.data(), (size_t)n * sizeof(SpOp), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_cta, cta.data(), cta.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(stream_program_kernel<8, 4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    e = cudaFuncSetAttribute(stream_program_kernel<8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(stream_program_kernel<12, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    e = cudaFuncSetAttribute(stream_program_kernel<12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&pr->l2_bytes, cudaDevAttrL2CacheSize, pr->device);
   if (e == cudaSuccess && M > 1) {
     e = cudaFuncSetAttribute(stream_batch_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e == cudaSuccess)
@@ -981,15 +998,18 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     return cudaLaunchKernelEx(&cfg, kern, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
                               p->sb_lmax, p->sb_nu_max, knob(3));
   }
-  // knob 9: consumer warps of the stream kernel: 8 (4 ring stages each, 4 units in flight; the default) or 12 (3 stages,
-  // 2 units).  No 16-warp variant: 17 warps put 5 on one of the SM's four register-file partitions, which caps a thread
-  // at 96 registers on sm_90 and spills the unit loop.
-  const int nw = knob(9) == 12 ? 12 : 8;
-  const int spw = nw == 8 ? 4 : 3;
+  // knob 9: consumer warps of the stream kernel: 8 (4 units in flight; the default) or 12 (2 units), each with the ring
+  // depth chosen at creation (at least 4 / 3 stages).  No 16-warp variant: 17 warps put 5 on one of the SM's four
+  // register-file partitions, which caps a thread at 96 registers on sm_90 and spills the unit loop.  The MoE, residual
+  // and rope kernels always run 8 warps.
+  const bool moe_k = p->d_rope != nullptr || p->d_res != nullptr || p->n_moe > 0;
+  const int nw = knob(9) == 12 && !moe_k ? 12 : 8;
+  const int spw = nw == 8 ? p->sp_spw8 : p->sp_spw12;
+  const int grid = prog_sm_count();
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(prog_sm_count());
+  cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(32 + nw * 32);
-  cfg.dynamicSmemBytes = sp_fixed_smem(nw, spw) + p->xs_bytes;
+  cfg.dynamicSmemBytes = sp_fixed_smem(nw, spw, moe_k) + p->xs_bytes;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: the hand-off polls are grid-wide waits
@@ -998,45 +1018,41 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
   cfg.numAttrs = 1;
   const SpOp* sops = p->d_sp_ops;
   const uint32_t* cta = p->d_cta;
-  // knob 8: HBM -> L2 prefetch window per producer lane in KB (<= 0 = off, the default: it can only help when the
-  // weight stream is the bottleneck, which the unit math is not; not re-measured on H100)
-  const int l2_ahead = knob(8) <= 0 ? 0 : knob(8) * 1024;
+  // knob 8: the HBM -> L2 run-ahead window of the weight stream, grid-wide, in MB, at most the device's L2 (<= 0: off,
+  // the default).  The producer advances its prefetch cursor only while it has no ring stage to fill - during op
+  // hand-offs and tails - and each of its grid x nw lanes keeps at most window / (grid x nw) bytes ahead of its ring.
+  // Off is the default: on the bench step no window beat it by more than its run-to-run spread (H100 SXM, DESIGN
+  // 3.5b: 8 and 16 MB within 0.5 %, 32 MB 4 % slower).
+  const size_t window = knob(8) <= 0 ? 0 : std::min((size_t)knob(8) << 20, (size_t)p->l2_bytes);
+  const int l2_ahead = (int)(window / ((size_t)grid * nw));
   // knob 10: ops ahead of the consumers' staging for which shared-memory loads may already be issued (0 = ungated,
-  // the default; n > 0: at most n - 1 ops ahead, 1 = strictly gated)
+  // the default: a gate of 2 measured 1.5-2 % slower on the bench step, DESIGN 3.5b; n > 0: at most n - 1 ops ahead,
+  // 1 = strictly gated)
   const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
   const SpMoe* no_moe = nullptr;
-  if (p->d_rope != nullptr) {
-    // programs with a ROPE_KV op (with or without adds / sparse-MoE blocks): 8 consumer warps x 4 ring stages
-    cfg.blockDim = dim3(32 + 8 * 32);
-    cfg.dynamicSmemBytes = sp_fixed_smem(8, 4, true) + p->xs_bytes;
+  if (p->d_rope != nullptr) {   // programs with a ROPE_KV op (with or without adds / sparse-MoE blocks)
     const SpMoe* md = p->d_moe;
     const SpRes* rd = p->d_res;
     const SpRope* qd = p->d_rope;
-    return cudaLaunchKernelEx(&cfg, stream_rope_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
+    return cudaLaunchKernelEx(&cfg, stream_rope_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
                               knob(3), l2_ahead, gate_ahead, md, rd, qd);
   }
-  if (p->d_res != nullptr) {
-    // programs with residual adds (with or without sparse-MoE blocks): always 8 consumer warps x 4 ring stages
-    cfg.blockDim = dim3(32 + 8 * 32);
-    cfg.dynamicSmemBytes = sp_fixed_smem(8, 4, true) + p->xs_bytes;
+  if (p->d_res != nullptr) {   // programs with residual adds (with or without sparse-MoE blocks)
     const SpMoe* md = p->d_moe;
     const SpRes* rd = p->d_res;
     return cudaLaunchKernelEx(&cfg, stream_residual_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
-                              knob(3), l2_ahead, gate_ahead, md, rd);
+                              spw, knob(3), l2_ahead, gate_ahead, md, rd);
   }
-  if (p->n_moe > 0) {
-    // programs with sparse-MoE blocks: the MOE instantiation, always 8 consumer warps x 4 ring stages
-    cfg.blockDim = dim3(32 + 8 * 32);
-    cfg.dynamicSmemBytes = sp_fixed_smem(8, 4, true) + p->xs_bytes;
+  if (p->n_moe > 0) {   // programs with sparse-MoE blocks: the MOE instantiation
     const SpMoe* md = p->d_moe;
-    return cudaLaunchKernelEx(&cfg, stream_moe_kernel, sops, cta, p->n_ops, p->d_rows,
-                              p->row_stride, p->d_state, knob(3), l2_ahead, gate_ahead, md);
+    return cudaLaunchKernelEx(&cfg, stream_moe_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
+                              knob(3), l2_ahead, gate_ahead, md);
   }
   if (nw == 8)
-    return cudaLaunchKernelEx(&cfg, stream_program_kernel<8, 4, 4>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                              p->d_state, knob(3), l2_ahead, gate_ahead, no_moe);
-  return cudaLaunchKernelEx(&cfg, stream_program_kernel<12, 3, 2>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                            p->d_state, knob(3), l2_ahead, gate_ahead, no_moe);
+    return cudaLaunchKernelEx(&cfg, stream_program_kernel<8, 4>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
+                              p->d_state, spw, knob(3), l2_ahead, gate_ahead, no_moe);
+  return cudaLaunchKernelEx(&cfg, stream_program_kernel<12, 2>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
+                            p->d_state, spw, knob(3), l2_ahead, gate_ahead, no_moe);
 }
 
 void program_destroy(Program* p) {

@@ -8,7 +8,7 @@
 // bulk-copy ring across op boundaries, the output-stationary CTA partition, the tagged (fp16 | tag) hand-off words
 // polled with ld.relaxed.gpu (M rows per op, one tag per (run, op)), the ProgWatch watchdog and its abort record.
 //
-// Bit identity with M = 1: the kernel keeps the cut of stream_program_kernel<8, 4, 4> - 8 consumer warps, the same
+// Bit identity with M = 1: the kernel keeps the cut of stream_program_kernel<8, 4> - 8 consumer warps, the same
 // unit-to-warp split, units folded and summed in the same order, the warps' partial sums reduced in the same fixed
 // order - and an MMA column does not depend on the other columns.  The RMSNorm of every row follows aux.cu's
 // rmsnorm_kernel (thread -> k mapping and summation order).  So token m of a batched run is bit-identical to an M = 1
@@ -23,7 +23,7 @@
 
 namespace b200awq {
 
-constexpr int kSbWarps = 8;   // consumer warps (the cut of stream_program_kernel<8, 4, 4>)
+constexpr int kSbWarps = 8;   // consumer warps (the cut of stream_program_kernel<8, 4>)
 constexpr int kSbGR = 4;      // units in flight per warp
 constexpr int kSbMaxStages = 4;
 // the kernel instance (MT) that runs M >= 2 tokens (M = 1 is stream_program_kernel: sizes with one row, not sb_mt(1))

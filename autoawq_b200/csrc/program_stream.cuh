@@ -82,12 +82,25 @@ struct SpMoe {
   int seg_a, seg_b, I;
 };
 
-// (moe: the MoE kernel's routing area, SpMoeSmem, follows the fixed part)
-__host__ __device__ constexpr size_t sp_fixed_smem(int nw, int spw, bool moe = false) {
-  return (size_t)nw * spw * kSpStageBytes + (size_t)kSpLMax * nw * 16 * 4 + (size_t)kSpXsumMax * 4 +
-         (size_t)2 * nw * spw * 8 + 2 * 128 + 256 + (moe ? kSpMoeSmem : 0);
+// Shared memory of the M = 1 stream kernels:
+//   sdesc [2] SpOp (256 B) | misc (256 B) | MoE routing area (SpMoeSmem, MOE kernels only) |
+//   part [kSpLMax][nw][16] f32 | xsum [kSpXsumMax] f32 | ring [spw][nw] stages | full / empty barriers [spw * nw] each |
+//   xs (the activations, K fp16)
+// spw = ring stages per consumer warp: the host picks the deepest ring that fits next to the program's activations
+// (sp_pick_spw in program.cu); at the minimum depth the layout is as large as with the fixed ring before.  Everything
+// in front of the ring sits at a compile-time offset: a base that depends on the program costs registers the kernels
+// do not have (9 warps cap a thread at 168, 13 at 128; sizing part and xsum from the program spills 24 / 60 bytes in
+// the 8-warp kernel).  Every part is a multiple of 16 bytes.
+constexpr int kSpMaxStages = 8;                   // ring stages per warp at most (227 KB allows 6 at 8 warps)
+constexpr int kSpMoeOff = 512;                    // the routing area (behind sdesc and misc)
+__host__ __device__ constexpr size_t sp_ring_off(int nw, bool moe) {
+  return kSpMoeOff + (moe ? kSpMoeSmem : 0) + (size_t)kSpLMax * nw * 16 * 4 + (size_t)kSpXsumMax * 4;
 }
-static_assert(sp_fixed_smem(8, 4) % 16 == 0 && sp_fixed_smem(12, 3) % 16 == 0 && sp_fixed_smem(16, 2) % 16 == 0,
+// bytes in front of the activations (xs)
+__host__ __device__ constexpr size_t sp_fixed_smem(int nw, int spw, bool moe) {
+  return sp_ring_off(nw, moe) + (size_t)nw * spw * (kSpStageBytes + 2 * 8);
+}
+static_assert(sp_fixed_smem(8, 4, false) % 16 == 0 && sp_fixed_smem(12, 3, true) % 16 == 0,
               "xs must stay 16-byte aligned");
 
 __device__ __forceinline__ uint4 ld_relaxed_u4(const void* p) {
@@ -393,25 +406,26 @@ __device__ __forceinline__ SpMoeSmem sp_moe_smem(uint8_t* area) {
   return s;
 }
 
-// The kernel body is program_stream_body.inc: stream_program_kernel<NW, SPW, GR> (MOE = false; `moe` unused) and
+// The kernel body is program_stream_body.inc: stream_program_kernel<NW, GR> (MOE = false; `moe` unused) and
 // stream_moe_kernel (programs with sparse-MoE blocks, SpMoe above) include it.  Every MoE-only step sits behind
 // `if constexpr (MOE)`: stream_program_kernel is the plain kernel, instruction for instruction.
 // (MOE is only ever false here; it is a template parameter rather than a local constant because a local constant,
 // unlike the parameter, changes the register assignment ptxas makes for this kernel)
-template <int NW, int SPW, int GR, bool MOE = false>
+// spw: ring stages per consumer warp (sp_fixed_smem above)
+template <int NW, int GR, bool MOE = false>
 __global__ void __launch_bounds__(32 + NW * 32, 1)
     stream_program_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
-                          uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
-                          int gate_ahead, const SpMoe* __restrict__ moe) {
+                          uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                          int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe) {
 #include "program_stream_body.inc"
 }
 
-// programs with sparse-MoE blocks: 8 consumer warps, 4 ring stages each
+// programs with sparse-MoE blocks: 8 consumer warps
 __global__ void __launch_bounds__(32 + 8 * 32, 1)
     stream_moe_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
-                      uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
-                      int gate_ahead, const SpMoe* __restrict__ moe) {
-  constexpr int NW = 8, SPW = 4, GR = 4;
+                      uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                      int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe) {
+  constexpr int NW = 8, GR = 4;
   constexpr bool MOE = true;
   pdl_wait();   // nothing is read before the predecessor is done, should it ever be launched with PDL (a no-op under
                 // the cooperative launch of program_run)
@@ -422,9 +436,9 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 // residual steps of the finish, which only SP_RESIDUAL compiles in (the kernels above do not see them at all)
 __global__ void __launch_bounds__(32 + 8 * 32, 1)
     stream_residual_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
-                           uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
-                           int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res) {
-  constexpr int NW = 8, SPW = 4, GR = 4;
+                           uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                           int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res) {
+  constexpr int NW = 8, GR = 4;
   constexpr bool MOE = true;
   pdl_wait();
 #define SP_RESIDUAL 1
@@ -436,10 +450,10 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 // kernel plus the rotation / cache stores of a mode-2 finish, which only SP_ROPE compiles in
 __global__ void __launch_bounds__(32 + 8 * 32, 1)
     stream_rope_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
-                       uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int dbg, int l2_ahead,
-                       int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                       uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                       int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
                        const SpRope* __restrict__ rope) {
-  constexpr int NW = 8, SPW = 4, GR = 4;
+  constexpr int NW = 8, GR = 4;
   constexpr bool MOE = true;
   pdl_wait();
 #define SP_RESIDUAL 1
