@@ -58,7 +58,18 @@ class Rope(ctypes.Structure):
     ]
 
 
+class QkNormRope(ctypes.Structure):
+    """b200awq_qk_norm_rope_t (include/b200awq.h): the descriptor of b200awq_qk_norm_rope_kv and of a QK_NORM_ROPE_KV
+    op's `weight`."""
+
+    _fields_ = [
+        ("rope", Rope), ("q_norm_weight", ctypes.c_void_p), ("k_norm_weight", ctypes.c_void_p), ("eps", ctypes.c_float),
+        ("pad_", ctypes.c_int32),
+    ]
+
+
 OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV = 1, 2, 3, 4, 5, 6
+OP_QK_NORM_ROPE_KV = 7
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -86,6 +97,7 @@ SIGNATURES = {
     "b200awq_rmsnorm": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_float, _c_void_p]),
     "b200awq_silu_and_mul": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_void_p]),
     "b200awq_rope_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Rope), _c_int, _c_void_p]),
+    "b200awq_qk_norm_rope_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(QkNormRope), _c_int, _c_void_p]),
     "b200awq_set_knob": (_c_int, [_c_int, _c_int]),
     "b200awq_get_knob": (_c_int, [_c_int]),
     "b200awq_debug_read": (_c_int, [_c_void_p, _c_size_t]),

@@ -82,6 +82,51 @@ __global__ void __launch_bounds__(256)
   rope_pair(r, pos, m, c, row[c], row[c + half]);
 }
 
+// one CTA per (token row, head), one thread per pair (a strided loop past 256 pairs); rope.cuh has the arithmetic and
+// the summation order of the head's sum of squares (set partials into shared memory, then summed in set order)
+__global__ void __launch_bounds__(256)
+    qk_norm_rope_kv_kernel(const __half* __restrict__ qkv, int64_t ldqkv, b200awq_qk_norm_rope_t q, float inv_d,
+                           int M) {
+  extern __shared__ float qk_part[];   // [D / 16] set partials of this head
+  pdl_trigger();
+  pdl_wait();
+  const b200awq_rope_t& r = q.rope;
+  const int pos = rope_pos(r);
+  const int D = r.head_dim, half = D >> 1, heads = r.n_heads + 2 * r.n_kv_heads;
+  const int m = static_cast<int>(blockIdx.x / heads), h = static_cast<int>(blockIdx.x - (unsigned)m * heads);
+  if (pos < 0 || m >= M) return;
+  const __half* row = qkv + (int64_t)m * ldqkv + (int64_t)h * D;
+  const int c0 = h * D;
+  if (h >= r.n_heads + r.n_kv_heads) {   // v head: not normalised
+    for (int p = threadIdx.x; p < half; p += blockDim.x) rope_pair(r, pos, m, c0 + p, row[p], row[p + half]);
+    return;
+  }
+  for (int p = threadIdx.x; p < half; p += blockDim.x) {   // blockDim % 8 == 0: a set's 8 lanes run together
+    const float s = qk_set_partial(row[p], row[p + half]);
+    if ((p & 7) == 0) qk_part[p >> 3] = s;
+  }
+  __syncthreads();
+  const float ss = qk_head_sum(D >> 4, [&](int t) { return qk_part[t]; });
+  for (int p = threadIdx.x; p < half; p += blockDim.x)
+    qk_norm_rope_pair(q, inv_d, pos, m, c0 + p, row[p], row[p + half], ss);
+}
+
+int qk_norm_validate(const b200awq_qk_norm_rope_t* q, int64_t ldqkv) {
+  if (q == nullptr) return B200AWQ_EINVAL;
+  const int v = rope_validate(&q->rope, ldqkv);
+  if (v != B200AWQ_OK) return v;
+  if (q->q_norm_weight == nullptr || q->k_norm_weight == nullptr) return B200AWQ_EINVAL;
+  return B200AWQ_OK;
+}
+
+cudaError_t qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t& q, int M, cudaStream_t st) {
+  const int half = q.rope.head_dim / 2, heads = q.rope.n_heads + 2 * q.rope.n_kv_heads;
+  const int threads = half < 256 ? half : 256;
+  return launch_kernel(qk_norm_rope_kv_kernel, dim3(static_cast<unsigned>((int64_t)M * heads)), dim3(threads),
+                       (size_t)(q.rope.head_dim / 16) * sizeof(float), st, reinterpret_cast<const __half*>(qkv), ldqkv, q,
+                       1.f / static_cast<float>(q.rope.head_dim), M);
+}
+
 int rope_validate(const b200awq_rope_t* r, int64_t ldqkv) {
   if (r == nullptr || r->pos == nullptr || r->freqs == nullptr || r->q_out == nullptr || r->k_cache == nullptr ||
       r->v_cache == nullptr)

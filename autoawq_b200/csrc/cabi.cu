@@ -214,6 +214,17 @@ int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, 
   return fold(rope_kv(qkv, ldqkv, *rope, M, static_cast<cudaStream_t>(stream)));
 }
 
+int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
+                            b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_qk_norm_rope_kv");
+  if (qkv == nullptr || M < 0) return B200AWQ_EINVAL;
+  const int v = qk_norm_validate(desc, ldqkv);
+  if (v != B200AWQ_OK) return v;
+  if ((desc->rope.head_dim % 16) != 0) return B200AWQ_EUNSUPPORTED;   // the fixed summation order works in sets of 16
+  if (M == 0) return B200AWQ_OK;
+  return fold(qk_norm_rope_kv(qkv, ldqkv, *desc, M, static_cast<cudaStream_t>(stream)));
+}
+
 
 int b200awq_program_create_batched(const b200awq_op_t* ops, int n_ops, int max_tokens, b200awq_program_t* out) {
   if (out == nullptr) return B200AWQ_EINVAL;

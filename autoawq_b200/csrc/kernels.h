@@ -7,6 +7,7 @@
 
 struct b200awq_op;
 struct b200awq_rope;
+struct b200awq_qk_norm_rope;
 
 namespace b200awq {
 
@@ -140,6 +141,11 @@ cudaError_t silu_and_mul(const void* gate_up, void* out, int rows, int d, cudaSt
 // B200AWQ_OK, or the code b200awq_rope_kv returns for a bad descriptor / qkv pitch (host only)
 int rope_validate(const struct ::b200awq_rope* r, int64_t ldqkv);
 cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_rope& r, int M, cudaStream_t st);
+// B200AWQ_OK, or the code b200awq_qk_norm_rope_kv returns for a bad descriptor / qkv pitch (host only; D % 16 is
+// checked by the callers)
+int qk_norm_validate(const struct ::b200awq_qk_norm_rope* q, int64_t ldqkv);
+cudaError_t qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_qk_norm_rope& q, int M,
+                            cudaStream_t st);
 cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
                                int G, int head_dim, cudaStream_t st);
 

@@ -119,7 +119,8 @@ struct ProgWatch {
 // wait codes of the abort record (the values are what b200awq_debug_read reports: they stay fixed)
 enum { kWEmpty = 3 /* producer: a free ring stage */, kWFull = 4 /* consumer: a landed ring stage */,
        kWCopy = 10 /* staging: the source row's tagged words */, kWRoute = 13 /* producer: a MoE block's routing */,
-       kWResidual = 14 /* finish: the tagged row of a residual add's source op */ };
+       kWResidual = 14 /* finish: the tagged row of a residual add's source op */,
+       kWQkNorm = 15 /* finish: a q / k head's tagged sum-of-squares partials (QK_NORM_ROPE_KV) */ };
 // returns false when the wait was abandoned (abort): the caller must not touch the barrier's stage any more
 __device__ __forceinline__ bool prog_mbar_wait(uint64_t* bar, uint32_t parity, int code, int op) {
   ProgWatch wd;
@@ -161,6 +162,10 @@ struct Program {
   // ROPE_KV ops (stream_rope_kernel / stream_batch_rope_kernel): one SpRope per kernel op, null without them (d_res is
   // then allocated too, empty where there is no add: the rope kernels are the residual kernels plus the rope steps)
   SpRope* d_rope = nullptr;
+  // QK_NORM_ROPE_KV ops (stream_qknorm_kernel / stream_batch_qknorm_kernel): one SpQkNorm per kernel op and the published
+  // set partials of their heads, null without them (d_res and d_rope are then allocated too)
+  SpQkNorm* d_qkn = nullptr;
+  unsigned long long* d_qkn_part = nullptr;
 };
 
 // An ADD folded into table entry i (program_create): the entry's y is swapped for the ADD's output (what its row
@@ -257,9 +262,11 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
 // Sparse-MoE blocks (`fold[i].kind` != 0, M = 1 only): the gate|up entry is a mode-1 op over top_k slots of 2I
 // columns, the down entry reads its published row (K' = top_k I); both stream E per-expert slices packed back to back.
 // ROPE_KV ops (`ropes[i].head_dim` != 0): entry i is packed in mode 2 and its finish rotates / appends (SpRope).
+// QK_NORM_ROPE_KV ops: as ROPE_KV, and `qkns[i]` carries the norm weights (q_norm_weight != null: SpQkNorm).
 static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
                          const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes,
-                         const std::vector<ResFold>& res, const std::vector<b200awq_rope_t>& ropes) {
+                         const std::vector<ResFold>& res, const std::vector<b200awq_rope_t>& ropes,
+                         const std::vector<b200awq_qk_norm_rope_t>& qkns) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
@@ -500,6 +507,36 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(stream_batch_residual_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   }
+  bool has_qkn = false;
+  for (int i = 0; i < n && !qkns.empty(); ++i) has_qkn = has_qkn || qkns[i].q_norm_weight != nullptr;
+  if (e == cudaSuccess && has_qkn) {
+    // the partials of op i live at [M][N_i / 16] words from its offset; zero tags are never a run's (sp_tag >= 1)
+    std::vector<SpQkNorm> qd(n);
+    size_t words = 0;
+    for (int i = 0; i < n; ++i)
+      if (qkns[i].q_norm_weight != nullptr) words += (size_t)M * (table[i].N / 16);
+    e = cudaMalloc(&pr->d_qkn_part, words * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemset(pr->d_qkn_part, 0, words * sizeof(unsigned long long));
+    size_t off = 0;
+    for (int i = 0; i < n; ++i) {
+      std::memset(&qd[i], 0, sizeof(SpQkNorm));
+      if (qkns[i].q_norm_weight == nullptr) continue;
+      qd[i].q = qkns[i];
+      qd[i].part = pr->d_qkn_part + off;
+      qd[i].inv_d = 1.f / static_cast<float>(qkns[i].rope.head_dim);
+      off += (size_t)M * (table[i].N / 16);
+    }
+    if (e == cudaSuccess) e = cudaMalloc(&pr->d_qkn, (size_t)n * sizeof(SpQkNorm));
+    if (e == cudaSuccess) e = cudaMemcpy(pr->d_qkn, qd.data(), (size_t)n * sizeof(SpQkNorm), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_qknorm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  }
   if (e == cudaSuccess && has_rope) {
     std::vector<SpRope> rp(n);
     for (int i = 0; i < n; ++i) rp[i].r = ropes[i];
@@ -538,8 +575,12 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     cudaFree(pr->d_moe);
     cudaFree(pr->d_res);
     cudaFree(pr->d_rope);
+    cudaFree(pr->d_qkn);
+    cudaFree(pr->d_qkn_part);
     pr->d_res = nullptr;
     pr->d_rope = nullptr;
+    pr->d_qkn = nullptr;
+    pr->d_qkn_part = nullptr;
     pr->d_stream = nullptr;
     pr->d_sp_ops = nullptr;
     pr->d_cta = nullptr;
@@ -665,6 +706,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   std::vector<std::pair<const void*, size_t>> ext_res;   // external residuals: no op of the program may write them
   std::vector<b200awq_rope_t> ropes;   // per table entry: the ROPE_KV folded into it (head_dim == 0: none)
   std::vector<int> rope_ops;           // table entries that carry one
+  std::vector<b200awq_qk_norm_rope_t> qkns;   // per table entry: a QK_NORM_ROPE_KV's descriptor (q_norm_weight == null:
+                                              // none, or a plain ROPE_KV)
   for (int i = 0; i < n; ++i) {
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
@@ -676,12 +719,17 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         if (res[j].raw_y != nullptr && overlaps(res[j].raw_y, rows_bytes(table[j].N), p, bytes)) return true;
       return false;
     };
-    if (op.kind == B200AWQ_OP_ROPE_KV) {
-      // RoPE + cache append, folded into the finish of the linear recorded just before it (whose whole output is qkv)
-      const b200awq_rope_t* r = static_cast<const b200awq_rope_t*>(op.weight);
+    if (op.kind == B200AWQ_OP_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV) {
+      // RoPE + cache append, folded into the finish of the linear recorded just before it (whose whole output is qkv);
+      // QK_NORM_ROPE_KV: the same op on its embedded descriptor, with q / k normalised first
+      const bool qkn = op.kind == B200AWQ_OP_QK_NORM_ROPE_KV;
+      const b200awq_qk_norm_rope_t* qd = qkn ? static_cast<const b200awq_qk_norm_rope_t*>(op.weight) : nullptr;
+      const b200awq_rope_t* r = qkn ? (qd != nullptr ? &qd->rope : nullptr) : static_cast<const b200awq_rope_t*>(op.weight);
       if (op.x == nullptr) return B200AWQ_EINVAL;
       const int v = rope_validate(r, M > 1 ? op.ldx : INT64_MAX);   // (one row: no pitch; N is checked below)
       if (v != B200AWQ_OK) return v;
+      if (qkn && (qd->q_norm_weight == nullptr || qd->k_norm_weight == nullptr)) return B200AWQ_EINVAL;
+      if (qkn && (!aligned16(qd->q_norm_weight) || !aligned16(qd->k_norm_weight))) return B200AWQ_EUNSUPPORTED;
       const int D = r->head_dim;
       if (op.N != (r->n_heads + 2 * r->n_kv_heads) * D || (D % 16) != 0) return B200AWQ_EUNSUPPORTED;
       // (an ADD or a glue op in between: the op before is not a linear; a SPARSE_MOE's entries are not plain linears)
@@ -690,6 +738,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       const ProgOp& pv = table.back();
       if (op.x != pv.y || op.N != pv.N || (M > 1 && op.ldx != op.N)) return B200AWQ_EUNSUPPORTED;
       ropes.back() = *r;
+      if (qkn) qkns.back() = *qd;
       rope_ops.push_back(static_cast<int>(table.size()) - 1);
       continue;
     }
@@ -840,6 +889,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     res.emplace_back();
     ropes.emplace_back();
     std::memset(&ropes.back(), 0, sizeof(b200awq_rope_t));
+    qkns.emplace_back();
+    std::memset(&qkns.back(), 0, sizeof(b200awq_qk_norm_rope_t));
   }
   for (const Glue& gl : glues)
     if (!gl.used) return B200AWQ_EUNSUPPORTED;   // a glue op nobody consumes would never run
@@ -869,19 +920,25 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   // ROPE_KV: the rotated q and the appended cache rows are written in a finish, while other CTAs run later ops.  No
   // other op of the program may read or write them, nor write the position / frequency table the finish reads; the
   // producer must not be a gate|up whose product a SiLU*mul reads (its row would hold silu(gate) * up).
+  // QK_NORM_ROPE_KV: its two norm weights are reads like the position and the frequency table.
   for (int ri : rope_ops) {
     const b200awq_rope_t& r = ropes[ri];
     const size_t cache = ((size_t)(M - 1) * r.cache_batch_stride + (size_t)r.cache_len * r.n_kv_heads * r.head_dim) * 2;
     const std::pair<const void*, size_t> outs[3] = {{r.q_out, (size_t)M * r.n_heads * r.head_dim * 2},
                                                     {r.k_cache, cache}, {r.v_cache, cache}};
-    const std::pair<const void*, size_t> ins[2] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * r.head_dim * 4}};
+    const size_t wn = qkns[ri].q_norm_weight != nullptr ? (size_t)r.head_dim * 2 : 0;   // (null, 0: overlaps nothing)
+    const std::pair<const void*, size_t> ins[4] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * r.head_dim * 4},
+                                                   {qkns[ri].q_norm_weight, wn}, {qkns[ri].k_norm_weight, wn}};
     auto hits_out = [&](const void* p, size_t b) {
       for (const auto& o : outs)
         if (overlaps(o.first, o.second, p, b)) return true;
       return false;
     };
     auto hits_any = [&](const void* p, size_t b) {
-      return hits_out(p, b) || overlaps(ins[0].first, ins[0].second, p, b) || overlaps(ins[1].first, ins[1].second, p, b);
+      if (hits_out(p, b)) return true;
+      for (const auto& in : ins)
+        if (overlaps(in.first, in.second, p, b)) return true;
+      return false;
     };
     if (overlaps(outs[0].first, outs[0].second, outs[1].first, outs[1].second) ||
         overlaps(outs[0].first, outs[0].second, outs[2].first, outs[2].second) ||
@@ -945,7 +1002,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   pr->n_ops = nt;
   pr->M = M;
   cudaError_t e = cudaGetDevice(&pr->device);
-  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes)) {
+  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes, qkns)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -979,6 +1036,15 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     cfg.numAttrs = 1;
     const SpOp* sops = p->d_sp_ops;
     const uint32_t* cta = p->d_cta;
+    if (p->d_qkn != nullptr) {   // a QK_NORM_ROPE_KV op: the rope kernel plus the two-phase q / k norm
+      auto nk = sb_mt(p->M) == 2 ? stream_batch_qknorm_kernel<2>
+                                 : (sb_mt(p->M) == 4 ? stream_batch_qknorm_kernel<4> : stream_batch_qknorm_kernel<8>);
+      const SpRes* rd = p->d_res;
+      const SpRope* qd = p->d_rope;
+      const SpQkNorm* nd = p->d_qkn;
+      return cudaLaunchKernelEx(&cfg, nk, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
+                                p->sb_lmax, p->sb_nu_max, knob(3), rd, qd, nd);
+    }
     if (p->d_rope != nullptr) {  // a ROPE_KV op: the residual kernel plus the rope steps of a mode-2 finish
       auto qk = sb_mt(p->M) == 2 ? stream_batch_rope_kernel<2>
                                  : (sb_mt(p->M) == 4 ? stream_batch_rope_kernel<4> : stream_batch_rope_kernel<8>);
@@ -1030,6 +1096,14 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
   // 1 = strictly gated)
   const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
   const SpMoe* no_moe = nullptr;
+  if (p->d_qkn != nullptr) {    // programs with a QK_NORM_ROPE_KV op (with or without other ROPE_KV ops, adds, MoE blocks)
+    const SpMoe* md = p->d_moe;
+    const SpRes* rd = p->d_res;
+    const SpRope* qd = p->d_rope;
+    const SpQkNorm* nd = p->d_qkn;
+    return cudaLaunchKernelEx(&cfg, stream_qknorm_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
+                              knob(3), l2_ahead, gate_ahead, md, rd, qd, nd);
+  }
   if (p->d_rope != nullptr) {   // programs with a ROPE_KV op (with or without adds / sparse-MoE blocks)
     const SpMoe* md = p->d_moe;
     const SpRes* rd = p->d_res;
@@ -1065,6 +1139,8 @@ void program_destroy(Program* p) {
   cudaFree(p->d_moe);
   cudaFree(p->d_res);
   cudaFree(p->d_rope);
+  cudaFree(p->d_qkn);
+  cudaFree(p->d_qkn_part);
   delete p;
 }
 

@@ -168,4 +168,22 @@ __global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
 #undef SP_RESIDUAL
 }
 
+// batched programs with a QK_NORM_ROPE_KV op (SpQkNorm, program_stream.cuh): the rope kernel plus the two-phase q / k
+// norm of the mode-2 finish (token row m publishes and polls its own partials)
+template <int MT>
+__global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
+    stream_batch_qknorm_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                               uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int M, int spw,
+                               int lmax, int nu_max, int dbg, const SpRes* __restrict__ res,
+                               const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn) {
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_QKNORM 1
+#include "program_batch_body.inc"
+#undef SP_QKNORM
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
 }  // namespace b200awq

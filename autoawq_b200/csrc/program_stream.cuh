@@ -163,6 +163,41 @@ struct SpRope {
   b200awq_rope_t r;
 };
 
+// QK_NORM_ROPE_KV folded into a qkv linear's finish (stream_qknorm_kernel / stream_batch_qknorm_kernel): one entry per
+// kernel op in a side table next to SpRope (whose descriptor is the embedded b200awq_rope_t); part == null on every op
+// without it.  A head's D / 16 sets can sit on different CTAs, so the finish runs in two phases: (a) every CTA publishes
+// the sum-of-squares partial of each of its q / k sets (rope.cuh: qk_set_partial) as one 64-bit word
+// (tag << 32 | float bits) into part[m * N / 16 + set]; (b) for each q / k pair it finishes it polls all partials of the
+// pair's head in set order (its own included), sums them (qk_head_sum), normalises, rotates and appends.  Every CTA
+// publishes before it waits and all CTAs are co-resident (cooperative launch), so no CTA waits on a waiting one.  Each
+// word is written once per run, under the run's tag of the op: nothing needs resetting.
+struct SpQkNorm {
+  b200awq_qk_norm_rope_t q;
+  unsigned long long* part;    // [M][N / 16] published set partials of this op (program-owned)
+  float inv_d;                 // fp32(1 / head_dim), rounded on the host (rope.cuh: qk_norm_rope_pair)
+  int pad_;
+};
+__device__ __forceinline__ void st_relaxed_u64(void* p, unsigned long long v) {
+  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_relaxed_u64(const void* p) {
+  unsigned long long r;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(r) : "l"(p) : "memory");
+  return r;
+}
+// phase (b): the published partial of one set, waited for under the op's tag
+__device__ __forceinline__ float sp_qk_partial(const unsigned long long* p, uint32_t tag, int op) {
+  unsigned long long v = ld_relaxed_u64(p);
+  if ((uint32_t)(v >> 32) != tag) {
+    ProgWatch wd;
+    do {
+      if (wd.tick(kWQkNorm, op)) break;
+      v = ld_relaxed_u64(p);
+    } while ((uint32_t)(v >> 32) != tag);
+  }
+  return __uint_as_float((uint32_t)v);
+}
+
 // set -> original columns (oracle/stream_format.py:set_columns)
 __device__ __forceinline__ void sp_cols(int mode, int N, int s, int g, int& lo, int& hi) {
   if (mode == 0) {
@@ -180,6 +215,29 @@ __device__ __forceinline__ void sp_cols_rot(int D, int s, int g, int& lo, int& h
   const int per_head = D >> 4, h = s / per_head, t = s - h * per_head;
   lo = h * D + 8 * t + g;
   hi = lo + (D >> 1);
+}
+
+// phase (b) of a QK_NORM_ROPE_KV finish (SpQkNorm above), shared by the M = 1 and the batched body: item t of this
+// thread (t = ct, ct + nthr, ... < nsets * per_set; per_set = 8 M) is lane group t % 8 of token row (t % per_set) / 8 of
+// local set t / per_set, whose fp16 pair phase (a) kept in part[(ls * kst + m) * 16 + g] / [.. + 8].
+__device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, int rpos, const float* part, int kst, int ct,
+                                          int nthr, int nsets, int per_set, int set0, int N, uint32_t tag, int op) {
+  const b200awq_rope_t& rp = qn->q.rope;
+  const int per_head = rp.head_dim >> 4, hqk = rp.n_heads + rp.n_kv_heads;
+  for (int t = ct; t < nsets * per_set; t += nthr) {
+    const int ls = t / per_set, r = t - ls * per_set, m = r >> 3, gg = r & 7, hd = (set0 + ls) / per_head;
+    const float* keep = part + ((size_t)ls * kst + m) * 16;
+    int clo, chi;
+    sp_cols_rot(rp.head_dim, set0 + ls, gg, clo, chi);
+    const __half a = __float2half_rn(keep[gg]), b = __float2half_rn(keep[gg + 8]);
+    if (hd >= hqk) {   // v head: not normalised, only appended
+      rope_pair(rp, rpos, m, clo, a, b);
+      continue;
+    }
+    const unsigned long long* hp = qn->part + (size_t)m * (N >> 4) + (size_t)hd * per_head;
+    const float ss = qk_head_sum(per_head, [&](int u) { return sp_qk_partial(hp + u, tag, op); });
+    qk_norm_rope_pair(qn->q, qn->inv_d, rpos, m, clo, a, b, ss);
+  }
 }
 
 // ------------------------------------------------------------------------------------------ re-layout kernel
@@ -459,6 +517,25 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 #define SP_RESIDUAL 1
 #define SP_ROPE 1
 #include "program_stream_body.inc"
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with a QK_NORM_ROPE_KV op (SpQkNorm above): the rope kernel plus the two-phase q / k norm of the
+// mode-2 finish, which only SP_QKNORM compiles in (programs with plain ROPE_KV ops only keep stream_rope_kernel)
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_qknorm_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                         uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                         int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                         const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn) {
+  constexpr int NW = 8, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_QKNORM 1
+#include "program_stream_body.inc"
+#undef SP_QKNORM
 #undef SP_ROPE
 #undef SP_RESIDUAL
 }

@@ -17,7 +17,8 @@ __all__ = [
     "gemm_forward_cuda", "dequantize_weights_cuda", "gemv_forward_cuda", "gemmv2_forward_cuda",
     "gemv_forward_cuda_decode", "gemm_forward_cuda_prefill", "layernorm_forward_cuda", "silu_and_mul",
     "topk_softmax", "moe_alig_block_size", "grouped_gemm_forward",
-    "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "set_knob", "get_knob",
+    "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "qk_norm_descriptor",
+    "set_knob", "get_knob",
     "B200AwqError",
 ]
 
@@ -281,20 +282,57 @@ def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_ou
     return r, q2, M
 
 
-def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None):
+def qk_norm_descriptor(rope, q_norm, k_norm, device):
+    """b200awq_qk_norm_rope_t around a b200awq_rope_t from Qwen3's two Qwen3RMSNorm modules (or None when both are None).
+    Each module needs .weight (float16 [D] on `device`) and .variance_epsilon; the two epsilons must be equal.  Returns
+    (descriptor or None, the tensors it names)."""
+    if q_norm is None and k_norm is None:
+        return None, []
+    if q_norm is None or k_norm is None:
+        raise B200AwqError("b200awq: give both q_norm and k_norm, or neither")
+    D = rope.head_dim
+    ws = []
+    for name, n in (("q_norm", q_norm), ("k_norm", k_norm)):
+        w = getattr(n, "weight", None)
+        if not isinstance(w, torch.Tensor) or not hasattr(n, "variance_epsilon"):
+            raise B200AwqError(f"b200awq: {name} must be a Qwen3RMSNorm (.weight, .variance_epsilon)")
+        w = w.detach()
+        if w.dtype != torch.float16 or tuple(w.shape) != (D,) or not w.is_contiguous() or w.device != device:
+            raise B200AwqError(f"b200awq: {name}.weight must be a contiguous float16 [{D}] tensor on {device}")
+        ws.append(w)
+    eps = float(q_norm.variance_epsilon)
+    if float(k_norm.variance_epsilon) != eps:
+        raise B200AwqError("b200awq: q_norm and k_norm must have the same variance_epsilon")
+    d = _cabi.QkNormRope()
+    d.rope = rope
+    d.q_norm_weight, d.k_norm_weight, d.eps = ws[0].data_ptr(), ws[1].data_ptr(), eps
+    return d, ws
+
+
+def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None, k_norm=None):
     """RoPE.forward on q and k of the fused qkv output and WindowedCache.update_kv of k and v at position *pos
     (awq/modules/fused/attn.py:243-267): writes q_out [M, H, D] and the row `pos` of cache batch entries 0..M-1, nothing
     else (nothing at all when pos is outside the cache or the frequency table).  pos is read on the device: a captured
-    CUDA graph replays at the position stored there.  Returns q_out (allocated when not given)."""
+    CUDA graph replays at the position stored there.  Returns q_out (allocated when not given).
+
+    q_norm / k_norm: Qwen3's two Qwen3RMSNorm modules (attn.py:250-253), both or neither.  With them every q head and
+    every k head is normalised per token before the rotation (b200awq_qk_norm_rope_kv; the head's sum of squares in the
+    fixed order of include/b200awq.h); v heads are not."""
     H = int(n_heads)
     D = (freqs_cis.shape[1] if freqs_cis.dtype == torch.complex64 else freqs_cis.shape[-2]) * 2
     if q_out is None:
         M = qkv.numel() // qkv.shape[-1] if qkv.shape[-1] else 0
         q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
     r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out)
+    qd, _ = qk_norm_descriptor(r, q_norm, k_norm, qkv.device)
+    ld = q2.stride(0) if M > 1 else q2.shape[1]
     with _DeviceGuard(qkv.device):
-        code = lib.b200awq_rope_kv(q2.data_ptr(), q2.stride(0) if M > 1 else q2.shape[1], r, M, _stream(qkv.device))
-    check(code, f"b200awq_rope_kv(M={M}, H={H}, KV={r.n_kv_heads}, D={D})")
+        if qd is None:
+            code = lib.b200awq_rope_kv(q2.data_ptr(), ld, r, M, _stream(qkv.device))
+        else:
+            code = lib.b200awq_qk_norm_rope_kv(q2.data_ptr(), ld, qd, M, _stream(qkv.device))
+    name = "b200awq_rope_kv" if qd is None else "b200awq_qk_norm_rope_kv"
+    check(code, f"{name}(M={M}, H={H}, KV={r.n_kv_heads}, D={D})")
     return q_out
 
 

@@ -33,7 +33,8 @@ program (DESIGN.md 3.5e).  Outside the folding rule `run()` replays per op, with
 (RoPE.forward on q and k, WindowedCache.update_kv of k and v: awq/modules/fused/attn.py:243-267).  It adds no kernel
 op either: it folds into the finish of the qkv linear recorded just before it, so the segment ends with q rotated and
 the cache row written, and attention reads them directly (DESIGN.md 3.5f).  `pos` is a device int32 tensor: advance it
-in place between runs (or graph replays).
+in place between runs (or graph replays).  With `q_norm=` / `k_norm=` (Qwen3's Qwen3RMSNorm modules) it also applies
+Qwen3's per-head q / k norm first, still inside the qkv linear's finish (DESIGN.md 3.5g).
 """
 from __future__ import annotations
 
@@ -131,12 +132,16 @@ class DecodeProgram:
         self._keep += [a, b, out]
         return out
 
-    def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None):
+    def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None,
+                      k_norm=None):
         """RoPE.forward(xq, xk, start_pos = *pos, seqlen = 1) + cache.update_kv(xv, xk) on the fused qkv output (q heads,
         then k heads, then v heads, as get_attention_shapes slices it): writes q_out [M, H, D] (allocated when not given,
         and returned) and row *pos of k_cache / v_cache batch entries 0..M-1, nothing when *pos is outside the cache or
         freqs_cis.  freqs_cis: the RoPE module's complex64 [S_f, D/2] table (any rope_theta / scaling it was built with
-        applies as is).  Partial rotary, q_norm / k_norm and ALiBi are not this op: the caller keeps those steps."""
+        applies as is).  q_norm / k_norm: Qwen3's two Qwen3RMSNorm modules (.weight fp16 [D], .variance_epsilon), both
+        or neither; with them q and k heads are normalised per head before the rotation (ext.rope_kv_cache), and the
+        fused kernel exchanges the heads' sums of squares across CTAs (DESIGN.md 3.5g).  Partial rotary and ALiBi are
+        not this op: the caller keeps those steps."""
         self._no_more()
         self._dev_of(qkv)
         H = int(n_heads)
@@ -154,10 +159,11 @@ class DecodeProgram:
         desc, q2, M = ext.rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out)
         if q2.data_ptr() != qkv.data_ptr():
             raise B200AwqError("b200awq: rope_kv_cache records qkv by address: pass its rows as they are")
+        qdesc, norm_w = ext.qk_norm_descriptor(desc, q_norm, k_norm, self._dev)
         self._ops.append(("rope", dict(qkv=q2, freqs=freqs_cis, pos=pos, k_cache=k_cache, v_cache=v_cache, q_out=q_out,
                                        H=H, KV=desc.n_kv_heads, M=M, N=q2.shape[1],
-                                       ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc)))
-        self._keep += [qkv, q2, freqs_cis, pos, k_cache, v_cache, q_out]
+                                       ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc, qdesc=qdesc)))
+        self._keep += [qkv, q2, freqs_cis, pos, k_cache, v_cache, q_out] + norm_w
         return q_out
 
     @staticmethod
@@ -269,6 +275,9 @@ class DecodeProgram:
             elif kind == "moe":
                 c.kind, c.M, c.K, c.N = _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
+            elif kind == "rope" and o["qdesc"] is not None:
+                c.kind, c.M, c.N, c.ldx = _cabi.OP_QK_NORM_ROPE_KV, o["M"], o["N"], o["ldx"]
+                c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["qdesc"])
             elif kind == "rope":
                 c.kind, c.M, c.N, c.ldx = _cabi.OP_ROPE_KV, o["M"], o["N"], o["ldx"]
                 c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["desc"])
@@ -328,7 +337,8 @@ class DecodeProgram:
     @property
     def launches_per_run(self) -> int:
         """Kernels launched by one run(): 1 when fused (adds and rope_kv_cache included); per op, one per recorded
-        call, 6 per sparse_moe, one torch.add launch per add and one b200awq_rope_kv launch per rope_kv_cache."""
+        call, 6 per sparse_moe, one torch.add launch per add and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch
+        per rope_kv_cache."""
         return 1 if self.fused else sum(6 if kind == "moe" else 1 for kind, _ in self._ops)
 
     def run(self) -> None:
@@ -349,6 +359,10 @@ class DecodeProgram:
                 self._moe_replay(o)
             elif kind == "add":
                 torch.add(o["a"], o["b"], out=o["out"])
+            elif kind == "rope" and o["qdesc"] is not None:
+                with ext._DeviceGuard(dev):
+                    code = lib.b200awq_qk_norm_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["qdesc"], o["M"], ext._stream(dev))
+                check(code, "b200awq_qk_norm_rope_kv")
             elif kind == "rope":
                 with ext._DeviceGuard(dev):
                     code = lib.b200awq_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["M"], ext._stream(dev))

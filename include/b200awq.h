@@ -19,6 +19,7 @@
  *   b200awq_rmsnorm .............. awq_ext.layernorm_forward_cuda   awq/modules/fused/norm.py:33-36
  *   b200awq_silu_and_mul ......... awq_ext.silu_and_mul             awq/modules/fused/moe.py:76
  *   b200awq_rope_kv .............. RoPE.forward + WindowedCache.update_kv   awq/modules/fused/attn.py:53-86,243-267
+ *   b200awq_qk_norm_rope_kv ...... q_norm / k_norm (Qwen3RMSNorm), then as b200awq_rope_kv   attn.py:250-253
  *
  * Tensor layouts (SURVEY.md Appendix A):
  *   GEMM  : qweight [K, N/8] i32 (AWQ interleave), qzeros [K/G, N/8] i32, scales [K/G, N] f16
@@ -245,9 +246,17 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     published row keep the raw qkv values.  B200AWQ_EUNSUPPORTED (the caller replays per op) when the op before it is
  *     not a plain linear (a glue op, an ADD, a gate|up whose product SiLU*mul reads, a SPARSE_MOE) or already carries an
  *     ADD, when N != (H + 2 KV) D or D % 16 != 0, or when any other op of the program reads or writes q_out or the
- *     caches. */
+ *     caches.
+ *
+ *   QK_NORM_ROPE_KV : ROPE_KV preceded by the per-head RMSNorm of q and k that Qwen3's attention applies
+ *                   (Qwen3RMSNorm q_norm / k_norm, awq/modules/fused/attn.py:250-253).  x, M, N as ROPE_KV, weight = a
+ *                   b200awq_qk_norm_rope_t descriptor (below).  As b200awq_qk_norm_rope_kv.
+ *     Folding: exactly ROPE_KV's rules and rejections (on the embedded descriptor), plus B200AWQ_EINVAL for a null norm
+ *     weight and B200AWQ_EUNSUPPORTED for one that is not 16-byte aligned or that an op of the program writes.  A head's
+ *     sums of squares span sets that other CTAs may finish: every CTA publishes the partials of its sets into a buffer
+ *     the program owns, then waits for all partials of each q / k head it finishes (DESIGN.md 3.5g). */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
-       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6 };
+       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -321,6 +330,25 @@ typedef struct b200awq_rope {
 } b200awq_rope_t;
 /* ldqkv: row pitch of qkv in elements (>= (H + 2 KV) D).  `rope` is a host pointer, read at the call. */
 int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream);
+
+/* Qwen3's q_norm / k_norm, then RoPE + KV-cache append (awq/modules/fused/attn.py:250-253, then as b200awq_rope_kv).
+ * For token row m and q or k head h (weight w = q_norm_weight for q heads, k_norm_weight for k heads, both [D] f16):
+ *   r     = rsqrtf(ss * fp32(1/D) + eps)  with ss the head's sum of squares in the fixed order below (fp32);
+ *                                         fp32(1/D) is torch.mean's scale (ss / D exactly for a power-of-two D)
+ *   x'_i  = fp16(w_i * fp16(x_i * r))      (Qwen3RMSNorm.forward on fp16 input)
+ * then the rotation and stores of b200awq_rope_kv on x'.  v heads are not normalised.  Summation order: set t of a head
+ * (t < D/16) holds the pairs (8 t + g, 8 t + g + D/2), g < 8; s_g = a_g^2 + b_g^2; the set partial is the xor
+ * butterfly of the 8 s_g at offsets 4, 2, 1; the head total is the sum of the D/16 set partials in ascending t.
+ * Requires D % 16 == 0.  Nothing is written when *pos is outside [0, min(cache_len, freqs_len)). */
+typedef struct b200awq_qk_norm_rope {
+  b200awq_rope_t rope;
+  const void* q_norm_weight;             /* [D] f16 */
+  const void* k_norm_weight;             /* [D] f16 */
+  float eps;                             /* variance_epsilon, shared by both norms */
+  int32_t pad_;
+} b200awq_qk_norm_rope_t;
+int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
+                            b200awq_stream_t stream);
 
 typedef struct b200awq_program* b200awq_program_t;
 
