@@ -110,6 +110,8 @@ SIGNATURES = {
         [_c_void_p, _c_int, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
          _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p, _c_size_t, _c_void_p],
     ),
+    "b200awq_moe_tc_plan": (_c_int, [_c_void_p, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p, _c_int,
+                                     _c_void_p]),
     "b200awq_comm_create": (_c_int, [_c_int, _c_int, _c_int, ctypes.POINTER(_c_void_p)]),
     "b200awq_comm_ipc_handle": (_c_int, [_c_void_p, _c_void_p]),
     "b200awq_comm_open": (_c_int, [_c_void_p, _c_void_p]),

@@ -380,6 +380,23 @@ int b200awq_grouped_gemm_forward(const void* x, int x_rows_per_token, const int3
     return B200AWQ_EINVAL;
   if ((block_size % 8) != 0) return B200AWQ_EUNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // prefill-sized problems: the grouped wgmma kernel, one token tile per BT slots of an expert's run.  The host sees
+  // only the average run T * topk / E (the per-expert counts live on the device).  Measured on Mixtral-8x7B shapes with a
+  // random router (H100 at 700 W, DESIGN 3.6): the whole MoE block takes 1.02 ms on this kernel from 12 to 24 slots per
+  // expert, against 0.81 / 1.12 / 1.32 / 1.37 ms on the register-staged kernel at 12 / 16 / 20 / 24 and 1.26 - 1.89 ms on
+  // the ring GEMV: the crossover lies between 12 and 16.  20 keeps every call of up to 18.5 slots per expert, the
+  // largest decode-sized shape the GPU tests pin to the other kernels, where it was.  Knob 12 = 3 runs the kernel
+  // regardless, 1 never (tools/moe_prefill_bench.py times both sides of the threshold with these).
+  constexpr int kMoeTcMinAvg = 20;
+  const int mode = knob(12);
+  if (mode != 1 && mode != 2 && moe_tc_supported(K, N, G, block_size, E) &&
+      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(scales)) & 15) == 0 &&
+      (mode == 3 || (int64_t)T * topk >= (int64_t)kMoeTcMinAvg * E)) {
+    const int n_slots = T * topk;
+    return fold(moe_tc_gemm(x, x_rows_per_token == 1 ? 0 : 1, qweight, scales, qzeros, mul_weights ? topk_weights : nullptr,
+                            sorted_ids, expert_ids, num_tokens_post_pad, y, n_slots, topk, sorted_len, E, K, N, G,
+                            block_size, moe_tc_token_tile(n_slots, E), st));
+  }
   const int hbs = sorted_len / 8;
   // decode-sized problems: the persistent TMA-ring GEMV, one job per 8 sorted slots (needs 8 rows of fp32 scratch
   // per job); anything larger, or without a workspace: the register-staged grouped kernel
@@ -396,5 +413,14 @@ int b200awq_grouped_gemm_forward(const void* x, int x_rows_per_token, const int3
   return fold(moe_grouped_gemm(x, x_rows_per_token == 1 ? 0 : 1, qweight, scales, qzeros, topk_weights, sorted_ids,
                                expert_ids, num_tokens_post_pad, y, T * topk, topk, sorted_len, K, N, G, mul_weights,
                                block_size, st));
+}
+
+int b200awq_moe_tc_plan(const int32_t* expert_ids_host, int n_blocks, int block_size, int E, int N, int BT, int sm_count,
+                        int32_t* tiles_out, int max_tiles, int* n_tiles) {
+  if (!expert_ids_host || !tiles_out || !n_tiles || n_blocks < 0 || max_tiles < 0 || sm_count <= 0) return B200AWQ_EINVAL;
+  if (N <= 0 || (N % 8) != 0 || (BT != 32 && BT != 64 && BT != 128)) return B200AWQ_EINVAL;
+  if (block_size <= 0 || (block_size % 16) != 0 || E < 1 || E > 256) return B200AWQ_EUNSUPPORTED;
+  *n_tiles = moe_tc_plan(expert_ids_host, n_blocks, block_size, E, N, BT, tiles_out, max_tiles);
+  return B200AWQ_OK;
 }
 }  // extern "C"

@@ -240,6 +240,17 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
       ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// 16-byte asynchronous copy global -> smem through L2 only (cp.async, not bulk: per-thread addresses, so the rows of a
+// gather may come from anywhere); src_bytes = 0 reads nothing and zero-fills the destination
+__device__ __forceinline__ void cp_async_16(uint32_t saddr, const void* gsrc, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(saddr), "l"(gsrc), "r"(src_bytes) : "memory");
+}
+// One arrival on the mbarrier once every cp.async this thread has issued so far has landed.  .noinc: the arrival is
+// part of the count the barrier was initialised with.  The copies are generic-proxy writes: a reader in the async
+// proxy (wgmma) fences (fence_proxy_async_smem) after its wait on the barrier.
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 // L2 cache policies (createpolicy) for the .L2::cache_hint forms below: evict_first for data that is dead once it has
 // been read, evict_last for data that must stay in L2 until it is read
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {

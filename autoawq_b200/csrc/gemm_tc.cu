@@ -770,6 +770,272 @@ __global__ void __launch_bounds__(TcqCfg<BT>::kThreads, 1)
   }
 }
 
+// ------------------------------------------------------------ grouped (MoE) kernel: one launch over all experts' runs
+// grouped_gemm_forward at prefill sizes: gemm_tc_kernel's tile, pipeline and MMA loop over stacked GEMM-layout experts.
+//   * tile = 128 output features x BT sorted slots of ONE expert; the expert only moves the three weight base pointers
+//     of the A-tile loader, so the A stage stays bit-identical to the dequant kernel;
+//   * the X stage is a GATHER: row j of a tile is slot sorted_ids[pos0 + j], whose activations are x[id / topk] or
+//     x[id] - no tensor map describes that.  Each of the 256 producer threads copies the 16-byte chunk (dt % 8) of rows
+//     dt / 8 + 32 i with cp.async straight into the 128B-swizzled K-major layout the TMA would have written (the XOR is
+//     applied to the destination address), zero-filling padding slots and rows past the run, and arrives on the
+//     stage's `full` barrier through cp.async.mbarrier.arrive.noinc: full = 8 warp arrivals (A tile) + 256 (X rows);
+//   * the work list is built ON THE DEVICE, so routing may change between replays of a captured graph: after
+//     griddepcontrol.wait every CTA scans expert_ids[0 .. num_post_pad / block_size) into the list of runs (maximal
+//     sequences of blocks of one expert) in shared memory; moe_tc_tile() then enumerates (run, n-tile, token tile) with
+//     the token tile fastest - CTAs resident together share an expert's 128-column weight slab in L2 - and a grid
+//     stride.  A token tile never crosses a run; the last one of a run is partial; experts without tokens have no run;
+//   * the epilogue scatters: token column j goes to y[id], times topk_weights[id] in fp32 when asked (one rounding).
+// No split-K and no workspace: calls with fewer tiles than SMs belong to the decode-sized kernels (see the routing).
+constexpr int kMoeTcMaxRuns = 256;   // = the largest E routed here: moe_align_block_size writes one run per used expert
+constexpr size_t kMoeTcTableBytes = (size_t)(2 * kMoeTcMaxRuns + 4) * sizeof(int);   // run_blk[257], run_e[256], n_runs
+
+struct MoeTcParams {
+  const __half* x;
+  const int32_t* qweight;
+  const __half* scales;
+  const int32_t* qzeros;
+  const float* topk_w;   // nullptr: outputs are not multiplied by the routing weight
+  const int* sorted_ids;
+  const int* expert_ids;
+  const int* num_post_pad;
+  __half* y;
+  int n_slots, topk, x_per_slot;
+  int E, K, N, groups, g_shift;
+  int block_size, max_blocks;   // blocks the sorted_ids buffer holds: the scan never trusts *num_post_pad beyond it
+};
+
+struct MoeTcTile {
+  int expert, pos0, rows, nt;   // expert, first sorted position, rows (<= BT), 128-column tile
+};
+struct MoeTcCursor {
+  int run, base;                // tiles that precede `run`
+};
+
+// Tile w of the fixed order (run, n-tile, token tile), walking `c` forward from the previous query (w never
+// decreases).  run_blk[r] .. run_blk[r + 1] are the blocks of run r; a run whose expert is out of range has no tiles.
+// The kernel's three warp roles and b200awq_moe_tc_plan all enumerate through this one function.
+__host__ __device__ inline bool moe_tc_tile(const int* run_blk, const int* run_e, int n_runs, int E, int block_size,
+                                            int n_tiles, int BT, int w, MoeTcCursor& c, MoeTcTile& t) {
+  for (; c.run < n_runs; ++c.run) {
+    const int e = run_e[c.run];
+    const int rows = (e >= 0 && e < E) ? (run_blk[c.run + 1] - run_blk[c.run]) * block_size : 0;
+    const int tt = (rows + BT - 1) / BT;
+    if (w < c.base + tt * n_tiles) {
+      const int local = w - c.base;
+      const int ti = local % tt;
+      t.expert = e;
+      t.nt = local / tt;
+      t.pos0 = run_blk[c.run] * block_size + ti * BT;
+      t.rows = rows - ti * BT < BT ? rows - ti * BT : BT;
+      return true;
+    }
+    c.base += tt * n_tiles;
+  }
+  return false;
+}
+
+template <int BT, int NG>
+__global__ void __launch_bounds__(kTcThreads, 1) moe_tc_kernel(const MoeTcParams p) {
+  using Cfg = TcCfg<BT>;
+  using Loader = GemmLayoutLoaderT<NG>;
+  constexpr int NS = Cfg::kStages;
+  constexpr int kRowsPerThread = BT / 32;   // gathered rows per producer thread and k-step
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* a_base = smem;                                  // NS x 16 KB
+  uint8_t* x_base = smem + (size_t)NS * kAStageBytes;      // NS x BT*128 B
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)NS * Cfg::kStageBytes);
+  uint64_t* full = bars;            // [NS]
+  uint64_t* empty = bars + NS;      // [NS]
+  int* run_blk = reinterpret_cast<int*>(smem + (size_t)NS * Cfg::kStageBytes + 256);   // [kMoeTcMaxRuns + 1]
+  int* run_e = run_blk + kMoeTcMaxRuns + 1;                                            // [kMoeTcMaxRuns]
+  int* s_runs = run_e + kMoeTcMaxRuns;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  pdl_trigger();
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&full[s], 8 + 256);  // one elected arrival per producer warp + every producer thread's gathered rows
+      mbar_init(&empty[s], 8);       // one arrival per consumer warp
+    }
+    fence_mbar_init();
+  }
+  // The routing tables decide WHICH weights are read, and they, the activations and y belong to predecessor kernels:
+  // nothing is loaded before the wait.
+  pdl_wait();
+  if (warp == 0) {
+    int nblk = *p.num_post_pad / p.block_size;
+    nblk = nblk < p.max_blocks ? nblk : p.max_blocks;
+    int n = 0;   // runs found so far
+    for (int i0 = 0; i0 < nblk; i0 += 32) {
+      const int i = i0 + lane;
+      const int e = i < nblk ? p.expert_ids[i] : -1;
+      const bool start = i < nblk && (i == 0 || p.expert_ids[i - 1] != e);
+      const uint32_t m = __ballot_sync(0xffffffffu, start);
+      const int r = n + __popc(m & ((1u << lane) - 1u));
+      if (start && r <= kMoeTcMaxRuns) {
+        run_blk[r] = i;
+        if (r < kMoeTcMaxRuns) run_e[r] = e;
+      }
+      n += __popc(m);
+    }
+    if (lane == 0) {
+      if (n <= kMoeTcMaxRuns) run_blk[n] = nblk;
+      *s_runs = n < kMoeTcMaxRuns ? n : kMoeTcMaxRuns;
+    }
+  }
+  __syncthreads();
+
+  const int n_runs = *s_runs;
+  const int n_tiles = (p.N + kTileN - 1) / kTileN;
+  const int KS = p.K / kBK;
+  auto locate = [&](int w, MoeTcCursor& c, MoeTcTile& t) {
+    return moe_tc_tile(run_blk, run_e, n_runs, p.E, p.block_size, n_tiles, BT, w, c, t);
+  };
+
+  if (warp < 8) {
+    // ================================================================= consumers: wgmma + scatter (2 warpgroups)
+    const int wg = warp >> 2;
+    const uint32_t a_s = smem_u32(a_base) + (uint32_t)wg * kAHalfBytes;
+    const uint32_t x_s = smem_u32(x_base);
+    int stage = 0;
+    uint32_t phase = 0;
+    MoeTcCursor cur{0, 0};
+    MoeTcTile t;
+    for (int w = blockIdx.x; locate(w, cur, t); w += gridDim.x) {
+      float acc[BT / 2];
+#pragma unroll
+      for (int i = 0; i < BT / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int s = 0; s < KS; ++s) {
+        mbar_wait(&full[stage], phase);
+        fence_proxy_async_smem();   // the gathered rows are generic-proxy writes that completed asynchronously
+        wgmma_fence();
+        tc_mma_stage<BT, true>(acc, a_s + (uint32_t)stage * kAStageBytes, x_s + (uint32_t)stage * Cfg::kXStageBytes);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == NS) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+      // accumulator elements 4 j + b (feature n_a) and 4 j + 2 + b (feature n_a + 8): tile row 8 j + 2 (lane % 4) + b
+      const int n_a = t.nt * kTileN + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BT / 8; ++j) {
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          const int m = 8 * j + 2 * (lane & 3) + b;
+          if (m >= t.rows) continue;
+          const int id = p.sorted_ids[t.pos0 + m];
+          if ((unsigned)id >= (unsigned)p.n_slots) continue;   // padding
+          const float v0 = p.topk_w != nullptr ? acc[4 * j + b] * p.topk_w[id] : acc[4 * j + b];
+          const float v1 = p.topk_w != nullptr ? acc[4 * j + 2 + b] * p.topk_w[id] : acc[4 * j + 2 + b];
+          __half* dst = p.y + (int64_t)id * p.N;
+          if (n_a < p.N) dst[n_a] = __float2half_rn(v0);
+          if (n_a + 8 < p.N) dst[n_a + 8] = __float2half_rn(v1);
+        }
+      }
+    }
+  } else {
+    // ================================================================= producers: dequant + activation gather (8 warps)
+    // As in gemm_tc_kernel the (tile, k-step) sequence of the CTA is one stream and the packed words run kPrefetch
+    // k-steps ahead of the dequantisation in a register ring, straight through tile boundaries.
+    constexpr int kPrefetch = Loader::kDepth;
+    const int dt = threadIdx.x - 256;  // 0..255
+    const uint32_t a_base_s = smem_u32(a_base);
+    const uint32_t x_base_s = smem_u32(x_base);
+    Loader ring[kPrefetch];
+    struct Cursor {
+      int w, s;
+      bool valid;
+      MoeTcCursor c;
+      MoeTcTile t;
+    };
+    auto advance = [&](Cursor& c) {   // true when it entered a new tile
+      if (++c.s < KS) return false;
+      c.s = 0;
+      c.w += gridDim.x;
+      c.valid = locate(c.w, c.c, c.t);
+      return c.valid;
+    };
+    // load cursor: the loader reads qweight / scales / qzeros / N / g_shift of a dense layer = this tile's expert
+    TcParams lp;
+    lp.N = p.N;
+    lp.g_shift = p.g_shift;
+    const int64_t NW = p.N >> 3;
+    auto set_expert = [&](int e) {
+      lp.qweight = p.qweight + (int64_t)e * p.K * NW;
+      lp.scales = p.scales + (int64_t)e * p.groups * p.N;
+      lp.qzeros = p.qzeros + (int64_t)e * p.groups * NW;
+    };
+    // store cursor: source row of each gathered tile row (-1: padding slot or past the run, zero-filled)
+    int xrow[kRowsPerThread];
+    auto set_rows = [&](const MoeTcTile& t) {
+#pragma unroll
+      for (int i = 0; i < kRowsPerThread; ++i) {
+        const int j = (dt >> 3) + 32 * i;
+        xrow[i] = -1;
+        if (j < t.rows) {
+          const int id = p.sorted_ids[t.pos0 + j];
+          if ((unsigned)id < (unsigned)p.n_slots) xrow[i] = p.x_per_slot ? id : id / p.topk;
+        }
+      }
+    };
+    Cursor L, S;
+    L.w = S.w = blockIdx.x;
+    L.s = S.s = 0;
+    L.c = S.c = MoeTcCursor{0, 0};
+    L.valid = S.valid = locate(L.w, L.c, L.t);
+    S.t = L.t;
+    if (L.valid) {
+      set_expert(L.t.expert);
+      set_rows(S.t);
+    }
+#pragma unroll
+    for (int d = 0; d < kPrefetch; ++d) {
+      ring[d].init();
+      if (L.valid) {
+        ring[d].load(lp, L.t.nt, L.s * kBK, dt);
+        if (advance(L)) set_expert(L.t.expert);
+      }
+    }
+    int stage = 0;
+    uint32_t phase = 0;
+    while (S.valid) {
+#pragma unroll
+      for (int d = 0; d < kPrefetch; ++d) {
+        if (S.valid) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          // K-major SW128: tile row j at j * 128 B, 16-byte chunk c at (c ^ (j % 8)); j % 8 == (dt / 8) % 8 for every i
+          const uint32_t x_dst = x_base_s + (uint32_t)stage * Cfg::kXStageBytes + (uint32_t)(dt >> 3) * 128u +
+                                 (uint32_t)(((dt & 7) ^ ((dt >> 3) & 7)) << 4);
+          const __half* x_src = p.x + S.s * kBK + (dt & 7) * 8;
+#pragma unroll
+          for (int i = 0; i < kRowsPerThread; ++i) {
+            const bool ok = xrow[i] >= 0;
+            cp_async_16(x_dst + (uint32_t)i * 4096u, x_src + (int64_t)(ok ? xrow[i] : 0) * p.K, ok ? 16u : 0u);
+          }
+          cp_async_mbar_arrive_noinc(&full[stage]);
+          ring[d].store(lp, 0, 0, dt, a_base_s + (uint32_t)stage * kAStageBytes);
+          fence_proxy_async_smem();   // every writer: generic-proxy stores -> visible to the tensor core
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&full[stage]);
+          if (++stage == NS) { stage = 0; phase ^= 1; }
+          if (advance(S)) set_rows(S.t);
+          if (L.valid) {
+            ring[d].load(lp, L.t.nt, L.s * kBK, dt);
+            if (advance(L)) set_expert(L.t.expert);
+          }
+        }
+      }
+    }
+  }
+}
+
 // -------------------------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -1024,6 +1290,102 @@ cudaError_t gemm_tc(const GemmArgs& a, int layout, float* acc_ws, int* tickets, 
     case 1: return dispatch_bt<1>(BT, tm, tmq, p, st);
     default: return dispatch_bt<2>(BT, tm, tmq, p, st);
   }
+}
+
+// ----------------------------------------------------------------------------- grouped (MoE) kernel, host side
+bool moe_tc_supported(int K, int N, int G, int block_size, int E) {
+  const bool g_ok = G == K || (G >= 32 && (G & (G - 1)) == 0);
+  return K > 0 && N > 0 && (K % kBK) == 0 && (N % 8) == 0 && g_ok && (K % G) == 0 && block_size > 0 &&
+         (block_size % 16) == 0 && E >= 1 && E <= kMoeTcMaxRuns;
+}
+
+// Token tile from the average run: a tile wider than the runs multiplies zeros.  The host never sees the per-expert
+// counts (they live on the device and must not be read back).
+int moe_tc_token_tile(int n_slots, int E) {
+  const int avg = n_slots / E;
+  return avg < 48 ? 32 : (avg < 96 ? 64 : 128);
+}
+
+template <int BT, int NG>
+static cudaError_t launch_moe_tc(const MoeTcParams& p, cudaStream_t st) {
+  constexpr size_t smem = TcCfg<BT>::kSmemBytes + kMoeTcTableBytes;
+  static_assert(smem <= 232448, "shared memory per CTA");
+  auto kern = moe_tc_kernel<BT, NG>;
+  static bool attr_set[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    if (dev >= 0 && dev < 64) attr_set[dev] = true;
+  }
+  // the tile count is only known on the device; a run of b blocks has at most b * ceil(block_size / BT) token tiles
+  const int64_t bound = (int64_t)((p.N + kTileN - 1) / kTileN) * p.max_blocks * ((p.block_size + BT - 1) / BT);
+  const int grid = bound < sm_count() ? (int)bound : sm_count();
+  return launch_kernel(kern, dim3(grid), dim3(kTcThreads), smem, st, p);
+}
+
+cudaError_t moe_tc_gemm(const void* x, int x_per_slot, const int32_t* qweight, const void* scales, const int32_t* qzeros,
+                        const float* topk_w, const int* sorted_ids, const int* expert_ids, const int* num_post_pad,
+                        void* y, int n_slots, int topk, int sorted_len, int E, int K, int N, int G, int block_size,
+                        int BT, cudaStream_t st) {
+  if (!moe_tc_supported(K, N, G, block_size, E)) return cudaErrorNotSupported;
+  if (((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(scales)) & 15) != 0) return cudaErrorMisalignedAddress;
+  MoeTcParams p;
+  p.x = reinterpret_cast<const __half*>(x);
+  p.qweight = qweight;
+  p.scales = reinterpret_cast<const __half*>(scales);
+  p.qzeros = qzeros;
+  p.topk_w = topk_w;
+  p.sorted_ids = sorted_ids;
+  p.expert_ids = expert_ids;
+  p.num_post_pad = num_post_pad;
+  p.y = reinterpret_cast<__half*>(y);
+  p.n_slots = n_slots; p.topk = topk; p.x_per_slot = x_per_slot;
+  p.E = E; p.K = K; p.N = N; p.groups = K / G;
+  p.g_shift = 31;
+  if ((G & (G - 1)) == 0) {   // else G == K: one group
+    p.g_shift = 0;
+    while ((1 << p.g_shift) < G) ++p.g_shift;
+  }
+  p.block_size = block_size;
+  p.max_blocks = sorted_len / block_size;
+  if (p.max_blocks == 0 || n_slots == 0) return cudaSuccess;
+  const bool ng2 = G == 32;   // two quantisation groups per 64-row k-step
+  switch (BT) {
+    case 32: return ng2 ? launch_moe_tc<32, 2>(p, st) : launch_moe_tc<32, 1>(p, st);
+    case 64: return ng2 ? launch_moe_tc<64, 2>(p, st) : launch_moe_tc<64, 1>(p, st);
+    case 128: return ng2 ? launch_moe_tc<128, 2>(p, st) : launch_moe_tc<128, 1>(p, st);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+// The kernel's tile list for a host copy of expert_ids: the same run list (built sequentially here, by one warp's
+// ballots there) walked by the same moe_tc_tile().
+int moe_tc_plan(const int32_t* expert_ids, int n_blocks, int block_size, int E, int N, int BT, int32_t* tiles_out,
+                int max_tiles) {
+  int run_blk[kMoeTcMaxRuns + 1], run_e[kMoeTcMaxRuns];
+  int n = 0;
+  for (int i = 0; i < n_blocks; ++i) {
+    if (i > 0 && expert_ids[i - 1] == expert_ids[i]) continue;
+    if (n <= kMoeTcMaxRuns) run_blk[n] = i;
+    if (n < kMoeTcMaxRuns) run_e[n] = expert_ids[i];
+    ++n;
+  }
+  if (n <= kMoeTcMaxRuns) run_blk[n] = n_blocks;
+  const int n_runs = n < kMoeTcMaxRuns ? n : kMoeTcMaxRuns;
+  MoeTcCursor c{0, 0};
+  MoeTcTile t;
+  int w = 0;
+  for (; moe_tc_tile(run_blk, run_e, n_runs, E, block_size, (N + kTileN - 1) / kTileN, BT, w, c, t); ++w) {
+    if (w < max_tiles) {
+      tiles_out[4 * w + 0] = t.expert;
+      tiles_out[4 * w + 1] = t.pos0;
+      tiles_out[4 * w + 2] = t.rows;
+      tiles_out[4 * w + 3] = t.nt;
+    }
+  }
+  return w;
 }
 
 }  // namespace b200awq

@@ -83,6 +83,18 @@ bool gemm_tcq_shape_ok(int M, int K, int N, int G);                       // the
 int gemm_tcq_grid(int n_tiles, int KP, int M, int sms, int mode);         // its work cut (host logic, CPU-testable)
 cudaError_t gemm_tcq_debug_read(void* dst, size_t bytes);   // phase timestamps of the last small-M launch (knob 3 == 9)
 
+// grouped (MoE) tensor-core kernel (gemm_tc.cu): the prefill-size path of grouped_gemm_forward.  BT = token tile (32 /
+// 64 / 128); x_per_slot and the routing tables as moe_grouped_gemm; topk_w == nullptr: no routing-weight multiply.
+bool moe_tc_supported(int K, int N, int G, int block_size, int E);        // the kernel's envelope
+int moe_tc_token_tile(int n_slots, int E);                                // BT the routing picks
+cudaError_t moe_tc_gemm(const void* x, int x_per_slot, const int32_t* qweight, const void* scales, const int32_t* qzeros,
+                        const float* topk_w, const int* sorted_ids, const int* expert_ids, const int* num_post_pad,
+                        void* y, int n_slots, int topk, int sorted_len, int E, int K, int N, int G, int block_size,
+                        int BT, cudaStream_t st);
+// its tile list for a HOST copy of expert_ids (host logic, CPU-testable): 4 ints per tile, returns the tile count
+int moe_tc_plan(const int32_t* expert_ids, int n_blocks, int block_size, int E, int N, int BT, int32_t* tiles_out,
+                int max_tiles);
+
 // decode program (program.cu)
 struct Program;
 // plan (b200awq_program_plan): fold only, for `grid` SMs and a residual window (<= 0: the library's); no CUDA call

@@ -7,11 +7,12 @@
 // The reference's kernels for these live in the un-vendored autoawq-kernels package (vLLM lineage); the contract
 // implemented here is the one its call sites and docstrings define (the test oracle restates it).
 //
-// grouped_gemm, first version: correctness and the decode case (bs = 1: two slots, two experts).  Eight sorted slots
+// grouped_gemm, decode-sized and fallback kernel (bs = 1: two slots, two experts).  Eight sorted slots
 // (half a 16-slot block: one expert) ride through mma.sync.m16n8k16 as the n = 8 dimension, exactly like the M <= 8
 // GEMV (gemv.cu): one CTA = 256 output columns x 8 slots, streaming the expert's K rows in chunks of 512 with
-// register-staged 128-bit loads.  HBM-bound at decode (each active expert's weights are read once per half-block);
-// a tensor-core grouped GEMM for prefill-sized token counts is the next step.
+// register-staged 128-bit loads.  HBM-bound at decode (each active expert's weights are read once per half-block).
+// Prefill-sized token counts run the grouped wgmma kernel instead (moe_tc_kernel, gemm_tc.cu), which reads an expert's
+// weights once per 32 - 128 slots.
 #include "common.cuh"
 #include "gemv_tile.cuh"
 #include "kernels.h"

@@ -104,11 +104,17 @@ int b200awq_silu_and_mul(const void* gate_up, void* out, int rows, int d, b200aw
  * y[id] = x_row(id) . deq(W[expert_ids[pos / block_size]]) (* topk_weights[id] if mul_weights), x_row(id) = x[id /
  * topk] when x_rows_per_token == 1 (x [T, 1, K]) and x[id] when x_rows_per_token == topk (x [T, topk, K]).
  * qweight [E, K, N/8], scales [E, K/G, N], qzeros [E, K/G, N/8] (stacked GEMM layout).  block_size is 16 at the
- * reference's call site (moe.py:54-56) and must be a multiple of 8 here.  Two kernels: with a workspace of
- * b200awq_workspace_bytes(sorted_len, K, N) bytes (zero-initialised, left zero; the per-op workspace serves) and
- * N % 256 == 0, K % 64 == 0, G in {64, 128, K} the persistent TMA-ring GEMV runs one job per 8 sorted slots (the
- * decode case); otherwise a register-staged grouped kernel (K % 512 == 0, N % 32 == 0, G % 64 == 0), else
- * B200AWQ_EUNSUPPORTED.  Knob 12 = 2 forces the second kernel. */
+ * reference's call site (moe.py:54-56) and must be a multiple of 8 here.  Three kernels:
+ *   - prefill-sized calls, T * topk >= 20 * E (an average of 20 slots per expert), with K % 64 == 0, G a power of two
+ *     >= 32 or G == K, block_size % 16 == 0, E <= 256, x and scales 16-byte aligned: the grouped tensor-core kernel
+ *     (wgmma), one tile per 128 output columns x 32 / 64 / 128 sorted slots of one expert.  It builds its tile list on
+ *     the device from expert_ids, which must list every expert's blocks contiguously (as moe_align_block_size
+ *     writes them); no workspace, no host read-back, CUDA-graph capturable with routing that changes between replays.
+ *   - otherwise, with a workspace of b200awq_workspace_bytes(sorted_len, K, N) bytes (zero-initialised, left zero;
+ *     the per-op workspace serves) and N % 256 == 0, K % 64 == 0, G in {64, 128, K}: the persistent TMA-ring GEMV, one
+ *     job per 8 sorted slots (the decode case);
+ *   - otherwise a register-staged grouped kernel (K % 512 == 0, N % 32 == 0, G % 64 == 0), else B200AWQ_EUNSUPPORTED.
+ * Knob 12 = 2 forces the third kernel, 3 the first wherever its shape conditions hold, 1 excludes the first. */
 int b200awq_topk_softmax(const float* gating_output, float* topk_weights, int32_t* topk_ids,
                          int32_t* token_expert_indices, int M, int E, int topk, b200awq_stream_t stream);
 int b200awq_moe_align_block_size(const int32_t* topk_ids, int numel, int num_experts, int block_size,
@@ -119,6 +125,14 @@ int b200awq_grouped_gemm_forward(const void* x, int x_rows_per_token, const int3
                                  const int32_t* expert_ids, const int32_t* num_tokens_post_pad, void* y, int T, int topk,
                                  int sorted_len, int E, int K, int N, int group_size, int mul_weights, int block_size,
                                  void* workspace, size_t workspace_bytes, b200awq_stream_t stream);
+
+/* Host-side tile list of the grouped tensor-core kernel (no GPU needed, no CUDA call): for a HOST copy of the first
+ * n_blocks = num_tokens_post_pad / block_size entries of expert_ids, the tiles in the kernel's order, 4 ints each:
+ * {expert, first sorted position, rows (<= BT), 128-column tile}.  Token tiles of one (expert, column tile) are
+ * adjacent; CTA b of a grid of min(*n_tiles, sm_count) CTAs runs tiles b, b + grid, ...  At most max_tiles tiles are
+ * written; *n_tiles is the full count.  BT in {32, 64, 128}; block_size % 16 == 0 and E <= 256 as the kernel. */
+int b200awq_moe_tc_plan(const int32_t* expert_ids_host, int n_blocks, int block_size, int E, int N, int BT, int sm_count,
+                        int32_t* tiles_out, int max_tiles, int* n_tiles);
 
 /* Host-side plan of the small-M tensor-core kernel (no GPU needed): for a GEMM-layout call of this shape on a device with
  * `sm_count` SMs, *grid = number of CTAs and *pairs_per_tile = K / 128; CTA b owns the contiguous range
@@ -156,7 +170,9 @@ int b200awq_tcq_plan(int M, int K, int N, int group_size, int sm_count, int mode
  *          spills on sm_90)
  *   key 10: decode program gate: 0 = ungated (the default: 1.93 vs 1.98 ms per Llama-3-8B step with 2 = gated one op
  *           ahead, H100 at 400 W), n > 0 = weight loads at most n - 1 ops ahead of the staging
- *   key 12: 2 = grouped_gemm_forward always uses the register-staged grouped kernel
+ *   key 12: grouped_gemm_forward kernel choice: 1 = never the grouped tensor-core kernel (the decode-sized kernels at
+ *           every token count); 2 = always the register-staged grouped kernel; 3 = the grouped tensor-core kernel
+ *           wherever its shape conditions hold, whatever the token count
  *   key 18: 1 = the persistent GEMV uses round 1's split-K epilogue (fp32 REDs, tickets, read-back) also at M = 1,
  *           instead of the packed one (one returning 64-bit atomic per element; bit-reproducible)
  *   key 17: 1 = b200awq_comm_all_reduce uses the flag protocol (push, fence, flag, wait, reduce) instead of the default
