@@ -69,7 +69,7 @@ class QkNormRope(ctypes.Structure):
 
 
 OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV = 1, 2, 3, 4, 5, 6
-OP_QK_NORM_ROPE_KV = 7
+OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE = 7, 8
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -123,6 +123,7 @@ SIGNATURES = {
     "b200awq_program_tokens": (_c_int, [_c_void_p]),
     "b200awq_program_plan": (_c_int, [ctypes.POINTER(Op), _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
+    "b200awq_qwen3_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_program_num_ops": (_c_int, [_c_void_p]),
     "b200awq_program_kind": (_c_int, [_c_void_p]),
     "b200awq_stream_bytes": (_c_size_t, [_c_int, _c_int, _c_int]),

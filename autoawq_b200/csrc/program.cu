@@ -120,7 +120,8 @@ struct ProgWatch {
 enum { kWEmpty = 3 /* producer: a free ring stage */, kWFull = 4 /* consumer: a landed ring stage */,
        kWCopy = 10 /* staging: the source row's tagged words */, kWRoute = 13 /* producer: a MoE block's routing */,
        kWResidual = 14 /* finish: the tagged row of a residual add's source op */,
-       kWQkNorm = 15 /* finish: a q / k head's tagged sum-of-squares partials (QK_NORM_ROPE_KV) */ };
+       kWQkNorm = 15 /* finish: a q / k head's tagged sum-of-squares partials (QK_NORM_ROPE_KV) */,
+       kWLogit = 16 /* routing: a QWEN3_MOE block's tagged router logits, published across the grid */ };
 // returns false when the wait was abandoned (abort): the caller must not touch the barrier's stage any more
 __device__ __forceinline__ bool prog_mbar_wait(uint64_t* bar, uint32_t parity, int code, int op) {
   ProgWatch wd;
@@ -157,6 +158,8 @@ struct Program {
   // sparse-MoE blocks (stream_moe_kernel): their descriptors
   SpMoe* d_moe = nullptr;
   int n_moe = 0;
+  unsigned long long* d_xlog = nullptr;   // QWEN3_MOE blocks: their published router logits ([E] words per block)
+  bool qwen3 = false;                      // QWEN3_MOE blocks: stream_qwen3moe_kernel
   // residual adds (stream_residual_kernel / stream_batch_residual_kernel): one SpRes per kernel op, null without adds
   SpRes* d_res = nullptr;
   // ROPE_KV ops (stream_rope_kernel / stream_batch_rope_kernel): one SpRope per kernel op, null without them (d_res is
@@ -182,11 +185,12 @@ struct MoeFold {
   int mi = -1;
 };
 
-// Envelope and partition of a sparse-MoE block in an M = 1 stream program (host only, see b200awq_moe_plan)
-int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
+// Envelope and partition of a sparse-MoE block in an M = 1 stream program (host only, see b200awq_moe_plan); e_max:
+// the experts the block's routing handles (kSpMoeEMax for SPARSE_MOE, kSpQwenEMax for QWEN3_MOE)
+static int moe_plan_e(int e_max, int E, int topk, int H, int I, int G, int grid, int* out8) {
   if (E <= 0 || topk <= 0 || topk > E || H <= 0 || I <= 0 || G <= 0 || grid <= 0 || out8 == nullptr)
     return B200AWQ_EINVAL;
-  if (E > kSpMoeEMax || topk > kSpMoeKMax) return B200AWQ_EUNSUPPORTED;
+  if (E > e_max || topk > kSpMoeKMax) return B200AWQ_EUNSUPPORTED;
   if (!stream_format_supported(H, 2 * I, G, 1) || !stream_format_supported(I, H, G, 0)) return B200AWQ_EUNSUPPORTED;
   const int UK = G < 128 ? G : 128;
   const int sets_a = topk * (2 * I / 16), nu_a = H / UK;
@@ -207,6 +211,12 @@ int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
   out8[6] = lmax_b;                    // down: most (set, slot) partial rows one CTA keeps
   out8[7] = (int)smem;                 // dynamic shared memory of the kernel for this block alone
   return B200AWQ_OK;
+}
+int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
+  return moe_plan_e(kSpMoeEMax, E, topk, H, I, G, grid, out8);
+}
+int qwen3_moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
+  return moe_plan_e(kSpQwenEMax, E, topk, H, I, G, grid, out8);
 }
 
 size_t stream_format_bytes(int K, int N, int G) {
@@ -266,16 +276,20 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
 static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
                          const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes,
                          const std::vector<ResFold>& res, const std::vector<b200awq_rope_t>& ropes,
-                         const std::vector<b200awq_qk_norm_rope_t>& qkns) {
+                         const std::vector<b200awq_qk_norm_rope_t>& qkns, const std::vector<int>& moe_hf) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
   const bool has_moe = !moes.empty();
   if (has_moe && M != 1) return false;
+  const bool has_hf = std::find(moe_hf.begin(), moe_hf.end(), 1) != moe_hf.end();
+  // a QWEN3_MOE program runs stream_qwen3moe_kernel, whose MoE blocks are all QWEN3_MOE blocks
+  if (has_hf && std::find(moe_hf.begin(), moe_hf.end(), 0) != moe_hf.end()) return false;
   std::vector<int> plan_a(moes.size() * 8);
   for (size_t b = 0; b < moes.size(); ++b) {
     const b200awq_moe_t& m = moes[b];
-    if (moe_plan(m.E, m.top_k, m.H, m.I, m.group_size, grid, &plan_a[b * 8]) != B200AWQ_OK) return false;
+    if ((moe_hf[b] ? qwen3_moe_plan : moe_plan)(m.E, m.top_k, m.H, m.I, m.group_size, grid, &plan_a[b * 8]) != B200AWQ_OK)
+      return false;
   }
   // creation is a load-time step (not capturable): whatever produced the checkpoint tensors on any stream is done
   // before the re-layout reads them
@@ -454,6 +468,12 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
                       table[i].G, mode[i], nullptr);
   }
   if (e == cudaSuccess && has_moe) {
+    // QWEN3_MOE blocks: [E] logit words each, zero (no run's tag) until the first run
+    size_t xwords = 0;
+    for (size_t b = 0; b < moes.size(); ++b) xwords += moe_hf[b] ? (size_t)moes[b].E : 0;
+    if (xwords > 0) e = cudaMalloc(&pr->d_xlog, xwords * sizeof(unsigned long long));
+    if (e == cudaSuccess && xwords > 0) e = cudaMemset(pr->d_xlog, 0, xwords * sizeof(unsigned long long));
+    size_t xoff = 0;
     std::vector<SpMoe> md(moes.size());
     for (size_t b = 0; b < moes.size(); ++b) {
       const b200awq_moe_t& m = moes[b];
@@ -476,17 +496,21 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       d.seg_a = plan_a[b * 8 + 2];
       d.seg_b = plan_a[b * 8 + 5];
       d.I = m.I;
+      if (moe_hf[b]) {
+        d.xlog = pr->d_xlog + xoff;
+        xoff += (size_t)m.E;
+      }
       for (int i = 0; i < n; ++i)
         if (moe_kind(i) != 0 && fold[i].mi == (int)b) (moe_kind(i) == 1 ? d.eb_a : d.eb_b) = (long long)expert_bytes(i);
     }
-    e = cudaMalloc(&pr->d_moe, md.size() * sizeof(SpMoe));
+    if (e == cudaSuccess) e = cudaMalloc(&pr->d_moe, md.size() * sizeof(SpMoe));
     if (e == cudaSuccess) e = cudaMemcpy(pr->d_moe, md.data(), md.size() * sizeof(SpMoe), cudaMemcpyHostToDevice);
     pr->n_moe = static_cast<int>(md.size());
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(stream_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)(227 * 1024));
   }
-  if (e == cudaSuccess && (has_res || has_rope)) {
+  if (e == cudaSuccess && (has_res || has_rope || has_hf)) {
     std::vector<SpRes> rd(n);
     for (int i = 0; i < n; ++i) {
       std::memset(&rd[i], 0, sizeof(SpRes));
@@ -509,14 +533,14 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   }
   bool has_qkn = false;
   for (int i = 0; i < n && !qkns.empty(); ++i) has_qkn = has_qkn || qkns[i].q_norm_weight != nullptr;
-  if (e == cudaSuccess && has_qkn) {
+  if (e == cudaSuccess && (has_qkn || has_hf)) {
     // the partials of op i live at [M][N_i / 16] words from its offset; zero tags are never a run's (sp_tag >= 1)
     std::vector<SpQkNorm> qd(n);
     size_t words = 0;
     for (int i = 0; i < n; ++i)
       if (qkns[i].q_norm_weight != nullptr) words += (size_t)M * (table[i].N / 16);
-    e = cudaMalloc(&pr->d_qkn_part, words * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMemset(pr->d_qkn_part, 0, words * sizeof(unsigned long long));
+    if (words > 0) e = cudaMalloc(&pr->d_qkn_part, words * sizeof(unsigned long long));
+    if (e == cudaSuccess && words > 0) e = cudaMemset(pr->d_qkn_part, 0, words * sizeof(unsigned long long));
     size_t off = 0;
     for (int i = 0; i < n; ++i) {
       std::memset(&qd[i], 0, sizeof(SpQkNorm));
@@ -537,9 +561,9 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   }
-  if (e == cudaSuccess && has_rope) {
+  if (e == cudaSuccess && (has_rope || has_hf)) {
     std::vector<SpRope> rp(n);
-    for (int i = 0; i < n; ++i) rp[i].r = ropes[i];
+    for (int i = 0; i < n; ++i) rp[i].r = ropes[i];   // (head_dim 0: no rotation)
     e = cudaMalloc(&pr->d_rope, (size_t)n * sizeof(SpRope));
     if (e == cudaSuccess) e = cudaMemcpy(pr->d_rope, rp.data(), (size_t)n * sizeof(SpRope), cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
@@ -553,6 +577,8 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   }
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_sp_ops, ops.data(), (size_t)n * sizeof(SpOp), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(pr->d_cta, cta.data(), cta.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && has_hf)
+    e = cudaFuncSetAttribute(stream_qwen3moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(stream_program_kernel<8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
   if (e == cudaSuccess)
@@ -573,6 +599,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     cudaFree(pr->d_rows);
     cudaFree(pr->d_state);
     cudaFree(pr->d_moe);
+    cudaFree(pr->d_xlog);
     cudaFree(pr->d_res);
     cudaFree(pr->d_rope);
     cudaFree(pr->d_qkn);
@@ -587,11 +614,13 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     pr->d_rows = nullptr;
     pr->d_state = nullptr;
     pr->d_moe = nullptr;
+    pr->d_xlog = nullptr;
     pr->n_moe = 0;
     *err = e;
     return false;
   }
   pr->stream_bytes = wbytes;
+  pr->qwen3 = has_hf;
   pr->xs_bytes = (size_t)max_K * (M == 1 ? 1 : sb_mt(M)) * 2;   // M = 1: one row (stream_program_kernel)
   return true;
 }
@@ -628,15 +657,16 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   *cuda_err = cudaSuccess;
   *out = nullptr;
   if (ops_in == nullptr || n_in <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
-  // A SPARSE_MOE op folds as two linears: gate|up (x [H] -> the recorded gate_up [top_k, 2I], N = top_k 2I) and down
+  // A SPARSE_MOE or QWEN3_MOE op folds as two linears: gate|up (x [H] -> the recorded gate_up [top_k, 2I], N = top_k 2I) and down
   // (the recorded activations [top_k, I] -> y [H], K = top_k I); the hazard rules below then see every buffer they touch.
   // Only the stream kernel runs them (M = 1; stream_build checks the envelope); otherwise the caller replays per op.
   std::vector<b200awq_op_t> xops;
   std::vector<MoeFold> xfold;
   std::vector<b200awq_moe_t> moes;
+  std::vector<int> moe_hf;       // per block: 1 for QWEN3_MOE (the same folding, Qwen3-MoE's routing and finishes)
   for (int i = 0; i < n_in; ++i) {
     const b200awq_op_t& op = ops_in[i];
-    if (op.kind != B200AWQ_OP_SPARSE_MOE) {
+    if (op.kind != B200AWQ_OP_SPARSE_MOE && op.kind != B200AWQ_OP_QWEN3_MOE) {
       xops.push_back(op);
       xfold.push_back(MoeFold{});
       continue;
@@ -655,6 +685,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (op.M != 1) return B200AWQ_EUNSUPPORTED;
     const int mi = static_cast<int>(moes.size());
     moes.push_back(*m);
+    moe_hf.push_back(op.kind == B200AWQ_OP_QWEN3_MOE ? 1 : 0);
     b200awq_op_t a;
     std::memset(&a, 0, sizeof(a));
     a.kind = B200AWQ_OP_LINEAR_GEMM;
@@ -1002,7 +1033,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   pr->n_ops = nt;
   pr->M = M;
   cudaError_t e = cudaGetDevice(&pr->device);
-  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes, qkns)) {
+  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes, qkns, moe_hf)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -1096,6 +1127,14 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
   // 1 = strictly gated)
   const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
   const SpMoe* no_moe = nullptr;
+  if (p->qwen3) {    // programs with QWEN3_MOE blocks (every side table allocated)
+    const SpMoe* md = p->d_moe;
+    const SpRes* rd = p->d_res;
+    const SpRope* qd = p->d_rope;
+    const SpQkNorm* nd = p->d_qkn;
+    return cudaLaunchKernelEx(&cfg, stream_qwen3moe_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
+                              spw, knob(3), l2_ahead, gate_ahead, md, rd, qd, nd);
+  }
   if (p->d_qkn != nullptr) {    // programs with a QK_NORM_ROPE_KV op (with or without other ROPE_KV ops, adds, MoE blocks)
     const SpMoe* md = p->d_moe;
     const SpRes* rd = p->d_res;
@@ -1137,6 +1176,7 @@ void program_destroy(Program* p) {
   cudaFree(p->d_rows);
   cudaFree(p->d_state);
   cudaFree(p->d_moe);
+  cudaFree(p->d_xlog);
   cudaFree(p->d_res);
   cudaFree(p->d_rope);
   cudaFree(p->d_qkn);

@@ -67,6 +67,16 @@ static_assert(sizeof(SpOp) == 128, "SpOp layout");
 constexpr int kSpMoeEMax = 64;                    // experts
 constexpr int kSpMoeKMax = 8;                     // top_k
 constexpr int kSpMoeSmem = 512;                   // logits [64] f32, weights [8] f32, ids [8] i32, routed op
+// QWEN3_MOE blocks (stream_qwen3moe_kernel, whose MoE blocks are all of this kind): up to 128 experts.  The logits are
+// not staged in shared memory: CTA c computes the logits e = c mod grid and publishes each as one 64-bit word
+// (tag << 32 | f32 bits of the fp16 value) into xlog[e]; warp 0 of every CTA then polls all E words into registers (lane l: experts l, l + 32, l + 64, l + 96) and runs the routing.
+// Every CTA publishes before it polls and all CTAs are co-resident (cooperative launch); each word has one writer per
+// run, under the run's tag of the op, so nothing is reset.  The routing area keeps its size: its logit slots hold the
+// slots' ascending-expert order (m_ord) instead, which the down finish sums in.
+constexpr int kSpQwenEMax = 128;
+// Finishes of a QWEN3_MOE block (transformers' Qwen3MoeSparseMoeBlock): gate|up publishes fp16(fp16(silu(g)) * u);
+// down rounds each slot's sum to fp16(y), takes c = fp16(y * w16) and adds the slots in ascending expert id with an
+// fp16 rounding after every add (index_add_ per expert).
 struct SpMoe {
   const __half* gate_w;        // router weight [E, H] fp16
   __half* logits;              // [E] fp16 (what nn.Linear returns)
@@ -80,6 +90,8 @@ struct SpMoe {
   long long eb_a, eb_b;        // bytes per expert slice of the gate|up / down stream copies
   int E, topk, renorm, block_size, sorted_len;
   int seg_a, seg_b, I;
+  unsigned long long* xlog;    // QWEN3_MOE: [E] published logits of this block (program-owned; topk_w then points at
+                               // fp16 weights), else null
 };
 
 // Shared memory of the M = 1 stream kernels:
@@ -185,17 +197,22 @@ __device__ __forceinline__ unsigned long long ld_relaxed_u64(const void* p) {
   asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(r) : "l"(p) : "memory");
   return r;
 }
-// phase (b): the published partial of one set, waited for under the op's tag
-__device__ __forceinline__ float sp_qk_partial(const unsigned long long* p, uint32_t tag, int op) {
+// a 64-bit word (tag << 32 | f32 bits) published by another CTA, waited for under the op's tag; `code` names the wait
+// in the abort record (QK_NORM_ROPE_KV's set partials, QWEN3_MOE's router logits)
+__device__ __forceinline__ float sp_tagged_f32(const unsigned long long* p, uint32_t tag, int code, int op) {
   unsigned long long v = ld_relaxed_u64(p);
   if ((uint32_t)(v >> 32) != tag) {
     ProgWatch wd;
     do {
-      if (wd.tick(kWQkNorm, op)) break;
+      if (wd.tick(code, op)) break;
       v = ld_relaxed_u64(p);
     } while ((uint32_t)(v >> 32) != tag);
   }
   return __uint_as_float((uint32_t)v);
+}
+// phase (b): the published partial of one set
+__device__ __forceinline__ float sp_qk_partial(const unsigned long long* p, uint32_t tag, int op) {
+  return sp_tagged_f32(p, tag, kWQkNorm, op);
 }
 
 // set -> original columns (oracle/stream_format.py:set_columns)
@@ -450,7 +467,7 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 // MOE kernel: the routing area in shared memory, right behind the fixed part
 struct SpMoeSmem {
-  float* m_logit;      // [64] widened fp16 logits
+  float* m_logit;      // [64] widened fp16 logits (QWEN3_MOE: int [8] ascending-expert order of the slots)
   float* m_w;          // [8] routing weights
   int* m_ids;          // [8] expert of each slot
   int* routed_op;      // last gate|up op whose routing is in m_w / m_ids (release / acquire at CTA scope)
@@ -535,6 +552,29 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 #define SP_ROPE 1
 #define SP_QKNORM 1
 #include "program_stream_body.inc"
+#undef SP_QKNORM
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with QWEN3_MOE blocks (with or without residual adds, ROPE_KV and QK_NORM_ROPE_KV ops): the qknorm
+// kernel with the Qwen3-MoE routing and finishes, which only SP_QWEN3 compiles in.  Every MoE block of such a program
+// is a QWEN3_MOE block (program_create replays a program that mixes them with SPARSE_MOE per op).  The side tables are
+// always allocated for it (empty entries where an op has no add, rotation or norm).
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_qwen3moe_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                           uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                           int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                           const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn) {
+  constexpr int NW = 8, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_QKNORM 1
+#define SP_QWEN3 1
+#include "program_stream_body.inc"
+#undef SP_QWEN3
 #undef SP_QKNORM
 #undef SP_ROPE
 #undef SP_RESIDUAL

@@ -223,3 +223,43 @@ def fuse_columns(parts: Iterable[PackedGemm]) -> PackedGemm:
     return PackedGemm(torch.cat([p.qweight for p in parts], dim=1).contiguous(),
                       torch.cat([p.qzeros for p in parts], dim=1).contiguous(),
                       torch.cat([p.scales for p in parts], dim=1).contiguous(), bias)
+
+
+def load_stacked_experts(path, prefix: str, E: int, device):
+    """The stacked GEMM-layout experts of one MoE block, read from the shards straight into their stacked tensors:
+    ((w1 qweight [E, H, 2I/8], scales [E, H/G, 2I], qzeros [E, H/G, 2I/8]), (w2 qweight [E, I, H/8], scales, qzeros)),
+    w1 = [gate | up] along N, from `prefix.experts.{e}.{gate,up,down}_proj.*` (Qwen3-MoE / Qwen2-MoE naming).  `path`
+    is a checkpoint directory or file, or a CheckpointIndex.  Each shard is opened once and each tensor is copied into
+    its place as it is read, so the checkpoint's experts are never held twice.  packing.stack_experts builds the same
+    tensors from loaded modules."""
+    from safetensors import safe_open
+
+    index = path if isinstance(path, CheckpointIndex) else CheckpointIndex(path)
+    kinds = ("qweight", "scales", "qzeros")
+    by_file: Dict[str, list] = {}
+    for e in range(E):
+        for proj in ("gate_proj", "up_proj", "down_proj"):
+            for t in kinds:
+                name = f"{prefix}.experts.{e}.{proj}.{t}"
+                if name not in index.files:
+                    raise KeyError(f"{name} is not in the checkpoint")
+                by_file.setdefault(index.files[name], []).append((name, e, proj, t))
+    w1: Dict[str, torch.Tensor] = {}
+    w2: Dict[str, torch.Tensor] = {}
+    for file, names in by_file.items():
+        with safe_open(file, framework="pt", device="cpu") as f:
+            for name, e, proj, t in names:
+                x = f.get_tensor(name)
+                if proj == "down_proj":
+                    if t not in w2:
+                        w2[t] = torch.empty((E,) + tuple(x.shape), dtype=x.dtype, device=device)
+                    w2[t][e].copy_(x)
+                    continue
+                n = x.shape[1]
+                if t not in w1:
+                    w1[t] = torch.empty((E, x.shape[0], 2 * n), dtype=x.dtype, device=device)
+                half = slice(0, n) if proj == "gate_proj" else slice(n, 2 * n)
+                if w1[t].shape[1:] != (x.shape[0], 2 * n):
+                    raise ValueError(f"{name}: shape {tuple(x.shape)} differs from the block's other experts")
+                w1[t][e, :, half].copy_(x)
+    return tuple(w1[t] for t in kinds), tuple(w2[t] for t in kinds)

@@ -109,3 +109,21 @@ def pack_gemv_fast(intweight_nk, zeros_ng, scales_ng, group_size: int):
     qz = torch.zeros_like(qs)
     qz[:, :ng] = -(qs[:, :ng] * zeros_ng.to(torch.float32)).to(torch.float16)
     return pack_gemv_fast_weight(intweight_nk), qs.t().contiguous(), qz.t().contiguous()
+
+
+def stack_experts(block):
+    """(gate_weight, w1, w2, top_k, norm_topk_prob) of a transformers-4.5x-shaped MoE block (Qwen3MoeSparseMoeBlock:
+    `.gate` nn.Linear, `.experts[e].{gate,up,down}_proj` with qweight / scales / qzeros, `.top_k`, `.norm_topk_prob`),
+    in the form DecodeProgram.qwen3_moe takes: w1 = (qweight, scales, qzeros) of [gate | up] concatenated along N and
+    stacked over the experts ([E, H, 2I/8], [E, H/G, 2I], [E, H/G, 2I/8]), w2 = the stacked down_proj tensors (the
+    concatenation and torch.stack of the reference's Mixtral fuser, awq/models/mixtral.py:131-151)."""
+    experts = list(block.experts)
+
+    def cat(a, b):
+        return torch.cat((a, b), dim=1)
+
+    w1 = tuple(torch.stack([cat(getattr(e.gate_proj, t), getattr(e.up_proj, t)) for e in experts], dim=0)
+               for t in ("qweight", "scales", "qzeros"))
+    w2 = tuple(torch.stack([getattr(e.down_proj, t) for e in experts], dim=0) for t in ("qweight", "scales", "qzeros"))
+    return (block.gate.weight.detach().contiguous(), w1, w2, int(block.top_k),
+            bool(getattr(block, "norm_topk_prob", True)))

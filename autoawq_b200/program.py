@@ -24,6 +24,11 @@ bit-identical to an M = 1 program on that token's row.  Without it, M > 1 replay
 at M = 1 the stream kernel runs it as two kernel ops with the routing computed inside (DESIGN.md 3.5d), otherwise
 `run()` replays apply_moe_weights' sequence through ext.  `moe_buffers(i)` returns the block's routing and intermediates.
 
+`qwen3_moe(x, gate_weight, w1, w2, top_k, norm_topk_prob)` records a Qwen3-MoE expert block with the arithmetic of
+transformers' Qwen3MoeSparseMoeBlock (fp16 routing weights, the experts combined in ascending id with fp16 adds); at
+M = 1 the stream kernel runs it as two kernel ops with the router logits exchanged across the grid (DESIGN.md 3.5h).
+`packing.stack_experts(block)` gives its arguments from a loaded block.
+
 `add(a, b)` records the decoder block's residual add (`h = hidden_states + attn_output`, awq/modules/fused/block.py:
 50-52,117-118).  It adds no kernel op: it folds into the epilogue of the linear (or sparse_moe) recorded just before it,
 so a layer splits only at attention - [o + h_in -> h, norm2(h), gate|up, silu, down + h -> out, norm1'(out), qkv'] is one
@@ -180,6 +185,17 @@ class DecodeProgram:
         weight, sum over the slots.  gate_weight: the router's nn.Linear weight [E, H] fp16 (no bias); w1 / w2: the
         stacked GEMM-layout experts of awq/models/mixtral.py:129-151 ([E, H, 2I/8] / [E, I, H/8] qweight).  Returns
         out [M, H] fp16; the routing and the intermediate tensors are the program's (moe_buffers)."""
+        return self._moe(x, gate_weight, w1, w2, top_k, renormalize, False)
+
+    def qwen3_moe(self, x, gate_weight, w1, w2, top_k, norm_topk_prob=True):
+        """Qwen3MoeSparseMoeBlock.forward (transformers 4.5x) on the normed rows x [.., H], arguments as sparse_moe
+        (packing.stack_experts makes them from a block): logits = fp16(x Wg^T), p = softmax_fp32(logits), top_k (ties to
+        the lower expert), w = p_k / sum p_k in fp32 when norm_topk_prob, w16 = fp16(w); then per selected expert in
+        ascending id a = fp16(fp16(silu(g)) u), y = fp16(W2 a), c = fp16(y w16), out = fp16(out + c) from 0.  E <= 128
+        and top_k <= 8 fuse at M = 1.  moe_buffers(i) holds topk_weights as fp16 w16 and down as the per-slot c."""
+        return self._moe(x, gate_weight, w1, w2, top_k, norm_topk_prob, True)
+
+    def _moe(self, x, gate_weight, w1, w2, top_k, renormalize, hf):
         self._no_more()
         self._dev_of(x)
         q1, s1, z1 = self._stacked(w1, "w1")
@@ -202,7 +218,7 @@ class DecodeProgram:
         dev, f16, i32 = x.device, torch.float16, torch.int32
         block = 16                                      # moe_align_block_size's block at moe.py:54-56
         b = dict(logits=torch.empty((M, E), dtype=f16, device=dev),
-                 topk_weights=torch.empty((M, top_k), dtype=torch.float32, device=dev),
+                 topk_weights=torch.empty((M, top_k), dtype=f16 if hf else torch.float32, device=dev),
                  topk_ids=torch.empty((M, top_k), dtype=i32, device=dev),
                  token_expert_indices=torch.empty((M, top_k), dtype=i32, device=dev),
                  sorted_ids=torch.empty((M * top_k + E * (block - 1),), dtype=i32, device=dev),
@@ -224,15 +240,16 @@ class DecodeProgram:
         x2 = x.reshape(M, H)
         self._ops.append(("moe", dict(x=x2, gate_weight=gate_weight, w1=(q1, s1, z1), w2=(q2, s2, z2), top_k=top_k,
                                       renormalize=bool(renormalize), E=E, H=H, I=I, M=M, out=out, raw_w=raw_w,
-                                      buffers=b, desc=d)))
+                                      buffers=b, desc=d, hf=bool(hf))))
         self._keep += [x, x2, gate_weight, q1, s1, z1, q2, s2, z2, out, raw_w] + list(b.values())
         return out.reshape(x.shape)
 
     def moe_buffers(self, i: int = 0) -> dict:
-        """The tensors the i-th recorded sparse_moe op owns (read-only views): logits [M, E] f16, topk_weights [M, top_k]
+        """The tensors the i-th recorded sparse_moe / qwen3_moe op (counted together, in recording order) owns (read-only views): logits [M, E] f16, topk_weights [M, top_k]
         f32 (after the renormalisation), topk_ids / token_expert_indices [M, top_k] i32, sorted_ids / expert_ids /
         num_tokens_post_pad (moe_alig_block_size), gate_up [M, top_k, 2I], act [M, top_k, I], down [M, top_k, H] (per-slot
-        down outputs x routing weight) and out [M, H].  A run overwrites them; the program reads none of them, so writing
+        down outputs x routing weight) and out [M, H].  For a qwen3_moe op topk_weights is the fp16 w16 [M, top_k] and
+        down holds the per-slot fp16(fp16(y) * w16).  A run overwrites them; the program reads none of them, so writing
         into them changes nothing but what the caller reads back."""
         o = [o for kind, o in self._ops if kind == "moe"][i]
         return dict(o["buffers"], out=o["out"])
@@ -258,6 +275,31 @@ class DecodeProgram:
         b["down"].copy_(dn)
         torch.sum(b["down"], dim=1, out=o["out"])
 
+    @staticmethod
+    def _qwen3_moe_replay(o) -> None:
+        """qwen3_moe's arithmetic through ext and torch, into the op's own buffers (no host synchronisation)."""
+        b, M, H, I, k = o["buffers"], o["M"], o["H"], o["I"], o["top_k"]
+        raw = o["raw_w"]
+        torch.matmul(o["x"], o["gate_weight"].t(), out=b["logits"])
+        ext.topk_softmax(raw, b["topk_ids"], b["token_expert_indices"], b["logits"].float())
+        if o["renormalize"]:
+            torch.div(raw, raw.sum(dim=-1, keepdim=True), out=raw)
+        b["topk_weights"].copy_(raw)                    # .half()
+        b["sorted_ids"].fill_(b["topk_ids"].numel())
+        ext.moe_alig_block_size(b["topk_ids"], o["E"], 16, b["sorted_ids"], b["expert_ids"], b["num_tokens_post_pad"])
+        gu = ext.grouped_gemm_forward(o["x"].view(M, 1, H), *o["w1"], raw, b["sorted_ids"], b["expert_ids"],
+                                      b["num_tokens_post_pad"], False, 8)
+        b["gate_up"].copy_(gu)
+        torch.mul(torch.nn.functional.silu(b["gate_up"][..., :I]), b["gate_up"][..., I:], out=b["act"])
+        dn = ext.grouped_gemm_forward(b["act"], *o["w2"], raw, b["sorted_ids"], b["expert_ids"],
+                                      b["num_tokens_post_pad"], False, 8)
+        torch.mul(dn, b["topk_weights"].unsqueeze(-1), out=b["down"])
+        order = torch.sort(b["topk_ids"], dim=-1).indices          # index_add_ per expert, ascending
+        slots = torch.gather(b["down"], 1, order.unsqueeze(-1).expand(M, k, H))
+        o["out"].zero_()
+        for j in range(k):
+            o["out"].add_(slots[:, j])
+
     # ------------------------------------------------------------------ build / run
     def _c_ops(self):
         arr = (Op * len(self._ops))()
@@ -273,7 +315,7 @@ class DecodeProgram:
                 c.kind, c.M, c.K = _cabi.OP_ADD, o["M"], o["K"]
                 c.x, c.weight, c.y = o["a"].data_ptr(), o["b"].data_ptr(), o["out"].data_ptr()
             elif kind == "moe":
-                c.kind, c.M, c.K, c.N = _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
+                c.kind, c.M, c.K, c.N = _cabi.OP_QWEN3_MOE if o["hf"] else _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
             elif kind == "rope" and o["qdesc"] is not None:
                 c.kind, c.M, c.N, c.ldx = _cabi.OP_QK_NORM_ROPE_KV, o["M"], o["N"], o["ldx"]
@@ -330,16 +372,21 @@ class DecodeProgram:
 
     @property
     def kernel_ops(self) -> int:
-        """Ops of the fused kernel: one per linear, two per sparse_moe (gate|up with the routing, down), none per add or
+        """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe (gate|up with the routing, down), none per add or
         rope_kv_cache (they fold into their producer's epilogue); 0 per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
     def launches_per_run(self) -> int:
         """Kernels launched by one run(): 1 when fused (adds and rope_kv_cache included); per op, one per recorded
-        call, 6 per sparse_moe, one torch.add launch per add and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch
-        per rope_kv_cache."""
-        return 1 if self.fused else sum(6 if kind == "moe" else 1 for kind, _ in self._ops)
+        call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), one torch.add launch per add
+        and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
+        kernel (torch.sort, torch.gather), so the kernel count can be higher."""
+        def per_op(kind, o):
+            if kind != "moe":
+                return 1
+            return 6 if not o["hf"] else 15 + o["top_k"] + (2 if o["renormalize"] else 0)
+        return 1 if self.fused else sum(per_op(kind, o) for kind, o in self._ops)
 
     def run(self) -> None:
         if not self._built:
@@ -355,6 +402,8 @@ class DecodeProgram:
                 ext.layernorm_forward_cuda(o["x"], o["weight"], o["out"], o["eps"])
             elif kind == "silu":
                 ext.silu_and_mul(o["out"], o["gate_up"])
+            elif kind == "moe" and o["hf"]:
+                self._qwen3_moe_replay(o)
             elif kind == "moe":
                 self._moe_replay(o)
             elif kind == "add":

@@ -270,9 +270,22 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     Folding: exactly ROPE_KV's rules and rejections (on the embedded descriptor), plus B200AWQ_EINVAL for a null norm
  *     weight and B200AWQ_EUNSUPPORTED for one that is not 16-byte aligned or that an op of the program writes.  A head's
  *     sums of squares span sets that other CTAs may finish: every CTA publishes the partials of its sets into a buffer
- *     the program owns, then waits for all partials of each q / k head it finishes (DESIGN.md 3.5g). */
+ *     the program owns, then waits for all partials of each q / k head it finishes (DESIGN.md 3.5g).
+ *
+ *   QWEN3_MOE     : a Qwen3-MoE expert block as transformers' Qwen3MoeSparseMoeBlock computes it (one token row),
+ *                   x, y, K and weight as SPARSE_MOE (renormalize = norm_topk_prob).  Arithmetic:
+ *                   logits = fp16(x Wg^T); p = softmax_fp32(logits) (topk_softmax's arithmetic); top_k, ties to the lower
+ *                   expert; w = p_k / sum p_k in fp32 when renormalize; w16 = fp16(w).  Then for each selected expert in
+ *                   ASCENDING EXPERT ID: a = fp16(fp16(silu(g)) * u) of its gate|up, y = fp16(W2 a), c = fp16(y * w16),
+ *                   out = fp16(out + c) from out = 0.  The descriptor's buffers hold what SPARSE_MOE's do, except
+ *                   topk_weights, which holds the fp16 w16 [top_k] (the pointer is reinterpreted), and down, which holds
+ *                   the per-slot c.
+ *     Folding: two kernel ops, as SPARSE_MOE.  The router logits are computed once across the grid (CTA c computes the
+ *     logits e = c mod grid) and exchanged through tagged words the program owns; every CTA then runs the routing from
+ *     all E logits (DESIGN.md 3.5h).  Envelope (else B200AWQ_EUNSUPPORTED): SPARSE_MOE's with E <= 128
+ *     (b200awq_qwen3_moe_plan below).  An ADD right after it folds into its down op. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
-       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7 };
+       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -321,6 +334,8 @@ typedef struct b200awq_moe {
  * CTA keeps in the down op, dynamic shared memory of the kernel for this block alone}.  B200AWQ_EUNSUPPORTED outside the
  * envelope above, B200AWQ_EINVAL for bad arguments. */
 int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8);
+/* The same plan for one QWEN3_MOE block: the same out8 layout and envelope, with E <= 128. */
+int b200awq_qwen3_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8);
 
 /* RoPE + KV-cache append of one decode step (awq/modules/fused/attn.py:53-86 RoPE.forward, cache.py:41-46
  * WindowedCache.update_kv).  For token row m < M, head h < H + 2 KV and pair i < D/2, with a = qkv[m, h D + i],
@@ -393,7 +408,7 @@ int b200awq_program_tokens(b200awq_program_t prog);
  * (csrc/program_stream.cuh).  1 (the split-K kernel on the checkpoint layout of earlier versions) is no longer
  * returned. */
 int b200awq_program_kind(b200awq_program_t prog);
-/* number of fused kernel ops (= linear ops, two per SPARSE_MOE op) of the program; 0 for a null handle */
+/* number of fused kernel ops (= linear ops, two per SPARSE_MOE / QWEN3_MOE op) of the program; 0 for a null handle */
 int b200awq_program_num_ops(b200awq_program_t prog);
 /* workspace / workspace_bytes: accepted and ignored (null is fine); the program owns its hand-off rows */
 int b200awq_program_run(b200awq_program_t prog, void* workspace, size_t workspace_bytes, b200awq_stream_t stream);
