@@ -47,6 +47,18 @@ class Moe(ctypes.Structure):
     ]
 
 
+class DeepseekMoe(ctypes.Structure):
+    """b200awq_deepseek_moe_t (include/b200awq.h): the descriptor a DEEPSEEK_MOE op's `weight` points at."""
+
+    _fields_ = [
+        ("moe", Moe), ("scoring", ctypes.c_int32), ("n_group", ctypes.c_int32), ("topk_group", ctypes.c_int32),
+        ("norm_topk_prob", ctypes.c_int32), ("routed_scaling_factor", ctypes.c_float), ("I_s", ctypes.c_int32),
+        ("bias", ctypes.c_void_p), ("ws1_qweight", ctypes.c_void_p), ("ws1_scales", ctypes.c_void_p),
+        ("ws1_qzeros", ctypes.c_void_p), ("ws2_qweight", ctypes.c_void_p), ("ws2_scales", ctypes.c_void_p),
+        ("ws2_qzeros", ctypes.c_void_p), ("shared_out", ctypes.c_void_p),
+    ]
+
+
 class Rope(ctypes.Structure):
     """b200awq_rope_t (include/b200awq.h): the descriptor of b200awq_rope_kv and of a ROPE_KV op's `weight`."""
 
@@ -69,7 +81,7 @@ class QkNormRope(ctypes.Structure):
 
 
 OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV = 1, 2, 3, 4, 5, 6
-OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE = 7, 8
+OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE, OP_DEEPSEEK_MOE = 7, 8, 9
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -124,6 +136,7 @@ SIGNATURES = {
     "b200awq_program_plan": (_c_int, [ctypes.POINTER(Op), _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_qwen3_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
+    "b200awq_deepseek_moe_plan": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_program_num_ops": (_c_int, [_c_void_p]),
     "b200awq_program_kind": (_c_int, [_c_void_p]),
     "b200awq_stream_bytes": (_c_size_t, [_c_int, _c_int, _c_int]),

@@ -263,6 +263,10 @@ int b200awq_qwen3_moe_plan(int E, int top_k, int H, int I, int group_size, int s
   return qwen3_moe_plan(E, top_k, H, I, group_size, sm_count, out8);
 }
 
+int b200awq_deepseek_moe_plan(int E, int top_k, int H, int I, int I_s, int group_size, int sm_count, int* out8) {
+  return deepseek_moe_plan(E, top_k, H, I, I_s, group_size, sm_count, out8);
+}
+
 int b200awq_program_num_ops(b200awq_program_t prog) {
   return prog == nullptr ? 0 : program_num_ops(reinterpret_cast<Program*>(prog));
 }

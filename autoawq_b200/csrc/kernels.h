@@ -107,6 +107,7 @@ int program_m(const Program* p);
 int program_num_ops(const Program* p);
 int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8);   // host only (b200awq_moe_plan)
 int qwen3_moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8);   // host only (b200awq_qwen3_moe_plan)
+int deepseek_moe_plan(int E, int topk, int H, int I, int I_s, int G, int grid, int* out8);   // (b200awq_deepseek_moe_plan)
 cudaError_t program_run(Program* p, cudaStream_t st);
 size_t program_stream_bytes(const Program* p);
 // stream format (program_stream.cuh; oracle/stream_format.py): one-time re-layout of a GEMM-layout linear

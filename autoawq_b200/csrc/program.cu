@@ -121,7 +121,7 @@ enum { kWEmpty = 3 /* producer: a free ring stage */, kWFull = 4 /* consumer: a 
        kWCopy = 10 /* staging: the source row's tagged words */, kWRoute = 13 /* producer: a MoE block's routing */,
        kWResidual = 14 /* finish: the tagged row of a residual add's source op */,
        kWQkNorm = 15 /* finish: a q / k head's tagged sum-of-squares partials (QK_NORM_ROPE_KV) */,
-       kWLogit = 16 /* routing: a QWEN3_MOE block's tagged router logits, published across the grid */ };
+       kWLogit = 16 /* routing: a QWEN3_MOE / DEEPSEEK_MOE block's tagged router logits, published across the grid */ };
 // returns false when the wait was abandoned (abort): the caller must not touch the barrier's stage any more
 __device__ __forceinline__ bool prog_mbar_wait(uint64_t* bar, uint32_t parity, int code, int op) {
   ProgWatch wd;
@@ -160,6 +160,7 @@ struct Program {
   int n_moe = 0;
   unsigned long long* d_xlog = nullptr;   // QWEN3_MOE blocks: their published router logits ([E] words per block)
   bool qwen3 = false;                      // QWEN3_MOE blocks: stream_qwen3moe_kernel
+  SpDsk* d_dsk = nullptr;                  // DEEPSEEK_MOE blocks (stream_deepseek_moe_kernel): one SpDsk per block
   // residual adds (stream_residual_kernel / stream_batch_residual_kernel): one SpRes per kernel op, null without adds
   SpRes* d_res = nullptr;
   // ROPE_KV ops (stream_rope_kernel / stream_batch_rope_kernel): one SpRope per kernel op, null without them (d_res is
@@ -217,6 +218,29 @@ int moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
 }
 int qwen3_moe_plan(int E, int topk, int H, int I, int G, int grid, int* out8) {
   return moe_plan_e(kSpQwenEMax, E, topk, H, I, G, grid, out8);
+}
+// A DEEPSEEK_MOE block (SpDsk in program_stream.cuh): the QWEN3_MOE plan of the routed experts; the shared expert
+// (I_s = nsh I) widens gate|up by 2 I_s / 16 sets and down by I_s / UK units and nsh partial rows per set
+int deepseek_moe_plan(int E, int topk, int H, int I, int I_s, int G, int grid, int* out8) {
+  if (I_s <= 0 || out8 == nullptr) return B200AWQ_EINVAL;
+  const int rc = moe_plan_e(kSpQwenEMax, E, topk, H, I, G, grid, out8);
+  if (rc != B200AWQ_OK) return rc;
+  if ((I_s % I) != 0) return B200AWQ_EUNSUPPORTED;
+  if (!stream_format_supported(H, 2 * I_s, G, 1) || !stream_format_supported(I_s, H, G, 0)) return B200AWQ_EUNSUPPORTED;
+  const int UK = G < 128 ? G : 128;
+  const int sets_a = (topk * 2 * I + 2 * I_s) / 16, kp = topk * I + I_s, sets_b = H / 16;
+  const int lmax_a = (sets_a + grid - 1) / grid, lmax_b = (sets_b + grid - 1) / grid * (topk + I_s / I);
+  // (the routing keeps E weights in the tail of the gate|up op's xsum: H / UK + kSpQwenEMax of its entries)
+  if (kp / UK > kSpXsumMax || H / UK + kSpQwenEMax > kSpXsumMax || lmax_a > kSpLMax || lmax_b > kSpLMax)
+    return B200AWQ_EUNSUPPORTED;
+  const size_t smem = sp_fixed_smem(8, 4, true) + (size_t)(H > kp ? H : kp) * 2;
+  if (smem > (size_t)227 * 1024) return B200AWQ_EUNSUPPORTED;
+  out8[1] = sets_a;
+  out8[3] = lmax_a;
+  out8[4] = kp / UK;
+  out8[6] = lmax_b;
+  out8[7] = (int)smem;
+  return B200AWQ_OK;
 }
 
 size_t stream_format_bytes(int K, int N, int G) {
@@ -276,20 +300,25 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
 static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
                          const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes,
                          const std::vector<ResFold>& res, const std::vector<b200awq_rope_t>& ropes,
-                         const std::vector<b200awq_qk_norm_rope_t>& qkns, const std::vector<int>& moe_hf) {
+                         const std::vector<b200awq_qk_norm_rope_t>& qkns, const std::vector<int>& moe_hf,
+                         const std::vector<b200awq_deepseek_moe_t>& dsks) {
   *err = cudaSuccess;
   const int n = static_cast<int>(table.size());
   if (n >= 60000) return false;
   const bool has_moe = !moes.empty();
   if (has_moe && M != 1) return false;
-  const bool has_hf = std::find(moe_hf.begin(), moe_hf.end(), 1) != moe_hf.end();
-  // a QWEN3_MOE program runs stream_qwen3moe_kernel, whose MoE blocks are all QWEN3_MOE blocks
-  if (has_hf && std::find(moe_hf.begin(), moe_hf.end(), 0) != moe_hf.end()) return false;
+  // moe_hf: 0 SPARSE_MOE, 1 QWEN3_MOE, 2 DEEPSEEK_MOE.  A QWEN3_MOE (DEEPSEEK_MOE) program runs stream_qwen3moe_kernel
+  // (stream_deepseek_moe_kernel), whose MoE blocks are all of that kind
+  const int mkind = moe_hf.empty() ? 0 : moe_hf[0];
+  if (std::find_if(moe_hf.begin(), moe_hf.end(), [&](int k) { return k != mkind; }) != moe_hf.end()) return false;
+  const bool has_hf = mkind != 0, has_ds = mkind == 2;
   std::vector<int> plan_a(moes.size() * 8);
   for (size_t b = 0; b < moes.size(); ++b) {
     const b200awq_moe_t& m = moes[b];
-    if ((moe_hf[b] ? qwen3_moe_plan : moe_plan)(m.E, m.top_k, m.H, m.I, m.group_size, grid, &plan_a[b * 8]) != B200AWQ_OK)
-      return false;
+    const int rc = moe_hf[b] == 2 ? deepseek_moe_plan(m.E, m.top_k, m.H, m.I, dsks[b].I_s, m.group_size, grid, &plan_a[b * 8])
+                                  : (moe_hf[b] ? qwen3_moe_plan : moe_plan)(m.E, m.top_k, m.H, m.I, m.group_size, grid,
+                                                                             &plan_a[b * 8]);
+    if (rc != B200AWQ_OK) return false;
   }
   // creation is a load-time step (not capturable): whatever produced the checkpoint tensors on any stream is done
   // before the re-layout reads them
@@ -315,6 +344,15 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
                                       : stream_format_bytes(m.I, m.H, m.group_size);
     return (b + 255) & ~(size_t)255;
   };
+  // bytes of the shared expert's stream copy of a DEEPSEEK_MOE entry (in front of its expert slices; 0 otherwise)
+  auto shared_bytes = [&](int i) {
+    if (moe_hf[fold[i].mi] != 2) return (size_t)0;
+    const b200awq_moe_t& m = moes[fold[i].mi];
+    const int I_s = dsks[fold[i].mi].I_s;
+    const size_t b = moe_kind(i) == 1 ? stream_format_bytes(m.H, 2 * I_s, m.group_size)
+                                      : stream_format_bytes(I_s, m.H, m.group_size);
+    return (b + 255) & ~(size_t)255;
+  };
   for (int i = 0; i < n; ++i)
     if (moe_kind(i) == 1) mode[i] = 1;
   bool has_rope = false;
@@ -338,7 +376,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     const ProgOp& p = table[i];
     if (moe_kind(i) != 0) {   // envelope checked by moe_plan (per-expert shapes, sets and partial rows per CTA)
       woff[i] = wbytes;
-      wbytes += (size_t)moes[fold[i].mi].E * expert_bytes(i);
+      wbytes += shared_bytes(i) + (size_t)moes[fold[i].mi].E * expert_bytes(i);
     } else {
       if (!stream_format_supported(p.K, p.N, p.G, mode[i] == 2 ? 0 : mode[i])) return false;
       const int UK = p.G < 128 ? p.G : 128;
@@ -454,10 +492,18 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       const b200awq_moe_t& m = moes[fold[i].mi];
       const int K = moe_kind(i) == 1 ? m.H : m.I, N = moe_kind(i) == 1 ? 2 * m.I : m.H, G = m.group_size;
       const int32_t* qw = static_cast<const int32_t*>(table[i].qw_src);
+      const size_t shb = shared_bytes(i);
       for (int x = 0; x < m.E && e == cudaSuccess; ++x)
         e = stream_pack(qw + (size_t)x * K * (N / 8), table[i].scales + (size_t)x * (K / G) * N,
-                        table[i].qzeros + (size_t)x * (K / G) * (N / 8), pr->d_stream + woff[i] + (size_t)x * expert_bytes(i),
-                        K, N, G, mode[i], nullptr);
+                        table[i].qzeros + (size_t)x * (K / G) * (N / 8),
+                        pr->d_stream + woff[i] + shb + (size_t)x * expert_bytes(i), K, N, G, mode[i], nullptr);
+      if (shb != 0 && e == cudaSuccess) {   // DEEPSEEK_MOE: the shared expert's copy, first
+        const b200awq_deepseek_moe_t& d = dsks[fold[i].mi];
+        const bool gu = moe_kind(i) == 1;
+        e = stream_pack(gu ? d.ws1_qweight : d.ws2_qweight, gu ? d.ws1_scales : d.ws2_scales,
+                        gu ? d.ws1_qzeros : d.ws2_qzeros, pr->d_stream + woff[i], gu ? m.H : d.I_s, gu ? 2 * d.I_s : m.H,
+                        G, mode[i], nullptr);
+      }
       continue;
     }
     if (mode[i] == 2)
@@ -509,6 +555,28 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(stream_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)(227 * 1024));
+    if (e == cudaSuccess && has_ds) {
+      std::vector<SpDsk> dd(moes.size());
+      for (size_t b = 0; b < moes.size(); ++b) {
+        const b200awq_deepseek_moe_t& d = dsks[b];
+        SpDsk& x = dd[b];
+        std::memset(&x, 0, sizeof(x));
+        x.bias = d.bias;
+        x.shared_out = static_cast<__half*>(d.shared_out);
+        x.scoring = d.scoring;
+        x.n_group = d.n_group;
+        x.topk_group = d.topk_group;
+        x.norm = d.norm_topk_prob != 0;
+        x.rsf = d.routed_scaling_factor;
+        x.nsh = d.I_s / d.moe.I;
+        for (int i = 0; i < n; ++i)
+          if (moe_kind(i) != 0 && fold[i].mi == (int)b) (moe_kind(i) == 1 ? x.shb_a : x.shb_b) = (long long)shared_bytes(i);
+      }
+      e = cudaMalloc(&pr->d_dsk, dd.size() * sizeof(SpDsk));
+      if (e == cudaSuccess) e = cudaMemcpy(pr->d_dsk, dd.data(), dd.size() * sizeof(SpDsk), cudaMemcpyHostToDevice);
+      if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(stream_deepseek_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    }
   }
   if (e == cudaSuccess && (has_res || has_rope || has_hf)) {
     std::vector<SpRes> rd(n);
@@ -600,6 +668,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     cudaFree(pr->d_state);
     cudaFree(pr->d_moe);
     cudaFree(pr->d_xlog);
+    cudaFree(pr->d_dsk);
     cudaFree(pr->d_res);
     cudaFree(pr->d_rope);
     cudaFree(pr->d_qkn);
@@ -615,6 +684,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     pr->d_state = nullptr;
     pr->d_moe = nullptr;
     pr->d_xlog = nullptr;
+    pr->d_dsk = nullptr;
     pr->n_moe = 0;
     *err = e;
     return false;
@@ -663,15 +733,19 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   std::vector<b200awq_op_t> xops;
   std::vector<MoeFold> xfold;
   std::vector<b200awq_moe_t> moes;
-  std::vector<int> moe_hf;       // per block: 1 for QWEN3_MOE (the same folding, Qwen3-MoE's routing and finishes)
+  std::vector<int> moe_hf;       // per block: 1 for QWEN3_MOE (the same folding, Qwen3-MoE's routing and finishes),
+                                 // 2 for DEEPSEEK_MOE (plus the shared expert: gate|up N and down K grow by it)
+  std::vector<b200awq_deepseek_moe_t> dsks;   // per block: DEEPSEEK_MOE's descriptor (zero for the other kinds)
   for (int i = 0; i < n_in; ++i) {
     const b200awq_op_t& op = ops_in[i];
-    if (op.kind != B200AWQ_OP_SPARSE_MOE && op.kind != B200AWQ_OP_QWEN3_MOE) {
+    if (op.kind != B200AWQ_OP_SPARSE_MOE && op.kind != B200AWQ_OP_QWEN3_MOE && op.kind != B200AWQ_OP_DEEPSEEK_MOE) {
       xops.push_back(op);
       xfold.push_back(MoeFold{});
       continue;
     }
-    const b200awq_moe_t* m = static_cast<const b200awq_moe_t*>(op.weight);
+    const bool ds = op.kind == B200AWQ_OP_DEEPSEEK_MOE;
+    const b200awq_deepseek_moe_t* dd = ds ? static_cast<const b200awq_deepseek_moe_t*>(op.weight) : nullptr;
+    const b200awq_moe_t* m = ds ? (dd != nullptr ? &dd->moe : nullptr) : static_cast<const b200awq_moe_t*>(op.weight);
     if (m == nullptr || op.x == nullptr || op.y == nullptr || m->gate_weight == nullptr || m->w1_qweight == nullptr ||
         m->w1_scales == nullptr || m->w1_qzeros == nullptr || m->w2_qweight == nullptr || m->w2_scales == nullptr ||
         m->w2_qzeros == nullptr || m->logits == nullptr || m->topk_weights == nullptr || m->topk_ids == nullptr ||
@@ -682,10 +756,25 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         (m->H % m->group_size) != 0 || (m->I % m->group_size) != 0 || m->block_size <= 0 ||
         m->sorted_len < m->top_k * op.M + m->E * (m->block_size - 1))
       return B200AWQ_EINVAL;
+    int I_s = 0;
+    if (ds) {
+      if (dd->ws1_qweight == nullptr || dd->ws1_scales == nullptr || dd->ws1_qzeros == nullptr ||
+          dd->ws2_qweight == nullptr || dd->ws2_scales == nullptr || dd->ws2_qzeros == nullptr ||
+          dd->shared_out == nullptr || (dd->scoring == 1 && dd->bias == nullptr))
+        return B200AWQ_EINVAL;
+      if (dd->I_s <= 0 || (dd->I_s % m->group_size) != 0 || (dd->scoring != 0 && dd->scoring != 1) || dd->n_group <= 0 ||
+          (m->E % dd->n_group) != 0 || dd->topk_group <= 0 || dd->topk_group > dd->n_group ||
+          (dd->n_group > 1 && m->E / dd->n_group < 2))
+        return B200AWQ_EINVAL;
+      I_s = dd->I_s;
+    }
     if (op.M != 1) return B200AWQ_EUNSUPPORTED;
     const int mi = static_cast<int>(moes.size());
     moes.push_back(*m);
-    moe_hf.push_back(op.kind == B200AWQ_OP_QWEN3_MOE ? 1 : 0);
+    moe_hf.push_back(ds ? 2 : (op.kind == B200AWQ_OP_QWEN3_MOE ? 1 : 0));
+    dsks.emplace_back();
+    if (ds) dsks.back() = *dd;
+    else std::memset(&dsks.back(), 0, sizeof(b200awq_deepseek_moe_t));
     b200awq_op_t a;
     std::memset(&a, 0, sizeof(a));
     a.kind = B200AWQ_OP_LINEAR_GEMM;
@@ -693,14 +782,14 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     a.group_size = m->group_size;
     b200awq_op_t b = a;
     a.K = m->H;
-    a.N = m->top_k * 2 * m->I;
+    a.N = m->top_k * 2 * m->I + 2 * I_s;
     a.ldx = a.K;
     a.x = op.x;
     a.qweight = m->w1_qweight;
     a.scales = m->w1_scales;
     a.qzeros = m->w1_qzeros;
     a.y = m->gate_up;
-    b.K = m->top_k * m->I;
+    b.K = m->top_k * m->I + I_s;
     b.N = m->H;
     b.ldx = b.K;
     b.x = m->act;
@@ -947,6 +1036,12 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
           overlaps(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4, er.first, er.second) ||
           overlaps(m.num_tokens_post_pad, 4, er.first, er.second))
         return B200AWQ_EUNSUPPORTED;
+    for (const b200awq_deepseek_moe_t& d : dsks)   // (zero for other blocks: overlaps nothing)
+      if (overlaps(d.moe.gate_up, (size_t)(d.moe.top_k * 2 * d.moe.I + 2 * d.I_s) * 2, er.first, er.second) ||
+          overlaps(d.moe.act, (size_t)(d.moe.top_k * d.moe.I + d.I_s) * 2, er.first, er.second) ||
+          overlaps(d.moe.logits, (size_t)d.moe.E * 4, er.first, er.second) ||
+          overlaps(d.shared_out, (size_t)d.moe.H * 2, er.first, er.second))
+        return B200AWQ_EUNSUPPORTED;
   }
   // ROPE_KV: the rotated q and the appended cache rows are written in a finish, while other CTAs run later ops.  No
   // other op of the program may read or write them, nor write the position / frequency table the finish reads; the
@@ -1002,6 +1097,11 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
           hits_any(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4) || hits_any(m.num_tokens_post_pad, 4) ||
           hits_out(m.gate_weight, (size_t)m.E * m.H * 2))
         return B200AWQ_EUNSUPPORTED;
+    for (const b200awq_deepseek_moe_t& d : dsks)
+      if (hits_any(d.moe.gate_up, (size_t)(d.moe.top_k * 2 * d.moe.I + 2 * d.I_s) * 2) ||
+          hits_any(d.moe.act, (size_t)(d.moe.top_k * d.moe.I + d.I_s) * 2) || hits_any(d.moe.logits, (size_t)d.moe.E * 4) ||
+          hits_any(d.shared_out, (size_t)d.moe.H * 2) || hits_out(d.bias, d.bias != nullptr ? (size_t)d.moe.E * 4 : 0))
+        return B200AWQ_EUNSUPPORTED;
   }
   for (int i = 0; i < nt; ++i) {
     // An in-program residual (row j % 4) is read in op i's finish, by the CTA that published those columns in op j (same
@@ -1033,7 +1133,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   pr->n_ops = nt;
   pr->M = M;
   cudaError_t e = cudaGetDevice(&pr->device);
-  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes, qkns, moe_hf)) {
+  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes, qkns, moe_hf, dsks)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -1127,6 +1227,15 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
   // 1 = strictly gated)
   const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
   const SpMoe* no_moe = nullptr;
+  if (p->d_dsk != nullptr) {    // programs with DEEPSEEK_MOE blocks (every side table allocated)
+    const SpMoe* md = p->d_moe;
+    const SpRes* rd = p->d_res;
+    const SpRope* qd = p->d_rope;
+    const SpQkNorm* nd = p->d_qkn;
+    const SpDsk* dd = p->d_dsk;
+    return cudaLaunchKernelEx(&cfg, stream_deepseek_moe_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride,
+                              p->d_state, spw, knob(3), l2_ahead, gate_ahead, md, rd, qd, nd, dd);
+  }
   if (p->qwen3) {    // programs with QWEN3_MOE blocks (every side table allocated)
     const SpMoe* md = p->d_moe;
     const SpRes* rd = p->d_res;
@@ -1177,6 +1286,7 @@ void program_destroy(Program* p) {
   cudaFree(p->d_state);
   cudaFree(p->d_moe);
   cudaFree(p->d_xlog);
+  cudaFree(p->d_dsk);
   cudaFree(p->d_res);
   cudaFree(p->d_rope);
   cudaFree(p->d_qkn);

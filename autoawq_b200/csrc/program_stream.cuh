@@ -94,6 +94,27 @@ struct SpMoe {
                                // fp16 weights), else null
 };
 
+// DEEPSEEK_MOE blocks (stream_deepseek_moe_kernel, whose MoE blocks are all of this kind): the QWEN3_MOE folding and
+// logit exchange (xlog, fp32 logits unrounded) plus one shared expert per block, in a side table indexed like SpMoe
+// (SpMoe keeps its layout, so the other MoE entries compile as before).  The shared expert's intermediate size is
+// I_s = nsh I (DeepSeek's n_shared_experts x moe_intermediate_size), so it runs as nsh more slots of the block's
+// segment length: after the top_k routed slots, in the shared expert's own stream copy (shb bytes, 256-byte aligned,
+// in front of the E expert slices).
+//   gate|up (K = H, N = top_k 2I + 2 I_s): segments q < top_k are routed slots, q >= top_k the shared expert's
+//     (unit u - top_k seg_a of its copy).  They need no routing: the producer issues them before the routed-op word is
+//     released, while the router logits are exchanged.
+//   down (K' = top_k I + I_s, N = H): a set has top_k + nsh partial rows of seg_b units; rows top_k.. read the shared
+//     copy (unit set I_s / UK + (row - top_k) seg_b + j).  The finish sums the shared rows in fp32 and rounds them on
+//     their own to y_s before adding it to the routed sum.
+struct SpDsk {
+  const float* bias;           // e_score_correction_bias [E] (sigmoid), else null
+  __half* shared_out;          // y_s [H]
+  long long shb_a, shb_b;      // bytes of the shared gate|up / down stream copies (in front of the expert slices)
+  int scoring, n_group, topk_group, norm;
+  float rsf;                   // routed_scaling_factor
+  int nsh;                     // I_s / I
+};
+
 // Shared memory of the M = 1 stream kernels:
 //   sdesc [2] SpOp (256 B) | misc (256 B) | MoE routing area (SpMoeSmem, MOE kernels only) |
 //   part [kSpLMax][nw][16] f32 | xsum [kSpXsumMax] f32 | ring [spw][nw] stages | full / empty barriers [spw * nw] each |
@@ -574,6 +595,31 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 #define SP_QKNORM 1
 #define SP_QWEN3 1
 #include "program_stream_body.inc"
+#undef SP_QWEN3
+#undef SP_QKNORM
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with DEEPSEEK_MOE blocks (SpDsk above; with or without residual adds, ROPE_KV and QK_NORM_ROPE_KV
+// ops): the Qwen3-MoE kernel with DeepSeek's routing, the shared expert and its finishes, which only SP_DEEPSEEK
+// compiles in.  Every MoE block of such a program is a DEEPSEEK_MOE block.
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_deepseek_moe_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                               uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                               int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                               const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn,
+                               const SpDsk* __restrict__ dsk) {
+  constexpr int NW = 8, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_QKNORM 1
+#define SP_QWEN3 1
+#define SP_DEEPSEEK 1
+#include "program_stream_body.inc"
+#undef SP_DEEPSEEK
 #undef SP_QWEN3
 #undef SP_QKNORM
 #undef SP_ROPE

@@ -263,3 +263,33 @@ def load_stacked_experts(path, prefix: str, E: int, device):
                     raise ValueError(f"{name}: shape {tuple(x.shape)} differs from the block's other experts")
                 w1[t][e, :, half].copy_(x)
     return tuple(w1[t] for t in kinds), tuple(w2[t] for t in kinds)
+
+
+def load_shared_expert(path, prefix: str, device):
+    """The shared expert of a DeepSeek-MoE block, read next to load_stacked_experts: ((qweight [H, 2 I_s / 8], scales
+    [H/G, 2 I_s], qzeros [H/G, 2 I_s / 8]) of [gate | up] along N, (down qweight [I_s, H/8], scales, qzeros)), from
+    `prefix.shared_experts.{gate,up,down}_proj.*`.  packing.stack_deepseek_experts builds the same tensors from loaded
+    modules."""
+    from safetensors import safe_open
+
+    index = path if isinstance(path, CheckpointIndex) else CheckpointIndex(path)
+    kinds = ("qweight", "scales", "qzeros")
+    got: Dict[str, torch.Tensor] = {}
+    by_file: Dict[str, list] = {}
+    for proj in ("gate_proj", "up_proj", "down_proj"):
+        for t in kinds:
+            name = f"{prefix}.shared_experts.{proj}.{t}"
+            if name not in index.files:
+                raise KeyError(f"{name} is not in the checkpoint")
+            by_file.setdefault(index.files[name], []).append(name)
+    for file, names in by_file.items():
+        with safe_open(file, framework="pt", device="cpu") as f:
+            for name in names:
+                got[name] = f.get_tensor(name)
+
+    def t(proj, k):
+        return got[f"{prefix}.shared_experts.{proj}.{k}"]
+
+    ws1 = tuple(torch.cat((t("gate_proj", k), t("up_proj", k)), dim=1).to(device).contiguous() for k in kinds)
+    ws2 = tuple(t("down_proj", k).to(device).contiguous() for k in kinds)
+    return ws1, ws2

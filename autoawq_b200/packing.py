@@ -127,3 +127,30 @@ def stack_experts(block):
     w2 = tuple(torch.stack([getattr(e.down_proj, t) for e in experts], dim=0) for t in ("qweight", "scales", "qzeros"))
     return (block.gate.weight.detach().contiguous(), w1, w2, int(block.top_k),
             bool(getattr(block, "norm_topk_prob", True)))
+
+
+def stack_deepseek_experts(block):
+    """(gate_weight, w1, w2, top_k, shared, routing) of a DeepSeek-V2 / V3 MoE block in the layout the reference
+    quantises (awq/models/deepseek_v2.py, deepseek_v3.py: `.gate` with `.weight` and, for V3, `.e_score_correction_bias`,
+    `.experts[e].{gate,up,down}_proj` and `.shared_experts.{gate,up,down}_proj` with qweight / scales / qzeros, and the
+    routing config `top_k`, `routed_scaling_factor`, `n_group` (or V2's `num_group`), `topk_group`, `norm_topk_prob`),
+    in the form DecodeProgram.deepseek_moe takes: prog.deepseek_moe(x, gate_weight, w1, w2, top_k, shared, **routing).
+    w1 / w2 as stack_experts; shared = ((qweight, scales, qzeros) of [gate | up] along N, those of down).  A gate with
+    e_score_correction_bias scores with sigmoid (V3), one without with softmax (V2 greedy)."""
+    gate_weight, w1, w2, top_k, _ = stack_experts(block)
+    sh = block.shared_experts
+
+    def cat(t):
+        return torch.cat((getattr(sh.gate_proj, t), getattr(sh.up_proj, t)), dim=1).contiguous()
+
+    shared = (tuple(cat(t) for t in ("qweight", "scales", "qzeros")),
+              tuple(getattr(sh.down_proj, t).contiguous() for t in ("qweight", "scales", "qzeros")))
+    bias = getattr(block.gate, "e_score_correction_bias", None)
+    n_group = int(getattr(block, "n_group", getattr(block, "num_group", 1)) or 1)
+    routing = dict(scoring="sigmoid" if bias is not None else "softmax",
+                   e_score_correction_bias=None if bias is None else bias.detach().float().contiguous(),
+                   n_group=n_group if bias is not None else 1,
+                   topk_group=int(getattr(block, "topk_group", 1) or 1) if bias is not None else 1,
+                   norm_topk_prob=bool(getattr(block, "norm_topk_prob", False)),
+                   routed_scaling_factor=float(getattr(block, "routed_scaling_factor", 1.0)))
+    return gate_weight, w1, w2, top_k, shared, routing

@@ -29,6 +29,13 @@ transformers' Qwen3MoeSparseMoeBlock (fp16 routing weights, the experts combined
 M = 1 the stream kernel runs it as two kernel ops with the router logits exchanged across the grid (DESIGN.md 3.5h).
 `packing.stack_experts(block)` gives its arguments from a loaded block.
 
+`deepseek_moe(x, gate_weight, w1, w2, top_k, shared, scoring, ...)` records a DeepSeek-V2 / V3 expert block
+(transformers' DeepseekV2Moe / DeepseekV3MoE over WQLinear_GEMM experts): fp32 router logits, softmax or sigmoid routing
+with expert groups and the correction bias, fp32 weights, the routed experts combined in ascending id, and the dense
+shared expert added last; at M = 1 the stream kernel runs it as two kernel ops with the shared expert's weights
+streamed while the router logits are exchanged (DESIGN.md 3.5i).  `packing.stack_deepseek_experts(block)` gives its
+arguments from a loaded block.
+
 `add(a, b)` records the decoder block's residual add (`h = hidden_states + attn_output`, awq/modules/fused/block.py:
 50-52,117-118).  It adds no kernel op: it folds into the epilogue of the linear (or sparse_moe) recorded just before it,
 so a layer splits only at attention - [o + h_in -> h, norm2(h), gate|up, silu, down + h -> out, norm1'(out), qkv'] is one
@@ -195,7 +202,29 @@ class DecodeProgram:
         and top_k <= 8 fuse at M = 1.  moe_buffers(i) holds topk_weights as fp16 w16 and down as the per-slot c."""
         return self._moe(x, gate_weight, w1, w2, top_k, norm_topk_prob, True)
 
-    def _moe(self, x, gate_weight, w1, w2, top_k, renormalize, hf):
+    def deepseek_moe(self, x, gate_weight, w1, w2, top_k, shared, scoring, e_score_correction_bias=None, n_group=1,
+                     topk_group=1, norm_topk_prob=False, routed_scaling_factor=1.0):
+        """DeepseekV2Moe / DeepseekV3MoE.forward (transformers 5.5) over WQLinear_GEMM experts on the normed rows
+        x [.., H]; gate_weight, w1, w2, top_k as qwen3_moe; shared = (ws1, ws2): the shared expert's [gate | up] and down
+        as (qweight, scales, qzeros) GEMM-layout tensors (2-D, or stacked with E = 1), intermediate size I_s.
+        l = fp32(x) fp32(Wg)^T.  scoring "softmax" (V2 greedy): p = softmax_fp32(l), top_k (ties to the lower expert),
+        w = p_k * routed_scaling_factor.  scoring "sigmoid" (V3 noaux_tc): s = sigmoid(l), c = s + e_score_correction_bias
+        (fp32 [E]); groups of E / n_group experts score their two largest c, the topk_group best stay and every other c
+        becomes 0.0; top_k of the masked c; w = s_k, / (sum + 1e-20) when norm_topk_prob, * routed_scaling_factor.  Then
+        per selected expert in ascending id a = fp16(fp16(silu(g)) u), y = fp16(W2 a), c = fp16(fp32(y) w),
+        r = fp16(r + c) from 0; y_s = the shared MLP with the same rounding; out = fp16(r + y_s).  E <= 128, top_k <= 8
+        and I_s a multiple of I fuse at M = 1.  moe_buffers(i) holds logits as fp32 [M, E], topk_weights as the fp32 w,
+        gate_up / act with the shared expert's columns after the slots' ([M, top_k 2I + 2 I_s] / [M, top_k I + I_s]),
+        down as the per-slot c and shared_out as y_s."""
+        if scoring not in ("softmax", "sigmoid"):
+            raise B200AwqError(f"b200awq: scoring must be 'softmax' or 'sigmoid', got {scoring!r}")
+        ws1 = tuple(t.reshape(t.shape[-2:]) for t in self._stacked(shared[0], "shared gate|up"))
+        ws2 = tuple(t.reshape(t.shape[-2:]) for t in self._stacked(shared[1], "shared down"))
+        return self._moe(x, gate_weight, w1, w2, top_k, bool(norm_topk_prob), False,
+                         ds=dict(ws1=ws1, ws2=ws2, scoring=scoring, bias=e_score_correction_bias, n_group=int(n_group),
+                                 topk_group=int(topk_group), rsf=float(routed_scaling_factor)))
+
+    def _moe(self, x, gate_weight, w1, w2, top_k, renormalize, hf, ds=None):
         self._no_more()
         self._dev_of(x)
         q1, s1, z1 = self._stacked(w1, "w1")
@@ -216,17 +245,38 @@ class DecodeProgram:
             raise B200AwqError(f"b200awq: sparse_moe expects contiguous float16 rows [.., {H}]")
         M = x.numel() // H
         dev, f16, i32 = x.device, torch.float16, torch.int32
+        I_s = 0
+        if ds is not None:
+            (sq1, ss1, sz1), (sq2, ss2, sz2) = ds["ws1"], ds["ws2"]
+            I_s = sq1.shape[1] * 4
+            for t, dt in ((sq1, torch.int32), (ss1, f16), (sz1, torch.int32), (sq2, torch.int32), (ss2, f16),
+                          (sz2, torch.int32)):
+                ext._require_cuda(t)
+                if t.dtype != dt or not t.is_contiguous():
+                    raise B200AwqError("b200awq: shared expert tensors must be contiguous GEMM-layout int32 / float16")
+            if (tuple(sq1.shape) != (H, 2 * I_s // 8) or tuple(sq2.shape) != (I_s, H // 8) or H // ss1.shape[0] != G
+                    or I_s // ss2.shape[0] != G):
+                raise B200AwqError("b200awq: shared does not describe the block's shared expert")
+            if not 1 <= ds["topk_group"] <= ds["n_group"] or E % ds["n_group"] != 0:
+                raise B200AwqError("b200awq: need E % n_group == 0 and 1 <= topk_group <= n_group")
+            if ds["scoring"] == "sigmoid":
+                bias = ds["bias"]
+                if bias is None or bias.dtype != torch.float32 or tuple(bias.shape) != (E,) or not bias.is_contiguous():
+                    raise B200AwqError(f"b200awq: sigmoid scoring needs e_score_correction_bias, float32 [{E}]")
+                ext._require_cuda(bias)
         block = 16                                      # moe_align_block_size's block at moe.py:54-56
-        b = dict(logits=torch.empty((M, E), dtype=f16, device=dev),
+        b = dict(logits=torch.empty((M, E), dtype=f16 if ds is None else torch.float32, device=dev),
                  topk_weights=torch.empty((M, top_k), dtype=f16 if hf else torch.float32, device=dev),
                  topk_ids=torch.empty((M, top_k), dtype=i32, device=dev),
                  token_expert_indices=torch.empty((M, top_k), dtype=i32, device=dev),
                  sorted_ids=torch.empty((M * top_k + E * (block - 1),), dtype=i32, device=dev),
                  expert_ids=torch.empty((M * top_k + E,), dtype=i32, device=dev),
                  num_tokens_post_pad=torch.empty((1,), dtype=i32, device=dev),
-                 gate_up=torch.empty((M, top_k, 2 * I), dtype=f16, device=dev),
-                 act=torch.empty((M, top_k, I), dtype=f16, device=dev),
+                 gate_up=torch.empty((M, top_k, 2 * I) if ds is None else (M, top_k * 2 * I + 2 * I_s), dtype=f16, device=dev),
+                 act=torch.empty((M, top_k, I) if ds is None else (M, top_k * I + I_s), dtype=f16, device=dev),
                  down=torch.empty((M, top_k, H), dtype=f16, device=dev))
+        if ds is not None:
+            b["shared_out"] = torch.empty((M, H), dtype=f16, device=dev)
         out = torch.empty((M, H), dtype=f16, device=dev)
         raw_w = torch.empty((M, top_k), dtype=torch.float32, device=dev)    # topk_softmax's output (replay)
         d = _cabi.Moe()
@@ -236,11 +286,25 @@ class DecodeProgram:
         d.w1_qweight, d.w1_scales, d.w1_qzeros = q1.data_ptr(), s1.data_ptr(), z1.data_ptr()
         d.w2_qweight, d.w2_scales, d.w2_qzeros = q2.data_ptr(), s2.data_ptr(), z2.data_ptr()
         for k, t in b.items():
-            setattr(d, k, t.data_ptr())
+            if k != "shared_out":
+                setattr(d, k, t.data_ptr())
+        if ds is not None:
+            dd = _cabi.DeepseekMoe()
+            dd.moe = d
+            dd.scoring = 0 if ds["scoring"] == "softmax" else 1
+            dd.n_group, dd.topk_group, dd.norm_topk_prob = ds["n_group"], ds["topk_group"], 1 if renormalize else 0
+            dd.routed_scaling_factor, dd.I_s = ds["rsf"], I_s
+            dd.bias = ds["bias"].data_ptr() if ds["scoring"] == "sigmoid" else None
+            dd.ws1_qweight, dd.ws1_scales, dd.ws1_qzeros = (t.data_ptr() for t in ds["ws1"])
+            dd.ws2_qweight, dd.ws2_scales, dd.ws2_qzeros = (t.data_ptr() for t in ds["ws2"])
+            dd.shared_out = b["shared_out"].data_ptr()
+            d = dd
+            ds = dict(ds, I_s=I_s, G=G)
+            self._keep += list(ds["ws1"]) + list(ds["ws2"]) + ([ds["bias"]] if ds["scoring"] == "sigmoid" else [])
         x2 = x.reshape(M, H)
         self._ops.append(("moe", dict(x=x2, gate_weight=gate_weight, w1=(q1, s1, z1), w2=(q2, s2, z2), top_k=top_k,
                                       renormalize=bool(renormalize), E=E, H=H, I=I, M=M, out=out, raw_w=raw_w,
-                                      buffers=b, desc=d, hf=bool(hf))))
+                                      buffers=b, desc=d, hf=bool(hf), ds=ds)))
         self._keep += [x, x2, gate_weight, q1, s1, z1, q2, s2, z2, out, raw_w] + list(b.values())
         return out.reshape(x.shape)
 
@@ -249,8 +313,9 @@ class DecodeProgram:
         f32 (after the renormalisation), topk_ids / token_expert_indices [M, top_k] i32, sorted_ids / expert_ids /
         num_tokens_post_pad (moe_alig_block_size), gate_up [M, top_k, 2I], act [M, top_k, I], down [M, top_k, H] (per-slot
         down outputs x routing weight) and out [M, H].  For a qwen3_moe op topk_weights is the fp16 w16 [M, top_k] and
-        down holds the per-slot fp16(fp16(y) * w16).  A run overwrites them; the program reads none of them, so writing
-        into them changes nothing but what the caller reads back."""
+        down holds the per-slot fp16(fp16(y) * w16).  A deepseek_moe op's are listed in deepseek_moe (with shared_out,
+        y_s [M, H]).  A run overwrites them; the program reads none of them, so writing into them changes nothing but
+        what the caller reads back."""
         o = [o for kind, o in self._ops if kind == "moe"][i]
         return dict(o["buffers"], out=o["out"])
 
@@ -300,6 +365,56 @@ class DecodeProgram:
         for j in range(k):
             o["out"].add_(slots[:, j])
 
+    @staticmethod
+    def _deepseek_moe_replay(o) -> None:
+        """deepseek_moe's arithmetic through ext and torch, into the op's own buffers (no host synchronisation)."""
+        b, M, H, I, k, E, ds = o["buffers"], o["M"], o["H"], o["I"], o["top_k"], o["E"], o["ds"]
+        I_s, G = ds["I_s"], ds["G"]
+        F = torch.nn.functional
+        torch.matmul(o["x"].float(), o["gate_weight"].float().t(), out=b["logits"])
+        if ds["scoring"] == "softmax":
+            w, ids = torch.topk(b["logits"].softmax(dim=-1), k, dim=-1)
+            w = w * ds["rsf"]
+        else:
+            s = b["logits"].sigmoid()
+            c = s + ds["bias"]
+            if ds["topk_group"] < ds["n_group"]:
+                gs = c.view(M, ds["n_group"], -1).topk(2, dim=-1)[0].sum(dim=-1)
+                gidx = torch.topk(gs, ds["topk_group"], dim=-1)[1]
+                gmask = torch.zeros_like(gs).scatter_(1, gidx, 1).bool()
+                c = c.masked_fill(~gmask.unsqueeze(-1).expand(M, ds["n_group"], E // ds["n_group"]).reshape(M, E), 0.0)
+            ids = torch.topk(c, k, dim=-1)[1]
+            w = s.gather(1, ids)
+            if o["renormalize"]:
+                w = w / (w.sum(dim=-1, keepdim=True) + 1e-20)
+            w = w * ds["rsf"]
+        b["topk_weights"].copy_(w)
+        b["topk_ids"].copy_(ids)
+        b["token_expert_indices"].copy_(torch.arange(k, device=ids.device, dtype=torch.int32) * M +
+                                        torch.arange(M, device=ids.device, dtype=torch.int32).unsqueeze(1))
+        b["sorted_ids"].fill_(b["topk_ids"].numel())
+        ext.moe_alig_block_size(b["topk_ids"], E, 16, b["sorted_ids"], b["expert_ids"], b["num_tokens_post_pad"])
+        tw = b["topk_weights"]
+        gu = ext.grouped_gemm_forward(o["x"].view(M, 1, H), *o["w1"], tw, b["sorted_ids"], b["expert_ids"],
+                                      b["num_tokens_post_pad"], False, 8)
+        gus = ext.linear_forward("gemm", o["x"], *ds["ws1"], G)
+        b["gate_up"][:, :k * 2 * I].copy_(gu.view(M, k * 2 * I))
+        b["gate_up"][:, k * 2 * I:].copy_(gus)
+        act = torch.mul(F.silu(gu[..., :I]), gu[..., I:])
+        act_s = torch.mul(F.silu(gus[:, :I_s]), gus[:, I_s:])
+        b["act"][:, :k * I].copy_(act.view(M, k * I))
+        b["act"][:, k * I:].copy_(act_s)
+        dn = ext.grouped_gemm_forward(act, *o["w2"], tw, b["sorted_ids"], b["expert_ids"], b["num_tokens_post_pad"],
+                                      False, 8)
+        b["down"].copy_(dn.float() * tw.unsqueeze(-1))                # .to(fp16)
+        ext.linear_forward("gemm", act_s, *ds["ws2"], G, out=b["shared_out"])
+        order = torch.sort(b["topk_ids"], dim=-1).indices             # index_add_ per expert, ascending
+        slots = torch.gather(b["down"], 1, order.unsqueeze(-1).expand(M, k, H))
+        o["out"].zero_()
+        for j in range(k):
+            o["out"].add_(slots[:, j])
+        o["out"].add_(b["shared_out"])
+
     # ------------------------------------------------------------------ build / run
     def _c_ops(self):
         arr = (Op * len(self._ops))()
@@ -315,7 +430,8 @@ class DecodeProgram:
                 c.kind, c.M, c.K = _cabi.OP_ADD, o["M"], o["K"]
                 c.x, c.weight, c.y = o["a"].data_ptr(), o["b"].data_ptr(), o["out"].data_ptr()
             elif kind == "moe":
-                c.kind, c.M, c.K, c.N = _cabi.OP_QWEN3_MOE if o["hf"] else _cabi.OP_SPARSE_MOE, o["M"], o["H"], o["H"]
+                c.kind, c.M, c.K, c.N = (_cabi.OP_DEEPSEEK_MOE if o["ds"] is not None else
+                                         _cabi.OP_QWEN3_MOE if o["hf"] else _cabi.OP_SPARSE_MOE), o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
             elif kind == "rope" and o["qdesc"] is not None:
                 c.kind, c.M, c.N, c.ldx = _cabi.OP_QK_NORM_ROPE_KV, o["M"], o["N"], o["ldx"]
@@ -372,19 +488,26 @@ class DecodeProgram:
 
     @property
     def kernel_ops(self) -> int:
-        """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe (gate|up with the routing, down), none per add or
+        """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe / deepseek_moe (gate|up with the routing, down), none per add or
         rope_kv_cache (they fold into their producer's epilogue); 0 per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
     def launches_per_run(self) -> int:
         """Kernels launched by one run(): 1 when fused (adds and rope_kv_cache included); per op, one per recorded
-        call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), one torch.add launch per add
+        call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), 34 + top_k per softmax
+        deepseek_moe (sigmoid: 36 + top_k, + 6 with expert groups, + 3 with norm_topk_prob), one torch.add launch per add
         and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
         kernel (torch.sort, torch.gather), so the kernel count can be higher."""
         def per_op(kind, o):
             if kind != "moe":
                 return 1
+            ds = o["ds"]
+            if ds is not None:
+                if ds["scoring"] == "softmax":
+                    return 34 + o["top_k"]
+                return (36 + o["top_k"] + (6 if ds["topk_group"] < ds["n_group"] else 0) +
+                        (3 if o["renormalize"] else 0))
             return 6 if not o["hf"] else 15 + o["top_k"] + (2 if o["renormalize"] else 0)
         return 1 if self.fused else sum(per_op(kind, o) for kind, o in self._ops)
 
@@ -402,6 +525,8 @@ class DecodeProgram:
                 ext.layernorm_forward_cuda(o["x"], o["weight"], o["out"], o["eps"])
             elif kind == "silu":
                 ext.silu_and_mul(o["out"], o["gate_up"])
+            elif kind == "moe" and o["ds"] is not None:
+                self._deepseek_moe_replay(o)
             elif kind == "moe" and o["hf"]:
                 self._qwen3_moe_replay(o)
             elif kind == "moe":

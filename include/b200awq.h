@@ -283,9 +283,36 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     Folding: two kernel ops, as SPARSE_MOE.  The router logits are computed once across the grid (CTA c computes the
  *     logits e = c mod grid) and exchanged through tagged words the program owns; every CTA then runs the routing from
  *     all E logits (DESIGN.md 3.5h).  Envelope (else B200AWQ_EUNSUPPORTED): SPARSE_MOE's with E <= 128
- *     (b200awq_qwen3_moe_plan below).  An ADD right after it folds into its down op. */
+ *     (b200awq_qwen3_moe_plan below).  An ADD right after it folds into its down op.
+ *
+ *   DEEPSEEK_MOE  : a DeepSeek-MoE expert block as transformers' DeepseekV2Moe / DeepseekV3MoE computes it over
+ *                   WQLinear_GEMM experts (one token row): routed experts plus one dense shared expert every token runs.
+ *                   x, y, K as SPARSE_MOE; weight = a b200awq_deepseek_moe_t descriptor (below).  Arithmetic:
+ *                   l = fp32(x) . fp32(Wg)^T, kept in fp32.
+ *                   scoring 0 (softmax, V2 "greedy"): p = softmax_fp32(l); the top_k largest p (ties to the lower
+ *                     expert); w = p_k * routed_scaling_factor.
+ *                   scoring 1 (sigmoid, V3 "noaux_tc"): s = sigmoid(l), c = s + bias; each of the n_group groups of
+ *                     E / n_group consecutive experts scores the sum of its two largest c; the topk_group best groups
+ *                     stay (ties to the lower group) and every other c becomes 0.0; the top_k largest masked c (ties to
+ *                     the lower expert); w = s_k, w = w / (sum w + 1e-20) when norm_topk_prob, w = w * routed_scaling_factor,
+ *                     all in fp32.
+ *                   Routed experts in ASCENDING EXPERT ID: a = fp16(fp16(silu(g)) * u), y = fp16(W2 a),
+ *                   c = fp16(fp32(y) * w), r = fp16(r + c) from r = 0.  Shared expert (gate|up concatenated along N):
+ *                   a_s = fp16(fp16(silu(g_s)) * u_s), y_s = fp16(W2s a_s).  y = fp16(r + y_s).
+ *                   The embedded descriptor's buffers hold what QWEN3_MOE's do, except: logits holds the fp32 l [E]
+ *                   and topk_weights the fp32 w [top_k] (pointers reinterpreted / as declared), gate_up holds
+ *                   [top_k 2I + 2 I_s] (the slots, then the shared gate|up) and act [top_k I + I_s] (the slots, then a_s);
+ *                   down holds the per-slot c.  renormalize is ignored (norm_topk_prob below).
+ *     Folding: two kernel ops.  gate|up has top_k 2I + 2 I_s columns, the shared sets after the slots; their weights do
+ *     not depend on the routing, so the producer streams them while the router logits are exchanged.  down reads
+ *     K' = top_k I + I_s (the shared expert concatenated along K after the slots) and keeps the shared expert's sum in
+ *     a partial row of its own.  Logit exchange as QWEN3_MOE, with the unrounded fp32 logits (DESIGN.md 3.5i).
+ *     Envelope (else B200AWQ_EUNSUPPORTED): M = 1, E <= 128, top_k <= 8, the shapes of b200awq_deepseek_moe_plan below.
+ *     A program that mixes SPARSE_MOE, QWEN3_MOE and DEEPSEEK_MOE blocks replays per op.  An ADD right after it folds
+ *     into its down op. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
-       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8 };
+       B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
+       B200AWQ_OP_DEEPSEEK_MOE = 9 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -336,6 +363,33 @@ typedef struct b200awq_moe {
 int b200awq_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8);
 /* The same plan for one QWEN3_MOE block: the same out8 layout and envelope, with E <= 128. */
 int b200awq_qwen3_moe_plan(int E, int top_k, int H, int I, int group_size, int sm_count, int* out8);
+
+/* DEEPSEEK_MOE descriptor (b200awq_op_t.weight points at it; copied at creation, tensors captured by address). */
+typedef struct b200awq_deepseek_moe {
+  b200awq_moe_t moe;            /* routed experts, router weight and the per-op buffers (see DEEPSEEK_MOE above) */
+  int32_t scoring;              /* 0: softmax (DeepSeek-V2), 1: sigmoid with e_score_correction_bias (DeepSeek-V3) */
+  int32_t n_group, topk_group;  /* expert groups (sigmoid): E % n_group == 0, E / n_group >= 2 unless n_group == 1 */
+  int32_t norm_topk_prob;       /* sigmoid: normalise the selected weights */
+  float routed_scaling_factor;
+  int32_t I_s;                  /* shared expert intermediate size (n_shared_experts x moe_intermediate_size) */
+  const float* bias;            /* e_score_correction_bias [E] f32 (sigmoid; null for softmax) */
+  const int32_t* ws1_qweight;   /* shared gate|up [H, 2 I_s / 8] (gate | up along N) */
+  const void* ws1_scales;       /* [H/G, 2 I_s] f16 */
+  const int32_t* ws1_qzeros;    /* [H/G, 2 I_s / 8] */
+  const int32_t* ws2_qweight;   /* shared down [I_s, H/8] */
+  const void* ws2_scales;       /* [I_s/G, H] f16 */
+  const int32_t* ws2_qzeros;    /* [I_s/G, H/8] */
+  void* shared_out;             /* y_s [H] f16 */
+} b200awq_deepseek_moe_t;
+
+/* Plan of one DEEPSEEK_MOE block, out8 as b200awq_moe_plan's with: [1] gate|up sets (top_k 2I + 2 I_s) / 16, [4] down
+ * units per set K' / min(G, 128) with K' = top_k I + I_s, [6] partial rows (top_k + I_s / I per set: the shared expert
+ * runs as I_s / I more slots).  Envelope (else B200AWQ_EUNSUPPORTED): E <= 128, top_k <= 8, I_s a multiple of I (DeepSeek's
+ * n_shared_experts x moe_intermediate_size), the expert and the shared shapes in the stream format, at most 32 gate|up
+ * sets and 32 partial rows per CTA, K' / min(G, 128) <= 1024, H / min(G, 128) <= 896 and the activations of K' in
+ * shared memory.  The routing arguments are checked at program creation (B200AWQ_EINVAL): scoring 0 or 1, a bias for
+ * sigmoid, n_group >= 1 dividing E with E / n_group >= 2 unless n_group == 1, 1 <= topk_group <= n_group. */
+int b200awq_deepseek_moe_plan(int E, int top_k, int H, int I, int I_s, int group_size, int sm_count, int* out8);
 
 /* RoPE + KV-cache append of one decode step (awq/modules/fused/attn.py:53-86 RoPE.forward, cache.py:41-46
  * WindowedCache.update_kv).  For token row m < M, head h < H + 2 KV and pair i < D/2, with a = qkv[m, h D + i],
@@ -408,7 +462,7 @@ int b200awq_program_tokens(b200awq_program_t prog);
  * (csrc/program_stream.cuh).  1 (the split-K kernel on the checkpoint layout of earlier versions) is no longer
  * returned. */
 int b200awq_program_kind(b200awq_program_t prog);
-/* number of fused kernel ops (= linear ops, two per SPARSE_MOE / QWEN3_MOE op) of the program; 0 for a null handle */
+/* number of fused kernel ops (= linear ops, two per SPARSE_MOE / QWEN3_MOE / DEEPSEEK_MOE op) of the program; 0 for a null handle */
 int b200awq_program_num_ops(b200awq_program_t prog);
 /* workspace / workspace_bytes: accepted and ignored (null is fine); the program owns its hand-off rows */
 int b200awq_program_run(b200awq_program_t prog, void* workspace, size_t workspace_bytes, b200awq_stream_t stream);
