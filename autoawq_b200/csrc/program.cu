@@ -6,19 +6,23 @@
 // those gaps, 128 times per decode step.  The packed weights never depend on the activations, so the producer warp of
 // every CTA walks the WHOLE op list and keeps its shared-memory ring full across op boundaries.
 //
-// This file is the host side of the stream kernels (program_stream.cuh: M = 1, with or without sparse-MoE blocks and
-// residual adds; program_batch.cuh: M = 2..8) plus what those kernels share:
-//   * program_create folds the recorded calls into a table of linears, each with the glue op that feeds it as an
-//     activation prologue, and enforces the hazard rules the kernels' ordering relies on;
-//   * stream_build re-lays out every linear once into the stream format and builds the kernels' op table; a
-//     sequence outside their envelope is not fused (B200AWQ_EUNSUPPORTED: the caller replays it per op);
-//   * program_run launches the kernel that matches the program;
+// This file is the host side of the stream kernels (program_stream.cuh: M = 1, with or without MoE blocks, residual
+// adds, ROPE_KV and QK_NORM_ROPE_KV ops; program_batch.cuh: M = 2..8) plus what those kernels share:
+//   * program_create folds the recorded calls into a FoldedProgram: one ProgOp per kernel op (a linear, the glue op
+//     that feeds it as an activation prologue, what is folded into its finish) and one MoeBlock per MoE op, and
+//     enforces the hazard rules the kernels' ordering relies on;
+//   * stream_build re-lays out every linear once into the stream format, builds the kernels' op table, chooses the
+//     kernel (ProgKernel) and uploads the side tables it takes; a sequence outside the kernels' envelope is not fused
+//     (B200AWQ_EUNSUPPORTED: the caller replays it per op);
+//   * program_run launches that kernel; the Program owns every device buffer and frees it when deleted;
 //   * the watchdog of every spin loop (ProgWatch, g_prog_abort) and the per-op phase timestamps (g_prog_dbg).
 //
 // Reference call sequence this replaces: awq/modules/fused/block.py:117-170 (norm -> qkv -> ... -> o -> norm ->
 // mlp) with awq/modules/fused/mlp.py:41-55 (gate/up GEMM, silu*mul, down GEMM), each a separate awq_ext call.
 #include <algorithm>
+#include <array>
 #include <cstring>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200awq.h"
@@ -30,26 +34,6 @@
 namespace b200awq {
 
 enum { kProCopy = 0, kProRmsnorm = 1, kProSilu = 2 };
-
-// One entry of the fold table program_create builds (host only): a linear and the activation prologue that feeds it.
-// stream_build turns the table into the kernels' SpOp table.
-struct ProgOp {
-  const __half* scales;
-  const int32_t* qzeros;
-  const __half* bias;
-  __half* y;
-  const __half* src;      // external source (fp16, global) when !src_prev: COPY x, RMSNORM row, SILU gate|up
-  const __half* norm_w;   // RMSNORM weight [K]
-  __half* xout;           // where the recorded glue op wanted its result, or null
-  int src_off;            // src_prev: first column of the previous op's output this op reads
-  int src_prev;           // 1: the source is the previous op's output
-  int K, N, G;
-  int prologue;
-  float eps;
-  int ext_dep;            // >= 0: the external source was written by that (older) op of this program
-  const int32_t* qw_src;  // the checkpoint-format qweight (re-laid-out by stream_build)
-  int src_ld;             // row pitch of src in elements (M > 1)
-};
 
 // knob 3 = 2: per-op phase timestamps (globaltimer ns) of the first 8 CTAs for the first 32 kernel ops; the slots are
 // listed in program_stream.cuh (SP_STAMP)
@@ -136,9 +120,85 @@ __device__ __forceinline__ bool prog_mbar_wait(uint64_t* bar, uint32_t parity, i
 namespace b200awq {
 
 // ------------------------------------------------------------------------------------------------ host side
+// One kernel op of a folded program (program_create): a linear, the activation prologue that feeds it and what is
+// folded into its finish.  stream_build turns the ops into the kernels' SpOp table and side tables.
+struct ProgOp {
+  const __half* scales = nullptr;
+  const int32_t* qzeros = nullptr;
+  const __half* bias = nullptr;
+  __half* y = nullptr;           // what the op's row publishes (an ADD folded in swaps the linear's y for its output)
+  const __half* src = nullptr;   // external source (fp16, global) when !src_prev: COPY x, RMSNORM row, SILU gate|up
+  const __half* norm_w = nullptr;   // RMSNORM weight [K]
+  __half* xout = nullptr;        // where the recorded glue op wanted its result, or null
+  int src_off = 0;               // src_prev: first column of the previous op's output this op reads
+  int src_prev = 0;              // 1: the source is the previous op's output
+  int K = 0, N = 0, G = 0;
+  int prologue = kProCopy;
+  float eps = 0.f;
+  int ext_dep = -1;              // >= 0: the external source was written by that (older) op of this program
+  const int32_t* qw_src = nullptr;   // the checkpoint-format qweight (re-laid-out by stream_build)
+  int src_ld = 0;                // row pitch of src in elements (M > 1)
+  int stage_row = -1;            // the op whose WHOLE published row this op's staging waits for, or -1
+  int moe = 0, mi = -1;          // 1: the gate|up op of MoE block `mi`, 2: its down op (0: a plain linear)
+  // an ADD folded into the finish (raw_y != null): raw_y is the linear's own output, still stored; the residual is the
+  // published row of the older op res_op, or res_ext, which no op of the program writes
+  const void* raw_y = nullptr;
+  const void* res_ext = nullptr;
+  int res_op = -1;
+  // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights
+  b200awq_qk_norm_rope_t qkr = {};
+};
+
+// One MoE op of a folded program (two kernel ops): kind is B200AWQ_OP_SPARSE_MOE, _QWEN3_MOE or _DEEPSEEK_MOE, ds.moe
+// the block's descriptor; the DeepSeek fields of ds are zero for the other kinds.
+struct MoeBlock {
+  int kind;
+  b200awq_deepseek_moe_t ds;
+  // What the block touches while the kernel runs, as (address, bytes): the kMoeWrites buffers it writes, then the
+  // router weight and the correction bias it only reads.  A DEEPSEEK_MOE block's gate_up and act include the shared
+  // expert and its logits are fp32.  (null, 0) overlaps nothing.
+  static constexpr int kMoeWrites = 11;
+  std::array<std::pair<const void*, size_t>, 13> extents(int M) const {
+    const b200awq_moe_t& m = ds.moe;
+    const bool dsk = kind == B200AWQ_OP_DEEPSEEK_MOE;
+    return {{{m.gate_up, ((size_t)m.top_k * 2 * m.I + 2 * (size_t)ds.I_s) * 2},
+             {m.act, ((size_t)m.top_k * m.I + ds.I_s) * 2},
+             {m.down, (size_t)m.top_k * m.H * 2},
+             {m.logits, (size_t)m.E * (dsk ? 4 : 2)},
+             {m.topk_weights, (size_t)m.top_k * M * 4},
+             {m.topk_ids, (size_t)m.top_k * M * 4},
+             {m.token_expert_indices, (size_t)m.top_k * M * 4},
+             {m.sorted_ids, (size_t)m.sorted_len * 4},
+             {m.expert_ids, (size_t)(m.top_k * M + m.E) * 4},
+             {m.num_tokens_post_pad, 4},
+             {ds.shared_out, dsk ? (size_t)m.H * 2 : 0},
+             {m.gate_weight, (size_t)m.E * m.H * 2},
+             {ds.bias, ds.bias != nullptr ? (size_t)m.E * 4 : 0}}};
+  }
+};
+
+// A folded program: its kernel ops and the MoE blocks they refer to
+struct FoldedProgram {
+  std::vector<ProgOp> table;
+  std::vector<MoeBlock> moes;
+};
+
+// The kernel entry that runs a program (chosen by stream_build).  M = 1: the plain kernel (8 or 12 consumer warps,
+// knob 9) or the 8-warp kernel of the program's features; M > 1: the batched kernels at MT = sb_mt(M).  Side tables:
+// the M = 1 kernels from kKernMoe on take SpMoe (null without MoE blocks), from kKernResidual on SpRes, from kKernRope on
+// SpRope, from kKernQkNorm on SpQkNorm, and kKernDeepseekMoe SpDsk; the batched ones take SpRes from
+// kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2 on.  The Qwen3-MoE and
+// DeepSeek-MoE kernels take every table, with empty entries where an op has no add, rotation or norm.
+enum ProgKernel {
+  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe,
+  kKernBatch2, kKernBatch4, kKernBatch8, kKernBatchResidual2, kKernBatchResidual4, kKernBatchResidual8,
+  kKernBatchRope2, kKernBatchRope4, kKernBatchRope8, kKernBatchQkNorm2, kKernBatchQkNorm4, kKernBatchQkNorm8
+};
+
 struct Program {
   int n_ops = 0;
   int M = 0;
+  ProgKernel kernel = kKernPlain;
   size_t xs_bytes = 0;
   int device = 0;
   // re-laid-out weights, per-op CTA partition, hand-off rows, tag state (program_stream.cuh)
@@ -155,35 +215,25 @@ struct Program {
   // device's L2 size (the run-ahead window, knob 8)
   int sp_spw8 = 0, sp_spw12 = 0;
   int l2_bytes = 0;
-  // sparse-MoE blocks (stream_moe_kernel): their descriptors
+  // side tables, null where the kernel does not take them (ProgKernel): one SpMoe per MoE block, with the published
+  // router logits of QWEN3_MOE / DEEPSEEK_MOE blocks ([E] words per block); one SpDsk per DEEPSEEK_MOE block; one
+  // SpRes, SpRope and SpQkNorm per kernel op, with the published set partials of QK_NORM_ROPE_KV ops
   SpMoe* d_moe = nullptr;
-  int n_moe = 0;
-  unsigned long long* d_xlog = nullptr;   // QWEN3_MOE blocks: their published router logits ([E] words per block)
-  bool qwen3 = false;                      // QWEN3_MOE blocks: stream_qwen3moe_kernel
-  SpDsk* d_dsk = nullptr;                  // DEEPSEEK_MOE blocks (stream_deepseek_moe_kernel): one SpDsk per block
-  // residual adds (stream_residual_kernel / stream_batch_residual_kernel): one SpRes per kernel op, null without adds
+  unsigned long long* d_xlog = nullptr;
+  SpDsk* d_dsk = nullptr;
   SpRes* d_res = nullptr;
-  // ROPE_KV ops (stream_rope_kernel / stream_batch_rope_kernel): one SpRope per kernel op, null without them (d_res is
-  // then allocated too, empty where there is no add: the rope kernels are the residual kernels plus the rope steps)
   SpRope* d_rope = nullptr;
-  // QK_NORM_ROPE_KV ops (stream_qknorm_kernel / stream_batch_qknorm_kernel): one SpQkNorm per kernel op and the published
-  // set partials of their heads, null without them (d_res and d_rope are then allocated too)
   SpQkNorm* d_qkn = nullptr;
   unsigned long long* d_qkn_part = nullptr;
-};
 
-// An ADD folded into table entry i (program_create): the entry's y is swapped for the ADD's output (what its row
-// publishes, so the hazard rules resolve later readers to the row); raw_y is the linear's own output, still stored
-struct ResFold {
-  const void* raw_y = nullptr;   // null: no ADD folded into this entry
-  const void* ext = nullptr;     // external residual (no op of the program writes it)
-  int op = -1;                   // >= 0: the residual is that older entry's published row
-};
-
-// One SPARSE_MOE op as the folding sees it: two table entries (gate|up, down) and the recorded descriptor
-struct MoeFold {
-  int kind = 0;        // 0: plain linear, 1: gate|up of block `mi`, 2: its down
-  int mi = -1;
+  Program() = default;
+  Program(const Program&) = delete;
+  Program& operator=(const Program&) = delete;
+  ~Program() {
+    for (void* d : std::initializer_list<void*>{d_sp_ops, d_stream, d_cta, d_rows, d_state, d_moe, d_xlog, d_dsk, d_res,
+                                                d_rope, d_qkn, d_qkn_part})
+      cudaFree(d);
+  }
 };
 
 // Envelope and partition of a sparse-MoE block in an M = 1 stream program (host only, see b200awq_moe_plan); e_max:
@@ -290,34 +340,40 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
   return cudaGetLastError();
 }
 
-// Builds the stream kernels' program from the folded op table, for M token rows (M > 1: the batched kernel of
-// program_batch.cuh).  Returns false when the sequence is outside their envelope.  *err != cudaSuccess reports a CUDA
-// failure.
-// Sparse-MoE blocks (`fold[i].kind` != 0, M = 1 only): the gate|up entry is a mode-1 op over top_k slots of 2I
-// columns, the down entry reads its published row (K' = top_k I); both stream E per-expert slices packed back to back.
-// ROPE_KV ops (`ropes[i].head_dim` != 0): entry i is packed in mode 2 and its finish rotates / appends (SpRope).
-// QK_NORM_ROPE_KV ops: as ROPE_KV, and `qkns[i]` carries the norm weights (q_norm_weight != null: SpQkNorm).
-static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid, int M, cudaError_t* err,
-                         const std::vector<MoeFold>& fold, const std::vector<b200awq_moe_t>& moes,
-                         const std::vector<ResFold>& res, const std::vector<b200awq_rope_t>& ropes,
-                         const std::vector<b200awq_qk_norm_rope_t>& qkns, const std::vector<int>& moe_hf,
-                         const std::vector<b200awq_deepseek_moe_t>& dsks) {
+// Allocates *d and copies h into it (an empty h leaves *d null)
+template <typename T>
+static cudaError_t upload(T** d, const std::vector<T>& h) {
+  if (h.empty()) return cudaSuccess;
+  const cudaError_t e = cudaMalloc(d, h.size() * sizeof(T));
+  return e != cudaSuccess ? e : cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
+}
+
+// Builds the stream kernels' program from the folded one, for pr->M token rows (M > 1: the batched kernel of
+// program_batch.cuh), and chooses the kernel that runs it.  Returns false when the sequence is outside their envelope.
+// *err != cudaSuccess reports a CUDA failure; what was allocated by then is pr's to free.
+// MoE blocks (`moe` != 0, M = 1 only): the gate|up op is a mode-1 op over top_k slots of 2I columns, the down op reads
+// its published row (K' = top_k I); both stream E per-expert slices packed back to back.
+// ROPE_KV ops (`qkr.rope.head_dim` != 0): packed in mode 2, the finish rotates / appends (SpRope).
+// QK_NORM_ROPE_KV ops: as ROPE_KV, and `qkr` carries the norm weights (q_norm_weight != null: SpQkNorm).
+static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaError_t* err) {
   *err = cudaSuccess;
-  const int n = static_cast<int>(table.size());
+  const std::vector<ProgOp>& table = f.table;
+  const int n = static_cast<int>(table.size()), M = pr->M;
   if (n >= 60000) return false;
-  const bool has_moe = !moes.empty();
+  const bool has_moe = !f.moes.empty();
   if (has_moe && M != 1) return false;
-  // moe_hf: 0 SPARSE_MOE, 1 QWEN3_MOE, 2 DEEPSEEK_MOE.  A QWEN3_MOE (DEEPSEEK_MOE) program runs stream_qwen3moe_kernel
-  // (stream_deepseek_moe_kernel), whose MoE blocks are all of that kind
-  const int mkind = moe_hf.empty() ? 0 : moe_hf[0];
-  if (std::find_if(moe_hf.begin(), moe_hf.end(), [&](int k) { return k != mkind; }) != moe_hf.end()) return false;
-  const bool has_hf = mkind != 0, has_ds = mkind == 2;
-  std::vector<int> plan_a(moes.size() * 8);
-  for (size_t b = 0; b < moes.size(); ++b) {
-    const b200awq_moe_t& m = moes[b];
-    const int rc = moe_hf[b] == 2 ? deepseek_moe_plan(m.E, m.top_k, m.H, m.I, dsks[b].I_s, m.group_size, grid, &plan_a[b * 8])
-                                  : (moe_hf[b] ? qwen3_moe_plan : moe_plan)(m.E, m.top_k, m.H, m.I, m.group_size, grid,
-                                                                             &plan_a[b * 8]);
+  // a QWEN3_MOE (DEEPSEEK_MOE) program runs stream_qwen3moe_kernel (stream_deepseek_moe_kernel), whose MoE blocks are
+  // all of that kind
+  const int mkind = has_moe ? f.moes[0].kind : B200AWQ_OP_SPARSE_MOE;
+  for (const MoeBlock& b : f.moes)
+    if (b.kind != mkind) return false;
+  std::vector<int> plan_a(f.moes.size() * 8);
+  for (size_t b = 0; b < f.moes.size(); ++b) {
+    const b200awq_moe_t& m = f.moes[b].ds.moe;
+    const int rc = mkind == B200AWQ_OP_DEEPSEEK_MOE
+                       ? deepseek_moe_plan(m.E, m.top_k, m.H, m.I, f.moes[b].ds.I_s, m.group_size, grid, &plan_a[b * 8])
+                       : (mkind == B200AWQ_OP_QWEN3_MOE ? qwen3_moe_plan : moe_plan)(m.E, m.top_k, m.H, m.I, m.group_size,
+                                                                                   grid, &plan_a[b * 8]);
     if (rc != B200AWQ_OK) return false;
   }
   // creation is a load-time step (not capturable): whatever produced the checkpoint tensors on any stream is done
@@ -336,47 +392,60 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
         mode[i - 1] = 1;
       }
     }
-  auto moe_kind = [&](int i) { return fold.empty() ? 0 : fold[i].kind; };
-  // bytes of one expert's slice of a MoE entry's stream copy (256-byte aligned)
+  // bytes of one expert's slice of a MoE op's stream copy (256-byte aligned)
   auto expert_bytes = [&](int i) {
-    const b200awq_moe_t& m = moes[fold[i].mi];
-    const size_t b = moe_kind(i) == 1 ? stream_format_bytes(m.H, 2 * m.I, m.group_size)
-                                      : stream_format_bytes(m.I, m.H, m.group_size);
+    const b200awq_moe_t& m = f.moes[table[i].mi].ds.moe;
+    const size_t b = table[i].moe == 1 ? stream_format_bytes(m.H, 2 * m.I, m.group_size)
+                                       : stream_format_bytes(m.I, m.H, m.group_size);
     return (b + 255) & ~(size_t)255;
   };
-  // bytes of the shared expert's stream copy of a DEEPSEEK_MOE entry (in front of its expert slices; 0 otherwise)
+  // bytes of the shared expert's stream copy of a DEEPSEEK_MOE op (in front of its expert slices; 0 otherwise)
   auto shared_bytes = [&](int i) {
-    if (moe_hf[fold[i].mi] != 2) return (size_t)0;
-    const b200awq_moe_t& m = moes[fold[i].mi];
-    const int I_s = dsks[fold[i].mi].I_s;
-    const size_t b = moe_kind(i) == 1 ? stream_format_bytes(m.H, 2 * I_s, m.group_size)
-                                      : stream_format_bytes(I_s, m.H, m.group_size);
+    const MoeBlock& blk = f.moes[table[i].mi];
+    if (blk.kind != B200AWQ_OP_DEEPSEEK_MOE) return (size_t)0;
+    const b200awq_moe_t& m = blk.ds.moe;
+    const size_t b = table[i].moe == 1 ? stream_format_bytes(m.H, 2 * blk.ds.I_s, m.group_size)
+                                       : stream_format_bytes(blk.ds.I_s, m.H, m.group_size);
     return (b + 255) & ~(size_t)255;
   };
   for (int i = 0; i < n; ++i)
-    if (moe_kind(i) == 1) mode[i] = 1;
-  bool has_rope = false;
-  for (int i = 0; i < n && !ropes.empty(); ++i)
-    if (ropes[i].head_dim != 0) {
+    if (table[i].moe == 1) mode[i] = 1;
+  bool has_rope = false, has_qkn = false, has_res = false;
+  for (int i = 0; i < n; ++i) {
+    if (table[i].qkr.rope.head_dim != 0) {
       if (mode[i] != 0) return false;   // (program_create rejects a gate|up producer already)
       mode[i] = 2;
       has_rope = true;
     }
+    has_qkn = has_qkn || table[i].qkr.q_norm_weight != nullptr;
+  }
   // residual adds: the producer and an in-program residual must publish plain columns (a mode-1 row holds SiLU*mul)
-  bool has_res = false;
-  for (int i = 0; i < n && !res.empty(); ++i)
-    if (res[i].raw_y != nullptr) {
-      if (mode[i] == 1 || (res[i].op >= 0 && mode[res[i].op] == 1)) return false;
+  for (int i = 0; i < n; ++i)
+    if (table[i].raw_y != nullptr) {
+      if (mode[i] == 1 || (table[i].res_op >= 0 && mode[table[i].res_op] == 1)) return false;
       has_res = true;
     }
+  // the kernel: the first of these the program needs (has_qkn implies has_rope; QWEN3_MOE and DEEPSEEK_MOE blocks only
+  // exist at M = 1)
+  const int mt = sb_mt(M) == 2 ? 0 : (sb_mt(M) == 4 ? 1 : 2);
+  const ProgKernel kern =
+      M > 1 ? ProgKernel((has_qkn ? kKernBatchQkNorm2 : has_rope ? kKernBatchRope2 : has_res ? kKernBatchResidual2
+                                                                                             : kKernBatch2) + mt)
+      : mkind == B200AWQ_OP_DEEPSEEK_MOE ? kKernDeepseekMoe
+      : mkind == B200AWQ_OP_QWEN3_MOE    ? kKernQwen3Moe
+      : has_qkn                          ? kKernQkNorm
+      : has_rope                         ? kKernRope
+      : has_res                          ? kKernResidual
+      : has_moe                          ? kKernMoe
+                                         : kKernPlain;
   size_t wbytes = 0, max_cols = 0;
   int max_K = 0, lmax = 0, nu_max = 0;
   std::vector<size_t> woff(n);
   for (int i = 0; i < n; ++i) {
     const ProgOp& p = table[i];
-    if (moe_kind(i) != 0) {   // envelope checked by moe_plan (per-expert shapes, sets and partial rows per CTA)
+    if (p.moe != 0) {   // envelope checked by moe_plan (per-expert shapes, sets and partial rows per CTA)
       woff[i] = wbytes;
-      wbytes += shared_bytes(i) + (size_t)moes[fold[i].mi].E * expert_bytes(i);
+      wbytes += shared_bytes(i) + (size_t)f.moes[p.mi].ds.moe.E * expert_bytes(i);
     } else {
       if (!stream_format_supported(p.K, p.N, p.G, mode[i] == 2 ? 0 : mode[i])) return false;
       const int UK = p.G < 128 ? p.G : 128;
@@ -393,7 +462,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   if (M == 1) {
     // the envelope: a ring of 4 stages at 8 warps (the MoE / residual / rope kernels, behind the routing area) or 3 at
     // 12 must fit; the program then runs the deepest ring its activations leave room for
-    const bool moe_k = has_moe || has_res || has_rope;
+    const bool moe_k = kern != kKernPlain;
     if (moe_k && sp_fixed_smem(8, 4, true) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
     if (!moe_k && sp_fixed_smem(12, 3, false) + (size_t)max_K * 2 > (size_t)227 * 1024) return false;
     pr->sp_spw8 = sp_pick_spw(8, moe_k, (size_t)max_K * 2);
@@ -412,7 +481,7 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     SpOp& o = ops[i];
     std::memset(&o, 0, sizeof(o));
     o.bias = p.bias;
-    o.y = (!res.empty() && res[i].raw_y != nullptr) ? static_cast<__half*>(const_cast<void*>(res[i].raw_y)) : p.y;
+    o.y = p.raw_y != nullptr ? static_cast<__half*>(const_cast<void*>(p.raw_y)) : p.y;
     o.K = p.K;
     o.N = p.N;
     const int UK = p.G < 128 ? p.G : 128;
@@ -454,13 +523,13 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
         o.ldx = p.src_ld;
       }
     }
-    if (moe_kind(i) != 0) {
-      o.moe = moe_kind(i);
-      o.moe_i = fold[i].mi;
+    if (p.moe != 0) {
+      o.moe = p.moe;
+      o.moe_i = p.mi;
       if (o.moe == 2) {
-        // the down entry stages the gate|up entry's published SiLU*mul row (top_k x I words, slot-major); the recorded
-        // activation tensor is written as a side effect of that entry
-        if (i == 0 || moe_kind(i - 1) != 1 || fold[i - 1].mi != fold[i].mi) return false;
+        // the down op stages the gate|up op's published SiLU*mul row (top_k x I words, slot-major); the recorded
+        // activation tensor is written as a side effect of that op
+        if (i == 0 || table[i - 1].moe != 1 || table[i - 1].mi != p.mi) return false;
         o.prologue = kProCopy;
         o.src = nullptr;
         o.src_op = i - 1;
@@ -477,29 +546,27 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
   }
   pr->row_stride = (int)((max_cols + 63) & ~(size_t)63);
   cudaError_t e = cudaMalloc(&pr->d_stream, wbytes);
-  if (e == cudaSuccess) e = cudaMalloc(&pr->d_sp_ops, (size_t)n * sizeof(SpOp));
-  if (e == cudaSuccess) e = cudaMalloc(&pr->d_cta, cta.size() * sizeof(uint32_t));
-  const size_t row_bytes = (size_t)kSpRows * M * pr->row_stride * sizeof(uint32_t);   // M hand-off rows per op
-  if (e == cudaSuccess) e = cudaMalloc(&pr->d_rows, row_bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&pr->d_state, 2 * sizeof(int));
-  if (e == cudaSuccess) e = cudaMemset(pr->d_rows, 0, row_bytes);
-  if (e == cudaSuccess) e = cudaMemset(pr->d_state, 0, 2 * sizeof(int));
+  if (e == cudaSuccess) e = upload(&pr->d_cta, cta);
+  // M hand-off rows per op and the tag state, zero (no run's tag) until the first run
+  if (e == cudaSuccess) e = upload(&pr->d_rows, std::vector<uint32_t>((size_t)kSpRows * M * pr->row_stride));
+  if (e == cudaSuccess) e = upload(&pr->d_state, std::vector<int>(2));
   for (int i = 0; i < n && e == cudaSuccess; ++i) {
     ops[i].wstream = pr->d_stream + woff[i];
     ops[i].cta_begin = pr->d_cta + (size_t)i * (grid + 1);
-    if (moe_kind(i) != 0) {
+    if (table[i].moe != 0) {
       // one stream copy per expert slice of the stacked tensors ([E, K, N/8], [E, K/G, N], [E, K/G, N/8])
-      const b200awq_moe_t& m = moes[fold[i].mi];
-      const int K = moe_kind(i) == 1 ? m.H : m.I, N = moe_kind(i) == 1 ? 2 * m.I : m.H, G = m.group_size;
-      const int32_t* qw = static_cast<const int32_t*>(table[i].qw_src);
+      const MoeBlock& blk = f.moes[table[i].mi];
+      const b200awq_moe_t& m = blk.ds.moe;
+      const bool gu = table[i].moe == 1;
+      const int K = gu ? m.H : m.I, N = gu ? 2 * m.I : m.H, G = m.group_size;
+      const int32_t* qw = table[i].qw_src;
       const size_t shb = shared_bytes(i);
       for (int x = 0; x < m.E && e == cudaSuccess; ++x)
         e = stream_pack(qw + (size_t)x * K * (N / 8), table[i].scales + (size_t)x * (K / G) * N,
                         table[i].qzeros + (size_t)x * (K / G) * (N / 8),
                         pr->d_stream + woff[i] + shb + (size_t)x * expert_bytes(i), K, N, G, mode[i], nullptr);
       if (shb != 0 && e == cudaSuccess) {   // DEEPSEEK_MOE: the shared expert's copy, first
-        const b200awq_deepseek_moe_t& d = dsks[fold[i].mi];
-        const bool gu = moe_kind(i) == 1;
+        const b200awq_deepseek_moe_t& d = blk.ds;
         e = stream_pack(gu ? d.ws1_qweight : d.ws2_qweight, gu ? d.ws1_scales : d.ws2_scales,
                         gu ? d.ws1_qzeros : d.ws2_qzeros, pr->d_stream + woff[i], gu ? m.H : d.I_s, gu ? 2 * d.I_s : m.H,
                         G, mode[i], nullptr);
@@ -508,23 +575,22 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
     }
     if (mode[i] == 2)
       e = stream_pack_rotary(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K,
-                             table[i].N, table[i].G, ropes[i].head_dim, nullptr);
+                             table[i].N, table[i].G, table[i].qkr.rope.head_dim, nullptr);
     else
       e = stream_pack(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K, table[i].N,
                       table[i].G, mode[i], nullptr);
   }
   if (e == cudaSuccess && has_moe) {
-    // QWEN3_MOE blocks: [E] logit words each, zero (no run's tag) until the first run
+    // QWEN3_MOE / DEEPSEEK_MOE blocks: [E] logit words each, zero (no run's tag) until the first run
     size_t xwords = 0;
-    for (size_t b = 0; b < moes.size(); ++b) xwords += moe_hf[b] ? (size_t)moes[b].E : 0;
-    if (xwords > 0) e = cudaMalloc(&pr->d_xlog, xwords * sizeof(unsigned long long));
-    if (e == cudaSuccess && xwords > 0) e = cudaMemset(pr->d_xlog, 0, xwords * sizeof(unsigned long long));
+    for (const MoeBlock& b : f.moes) xwords += b.kind != B200AWQ_OP_SPARSE_MOE ? (size_t)b.ds.moe.E : 0;
+    e = upload(&pr->d_xlog, std::vector<unsigned long long>(xwords));
     size_t xoff = 0;
-    std::vector<SpMoe> md(moes.size());
-    for (size_t b = 0; b < moes.size(); ++b) {
-      const b200awq_moe_t& m = moes[b];
+    std::vector<SpMoe> md(f.moes.size());
+    std::vector<SpDsk> dd(f.moes.size());
+    for (size_t b = 0; b < f.moes.size(); ++b) {
+      const b200awq_moe_t& m = f.moes[b].ds.moe;
       SpMoe& d = md[b];
-      std::memset(&d, 0, sizeof(d));
       d.gate_w = static_cast<const __half*>(m.gate_weight);
       d.logits = static_cast<__half*>(m.logits);
       d.topk_w = m.topk_weights;
@@ -542,157 +608,86 @@ static bool stream_build(Program* pr, const std::vector<ProgOp>& table, int grid
       d.seg_a = plan_a[b * 8 + 2];
       d.seg_b = plan_a[b * 8 + 5];
       d.I = m.I;
-      if (moe_hf[b]) {
+      if (f.moes[b].kind != B200AWQ_OP_SPARSE_MOE) {
         d.xlog = pr->d_xlog + xoff;
         xoff += (size_t)m.E;
       }
-      for (int i = 0; i < n; ++i)
-        if (moe_kind(i) != 0 && fold[i].mi == (int)b) (moe_kind(i) == 1 ? d.eb_a : d.eb_b) = (long long)expert_bytes(i);
+      const b200awq_deepseek_moe_t& s = f.moes[b].ds;
+      SpDsk& x = dd[b];
+      x.bias = s.bias;
+      x.shared_out = static_cast<__half*>(s.shared_out);
+      x.scoring = s.scoring;
+      x.n_group = s.n_group;
+      x.topk_group = s.topk_group;
+      x.norm = s.norm_topk_prob != 0;
+      x.rsf = s.routed_scaling_factor;
+      x.nsh = s.I_s / m.I;
     }
-    if (e == cudaSuccess) e = cudaMalloc(&pr->d_moe, md.size() * sizeof(SpMoe));
-    if (e == cudaSuccess) e = cudaMemcpy(pr->d_moe, md.data(), md.size() * sizeof(SpMoe), cudaMemcpyHostToDevice);
-    pr->n_moe = static_cast<int>(md.size());
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)(227 * 1024));
-    if (e == cudaSuccess && has_ds) {
-      std::vector<SpDsk> dd(moes.size());
-      for (size_t b = 0; b < moes.size(); ++b) {
-        const b200awq_deepseek_moe_t& d = dsks[b];
-        SpDsk& x = dd[b];
-        std::memset(&x, 0, sizeof(x));
-        x.bias = d.bias;
-        x.shared_out = static_cast<__half*>(d.shared_out);
-        x.scoring = d.scoring;
-        x.n_group = d.n_group;
-        x.topk_group = d.topk_group;
-        x.norm = d.norm_topk_prob != 0;
-        x.rsf = d.routed_scaling_factor;
-        x.nsh = d.I_s / d.moe.I;
-        for (int i = 0; i < n; ++i)
-          if (moe_kind(i) != 0 && fold[i].mi == (int)b) (moe_kind(i) == 1 ? x.shb_a : x.shb_b) = (long long)shared_bytes(i);
+    for (int i = 0; i < n; ++i)
+      if (table[i].moe != 0) {
+        (table[i].moe == 1 ? md[table[i].mi].eb_a : md[table[i].mi].eb_b) = (long long)expert_bytes(i);
+        (table[i].moe == 1 ? dd[table[i].mi].shb_a : dd[table[i].mi].shb_b) = (long long)shared_bytes(i);
       }
-      e = cudaMalloc(&pr->d_dsk, dd.size() * sizeof(SpDsk));
-      if (e == cudaSuccess) e = cudaMemcpy(pr->d_dsk, dd.data(), dd.size() * sizeof(SpDsk), cudaMemcpyHostToDevice);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(stream_deepseek_moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    }
+    if (e == cudaSuccess) e = upload(&pr->d_moe, md);
+    if (e == cudaSuccess && kern == kKernDeepseekMoe) e = upload(&pr->d_dsk, dd);
   }
-  if (e == cudaSuccess && (has_res || has_rope || has_hf)) {
+  // the side tables the kernel takes (ProgKernel)
+  const bool takes_res = (kern >= kKernResidual && kern <= kKernDeepseekMoe) || kern >= kKernBatchResidual2;
+  const bool takes_rope = (kern >= kKernRope && kern <= kKernDeepseekMoe) || kern >= kKernBatchRope2;
+  const bool takes_qkn = (kern >= kKernQkNorm && kern <= kKernDeepseekMoe) || kern >= kKernBatchQkNorm2;
+  if (e == cudaSuccess && takes_res) {
     std::vector<SpRes> rd(n);
     for (int i = 0; i < n; ++i) {
-      std::memset(&rd[i], 0, sizeof(SpRes));
-      rd[i].op = -1;
-      if (res.empty() || res[i].raw_y == nullptr) continue;
-      rd[i].out = table[i].y;                       // the ADD's output (the entry's y was swapped for it)
-      rd[i].op = res[i].op;
-      rd[i].ext = static_cast<const __half*>(res[i].ext);
+      rd[i].op = table[i].res_op;
+      if (table[i].raw_y == nullptr) continue;
+      rd[i].out = table[i].y;                       // the ADD's output (the op's y was swapped for it)
+      rd[i].ext = static_cast<const __half*>(table[i].res_ext);
     }
-    e = cudaMalloc(&pr->d_res, (size_t)n * sizeof(SpRes));
-    if (e == cudaSuccess) e = cudaMemcpy(pr->d_res, rd.data(), (size_t)n * sizeof(SpRes), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_residual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_residual_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_residual_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_residual_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    e = upload(&pr->d_res, rd);
   }
-  bool has_qkn = false;
-  for (int i = 0; i < n && !qkns.empty(); ++i) has_qkn = has_qkn || qkns[i].q_norm_weight != nullptr;
-  if (e == cudaSuccess && (has_qkn || has_hf)) {
+  if (e == cudaSuccess && takes_rope) {
+    std::vector<SpRope> rp(n);
+    for (int i = 0; i < n; ++i) rp[i].r = table[i].qkr.rope;   // (head_dim 0: no rotation)
+    e = upload(&pr->d_rope, rp);
+  }
+  if (e == cudaSuccess && takes_qkn) {
     // the partials of op i live at [M][N_i / 16] words from its offset; zero tags are never a run's (sp_tag >= 1)
-    std::vector<SpQkNorm> qd(n);
     size_t words = 0;
-    for (int i = 0; i < n; ++i)
-      if (qkns[i].q_norm_weight != nullptr) words += (size_t)M * (table[i].N / 16);
-    if (words > 0) e = cudaMalloc(&pr->d_qkn_part, words * sizeof(unsigned long long));
-    if (e == cudaSuccess && words > 0) e = cudaMemset(pr->d_qkn_part, 0, words * sizeof(unsigned long long));
+    for (const ProgOp& p : table) words += p.qkr.q_norm_weight != nullptr ? (size_t)M * (p.N / 16) : 0;
+    e = upload(&pr->d_qkn_part, std::vector<unsigned long long>(words));
+    std::vector<SpQkNorm> qd(n);
     size_t off = 0;
     for (int i = 0; i < n; ++i) {
-      std::memset(&qd[i], 0, sizeof(SpQkNorm));
-      if (qkns[i].q_norm_weight == nullptr) continue;
-      qd[i].q = qkns[i];
+      if (table[i].qkr.q_norm_weight == nullptr) continue;
+      qd[i].q = table[i].qkr;
       qd[i].part = pr->d_qkn_part + off;
-      qd[i].inv_d = 1.f / static_cast<float>(qkns[i].rope.head_dim);
+      qd[i].inv_d = 1.f / static_cast<float>(table[i].qkr.rope.head_dim);
       off += (size_t)M * (table[i].N / 16);
     }
-    if (e == cudaSuccess) e = cudaMalloc(&pr->d_qkn, (size_t)n * sizeof(SpQkNorm));
-    if (e == cudaSuccess) e = cudaMemcpy(pr->d_qkn, qd.data(), (size_t)n * sizeof(SpQkNorm), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_qknorm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_qknorm_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    if (e == cudaSuccess) e = upload(&pr->d_qkn, qd);
   }
-  if (e == cudaSuccess && (has_rope || has_hf)) {
-    std::vector<SpRope> rp(n);
-    for (int i = 0; i < n; ++i) rp[i].r = ropes[i];   // (head_dim 0: no rotation)
-    e = cudaMalloc(&pr->d_rope, (size_t)n * sizeof(SpRope));
-    if (e == cudaSuccess) e = cudaMemcpy(pr->d_rope, rp.data(), (size_t)n * sizeof(SpRope), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_rope_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_rope_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_rope_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_rope_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-  }
-  if (e == cudaSuccess) e = cudaMemcpy(pr->d_sp_ops, ops.data(), (size_t)n * sizeof(SpOp), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(pr->d_cta, cta.data(), cta.size() * sizeof(uint32_t), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && has_hf)
-    e = cudaFuncSetAttribute(stream_qwen3moe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(stream_program_kernel<8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(stream_program_kernel<12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+  if (e == cudaSuccess) e = upload(&pr->d_sp_ops, ops);
+  // the kernel may use all 227 KB of shared memory (the plain one at both warp counts: knob 9 is read at run time)
+  static const void* const entry[] = {
+      (const void*)stream_program_kernel<8, 4>, (const void*)stream_moe_kernel, (const void*)stream_residual_kernel,
+      (const void*)stream_rope_kernel, (const void*)stream_qknorm_kernel, (const void*)stream_qwen3moe_kernel,
+      (const void*)stream_deepseek_moe_kernel, (const void*)stream_batch_kernel<2>, (const void*)stream_batch_kernel<4>,
+      (const void*)stream_batch_kernel<8>, (const void*)stream_batch_residual_kernel<2>,
+      (const void*)stream_batch_residual_kernel<4>, (const void*)stream_batch_residual_kernel<8>,
+      (const void*)stream_batch_rope_kernel<2>, (const void*)stream_batch_rope_kernel<4>,
+      (const void*)stream_batch_rope_kernel<8>, (const void*)stream_batch_qknorm_kernel<2>,
+      (const void*)stream_batch_qknorm_kernel<4>, (const void*)stream_batch_qknorm_kernel<8>};
+  static_assert(sizeof(entry) / sizeof(entry[0]) == kKernBatchQkNorm8 + 1, "one entry per ProgKernel");
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(entry[kern], cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  if (e == cudaSuccess && kern == kKernPlain)
+    e = cudaFuncSetAttribute(stream_program_kernel<12, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&pr->l2_bytes, cudaDevAttrL2CacheSize, pr->device);
-  if (e == cudaSuccess && M > 1) {
-    e = cudaFuncSetAttribute(stream_batch_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(stream_batch_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-  }
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    cudaFree(pr->d_stream);
-    cudaFree(pr->d_sp_ops);
-    cudaFree(pr->d_cta);
-    cudaFree(pr->d_rows);
-    cudaFree(pr->d_state);
-    cudaFree(pr->d_moe);
-    cudaFree(pr->d_xlog);
-    cudaFree(pr->d_dsk);
-    cudaFree(pr->d_res);
-    cudaFree(pr->d_rope);
-    cudaFree(pr->d_qkn);
-    cudaFree(pr->d_qkn_part);
-    pr->d_res = nullptr;
-    pr->d_rope = nullptr;
-    pr->d_qkn = nullptr;
-    pr->d_qkn_part = nullptr;
-    pr->d_stream = nullptr;
-    pr->d_sp_ops = nullptr;
-    pr->d_cta = nullptr;
-    pr->d_rows = nullptr;
-    pr->d_state = nullptr;
-    pr->d_moe = nullptr;
-    pr->d_xlog = nullptr;
-    pr->d_dsk = nullptr;
-    pr->n_moe = 0;
-    *err = e;
-    return false;
-  }
+  pr->kernel = kern;
   pr->stream_bytes = wbytes;
-  pr->qwen3 = has_hf;
   pr->xs_bytes = (size_t)max_K * (M == 1 ? 1 : sb_mt(M)) * 2;   // M = 1: one row (stream_program_kernel)
-  return true;
+  *err = e;
+  return e == cudaSuccess;
 }
 
 static int prog_sm_count() {
@@ -727,20 +722,20 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   *cuda_err = cudaSuccess;
   *out = nullptr;
   if (ops_in == nullptr || n_in <= 0 || max_tokens < 1 || max_tokens > 8) return B200AWQ_EINVAL;
-  // A SPARSE_MOE or QWEN3_MOE op folds as two linears: gate|up (x [H] -> the recorded gate_up [top_k, 2I], N = top_k 2I) and down
-  // (the recorded activations [top_k, I] -> y [H], K = top_k I); the hazard rules below then see every buffer they touch.
-  // Only the stream kernel runs them (M = 1; stream_build checks the envelope); otherwise the caller replays per op.
+  // A MoE op folds as two linears: gate|up (x [H] -> the recorded gate_up [top_k, 2I], N = top_k 2I) and down (the
+  // recorded activations [top_k, I] -> y [H], K = top_k I); a DEEPSEEK_MOE op's shared expert widens both by I_s.  The
+  // hazard rules below then see every buffer they touch.  Only the stream kernel runs them (M = 1; stream_build checks
+  // the envelope); otherwise the caller replays per op.
+  FoldedProgram f;
+  std::vector<ProgOp>& table = f.table;
+  std::vector<MoeBlock>& moes = f.moes;
   std::vector<b200awq_op_t> xops;
-  std::vector<MoeFold> xfold;
-  std::vector<b200awq_moe_t> moes;
-  std::vector<int> moe_hf;       // per block: 1 for QWEN3_MOE (the same folding, Qwen3-MoE's routing and finishes),
-                                 // 2 for DEEPSEEK_MOE (plus the shared expert: gate|up N and down K grow by it)
-  std::vector<b200awq_deepseek_moe_t> dsks;   // per block: DEEPSEEK_MOE's descriptor (zero for the other kinds)
+  std::vector<std::pair<int, int>> xmoe;   // per entry of xops: ProgOp::moe and ProgOp::mi
   for (int i = 0; i < n_in; ++i) {
     const b200awq_op_t& op = ops_in[i];
     if (op.kind != B200AWQ_OP_SPARSE_MOE && op.kind != B200AWQ_OP_QWEN3_MOE && op.kind != B200AWQ_OP_DEEPSEEK_MOE) {
       xops.push_back(op);
-      xfold.push_back(MoeFold{});
+      xmoe.emplace_back(0, -1);
       continue;
     }
     const bool ds = op.kind == B200AWQ_OP_DEEPSEEK_MOE;
@@ -770,11 +765,9 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     }
     if (op.M != 1) return B200AWQ_EUNSUPPORTED;
     const int mi = static_cast<int>(moes.size());
-    moes.push_back(*m);
-    moe_hf.push_back(ds ? 2 : (op.kind == B200AWQ_OP_QWEN3_MOE ? 1 : 0));
-    dsks.emplace_back();
-    if (ds) dsks.back() = *dd;
-    else std::memset(&dsks.back(), 0, sizeof(b200awq_deepseek_moe_t));
+    moes.push_back(MoeBlock{op.kind, {}});
+    if (ds) moes.back().ds = *dd;
+    else moes.back().ds.moe = *m;
     b200awq_op_t a;
     std::memset(&a, 0, sizeof(a));
     a.kind = B200AWQ_OP_LINEAR_GEMM;
@@ -798,14 +791,12 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     b.qzeros = m->w2_qzeros;
     b.y = op.y;
     xops.push_back(a);
-    xfold.push_back(MoeFold{1, mi});
+    xmoe.emplace_back(1, mi);
     xops.push_back(b);
-    xfold.push_back(MoeFold{2, mi});
+    xmoe.emplace_back(2, mi);
   }
   const b200awq_op_t* ops = xops.data();
   const int n = static_cast<int>(xops.size());
-  std::vector<MoeFold> fold;     // per table entry
-  std::vector<ProgOp> table;
   struct Glue {
     int kind;
     const void* src;
@@ -820,25 +811,37 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   // plan: the folding alone, for `plan->grid` SMs and residual window `plan->window`, without any CUDA call
   const int grid = plan != nullptr ? plan->grid : prog_sm_count();
   const int res_window = plan != nullptr && plan->window > 0 ? plan->window : kSpResWindow;
-  std::vector<int> stage_row;    // per table entry: the op whose WHOLE published row its staging waits for, or -1
   int M = -1;
-  std::vector<ResFold> res;     // per table entry: the ADD folded into it, if any
-  std::vector<std::pair<const void*, size_t>> ext_res;   // external residuals: no op of the program may write them
-  std::vector<b200awq_rope_t> ropes;   // per table entry: the ROPE_KV folded into it (head_dim == 0: none)
-  std::vector<int> rope_ops;           // table entries that carry one
-  std::vector<b200awq_qk_norm_rope_t> qkns;   // per table entry: a QK_NORM_ROPE_KV's descriptor (q_norm_weight == null:
-                                              // none, or a plain ROPE_KV)
+  // extents in bytes: M contiguous fp16 rows of `width`; an op's source (M rows at pitch src_ld, gate|up for SiLU*mul)
+  // and output; a glue record's output and source
+  auto rows_bytes = [&](int width) { return (size_t)(M > 0 ? M : 1) * width * 2; };
+  auto src_bytes = [&](const ProgOp& p) {
+    return ((size_t)(M - 1) * p.src_ld + (size_t)(p.prologue == kProSilu ? 2 : 1) * p.K) * 2;
+  };
+  auto y_bytes = [&](const ProgOp& p) { return rows_bytes(p.N); };
+  auto glue_out_bytes = [&](const Glue& gl) { return rows_bytes(gl.width); };
+  auto glue_src_bytes = [&](const Glue& gl) { return rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width); };
+  // a write over something a live glue record (other than `keep`) still needs ends that record; false: the record was
+  // never used, so it would never run
+  auto glue_write = [&](const void* p, size_t bytes, const Glue* keep) {
+    for (Glue& gl : glues)
+      if (gl.live && &gl != keep &&
+          (overlaps(gl.out, glue_out_bytes(gl), p, bytes) || overlaps(gl.src, glue_src_bytes(gl), p, bytes))) {
+        if (!gl.used) return false;
+        gl.live = false;
+      }
+    return true;
+  };
+  // a read of a linear's raw output after an ADD was folded into it: its row carries the sum, not y
+  auto reads_raw_y = [&](const void* p, size_t bytes) {
+    for (const ProgOp& t : table)
+      if (t.raw_y != nullptr && overlaps(t.raw_y, y_bytes(t), p, bytes)) return true;
+    return false;
+  };
   for (int i = 0; i < n; ++i) {
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
     if (op.M != M) return B200AWQ_EUNSUPPORTED;
-    auto rows_bytes = [&](int width) { return (size_t)(M > 0 ? M : 1) * width * 2; };   // M contiguous fp16 rows
-    // a read of a linear's raw output after an ADD was folded into it: its row carries the sum, not y
-    auto reads_raw_y = [&](const void* p, size_t bytes) {
-      for (size_t j = 0; j < table.size(); ++j)
-        if (res[j].raw_y != nullptr && overlaps(res[j].raw_y, rows_bytes(table[j].N), p, bytes)) return true;
-      return false;
-    };
     if (op.kind == B200AWQ_OP_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV) {
       // RoPE + cache append, folded into the finish of the linear recorded just before it (whose whole output is qkv);
       // QK_NORM_ROPE_KV: the same op on its embedded descriptor, with q / k normalised first
@@ -852,14 +855,13 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       if (qkn && (!aligned16(qd->q_norm_weight) || !aligned16(qd->k_norm_weight))) return B200AWQ_EUNSUPPORTED;
       const int D = r->head_dim;
       if (op.N != (r->n_heads + 2 * r->n_kv_heads) * D || (D % 16) != 0) return B200AWQ_EUNSUPPORTED;
-      // (an ADD or a glue op in between: the op before is not a linear; a SPARSE_MOE's entries are not plain linears)
-      if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty() || fold.back().kind != 0)
+      // (an ADD or a glue op in between: the op before is not a linear; a MoE block's ops are not plain linears)
+      if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty() || table.back().moe != 0)
         return B200AWQ_EUNSUPPORTED;
-      const ProgOp& pv = table.back();
+      ProgOp& pv = table.back();
       if (op.x != pv.y || op.N != pv.N || (M > 1 && op.ldx != op.N)) return B200AWQ_EUNSUPPORTED;
-      ropes.back() = *r;
-      if (qkn) qkns.back() = *qd;
-      rope_ops.push_back(static_cast<int>(table.size()) - 1);
+      if (qkn) pv.qkr = *qd;
+      else pv.qkr.rope = *r;
       continue;
     }
     if (op.kind == B200AWQ_OP_ADD) {
@@ -875,35 +877,26 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       else if (op.weight == pv.y) r = op.x;
       else return B200AWQ_EUNSUPPORTED;  // neither operand is the producer's output (both external)
       if (op.K != pv.N || overlaps(r, bytes, pv.y, bytes)) return B200AWQ_EUNSUPPORTED;
-      ResFold rf;
-      rf.raw_y = pv.y;
       // in-program residual: the newest op that wrote any of it must have published exactly it, kSpResWindow ops back
-      for (int j = static_cast<int>(table.size()) - 2; j >= 0 && rf.op < 0; --j) {
-        const bool hit = overlaps(table[j].y, rows_bytes(table[j].N), r, bytes) ||
-                         (res[j].raw_y != nullptr && overlaps(res[j].raw_y, rows_bytes(table[j].N), r, bytes));
+      int res_op = -1;
+      for (int j = static_cast<int>(table.size()) - 2; j >= 0 && res_op < 0; --j) {
+        const bool hit = overlaps(table[j].y, y_bytes(table[j]), r, bytes) ||
+                         (table[j].raw_y != nullptr && overlaps(table[j].raw_y, y_bytes(table[j]), r, bytes));
         if (!hit) continue;
         if (r != table[j].y || table[j].N != op.K) return B200AWQ_EUNSUPPORTED;
         if (static_cast<int>(table.size()) - 1 - j > res_window) return B200AWQ_EUNSUPPORTED;
-        rf.op = j;
+        res_op = j;
       }
       for (const Glue& gl : glues)   // a glue output is written by CTA slices, never published as a row
-        if (overlaps(gl.out, rows_bytes(gl.width), r, bytes)) return B200AWQ_EUNSUPPORTED;
-      if (rf.op < 0) {
-        rf.ext = r;
-        ext_res.emplace_back(r, bytes);
-      }
+        if (overlaps(gl.out, glue_out_bytes(gl), r, bytes)) return B200AWQ_EUNSUPPORTED;
       // the output must not overlap what the producer reads (other CTAs may still be staging it) or publishes
-      const size_t pv_src = ((size_t)(M - 1) * pv.src_ld + (size_t)(pv.prologue == kProSilu ? 2 : 1) * pv.K) * 2;
-      if (overlaps(op.y, bytes, pv.src, pv_src) || (pv.xout != nullptr && overlaps(op.y, bytes, pv.xout, rows_bytes(pv.K))))
+      if (overlaps(op.y, bytes, pv.src, src_bytes(pv)) || (pv.xout != nullptr && overlaps(op.y, bytes, pv.xout, rows_bytes(pv.K))))
         return B200AWQ_EUNSUPPORTED;
-      for (Glue& gl : glues)         // writing the output over something a live glue record still needs ends that record
-        if (gl.live && (overlaps(gl.out, rows_bytes(gl.width), op.y, bytes) ||
-                        overlaps(gl.src, rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width), op.y, bytes))) {
-          if (!gl.used) return B200AWQ_EUNSUPPORTED;
-          gl.live = false;
-        }
+      if (!glue_write(op.y, bytes, nullptr)) return B200AWQ_EUNSUPPORTED;
+      pv.raw_y = pv.y;
+      pv.res_op = res_op;
+      pv.res_ext = res_op < 0 ? r : nullptr;
       pv.y = static_cast<__half*>(op.y);   // the producer's row now publishes the sum
-      res.back() = rf;
       continue;
     }
     if (op.kind == B200AWQ_OP_RMSNORM || op.kind == B200AWQ_OP_SILU_AND_MUL) {
@@ -913,16 +906,11 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         return B200AWQ_EUNSUPPORTED;
       const size_t in_bytes = (size_t)M * (op.kind == B200AWQ_OP_SILU_AND_MUL ? 2 : 1) * op.K * 2;
       if (overlaps(op.y, rows_bytes(op.K), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;  // in-place glue op
-      for (Glue& gl : glues)
-        if (gl.live && (overlaps(gl.out, rows_bytes(gl.width), op.y, rows_bytes(op.K)) ||
-                        overlaps(gl.src, rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width), op.y, rows_bytes(op.K)))) {
-          if (!gl.used) return B200AWQ_EUNSUPPORTED;
-          gl.live = false;
-        }
+      if (!glue_write(op.y, rows_bytes(op.K), nullptr)) return B200AWQ_EUNSUPPORTED;
       if (reads_raw_y(op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
       // its input must not be a buffer only CTA 0 publishes
       for (const Glue& gl : glues)
-        if (overlaps(gl.out, rows_bytes(gl.width), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
+        if (overlaps(gl.out, glue_out_bytes(gl), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
       glues.push_back(Glue{op.kind == B200AWQ_OP_RMSNORM ? kProRmsnorm : kProSilu, op.x, op.weight, op.y, op.K, op.eps,
                            false, true});
       continue;
@@ -934,8 +922,6 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (M < 1 || M > max_tokens) return B200AWQ_EUNSUPPORTED;
     if (M > 1 && op.ldx < op.K) return B200AWQ_EINVAL;
     ProgOp p;
-    std::memset(&p, 0, sizeof(p));
-    p.ext_dep = -1;
     p.qw_src = static_cast<const int32_t*>(op.qweight);
     p.scales = static_cast<const __half*>(op.scales);
     p.qzeros = static_cast<const int32_t*>(op.qzeros);
@@ -944,6 +930,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     p.K = op.K;
     p.N = op.N;
     p.G = op.group_size;
+    p.moe = xmoe[i].first;
+    p.mi = xmoe[i].second;
     Glue* hit = nullptr;
     for (Glue& gl : glues)
       if (gl.live && gl.out == op.x && gl.width == op.K) hit = &gl;
@@ -962,99 +950,76 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       p.src_ld = M > 1 ? static_cast<int>(op.ldx) : op.K;
       if (!aligned16(op.x)) return B200AWQ_EUNSUPPORTED;
       for (const Glue& gl : glues)   // reading a buffer only CTA 0 publishes (a dead or mismatching record)
-        if (overlaps(gl.out, rows_bytes(gl.width), op.x, ((size_t)(M - 1) * p.src_ld + op.K) * 2)) return B200AWQ_EUNSUPPORTED;
+        if (overlaps(gl.out, glue_out_bytes(gl), op.x, src_bytes(p))) return B200AWQ_EUNSUPPORTED;
     }
     // the source's M rows (row pitch src_ld), this op's output (M rows of N)
-    const size_t src_bytes = ((size_t)(M - 1) * p.src_ld + (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K) * 2;
-    const size_t y_bytes = rows_bytes(op.N);
-    if (overlaps(p.y, y_bytes, p.src, src_bytes) || reads_raw_y(p.src, src_bytes)) return B200AWQ_EUNSUPPORTED;
-    if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), p.y, y_bytes)) return B200AWQ_EUNSUPPORTED;
+    const size_t sb = src_bytes(p), yb = y_bytes(p);
+    if (overlaps(p.y, yb, p.src, sb) || reads_raw_y(p.src, sb)) return B200AWQ_EUNSUPPORTED;
+    if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), p.y, yb)) return B200AWQ_EUNSUPPORTED;
     if (!table.empty()) {
       // the previous op's fp16 output reaches memory only while THIS op stages its activations: a source inside it
       // is taken from the previous op's fp32 accumulators instead (same values), anything else touching it is a race
       const ProgOp& pv = table.back();
       const uintptr_t y0 = reinterpret_cast<uintptr_t>(pv.y), s0 = reinterpret_cast<uintptr_t>(p.src);
-      if (s0 >= y0 && s0 + src_bytes <= y0 + rows_bytes(pv.N)) {
+      if (s0 >= y0 && s0 + sb <= y0 + y_bytes(pv)) {
         if (((s0 - y0) & 15) != 0) return B200AWQ_EUNSUPPORTED;
         p.src_prev = 1;
         p.src_off = static_cast<int>((s0 - y0) / 2);
-      } else if (overlaps(pv.y, rows_bytes(pv.N), p.src, src_bytes)) {
+      } else if (overlaps(pv.y, y_bytes(pv), p.src, sb)) {
         return B200AWQ_EUNSUPPORTED;
       } else {
         // a source written by an older op of this program: wait for that op's duty-warp stores
         for (int j = static_cast<int>(table.size()) - 2; j >= 0; --j)
-          if (overlaps(table[j].y, rows_bytes(table[j].N), p.src, src_bytes)) {
+          if (overlaps(table[j].y, y_bytes(table[j]), p.src, sb)) {
             p.ext_dep = j;
             break;
           }
       }
-      if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), pv.y, rows_bytes(pv.N))) return B200AWQ_EUNSUPPORTED;
+      if (p.xout != nullptr && overlaps(p.xout, rows_bytes(op.K), pv.y, y_bytes(pv))) return B200AWQ_EUNSUPPORTED;
     }
-    // writing y over something a live glue record still needs ends that record
-    for (Glue& gl : glues)
-      if (gl.live && &gl != hit &&
-          (overlaps(gl.out, rows_bytes(gl.width), p.y, y_bytes) ||
-           overlaps(gl.src, rows_bytes((gl.kind == kProSilu ? 2 : 1) * gl.width), p.y, y_bytes))) {
-        if (!gl.used) return B200AWQ_EUNSUPPORTED;
-        gl.live = false;
-      }
-    {
-      // a staging wait on the whole row of op s waits for every CTA that owns columns of s
-      const int s = p.src_prev ? static_cast<int>(table.size()) - 1 : p.ext_dep;
-      const size_t width = (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K;
-      stage_row.push_back(s >= 0 && p.src == table[s].y && width == (size_t)table[s].N ? s : -1);
-    }
+    if (!glue_write(p.y, yb, hit)) return B200AWQ_EUNSUPPORTED;
+    // a staging wait on the whole row of op s waits for every CTA that owns columns of s
+    const int s = p.src_prev ? static_cast<int>(table.size()) - 1 : p.ext_dep;
+    const size_t width = (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K;
+    p.stage_row = s >= 0 && p.src == table[s].y && width == (size_t)table[s].N ? s : -1;
     table.push_back(p);
-    fold.push_back(xfold[i]);
-    res.emplace_back();
-    ropes.emplace_back();
-    std::memset(&ropes.back(), 0, sizeof(b200awq_rope_t));
-    qkns.emplace_back();
-    std::memset(&qkns.back(), 0, sizeof(b200awq_qk_norm_rope_t));
   }
   for (const Glue& gl : glues)
     if (!gl.used) return B200AWQ_EUNSUPPORTED;   // a glue op nobody consumes would never run
   if (table.empty()) return B200AWQ_EUNSUPPORTED;
   const int nt = static_cast<int>(table.size());
-  for (const auto& er : ext_res) {
+  for (const ProgOp& t : table) {
     // an external residual is read at the finish of its op, any time during the run: nothing of the program may write it
-    for (int j = 0; j < nt; ++j)
-      if (overlaps(table[j].y, (size_t)M * table[j].N * 2, er.first, er.second) ||
-          (res[j].raw_y != nullptr && overlaps(res[j].raw_y, (size_t)M * table[j].N * 2, er.first, er.second)))
+    if (t.res_ext == nullptr) continue;
+    const size_t eb = y_bytes(t);
+    for (const ProgOp& o : table)
+      if (overlaps(o.y, y_bytes(o), t.res_ext, eb) || (o.raw_y != nullptr && overlaps(o.raw_y, y_bytes(o), t.res_ext, eb)))
         return B200AWQ_EUNSUPPORTED;
     for (const Glue& gl : glues)
-      if (overlaps(gl.out, (size_t)M * gl.width * 2, er.first, er.second)) return B200AWQ_EUNSUPPORTED;
-    for (const b200awq_moe_t& m : moes)
-      if (overlaps(m.gate_up, (size_t)m.top_k * 2 * m.I * 2, er.first, er.second) ||
-          overlaps(m.act, (size_t)m.top_k * m.I * 2, er.first, er.second) ||
-          overlaps(m.down, (size_t)m.top_k * m.H * 2, er.first, er.second) ||
-          overlaps(m.logits, (size_t)m.E * 2, er.first, er.second) ||
-          overlaps(m.topk_weights, (size_t)m.top_k * M * 4, er.first, er.second) ||
-          overlaps(m.topk_ids, (size_t)m.top_k * M * 4, er.first, er.second) ||
-          overlaps(m.token_expert_indices, (size_t)m.top_k * M * 4, er.first, er.second) ||
-          overlaps(m.sorted_ids, (size_t)m.sorted_len * 4, er.first, er.second) ||
-          overlaps(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4, er.first, er.second) ||
-          overlaps(m.num_tokens_post_pad, 4, er.first, er.second))
-        return B200AWQ_EUNSUPPORTED;
-    for (const b200awq_deepseek_moe_t& d : dsks)   // (zero for other blocks: overlaps nothing)
-      if (overlaps(d.moe.gate_up, (size_t)(d.moe.top_k * 2 * d.moe.I + 2 * d.I_s) * 2, er.first, er.second) ||
-          overlaps(d.moe.act, (size_t)(d.moe.top_k * d.moe.I + d.I_s) * 2, er.first, er.second) ||
-          overlaps(d.moe.logits, (size_t)d.moe.E * 4, er.first, er.second) ||
-          overlaps(d.shared_out, (size_t)d.moe.H * 2, er.first, er.second))
-        return B200AWQ_EUNSUPPORTED;
+      if (overlaps(gl.out, glue_out_bytes(gl), t.res_ext, eb)) return B200AWQ_EUNSUPPORTED;
+    for (const MoeBlock& b : moes) {
+      const auto x = b.extents(M);
+      for (int k = 0; k < MoeBlock::kMoeWrites; ++k)
+        if (overlaps(x[k].first, x[k].second, t.res_ext, eb)) return B200AWQ_EUNSUPPORTED;
+    }
   }
   // ROPE_KV: the rotated q and the appended cache rows are written in a finish, while other CTAs run later ops.  No
   // other op of the program may read or write them, nor write the position / frequency table the finish reads; the
   // producer must not be a gate|up whose product a SiLU*mul reads (its row would hold silu(gate) * up).
   // QK_NORM_ROPE_KV: its two norm weights are reads like the position and the frequency table.
-  for (int ri : rope_ops) {
-    const b200awq_rope_t& r = ropes[ri];
+  auto rope_outs = [&](const b200awq_rope_t& r) {
     const size_t cache = ((size_t)(M - 1) * r.cache_batch_stride + (size_t)r.cache_len * r.n_kv_heads * r.head_dim) * 2;
-    const std::pair<const void*, size_t> outs[3] = {{r.q_out, (size_t)M * r.n_heads * r.head_dim * 2},
-                                                    {r.k_cache, cache}, {r.v_cache, cache}};
-    const size_t wn = qkns[ri].q_norm_weight != nullptr ? (size_t)r.head_dim * 2 : 0;   // (null, 0: overlaps nothing)
+    return std::array<std::pair<const void*, size_t>, 3>{
+        {{r.q_out, (size_t)M * r.n_heads * r.head_dim * 2}, {r.k_cache, cache}, {r.v_cache, cache}}};
+  };
+  for (int ri = 0; ri < nt; ++ri) {
+    const b200awq_qk_norm_rope_t& q = table[ri].qkr;
+    const b200awq_rope_t& r = q.rope;
+    if (r.head_dim == 0) continue;
+    const auto outs = rope_outs(r);
+    const size_t wn = q.q_norm_weight != nullptr ? (size_t)r.head_dim * 2 : 0;   // (null, 0: overlaps nothing)
     const std::pair<const void*, size_t> ins[4] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * r.head_dim * 4},
-                                                   {qkns[ri].q_norm_weight, wn}, {qkns[ri].k_norm_weight, wn}};
+                                                   {q.q_norm_weight, wn}, {q.k_norm_weight, wn}};
     auto hits_out = [&](const void* p, size_t b) {
       for (const auto& o : outs)
         if (overlaps(o.first, o.second, p, b)) return true;
@@ -1071,37 +1036,24 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         overlaps(outs[1].first, outs[1].second, outs[2].first, outs[2].second))
       return B200AWQ_EUNSUPPORTED;
     for (int j = 0; j < nt; ++j) {
-      const size_t src_bytes = ((size_t)(M - 1) * table[j].src_ld + (size_t)(table[j].prologue == kProSilu ? 2 : 1) * table[j].K) * 2;
-      if (hits_any(table[j].y, (size_t)M * table[j].N * 2) ||
-          (res[j].raw_y != nullptr && hits_any(res[j].raw_y, (size_t)M * table[j].N * 2)) ||
-          (table[j].src != nullptr && hits_out(table[j].src, src_bytes)) ||
-          (res[j].ext != nullptr && hits_out(res[j].ext, (size_t)M * table[j].N * 2)))
+      const ProgOp& o = table[j];
+      if (hits_any(o.y, y_bytes(o)) || (o.raw_y != nullptr && hits_any(o.raw_y, y_bytes(o))) ||
+          (o.src != nullptr && hits_out(o.src, src_bytes(o))) || (o.res_ext != nullptr && hits_out(o.res_ext, y_bytes(o))))
         return B200AWQ_EUNSUPPORTED;
-      if (table[j].prologue == kProSilu && overlaps(table[j].src, src_bytes, table[ri].y, (size_t)M * table[ri].N * 2))
+      if (o.prologue == kProSilu && overlaps(o.src, src_bytes(o), table[ri].y, y_bytes(table[ri])))
         return B200AWQ_EUNSUPPORTED;   // a SiLU*mul of the qkv output: the producer would be a mode-1 gate|up
-      if (j != ri && ropes[j].head_dim != 0) {   // another ROPE_KV: its outputs are writes, its inputs reads
-        const b200awq_rope_t& o = ropes[j];
-        const size_t oc = ((size_t)(M - 1) * o.cache_batch_stride + (size_t)o.cache_len * o.n_kv_heads * o.head_dim) * 2;
-        if (hits_any(o.q_out, (size_t)M * o.n_heads * o.head_dim * 2) || hits_any(o.k_cache, oc) || hits_any(o.v_cache, oc))
-          return B200AWQ_EUNSUPPORTED;
-      }
+      if (j != ri && o.qkr.rope.head_dim != 0)   // another ROPE_KV: its outputs are writes, its inputs reads
+        for (const auto& w : rope_outs(o.qkr.rope))
+          if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
     }
     for (const Glue& gl : glues)
-      if (hits_any(gl.out, (size_t)M * gl.width * 2) || hits_out(gl.src, (size_t)M * (gl.kind == kProSilu ? 2 : 1) * gl.width * 2))
-        return B200AWQ_EUNSUPPORTED;
-    for (const b200awq_moe_t& m : moes)
-      if (hits_any(m.gate_up, (size_t)m.top_k * 2 * m.I * 2) || hits_any(m.act, (size_t)m.top_k * m.I * 2) ||
-          hits_any(m.down, (size_t)m.top_k * m.H * 2) || hits_any(m.logits, (size_t)m.E * 2) ||
-          hits_any(m.topk_weights, (size_t)m.top_k * M * 4) || hits_any(m.topk_ids, (size_t)m.top_k * M * 4) ||
-          hits_any(m.token_expert_indices, (size_t)m.top_k * M * 4) || hits_any(m.sorted_ids, (size_t)m.sorted_len * 4) ||
-          hits_any(m.expert_ids, (size_t)(m.top_k * M + m.E) * 4) || hits_any(m.num_tokens_post_pad, 4) ||
-          hits_out(m.gate_weight, (size_t)m.E * m.H * 2))
-        return B200AWQ_EUNSUPPORTED;
-    for (const b200awq_deepseek_moe_t& d : dsks)
-      if (hits_any(d.moe.gate_up, (size_t)(d.moe.top_k * 2 * d.moe.I + 2 * d.I_s) * 2) ||
-          hits_any(d.moe.act, (size_t)(d.moe.top_k * d.moe.I + d.I_s) * 2) || hits_any(d.moe.logits, (size_t)d.moe.E * 4) ||
-          hits_any(d.shared_out, (size_t)d.moe.H * 2) || hits_out(d.bias, d.bias != nullptr ? (size_t)d.moe.E * 4 : 0))
-        return B200AWQ_EUNSUPPORTED;
+      if (hits_any(gl.out, glue_out_bytes(gl)) || hits_out(gl.src, glue_src_bytes(gl))) return B200AWQ_EUNSUPPORTED;
+    for (const MoeBlock& b : moes) {
+      const auto x = b.extents(M);
+      for (int k = 0; k < (int)x.size(); ++k)
+        if (k < MoeBlock::kMoeWrites ? hits_any(x[k].first, x[k].second) : hits_out(x[k].first, x[k].second))
+          return B200AWQ_EUNSUPPORTED;
+    }
   }
   for (int i = 0; i < nt; ++i) {
     // An in-program residual (row j % 4) is read in op i's finish, by the CTA that published those columns in op j (same
@@ -1110,14 +1062,14 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     // finished op i: some op in (i, k] must stage the WHOLE row of an op >= i that every CTA owns columns of (a wait on a
     // slice of a row, or on a narrow op, waits for a few CTAs only).  tests/test_stream_residual_model.py replays random
     // programs through this rule (b200awq_program_plan).
-    const int j = res[i].op;
+    const int j = table[i].res_op;
     if (j < 0) continue;
     int k = j + kSpRows;
     while (k <= i) k += kSpRows;
     if (k >= nt) continue;
     int reach = -1;
     for (int m = i + 1; m <= k; ++m) {
-      const int s = stage_row[m];
+      const int s = table[m].stage_row;
       if (s >= 0 && table[s].N / 16 >= grid) reach = std::max(reach, s);
     }
     if (reach < i) return B200AWQ_EUNSUPPORTED;
@@ -1133,7 +1085,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   pr->n_ops = nt;
   pr->M = M;
   cudaError_t e = cudaGetDevice(&pr->device);
-  if (e == cudaSuccess && stream_build(pr, table, grid, M, &e, fold, moes, res, ropes, qkns, moe_hf, dsks)) {
+  if (e == cudaSuccess && stream_build(pr, f, grid, &e)) {
     *out = pr;
     return B200AWQ_OK;
   }
@@ -1153,145 +1105,71 @@ size_t program_stream_bytes(const Program* p) { return p->stream_bytes; }
 cudaError_t program_run(Program* p, cudaStream_t st) {
   cudaError_t e = program_abort_clear(st);
   if (e != cudaSuccess) return e;
-  if (p->M > 1) {
-    // batched stream variant: 8 consumer warps, the ring depth chosen at creation, MT = the smallest of 2 / 4 / 8 >= M
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(prog_sm_count());
-    cfg.blockDim = dim3(32 + kSbWarps * 32);
-    cfg.dynamicSmemBytes = sb_fixed_smem(p->sb_spw, p->sb_lmax, sb_mt(p->M), p->sb_nu_max) + p->xs_bytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: the hand-off polls are grid-wide waits
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    const SpOp* sops = p->d_sp_ops;
-    const uint32_t* cta = p->d_cta;
-    if (p->d_qkn != nullptr) {   // a QK_NORM_ROPE_KV op: the rope kernel plus the two-phase q / k norm
-      auto nk = sb_mt(p->M) == 2 ? stream_batch_qknorm_kernel<2>
-                                 : (sb_mt(p->M) == 4 ? stream_batch_qknorm_kernel<4> : stream_batch_qknorm_kernel<8>);
-      const SpRes* rd = p->d_res;
-      const SpRope* qd = p->d_rope;
-      const SpQkNorm* nd = p->d_qkn;
-      return cudaLaunchKernelEx(&cfg, nk, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
-                                p->sb_lmax, p->sb_nu_max, knob(3), rd, qd, nd);
-    }
-    if (p->d_rope != nullptr) {  // a ROPE_KV op: the residual kernel plus the rope steps of a mode-2 finish
-      auto qk = sb_mt(p->M) == 2 ? stream_batch_rope_kernel<2>
-                                 : (sb_mt(p->M) == 4 ? stream_batch_rope_kernel<4> : stream_batch_rope_kernel<8>);
-      const SpRes* rd = p->d_res;
-      const SpRope* qd = p->d_rope;
-      return cudaLaunchKernelEx(&cfg, qk, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
-                                p->sb_lmax, p->sb_nu_max, knob(3), rd, qd);
-    }
-    if (p->d_res != nullptr) {   // residual adds: the same kernel with the residual steps in its finish
-      auto rk = sb_mt(p->M) == 2 ? stream_batch_residual_kernel<2>
-                                 : (sb_mt(p->M) == 4 ? stream_batch_residual_kernel<4> : stream_batch_residual_kernel<8>);
-      const SpRes* rd = p->d_res;
-      return cudaLaunchKernelEx(&cfg, rk, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
-                                p->sb_lmax, p->sb_nu_max, knob(3), rd);
-    }
-    auto kern = sb_mt(p->M) == 2 ? stream_batch_kernel<2> : (sb_mt(p->M) == 4 ? stream_batch_kernel<4> : stream_batch_kernel<8>);
-    return cudaLaunchKernelEx(&cfg, kern, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M, p->sb_spw,
-                              p->sb_lmax, p->sb_nu_max, knob(3));
-  }
-  // knob 9: consumer warps of the stream kernel: 8 (4 units in flight; the default) or 12 (2 units), each with the ring
-  // depth chosen at creation (at least 4 / 3 stages).  No 16-warp variant: 17 warps put 5 on one of the SM's four
-  // register-file partitions, which caps a thread at 96 registers on sm_90 and spills the unit loop.  The MoE, residual
-  // and rope kernels always run 8 warps.
-  const bool moe_k = p->d_rope != nullptr || p->d_res != nullptr || p->n_moe > 0;
-  const int nw = knob(9) == 12 && !moe_k ? 12 : 8;
+  const ProgKernel k = p->kernel;
+  // knob 9: consumer warps of the plain M = 1 kernel: 8 (4 units in flight; the default) or 12 (2 units), each with the
+  // ring depth chosen at creation (at least 4 / 3 stages).  No 16-warp variant: 17 warps put 5 on one of the SM's four
+  // register-file partitions, which caps a thread at 96 registers on sm_90 and spills the unit loop.  Every other
+  // kernel runs 8 warps; a batched one the ring depth chosen at creation, at MT = the smallest of 2 / 4 / 8 >= M.
+  const int nw = k == kKernPlain && knob(9) == 12 ? 12 : 8;
   const int spw = nw == 8 ? p->sp_spw8 : p->sp_spw12;
   const int grid = prog_sm_count();
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(32 + nw * 32);
-  cfg.dynamicSmemBytes = sp_fixed_smem(nw, spw, moe_k) + p->xs_bytes;
+  cfg.dynamicSmemBytes = p->xs_bytes + (p->M > 1 ? sb_fixed_smem(p->sb_spw, p->sb_lmax, sb_mt(p->M), p->sb_nu_max)
+                                                 : sp_fixed_smem(nw, spw, k != kKernPlain));
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: the hand-off polls are grid-wide waits
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  const SpOp* sops = p->d_sp_ops;
-  const uint32_t* cta = p->d_cta;
-  // knob 8: the HBM -> L2 run-ahead window of the weight stream, grid-wide, in MB, at most the device's L2 (<= 0: off,
-  // the default).  The producer advances its prefetch cursor only while it has no ring stage to fill - during op
-  // hand-offs and tails - and each of its grid x nw lanes keeps at most window / (grid x nw) bytes ahead of its ring.
-  // Off is the default: on the bench step no window beat it by more than its run-to-run spread (H100 SXM, DESIGN
-  // 3.5b: 8 and 16 MB within 0.5 %, 32 MB 4 % slower).
-  const size_t window = knob(8) <= 0 ? 0 : std::min((size_t)knob(8) << 20, (size_t)p->l2_bytes);
-  const int l2_ahead = (int)(window / ((size_t)grid * nw));
-  // knob 10: ops ahead of the consumers' staging for which shared-memory loads may already be issued (0 = ungated,
-  // the default: a gate of 2 measured 1.5-2 % slower on the bench step, DESIGN 3.5b; n > 0: at most n - 1 ops ahead,
-  // 1 = strictly gated)
-  const int gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
-  const SpMoe* no_moe = nullptr;
-  if (p->d_dsk != nullptr) {    // programs with DEEPSEEK_MOE blocks (every side table allocated)
-    const SpMoe* md = p->d_moe;
-    const SpRes* rd = p->d_res;
-    const SpRope* qd = p->d_rope;
-    const SpQkNorm* nd = p->d_qkn;
-    const SpDsk* dd = p->d_dsk;
-    return cudaLaunchKernelEx(&cfg, stream_deepseek_moe_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                              p->d_state, spw, knob(3), l2_ahead, gate_ahead, md, rd, qd, nd, dd);
+  int l2_ahead = 0, gate_ahead = 0;
+  if (p->M == 1) {
+    // knob 8: the HBM -> L2 run-ahead window of the weight stream, grid-wide, in MB, at most the device's L2 (<= 0:
+    // off, the default).  The producer advances its prefetch cursor only while it has no ring stage to fill - during op
+    // hand-offs and tails - and each of its grid x nw lanes keeps at most window / (grid x nw) bytes ahead of its ring.
+    // Off is the default: on the bench step no window beat it by more than its run-to-run spread (H100 SXM, DESIGN
+    // 3.5b: 8 and 16 MB within 0.5 %, 32 MB 4 % slower).
+    const size_t window = knob(8) <= 0 ? 0 : std::min((size_t)knob(8) << 20, (size_t)p->l2_bytes);
+    l2_ahead = (int)(window / ((size_t)grid * nw));
+    // knob 10: ops ahead of the consumers' staging for which shared-memory loads may already be issued (0 = ungated,
+    // the default: a gate of 2 measured 1.5-2 % slower on the bench step, DESIGN 3.5b; n > 0: at most n - 1 ops ahead,
+    // 1 = strictly gated)
+    gate_ahead = knob(10) <= 0 ? 1 << 20 : knob(10) - 1;
   }
-  if (p->qwen3) {    // programs with QWEN3_MOE blocks (every side table allocated)
-    const SpMoe* md = p->d_moe;
-    const SpRes* rd = p->d_res;
-    const SpRope* qd = p->d_rope;
-    const SpQkNorm* nd = p->d_qkn;
-    return cudaLaunchKernelEx(&cfg, stream_qwen3moe_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
-                              spw, knob(3), l2_ahead, gate_ahead, md, rd, qd, nd);
+  auto batch = [&](auto kern, auto... side) {
+    return cudaLaunchKernelEx(&cfg, kern, p->d_sp_ops, p->d_cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, p->M,
+                              p->sb_spw, p->sb_lmax, p->sb_nu_max, knob(3), side...);
+  };
+  auto stream = [&](auto kern, auto... side) {   // (d_moe: null without MoE blocks)
+    return cudaLaunchKernelEx(&cfg, kern, p->d_sp_ops, p->d_cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
+                              knob(3), l2_ahead, gate_ahead, p->d_moe, side...);
+  };
+  switch (k) {
+    case kKernPlain: return nw == 8 ? stream(stream_program_kernel<8, 4>) : stream(stream_program_kernel<12, 2>);
+    case kKernMoe: return stream(stream_moe_kernel);
+    case kKernResidual: return stream(stream_residual_kernel, p->d_res);
+    case kKernRope: return stream(stream_rope_kernel, p->d_res, p->d_rope);
+    case kKernQkNorm: return stream(stream_qknorm_kernel, p->d_res, p->d_rope, p->d_qkn);
+    case kKernQwen3Moe: return stream(stream_qwen3moe_kernel, p->d_res, p->d_rope, p->d_qkn);
+    case kKernDeepseekMoe: return stream(stream_deepseek_moe_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk);
+    case kKernBatch2: return batch(stream_batch_kernel<2>);
+    case kKernBatch4: return batch(stream_batch_kernel<4>);
+    case kKernBatch8: return batch(stream_batch_kernel<8>);
+    case kKernBatchResidual2: return batch(stream_batch_residual_kernel<2>, p->d_res);
+    case kKernBatchResidual4: return batch(stream_batch_residual_kernel<4>, p->d_res);
+    case kKernBatchResidual8: return batch(stream_batch_residual_kernel<8>, p->d_res);
+    case kKernBatchRope2: return batch(stream_batch_rope_kernel<2>, p->d_res, p->d_rope);
+    case kKernBatchRope4: return batch(stream_batch_rope_kernel<4>, p->d_res, p->d_rope);
+    case kKernBatchRope8: return batch(stream_batch_rope_kernel<8>, p->d_res, p->d_rope);
+    case kKernBatchQkNorm2: return batch(stream_batch_qknorm_kernel<2>, p->d_res, p->d_rope, p->d_qkn);
+    case kKernBatchQkNorm4: return batch(stream_batch_qknorm_kernel<4>, p->d_res, p->d_rope, p->d_qkn);
+    case kKernBatchQkNorm8: return batch(stream_batch_qknorm_kernel<8>, p->d_res, p->d_rope, p->d_qkn);
   }
-  if (p->d_qkn != nullptr) {    // programs with a QK_NORM_ROPE_KV op (with or without other ROPE_KV ops, adds, MoE blocks)
-    const SpMoe* md = p->d_moe;
-    const SpRes* rd = p->d_res;
-    const SpRope* qd = p->d_rope;
-    const SpQkNorm* nd = p->d_qkn;
-    return cudaLaunchKernelEx(&cfg, stream_qknorm_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
-                              knob(3), l2_ahead, gate_ahead, md, rd, qd, nd);
-  }
-  if (p->d_rope != nullptr) {   // programs with a ROPE_KV op (with or without adds / sparse-MoE blocks)
-    const SpMoe* md = p->d_moe;
-    const SpRes* rd = p->d_res;
-    const SpRope* qd = p->d_rope;
-    return cudaLaunchKernelEx(&cfg, stream_rope_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
-                              knob(3), l2_ahead, gate_ahead, md, rd, qd);
-  }
-  if (p->d_res != nullptr) {   // programs with residual adds (with or without sparse-MoE blocks)
-    const SpMoe* md = p->d_moe;
-    const SpRes* rd = p->d_res;
-    return cudaLaunchKernelEx(&cfg, stream_residual_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state,
-                              spw, knob(3), l2_ahead, gate_ahead, md, rd);
-  }
-  if (p->n_moe > 0) {   // programs with sparse-MoE blocks: the MOE instantiation
-    const SpMoe* md = p->d_moe;
-    return cudaLaunchKernelEx(&cfg, stream_moe_kernel, sops, cta, p->n_ops, p->d_rows, p->row_stride, p->d_state, spw,
-                              knob(3), l2_ahead, gate_ahead, md);
-  }
-  if (nw == 8)
-    return cudaLaunchKernelEx(&cfg, stream_program_kernel<8, 4>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                              p->d_state, spw, knob(3), l2_ahead, gate_ahead, no_moe);
-  return cudaLaunchKernelEx(&cfg, stream_program_kernel<12, 2>, sops, cta, p->n_ops, p->d_rows, p->row_stride,
-                            p->d_state, spw, knob(3), l2_ahead, gate_ahead, no_moe);
+  return cudaErrorInvalidValue;   // (not reached: stream_build sets one of the above)
 }
 
-void program_destroy(Program* p) {
-  if (p == nullptr) return;
-  cudaFree(p->d_sp_ops);
-  cudaFree(p->d_stream);
-  cudaFree(p->d_cta);
-  cudaFree(p->d_rows);
-  cudaFree(p->d_state);
-  cudaFree(p->d_moe);
-  cudaFree(p->d_xlog);
-  cudaFree(p->d_dsk);
-  cudaFree(p->d_res);
-  cudaFree(p->d_rope);
-  cudaFree(p->d_qkn);
-  cudaFree(p->d_qkn_part);
-  delete p;
-}
+void program_destroy(Program* p) { delete p; }
 
 }  // namespace b200awq

@@ -580,8 +580,8 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 
 // M = 1 programs with QWEN3_MOE blocks (with or without residual adds, ROPE_KV and QK_NORM_ROPE_KV ops): the qknorm
 // kernel with the Qwen3-MoE routing and finishes, which only SP_QWEN3 compiles in.  Every MoE block of such a program
-// is a QWEN3_MOE block (program_create replays a program that mixes them with SPARSE_MOE per op).  The side tables are
-// always allocated for it (empty entries where an op has no add, rotation or norm).
+// is a QWEN3_MOE block (program_create replays a program that mixes them with SPARSE_MOE per op).  It takes every side
+// table (ProgKernel in program.cu), with empty entries where an op has no add, rotation or norm.
 __global__ void __launch_bounds__(32 + 8 * 32, 1)
     stream_qwen3moe_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
                            uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
