@@ -80,8 +80,22 @@ class QkNormRope(ctypes.Structure):
     ]
 
 
+class Mla(ctypes.Structure):
+    """b200awq_mla_t (include/b200awq.h): the descriptor of b200awq_mla_rope / b200awq_mla_kv and of an MLA_ROPE /
+    MLA_KV op's `weight`."""
+
+    _fields_ = [
+        ("n_heads", ctypes.c_int32), ("nope_dim", ctypes.c_int32), ("rope_dim", ctypes.c_int32),
+        ("v_dim", ctypes.c_int32), ("kv_lora_rank", ctypes.c_int32), ("style", ctypes.c_int32),
+        ("cache_len", ctypes.c_int32), ("freqs_len", ctypes.c_int32), ("k_batch_stride", ctypes.c_int64),
+        ("v_batch_stride", ctypes.c_int64), ("v_head_stride", ctypes.c_int32), ("pad_", ctypes.c_int32),
+        ("pos", ctypes.c_void_p), ("freqs", ctypes.c_void_p), ("q_out", ctypes.c_void_p), ("k_cache", ctypes.c_void_p),
+        ("v_cache", ctypes.c_void_p),
+    ]
+
+
 OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV = 1, 2, 3, 4, 5, 6
-OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE, OP_DEEPSEEK_MOE = 7, 8, 9
+OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE, OP_DEEPSEEK_MOE, OP_MLA_ROPE, OP_MLA_KV = 7, 8, 9, 10, 11
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -110,6 +124,8 @@ SIGNATURES = {
     "b200awq_silu_and_mul": (_c_int, [_c_void_p, _c_void_p, _c_int, _c_int, _c_void_p]),
     "b200awq_rope_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Rope), _c_int, _c_void_p]),
     "b200awq_qk_norm_rope_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(QkNormRope), _c_int, _c_void_p]),
+    "b200awq_mla_rope": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
+    "b200awq_mla_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
     "b200awq_set_knob": (_c_int, [_c_int, _c_int]),
     "b200awq_get_knob": (_c_int, [_c_int]),
     "b200awq_debug_read": (_c_int, [_c_void_p, _c_size_t]),

@@ -2,6 +2,8 @@
 //   rmsnorm       <- awq_ext.layernorm_forward_cuda   (awq/modules/fused/norm.py:33-36)
 //   silu_and_mul  <- awq_ext.silu_and_mul             (awq/modules/fused/moe.py:76)
 //   rope_kv       <- RoPE.forward + WindowedCache.update_kv (awq/modules/fused/attn.py:53-86,243-267)
+//   mla_rope / mla_kv <- the glue of transformers' DeepseekV2Attention / DeepseekV3Attention between the projections
+//                    and attention (rotary, head split, cache write)
 // fp16 in/out, fp32 math.  Bandwidth-trivial (KBs per decode step); kept simple.
 #include "common.cuh"
 #include "kernels.h"
@@ -142,6 +144,63 @@ cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t& r, int
   const int64_t n = (int64_t)M * (r.n_heads + 2 * r.n_kv_heads) * (r.head_dim / 2);
   return launch_kernel(rope_kv_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
                        reinterpret_cast<const __half*>(qkv), ldqkv, r, M);
+}
+
+// one thread per (token row, column pair) of the q_proj | kv_a_proj_with_mqa row; rope.cuh has the arithmetic
+__global__ void __launch_bounds__(256)
+    mla_rope_kernel(const __half* __restrict__ row, int64_t ld, b200awq_mla_t d, int M) {
+  pdl_trigger();
+  pdl_wait();
+  const int pos = mla_pos(d, true);
+  const int pairs = (d.n_heads * (d.nope_dim + d.rope_dim) + d.kv_lora_rank + d.rope_dim) >> 1;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pos < 0 || i >= (int64_t)M * pairs) return;
+  const int m = static_cast<int>(i / pairs), c = 2 * static_cast<int>(i - (int64_t)m * pairs);
+  const __half* r = row + m * ld;
+  mla_rope_pair(d, pos, m, c, r[c], r[c + 1]);
+}
+
+// one thread per (token row, column) of the kv_b_proj row
+__global__ void __launch_bounds__(256)
+    mla_kv_kernel(const __half* __restrict__ row, int64_t ld, b200awq_mla_t d, int M) {
+  pdl_trigger();
+  pdl_wait();
+  const int pos = mla_pos(d, false);
+  const int n = d.n_heads * (d.nope_dim + d.v_dim);
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pos < 0 || i >= (int64_t)M * n) return;
+  const int m = static_cast<int>(i / n), c = static_cast<int>(i - (int64_t)m * n);
+  mla_kv_col(d, pos, m, c, row[m * ld + c]);
+}
+
+// rope: the fields MLA_ROPE reads (q_out, freqs, style, C), else MLA_KV's (v_cache and its geometry); both read pos and
+// k_cache with its geometry
+int mla_validate(const b200awq_mla_t* d, bool rope) {
+  if (d == nullptr || d->pos == nullptr || d->k_cache == nullptr) return B200AWQ_EINVAL;
+  if (d->n_heads <= 0 || d->nope_dim <= 0 || d->rope_dim <= 0 || (d->rope_dim % 2) != 0 || d->cache_len <= 0 ||
+      d->k_batch_stride < (int64_t)d->cache_len * d->n_heads * (d->nope_dim + d->rope_dim))
+    return B200AWQ_EINVAL;
+  if (rope)
+    return d->q_out == nullptr || d->freqs == nullptr || d->kv_lora_rank <= 0 || (d->style != 0 && d->style != 1) ||
+                   d->freqs_len <= 0
+               ? B200AWQ_EINVAL
+               : B200AWQ_OK;
+  return d->v_cache == nullptr || d->v_dim <= 0 || d->v_head_stride < d->v_dim ||
+                 d->v_batch_stride < (int64_t)d->cache_len * d->n_heads * d->v_head_stride
+             ? B200AWQ_EINVAL
+             : B200AWQ_OK;
+}
+
+cudaError_t mla_rope(const void* row, int64_t ld, const b200awq_mla_t& d, int M, cudaStream_t st) {
+  const int64_t n = (int64_t)M * ((d.n_heads * (d.nope_dim + d.rope_dim) + d.kv_lora_rank + d.rope_dim) / 2);
+  return launch_kernel(mla_rope_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
+                       reinterpret_cast<const __half*>(row), ld, d, M);
+}
+
+cudaError_t mla_kv(const void* row, int64_t ld, const b200awq_mla_t& d, int M, cudaStream_t st) {
+  const int64_t n = (int64_t)M * d.n_heads * (d.nope_dim + d.v_dim);
+  return launch_kernel(mla_kv_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
+                       reinterpret_cast<const __half*>(row), ld, d, M);
 }
 
 cudaError_t rmsnorm(const void* x, const void* w, void* out, int rows, int hidden, float eps, cudaStream_t st) {

@@ -147,6 +147,9 @@ struct ProgOp {
   int res_op = -1;
   // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights
   b200awq_qk_norm_rope_t qkr = {};
+  // an MLA_ROPE (mla_kind 1) or MLA_KV (2) folded into the finish
+  b200awq_mla_t mla = {};
+  int mla_kind = 0;
 };
 
 // One MoE op of a folded program (two kernel ops): kind is B200AWQ_OP_SPARSE_MOE, _QWEN3_MOE or _DEEPSEEK_MOE, ds.moe
@@ -186,11 +189,11 @@ struct FoldedProgram {
 // The kernel entry that runs a program (chosen by stream_build).  M = 1: the plain kernel (8 or 12 consumer warps,
 // knob 9) or the 8-warp kernel of the program's features; M > 1: the batched kernels at MT = sb_mt(M).  Side tables:
 // the M = 1 kernels from kKernMoe on take SpMoe (null without MoE blocks), from kKernResidual on SpRes, from kKernRope on
-// SpRope, from kKernQkNorm on SpQkNorm, and kKernDeepseekMoe SpDsk; the batched ones take SpRes from
-// kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2 on.  The Qwen3-MoE and
-// DeepSeek-MoE kernels take every table, with empty entries where an op has no add, rotation or norm.
+// SpRope, from kKernQkNorm on SpQkNorm, kKernDeepseekMoe and kKernMla SpDsk, and kKernMla SpMla; the batched ones take
+// SpRes from kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2 on.  The Qwen3-MoE,
+// DeepSeek-MoE and MLA kernels take every table, with empty entries where an op has no add, rotation or norm.
 enum ProgKernel {
-  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe,
+  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe, kKernMla,
   kKernBatch2, kKernBatch4, kKernBatch8, kKernBatchResidual2, kKernBatchResidual4, kKernBatchResidual8,
   kKernBatchRope2, kKernBatchRope4, kKernBatchRope8, kKernBatchQkNorm2, kKernBatchQkNorm4, kKernBatchQkNorm8
 };
@@ -225,13 +228,14 @@ struct Program {
   SpRope* d_rope = nullptr;
   SpQkNorm* d_qkn = nullptr;
   unsigned long long* d_qkn_part = nullptr;
+  SpMla* d_mla = nullptr;
 
   Program() = default;
   Program(const Program&) = delete;
   Program& operator=(const Program&) = delete;
   ~Program() {
     for (void* d : std::initializer_list<void*>{d_sp_ops, d_stream, d_cta, d_rows, d_state, d_moe, d_xlog, d_dsk, d_res,
-                                                d_rope, d_qkn, d_qkn_part})
+                                                d_rope, d_qkn, d_qkn_part, d_mla})
       cudaFree(d);
   }
 };
@@ -302,7 +306,7 @@ bool stream_format_supported(int K, int N, int G, int mode) {
   if (K <= 0 || N <= 0 || G <= 0 || (K % G) != 0 || (N % 16) != 0 || (K % 128) != 0) return false;
   if (!(G == 32 || G == 64 || (G % 128) == 0)) return false;
   if (mode == 1 && ((N / 2) % 8) != 0) return false;
-  return mode == 0 || mode == 1;
+  return mode == 0 || mode == 1 || mode == 3;
 }
 static int prog_sm_count();   // device SM count (defined below)
 
@@ -335,8 +339,12 @@ cudaError_t stream_pack(const int32_t* qweight, const void* scales, const int32_
   const int64_t total = (int64_t)(N / 16) * (K / UK) * ((UK / 16) * 32 + 12);
   const int cap = prog_sm_count() * 16;
   const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
-  stream_pack_kernel<<<blocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros,
-                                             static_cast<uint8_t*>(out), K, N, G, mode);
+  if (mode == 3)   // (a kernel of its own: stream_pack_kernel keeps its code)
+    stream_pack_pairs_kernel<<<blocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros,
+                                                     static_cast<uint8_t*>(out), K, N, G);
+  else
+    stream_pack_kernel<<<blocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros,
+                                               static_cast<uint8_t*>(out), K, N, G, mode);
   return cudaGetLastError();
 }
 
@@ -355,6 +363,8 @@ static cudaError_t upload(T** d, const std::vector<T>& h) {
 // its published row (K' = top_k I); both stream E per-expert slices packed back to back.
 // ROPE_KV ops (`qkr.rope.head_dim` != 0): packed in mode 2, the finish rotates / appends (SpRope).
 // QK_NORM_ROPE_KV ops: as ROPE_KV, and `qkr` carries the norm weights (q_norm_weight != null: SpQkNorm).
+// MLA_ROPE ops (`mla_kind` 1): packed in mode 3, the finish rotates / stores (SpMla); MLA_KV (2): mode 0, the finish
+// stores the cache columns.  Such a program runs stream_mla_kernel, whose MoE blocks are DEEPSEEK_MOE blocks.
 static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaError_t* err) {
   *err = cudaSuccess;
   const std::vector<ProgOp>& table = f.table;
@@ -365,6 +375,9 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   // a QWEN3_MOE (DEEPSEEK_MOE) program runs stream_qwen3moe_kernel (stream_deepseek_moe_kernel), whose MoE blocks are
   // all of that kind
   const int mkind = has_moe ? f.moes[0].kind : B200AWQ_OP_SPARSE_MOE;
+  // MLA ops run on stream_mla_kernel, whose MoE blocks are DEEPSEEK_MOE blocks
+  for (const ProgOp& p : table)
+    if (p.mla_kind != 0 && has_moe && mkind != B200AWQ_OP_DEEPSEEK_MOE) return false;
   for (const MoeBlock& b : f.moes)
     if (b.kind != mkind) return false;
   std::vector<int> plan_a(f.moes.size() * 8);
@@ -410,7 +423,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   };
   for (int i = 0; i < n; ++i)
     if (table[i].moe == 1) mode[i] = 1;
-  bool has_rope = false, has_qkn = false, has_res = false;
+  bool has_rope = false, has_qkn = false, has_res = false, has_mla = false;
   for (int i = 0; i < n; ++i) {
     if (table[i].qkr.rope.head_dim != 0) {
       if (mode[i] != 0) return false;   // (program_create rejects a gate|up producer already)
@@ -418,7 +431,13 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
       has_rope = true;
     }
     has_qkn = has_qkn || table[i].qkr.q_norm_weight != nullptr;
+    if (table[i].mla_kind != 0) {
+      if (mode[i] != 0) return false;
+      if (table[i].mla_kind == 1) mode[i] = 3;
+      has_mla = true;
+    }
   }
+  if (has_mla && M != 1) return false;   // (program_create rejects it already)
   // residual adds: the producer and an in-program residual must publish plain columns (a mode-1 row holds SiLU*mul)
   for (int i = 0; i < n; ++i)
     if (table[i].raw_y != nullptr) {
@@ -431,6 +450,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   const ProgKernel kern =
       M > 1 ? ProgKernel((has_qkn ? kKernBatchQkNorm2 : has_rope ? kKernBatchRope2 : has_res ? kKernBatchResidual2
                                                                                              : kKernBatch2) + mt)
+      : has_mla                          ? kKernMla
       : mkind == B200AWQ_OP_DEEPSEEK_MOE ? kKernDeepseekMoe
       : mkind == B200AWQ_OP_QWEN3_MOE    ? kKernQwen3Moe
       : has_qkn                          ? kKernQkNorm
@@ -629,12 +649,12 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
         (table[i].moe == 1 ? dd[table[i].mi].shb_a : dd[table[i].mi].shb_b) = (long long)shared_bytes(i);
       }
     if (e == cudaSuccess) e = upload(&pr->d_moe, md);
-    if (e == cudaSuccess && kern == kKernDeepseekMoe) e = upload(&pr->d_dsk, dd);
+    if (e == cudaSuccess && (kern == kKernDeepseekMoe || kern == kKernMla)) e = upload(&pr->d_dsk, dd);
   }
   // the side tables the kernel takes (ProgKernel)
-  const bool takes_res = (kern >= kKernResidual && kern <= kKernDeepseekMoe) || kern >= kKernBatchResidual2;
-  const bool takes_rope = (kern >= kKernRope && kern <= kKernDeepseekMoe) || kern >= kKernBatchRope2;
-  const bool takes_qkn = (kern >= kKernQkNorm && kern <= kKernDeepseekMoe) || kern >= kKernBatchQkNorm2;
+  const bool takes_res = (kern >= kKernResidual && kern <= kKernMla) || kern >= kKernBatchResidual2;
+  const bool takes_rope = (kern >= kKernRope && kern <= kKernMla) || kern >= kKernBatchRope2;
+  const bool takes_qkn = (kern >= kKernQkNorm && kern <= kKernMla) || kern >= kKernBatchQkNorm2;
   if (e == cudaSuccess && takes_res) {
     std::vector<SpRes> rd(n);
     for (int i = 0; i < n; ++i) {
@@ -666,12 +686,22 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     }
     if (e == cudaSuccess) e = upload(&pr->d_qkn, qd);
   }
+  if (e == cudaSuccess && kern == kKernMla) {
+    std::vector<SpMla> ml(n);
+    for (int i = 0; i < n; ++i) {
+      ml[i].d = table[i].mla;
+      ml[i].kind = table[i].mla_kind;
+      const int s = table[i].stage_row;
+      if (s >= 0 && table[s].mla_kind == 1 && ops[i].src_op == s) ml[i].wait_words = table[s].N;
+    }
+    e = upload(&pr->d_mla, ml);
+  }
   if (e == cudaSuccess) e = upload(&pr->d_sp_ops, ops);
   // the kernel may use all 227 KB of shared memory (the plain one at both warp counts: knob 9 is read at run time)
   static const void* const entry[] = {
       (const void*)stream_program_kernel<8, 4>, (const void*)stream_moe_kernel, (const void*)stream_residual_kernel,
       (const void*)stream_rope_kernel, (const void*)stream_qknorm_kernel, (const void*)stream_qwen3moe_kernel,
-      (const void*)stream_deepseek_moe_kernel, (const void*)stream_batch_kernel<2>, (const void*)stream_batch_kernel<4>,
+      (const void*)stream_deepseek_moe_kernel, (const void*)stream_mla_kernel, (const void*)stream_batch_kernel<2>, (const void*)stream_batch_kernel<4>,
       (const void*)stream_batch_kernel<8>, (const void*)stream_batch_residual_kernel<2>,
       (const void*)stream_batch_residual_kernel<4>, (const void*)stream_batch_residual_kernel<8>,
       (const void*)stream_batch_rope_kernel<2>, (const void*)stream_batch_rope_kernel<4>,
@@ -864,6 +894,28 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       else pv.qkr.rope = *r;
       continue;
     }
+    if (op.kind == B200AWQ_OP_MLA_ROPE || op.kind == B200AWQ_OP_MLA_KV) {
+      // MLA's rotation / cache stores, folded into the finish of the linear recorded just before it (whose whole output
+      // is the op's row): q_proj | kv_a_proj_with_mqa for MLA_ROPE, kv_b_proj for MLA_KV
+      const bool mrope = op.kind == B200AWQ_OP_MLA_ROPE;
+      const b200awq_mla_t* d = static_cast<const b200awq_mla_t*>(op.weight);
+      if (op.x == nullptr) return B200AWQ_EINVAL;
+      const int v = mla_validate(d, mrope);
+      if (v != B200AWQ_OK) return v;
+      if (M != 1) return B200AWQ_EUNSUPPORTED;
+      if ((d->nope_dim % 16) != 0 || (d->rope_dim % 16) != 0 || (mrope ? d->kv_lora_rank : d->v_dim) % 16 != 0)
+        return B200AWQ_EUNSUPPORTED;
+      const int64_t want = mrope ? (int64_t)d->n_heads * (d->nope_dim + d->rope_dim) + d->kv_lora_rank + d->rope_dim
+                                 : (int64_t)d->n_heads * (d->nope_dim + d->v_dim);
+      if (op.N != want) return B200AWQ_EUNSUPPORTED;
+      if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty() || table.back().moe != 0)
+        return B200AWQ_EUNSUPPORTED;
+      ProgOp& pv = table.back();
+      if (op.x != pv.y || op.N != pv.N) return B200AWQ_EUNSUPPORTED;
+      pv.mla = *d;
+      pv.mla_kind = mrope ? 1 : 2;
+      continue;
+    }
     if (op.kind == B200AWQ_OP_ADD) {
       // y = x + weight, folded into the epilogue of the op recorded just before it (a linear / a MoE block's down)
       if (op.x == nullptr || op.weight == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
@@ -902,6 +954,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (op.kind == B200AWQ_OP_RMSNORM || op.kind == B200AWQ_OP_SILU_AND_MUL) {
       if (op.x == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
       if (op.kind == B200AWQ_OP_RMSNORM && op.weight == nullptr) return B200AWQ_EINVAL;
+      // an RMSNORM over rows of a wider tensor (ldx > K): the kernels stage contiguous rows only
+      if (op.kind == B200AWQ_OP_RMSNORM && M > 1 && op.ldx != 0 && op.ldx != op.K) return B200AWQ_EUNSUPPORTED;
       if ((op.K % 8) != 0 || !aligned16(op.x) || !aligned16(op.y) || (op.weight != nullptr && !aligned16(op.weight)))
         return B200AWQ_EUNSUPPORTED;
       const size_t in_bytes = (size_t)M * (op.kind == B200AWQ_OP_SILU_AND_MUL ? 2 : 1) * op.K * 2;
@@ -982,6 +1036,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     const int s = p.src_prev ? static_cast<int>(table.size()) - 1 : p.ext_dep;
     const size_t width = (size_t)(p.prologue == kProSilu ? 2 : 1) * op.K;
     p.stage_row = s >= 0 && p.src == table[s].y && width == (size_t)table[s].N ? s : -1;
+    // a slice of an MLA_ROPE producer's row: stream_mla_kernel stages it after the whole row (SpMla::wait_words)
+    if (s >= 0 && table[s].mla_kind == 1 && p.prologue != kProSilu) p.stage_row = s;
     table.push_back(p);
   }
   for (const Glue& gl : glues)
@@ -1045,6 +1101,76 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       if (j != ri && o.qkr.rope.head_dim != 0)   // another ROPE_KV: its outputs are writes, its inputs reads
         for (const auto& w : rope_outs(o.qkr.rope))
           if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
+    }
+    for (const Glue& gl : glues)
+      if (hits_any(gl.out, glue_out_bytes(gl)) || hits_out(gl.src, glue_src_bytes(gl))) return B200AWQ_EUNSUPPORTED;
+    for (const MoeBlock& b : moes) {
+      const auto x = b.extents(M);
+      for (int k = 0; k < (int)x.size(); ++k)
+        if (k < MoeBlock::kMoeWrites ? hits_any(x[k].first, x[k].second) : hits_out(x[k].first, x[k].second))
+          return B200AWQ_EUNSUPPORTED;
+    }
+  }
+  // MLA_ROPE / MLA_KV: the same rule as ROPE_KV for q_out, the caches, pos and (MLA_ROPE) freqs, against every op,
+  // glue record, MoE block and ROPE_KV op.  The MLA_ROPE and MLA_KV ops of one layer may share k_cache: with the same
+  // geometry they write disjoint columns of its rows (k_pe, k_nope).
+  auto mla_outs = [&](const ProgOp& p) {
+    const b200awq_mla_t& d = p.mla;
+    const bool r = p.mla_kind == 1;
+    const size_t kb = ((size_t)(M - 1) * d.k_batch_stride + (size_t)d.cache_len * d.n_heads * (d.nope_dim + d.rope_dim)) * 2;
+    const size_t vb = ((size_t)(M - 1) * d.v_batch_stride + (size_t)d.cache_len * d.n_heads * d.v_head_stride) * 2;
+    return std::array<std::pair<const void*, size_t>, 3>{
+        {{r ? d.q_out : nullptr, r ? (size_t)M * d.n_heads * (d.nope_dim + d.rope_dim) * 2 : 0},
+         {d.k_cache, kb},
+         {r ? nullptr : d.v_cache, r ? 0 : vb}}};
+  };
+  auto shares_k = [&](const ProgOp& a, const ProgOp& b) {
+    const b200awq_mla_t &x = a.mla, &y = b.mla;
+    return a.mla_kind != b.mla_kind && x.k_cache == y.k_cache && x.n_heads == y.n_heads && x.nope_dim == y.nope_dim &&
+           x.rope_dim == y.rope_dim && x.cache_len == y.cache_len && x.k_batch_stride == y.k_batch_stride;
+  };
+  for (int ri = 0; ri < nt; ++ri) {
+    const ProgOp& mp = table[ri];
+    if (mp.mla_kind == 0) continue;
+    const b200awq_mla_t& d = mp.mla;
+    const auto outs = mla_outs(mp);
+    const std::pair<const void*, size_t> ins[2] = {
+        {d.pos, 4}, {mp.mla_kind == 1 ? d.freqs : nullptr, mp.mla_kind == 1 ? (size_t)d.freqs_len * d.rope_dim * 4 : 0}};
+    auto hits_out = [&](const void* p, size_t b) {
+      for (const auto& o : outs)
+        if (overlaps(o.first, o.second, p, b)) return true;
+      return false;
+    };
+    // (skip: the one output of this op the other write may overlap, or -1)
+    auto hits_any = [&](const void* p, size_t b, int skip = -1) {
+      for (int k = 0; k < 3; ++k)
+        if (k != skip && overlaps(outs[k].first, outs[k].second, p, b)) return true;
+      for (const auto& in : ins)
+        if (overlaps(in.first, in.second, p, b)) return true;
+      return false;
+    };
+    for (int a = 0; a < 3; ++a)
+      for (int b = a + 1; b < 3; ++b)
+        if (overlaps(outs[a].first, outs[a].second, outs[b].first, outs[b].second)) return B200AWQ_EUNSUPPORTED;
+    for (int j = 0; j < nt; ++j) {
+      const ProgOp& o = table[j];
+      if (hits_any(o.y, y_bytes(o)) || (o.raw_y != nullptr && hits_any(o.raw_y, y_bytes(o))) ||
+          (o.src != nullptr && hits_out(o.src, src_bytes(o))) || (o.res_ext != nullptr && hits_out(o.res_ext, y_bytes(o))))
+        return B200AWQ_EUNSUPPORTED;
+      if (o.qkr.rope.head_dim != 0) {   // a ROPE_KV: its outputs are writes, its inputs reads
+        const b200awq_qk_norm_rope_t& q = o.qkr;
+        for (const auto& w : rope_outs(q.rope))
+          if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
+        const size_t wn = q.q_norm_weight != nullptr ? (size_t)q.rope.head_dim * 2 : 0;
+        if (hits_out(q.rope.pos, 4) || hits_out(q.rope.freqs, (size_t)q.rope.freqs_len * q.rope.head_dim * 4) ||
+            hits_out(q.q_norm_weight, wn) || hits_out(q.k_norm_weight, wn))
+          return B200AWQ_EUNSUPPORTED;
+      }
+      if (j != ri && o.mla_kind != 0) {   // another MLA op: its outputs are writes (its reads: its own pass of this loop)
+        const auto w = mla_outs(o);
+        for (int k = 0; k < 3; ++k)
+          if (hits_any(w[k].first, w[k].second, k == 1 && shares_k(mp, o) ? 1 : -1)) return B200AWQ_EUNSUPPORTED;
+      }
     }
     for (const Glue& gl : glues)
       if (hits_any(gl.out, glue_out_bytes(gl)) || hits_out(gl.src, glue_src_bytes(gl))) return B200AWQ_EUNSUPPORTED;
@@ -1154,6 +1280,7 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     case kKernQkNorm: return stream(stream_qknorm_kernel, p->d_res, p->d_rope, p->d_qkn);
     case kKernQwen3Moe: return stream(stream_qwen3moe_kernel, p->d_res, p->d_rope, p->d_qkn);
     case kKernDeepseekMoe: return stream(stream_deepseek_moe_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk);
+    case kKernMla: return stream(stream_mla_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk, p->d_mla);
     case kKernBatch2: return batch(stream_batch_kernel<2>);
     case kKernBatch4: return batch(stream_batch_kernel<4>);
     case kKernBatch8: return batch(stream_batch_kernel<8>);

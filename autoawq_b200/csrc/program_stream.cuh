@@ -255,6 +255,26 @@ __device__ __forceinline__ void sp_cols_rot(int D, int s, int g, int& lo, int& h
   hi = lo + (D >> 1);
 }
 
+// mode 3 (a q_proj | kv_a_proj_with_mqa linear whose MLA_ROPE folds into its finish): set s holds the adjacent pairs
+// lo = 16 s + 2 g, hi = lo + 1, so one lane finishes both elements of an interleaved rotary pair
+__device__ __forceinline__ void sp_cols_pairs(int s, int g, int& lo, int& hi) {
+  lo = 16 * s + 2 * g;
+  hi = lo + 1;
+}
+
+// MLA_ROPE / MLA_KV folded into a linear's finish (stream_mla_kernel): one entry per kernel op in a side table, like
+// SpRope.  kind 1: the op is packed in mode 3 and its finish runs rope.cuh's mla_rope_pair on every pair; kind 2: a
+// mode-0 kv_b_proj op whose finish stores every column with mla_kv_col; kind 0 on every other op.
+// wait_words > 0: the op stages a slice of an MLA_ROPE producer's row (kv_a_layernorm of c_kv, kv_b_proj's prologue) and
+// first waits for one word of every 16-column set of that row (wait_words columns): each is published by the set's owner
+// after it finished every earlier op, as a whole-row staging shows, so program_create's residual rule may count this
+// staging as one (ProgOp::stage_row).
+struct SpMla {
+  b200awq_mla_t d;
+  int kind;
+  int wait_words;
+};
+
 // phase (b) of a QK_NORM_ROPE_KV finish (SpQkNorm above), shared by the M = 1 and the batched body: item t of this
 // thread (t = ct, ct + nthr, ... < nsets * per_set; per_set = 8 M) is lane group t % 8 of token row (t % per_set) / 8 of
 // local set t / per_set, whose fp16 pair phase (a) kept in part[(ls * kst + m) * 16 + g] / [.. + 8].
@@ -356,6 +376,13 @@ __global__ void __launch_bounds__(256)
   pdl_wait();   // (launched without the PDL attribute: a no-op, kept so the kernel stays safe under one)
   sp_pack(qweight, scales, qzeros, out, K, N, G,
           [=](int s, int g, int& lo, int& hi) { sp_cols_rot(head_dim, s, g, lo, hi); });
+}
+
+__global__ void __launch_bounds__(256)
+    stream_pack_pairs_kernel(const int32_t* __restrict__ qweight, const __half* __restrict__ scales,
+                             const int32_t* __restrict__ qzeros, uint8_t* __restrict__ out, int K, int N, int G) {
+  pdl_wait();   // (launched without the PDL attribute: a no-op, kept so the kernel stays safe under one)
+  sp_pack(qweight, scales, qzeros, out, K, N, G, [=](int s, int g, int& lo, int& hi) { sp_cols_pairs(s, g, lo, hi); });
 }
 
 // ------------------------------------------------------------------------------------------ the kernel
@@ -619,6 +646,33 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 #define SP_QWEN3 1
 #define SP_DEEPSEEK 1
 #include "program_stream_body.inc"
+#undef SP_DEEPSEEK
+#undef SP_QWEN3
+#undef SP_QKNORM
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with MLA_ROPE / MLA_KV ops (SpMla above), with or without DEEPSEEK_MOE blocks (a DeepSeek segment, or
+// its dense first layer): the DeepSeek-MoE kernel plus the mode-3 rotation and the q / k / v stores of the finish, which
+// only SP_MLA compiles in.  Every rotated pair lives in one lane: no cross-CTA exchange.
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_mla_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                      uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                      int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                      const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn, const SpDsk* __restrict__ dsk,
+                      const SpMla* __restrict__ mla) {
+  constexpr int NW = 8, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_QKNORM 1
+#define SP_QWEN3 1
+#define SP_DEEPSEEK 1
+#define SP_MLA 1
+#include "program_stream_body.inc"
+#undef SP_MLA
 #undef SP_DEEPSEEK
 #undef SP_QWEN3
 #undef SP_QKNORM

@@ -87,4 +87,81 @@ __device__ __forceinline__ void qk_norm_rope_pair(const b200awq_qk_norm_rope_t& 
   rope_pair(q.rope, pos, m, col, wa, wb);
 }
 
+// ---- MLA (B200AWQ_OP_MLA_ROPE / _MLA_KV, include/b200awq.h): the per-pair / per-column steps shared by the stand-alone
+// kernels (aux.cu) and the finish of the decode-program kernel that folds them (program_stream_body.inc under SP_MLA).
+// Reference: transformers 5.5 DeepseekV2Attention.forward (apply_rotary_emb) and DeepseekV3Attention.forward
+// (apply_rotary_pos_emb_interleave).
+
+// the position of this step, or -1 when it is outside the cache (MLA_ROPE: or the frequency table; MLA_KV reads none)
+__device__ __forceinline__ int mla_pos(const b200awq_mla_t& d, bool rope) {
+  const int p = *d.pos;
+  return (p >= 0 && p < d.cache_len && (!rope || p < d.freqs_len)) ? p : -1;
+}
+
+// Rotary pair i (a = x[2i], b = x[2i + 1]) of a rope slice of Dr elements: the two results and their places in the
+// rotated slice.  Style 0 is the complex<float> product of apply_rotary_emb with rope_pair's contraction, back at the
+// interleaved places 2i, 2i + 1.  Style 1 is apply_rotary_pos_emb_interleave's fp16 tensor arithmetic: cos / sin cast
+// to fp16, every product and the sum rounded to fp16 (each an exact fp32 value rounded once, as torch's half kernels
+// compute them), de-interleaved to i, i + Dr/2.
+struct MlaRot {
+  int j0, j1;
+  __half o0, o1;
+};
+__device__ __forceinline__ MlaRot mla_rotate(const b200awq_mla_t& d, int pos, int i, __half a, __half b) {
+  const int half = d.rope_dim >> 1;
+  const float2 cs = reinterpret_cast<const float2*>(d.freqs)[(size_t)pos * half + i];
+  const float fa = __half2float(a), fb = __half2float(b);
+  MlaRot r;
+  if (d.style == 0) {
+    r.j0 = 2 * i;
+    r.j1 = 2 * i + 1;
+    r.o0 = __float2half_rn(__fmaf_rn(fa, cs.x, -__fmul_rn(fb, cs.y)));
+    r.o1 = __float2half_rn(__fmaf_rn(fb, cs.x, __fmul_rn(fa, cs.y)));
+    return r;
+  }
+  const float c = __half2float(__float2half_rn(cs.x)), s = __half2float(__float2half_rn(cs.y));
+  auto h = [](float v) { return __half2float(__float2half_rn(v)); };
+  r.j0 = i;
+  r.j1 = i + half;
+  r.o0 = __float2half_rn(__fadd_rn(h(__fmul_rn(fa, c)), h(__fmul_rn(-fb, s))));
+  r.o1 = __float2half_rn(__fadd_rn(h(__fmul_rn(fb, c)), h(__fmul_rn(fa, s))));
+  return r;
+}
+
+// MLA_ROPE on columns (col, col + 1) of token row m's q_proj | kv_a_proj_with_mqa row (col even; a, b their values):
+// q_nope copied and q_pe rotated into q_out, c_kv nothing, k_pe rotated into the k rows of all H heads at position pos
+__device__ __forceinline__ void mla_rope_pair(const b200awq_mla_t& d, int pos, int m, int col, __half a, __half b) {
+  const int W = d.nope_dim + d.rope_dim, H = d.n_heads, qn = H * W;
+  if (col < qn) {
+    const int h = col / W, i = col - h * W;
+    __half* q = static_cast<__half*>(d.q_out) + ((size_t)m * H + h) * W;
+    if (i < d.nope_dim) {
+      q[i] = a;
+      q[i + 1] = b;
+    } else {
+      const MlaRot r = mla_rotate(d, pos, (i - d.nope_dim) >> 1, a, b);
+      q[d.nope_dim + r.j0] = r.o0;
+      q[d.nope_dim + r.j1] = r.o1;
+    }
+    return;
+  }
+  const int kp = col - qn - d.kv_lora_rank;
+  if (kp < 0) return;
+  const MlaRot r = mla_rotate(d, pos, kp >> 1, a, b);
+  __half* k = static_cast<__half*>(d.k_cache) + (size_t)m * d.k_batch_stride + (size_t)pos * qn + d.nope_dim;
+  for (int h = 0; h < H; ++h) {
+    k[(size_t)h * W + r.j0] = r.o0;
+    k[(size_t)h * W + r.j1] = r.o1;
+  }
+}
+
+// MLA_KV on column col of token row m's kv_b_proj row (value x): k_nope into k_cache, v into v_cache, at position pos
+__device__ __forceinline__ void mla_kv_col(const b200awq_mla_t& d, int pos, int m, int col, __half x) {
+  const int W = d.nope_dim + d.v_dim, h = col / W, i = col - h * W, H = d.n_heads;
+  if (i < d.nope_dim)
+    static_cast<__half*>(d.k_cache)[(size_t)m * d.k_batch_stride + ((size_t)pos * H + h) * (d.nope_dim + d.rope_dim) + i] = x;
+  else
+    static_cast<__half*>(d.v_cache)[(size_t)m * d.v_batch_stride + ((size_t)pos * H + h) * d.v_head_stride + i - d.nope_dim] = x;
+}
+
 }  // namespace b200awq

@@ -18,6 +18,7 @@ __all__ = [
     "gemv_forward_cuda_decode", "gemm_forward_cuda_prefill", "layernorm_forward_cuda", "silu_and_mul",
     "topk_softmax", "moe_alig_block_size", "grouped_gemm_forward",
     "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "qk_norm_descriptor",
+    "mla_descriptor", "mla_rope", "mla_kv_cache",
     "set_knob", "get_knob",
     "B200AwqError",
 ]
@@ -334,6 +335,121 @@ def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_
     name = "b200awq_rope_kv" if qd is None else "b200awq_qk_norm_rope_kv"
     check(code, f"{name}(M={M}, H={H}, KV={r.n_kv_heads}, D={D})")
     return q_out
+
+
+def _rows(x, N, name):
+    if x.dtype != torch.float16 or x.shape[-1] != N:
+        raise B200AwqError(f"b200awq: {name} must be float16 [.., {N}]")
+    x2 = x.reshape(-1, N)
+    if x2.stride(-1) != 1:
+        raise B200AwqError(f"b200awq: {name} rows must have a unit stride")
+    return x2
+
+
+def _mla_freqs(freqs, rope_dim, style):
+    """The [S_f, Dr/2, 2] f32 (cos, sin) table of b200awq_mla_t.  style 0: DeepseekV2RotaryEmbedding's complex64
+    freqs_cis [S_f, Dr/2] or its f32 real view.  style 1: a (cos, sin) pair of f32 [S_f, Dr] tensors as
+    DeepseekV3RotaryEmbedding returns them (attention_scaling applied, before the cast to the activations' dtype); their
+    halves repeat, so the first Dr/2 columns are taken (a new tensor)."""
+    if style == 0:
+        if isinstance(freqs, torch.Tensor) and freqs.dtype == torch.complex64:
+            freqs = torch.view_as_real(freqs)
+        if (not isinstance(freqs, torch.Tensor) or freqs.dtype != torch.float32 or freqs.dim() != 3
+                or tuple(freqs.shape[1:]) != (rope_dim // 2, 2)):
+            raise B200AwqError(f"b200awq: style 0 freqs must be freqs_cis (complex64 [S, {rope_dim // 2}]) or its "
+                               "real view")
+        return freqs.contiguous()          # (the rotary module's table is a transposed product: a copy then)
+    if isinstance(freqs, torch.Tensor) and freqs.dtype == torch.float32 and freqs.dim() == 3:
+        t = freqs                                   # already the descriptor's table
+    else:
+        cos, sin = freqs
+        if cos.dtype != torch.float32 or sin.shape != cos.shape or cos.shape[-1] != rope_dim:
+            raise B200AwqError(f"b200awq: style 1 freqs must be the f32 (cos, sin) pair [S, {rope_dim}]")
+        h = rope_dim // 2
+        t = torch.stack((cos.reshape(-1, rope_dim)[:, :h], sin.reshape(-1, rope_dim)[:, :h]), dim=-1).contiguous()
+    if tuple(t.shape[1:]) != (rope_dim // 2, 2) or not t.is_contiguous():
+        raise B200AwqError(f"b200awq: style 1 freqs must be [S, {rope_dim // 2}, 2] f32")
+    return t
+
+
+def mla_descriptor(pos, freqs, k_cache, v_cache, q_out, M, n_heads, nope_dim, rope_dim, v_dim, kv_lora_rank, style):
+    """Checks the tensors of the MLA glue for M token rows and returns the b200awq_mla_t.  freqs: the [S_f, Dr/2, 2] f32
+    table (_mla_freqs) or None (MLA_KV); k_cache f16 [B >= M, S, H, Dn + Dr] with contiguous [S, H, Dn + Dr] entries;
+    v_cache f16 [B >= M, S, H, >= Dv] (padded heads allowed: the head stride is its last dimension) with contiguous
+    entries, or None (MLA_ROPE); q_out contiguous f16 [M, H, Dn + Dr] (any shape of M H (Dn + Dr) elements ending in
+    [H, Dn + Dr]) or None (MLA_KV); pos a device int32 tensor of one element.  The kernels write batch entry m and q_out
+    row m for every m < M, so every size is checked against M before a pointer is taken."""
+    H, Dn, Dr, Dv, C, M = int(n_heads), int(nope_dim), int(rope_dim), int(v_dim), int(kv_lora_rank), int(M)
+    W = Dn + Dr
+    d = _cabi.Mla()
+    d.n_heads, d.nope_dim, d.rope_dim, d.v_dim, d.kv_lora_rank, d.style = H, Dn, Dr, Dv, C, int(style)
+    if pos.dtype != torch.int32 or pos.numel() != 1:
+        raise B200AwqError("b200awq: pos must be a device int32 tensor with one element")
+    if (k_cache.dtype != torch.float16 or k_cache.dim() != 4 or tuple(k_cache.shape[2:]) != (H, W)
+            or k_cache.stride(3) != 1 or k_cache.stride(2) != W or k_cache.stride(1) != H * W):
+        raise B200AwqError(f"b200awq: k_cache must be float16 [B, S, {H}, {W}] with contiguous [S, H, D] entries")
+    if k_cache.shape[0] < M:
+        raise B200AwqError(f"b200awq: k_cache has {k_cache.shape[0]} batch entries for {M} token rows")
+    if v_cache is not None:
+        if (v_cache.dtype != torch.float16 or v_cache.dim() != 4 or v_cache.shape[2] != H or v_cache.shape[3] < Dv
+                or v_cache.stride(3) != 1 or v_cache.stride(2) != v_cache.shape[3]
+                or v_cache.stride(1) != H * v_cache.shape[3] or v_cache.shape[1] != k_cache.shape[1]):
+            raise B200AwqError(f"b200awq: v_cache must be float16 [B, S, {H}, >= {Dv}] with contiguous entries and "
+                               "k_cache's S")
+        if v_cache.shape[0] < M:
+            raise B200AwqError(f"b200awq: v_cache has {v_cache.shape[0]} batch entries for {M} token rows")
+    if q_out is not None and (q_out.dtype != torch.float16 or not q_out.is_contiguous()
+                              or tuple(q_out.shape[-2:]) != (H, W) or q_out.numel() != M * H * W):
+        raise B200AwqError(f"b200awq: q_out must be a contiguous float16 [{M}, {H}, {W}] tensor")
+    _require_cuda(pos, k_cache, v_cache, freqs, q_out)
+    d.cache_len, d.k_batch_stride = k_cache.shape[1], k_cache.stride(0)
+    d.pos, d.k_cache = pos.data_ptr(), k_cache.data_ptr()
+    if v_cache is not None:
+        d.v_batch_stride, d.v_head_stride, d.v_cache = v_cache.stride(0), v_cache.shape[3], v_cache.data_ptr()
+    if freqs is not None:
+        d.freqs_len, d.freqs = freqs.shape[0], freqs.data_ptr()
+    if q_out is not None:
+        d.q_out = q_out.data_ptr()
+    return d
+
+
+def _mla_call(fn, row2, d, M, name):
+    ld = row2.stride(0) if M > 1 else row2.shape[1]
+    with _DeviceGuard(row2.device):
+        code = fn(row2.data_ptr(), ld, d, M, _stream(row2.device))
+    check(code, f"{name}(M={M}, H={d.n_heads}, Dn={d.nope_dim}, Dr={d.rope_dim})")
+
+
+def mla_rope(qkva, freqs, pos, k_cache, n_heads, nope_dim, rope_dim, kv_lora_rank, style, q_out=None):
+    """The glue of transformers' DeepseekV2Attention / DeepseekV3Attention (no q LoRA) after the fused
+    q_proj | kv_a_proj_with_mqa linear: qkva [.., H (Dn + Dr) + C + Dr] f16 = [q | c_kv | k_pe].  Writes q_out
+    [M, H, Dn + Dr] = [q_nope | rotated q_pe] per head (allocated when not given, and returned) and k_cache[m, *pos, h,
+    Dn:] = the rotated k_pe for every head h, for token rows m < M <= 8; nothing when *pos is outside the cache or the
+    table.  style 0: V2's apply_rotary_emb, freqs = freqs_cis; style 1: V3's apply_rotary_pos_emb_interleave, freqs =
+    the (cos, sin) pair (include/b200awq.h states both arithmetics).  c_kv is left to kv_a_layernorm."""
+    H, Dn, Dr, C = int(n_heads), int(nope_dim), int(rope_dim), int(kv_lora_rank)
+    row2 = _rows(qkva, H * (Dn + Dr) + C + Dr, "qkva")
+    M = row2.shape[0]
+    if q_out is None:
+        q_out = torch.empty((M, H, Dn + Dr), dtype=torch.float16, device=qkva.device)
+    f = _mla_freqs(freqs, Dr, int(style))
+    d = mla_descriptor(pos, f, k_cache, None, q_out, M, H, Dn, Dr, 0, C, style)
+    _require_cuda(qkva)
+    _mla_call(lib.b200awq_mla_rope, row2, d, M, "b200awq_mla_rope")
+    return q_out
+
+
+def mla_kv_cache(kv, pos, k_cache, v_cache, n_heads, nope_dim, v_dim):
+    """kv_b_proj's output kv [.., H (Dn + Dv)] f16 (per head [k_nope | v]) into the caches at position *pos:
+    k_cache[m, *pos, h, :Dn] = k_nope, v_cache[m, *pos, h, :Dv] = v, for token rows m < M <= 8; nothing when *pos is
+    outside the cache.  k_cache [B, S, H, Dn + Dr] fixes Dr; v_cache [B, S, H, >= Dv]."""
+    H, Dn, Dv = int(n_heads), int(nope_dim), int(v_dim)
+    row2 = _rows(kv, H * (Dn + Dv), "kv")
+    M = row2.shape[0]
+    Dr = k_cache.shape[-1] - Dn
+    d = mla_descriptor(pos, None, k_cache, v_cache, None, M, H, Dn, Dr, Dv, 0, 0)
+    _require_cuda(kv)
+    _mla_call(lib.b200awq_mla_kv, row2, d, M, "b200awq_mla_kv")
 
 
 # ------------------------------------------------------------------------------------ MoE (awq_ext surface)

@@ -154,3 +154,20 @@ def stack_deepseek_experts(block):
                    norm_topk_prob=bool(getattr(block, "norm_topk_prob", False)),
                    routed_scaling_factor=float(getattr(block, "routed_scaling_factor", 1.0)))
     return gate_weight, w1, w2, top_k, shared, routing
+
+
+def fuse_mla_input(attn):
+    """(qweight, scales, qzeros, bias) of the fused q_proj | kv_a_proj_with_mqa linear of a transformers
+    DeepseekV2Attention / DeepseekV3Attention without a q LoRA whose two projections are WQLinear_GEMM modules: both read
+    the hidden state, so one GEMM-layout linear with N = H (Dn + Dr) + C + Dr gives the row [q | c_kv | k_pe] that
+    DecodeProgram.mla_rope takes (loader.fuse_columns' concatenation along N).  bias is None when neither projection
+    has one."""
+    from .loader import fuse_columns
+    from .shard import PackedGemm
+
+    if getattr(attn, "q_lora_rank", None) is not None:
+        raise ValueError("fuse_mla_input: the attention has a q LoRA (q_a_proj / q_b_proj); only q_proj is supported")
+    parts = [PackedGemm(m.qweight, m.qzeros, m.scales, getattr(m, "bias", None))
+             for m in (attn.q_proj, attn.kv_a_proj_with_mqa)]
+    f = fuse_columns(parts)
+    return f.qweight, f.scales, f.qzeros, f.bias

@@ -47,6 +47,13 @@ op either: it folds into the finish of the qkv linear recorded just before it, s
 the cache row written, and attention reads them directly (DESIGN.md 3.5f).  `pos` is a device int32 tensor: advance it
 in place between runs (or graph replays).  With `q_norm=` / `k_norm=` (Qwen3's Qwen3RMSNorm modules) it also applies
 Qwen3's per-head q / k norm first, still inside the qkv linear's finish (DESIGN.md 3.5g).
+
+`mla_rope(qkva, freqs, pos, k_cache, ...)` and `mla_kv_cache(kv, pos, k_cache, v_cache, ...)` record the glue of
+DeepSeek-V2 / V3 multi-head latent attention (transformers' DeepseekV2Attention / DeepseekV3Attention, no q LoRA) in
+transformers' order: the fused q_proj | kv_a_proj_with_mqa linear (packing.fuse_mla_input), mla_rope, kv_a_layernorm as
+an RMSNorm on the c_kv slice of that linear's output, kv_b_proj, mla_kv_cache.  Each folds into the finish of the linear
+recorded just before it, so at M = 1 a DeepSeek segment runs as one launch from one attention call to the next
+(DESIGN.md 3.5j).
 """
 from __future__ import annotations
 
@@ -83,15 +90,24 @@ class DecodeProgram:
             raise B200AwqError("b200awq: program already built")
 
     def layernorm_forward_cuda(self, x, weight, out, eps):
+        """x may also be rows of a wider tensor (unit stride, one row pitch: kv_a_layernorm on the c_kv slice of
+        M > 1 q_proj | kv_a_proj_with_mqa rows).  Such a source has its pitch recorded (ldx); the fused kernels stage
+        contiguous rows only, so a program with one replays per op."""
         self._no_more()
         self._dev_of(x)
         if x.dtype != torch.float16 or weight.dtype != torch.float16 or out.dtype != torch.float16:
             raise B200AwqError("b200awq: rmsnorm expects float16 tensors")
-        if not x.is_contiguous() or not out.is_contiguous() or not weight.is_contiguous():
-            raise B200AwqError("b200awq: program rmsnorm expects contiguous tensors")
         hidden = x.shape[-1]
+        ldx = 0
+        if not x.is_contiguous():
+            x2 = x.reshape(-1, hidden) if x.stride(-1) == 1 else None
+            if x2 is None or x2.data_ptr() != x.data_ptr() or x2.stride(-1) != 1:
+                raise B200AwqError("b200awq: program rmsnorm expects contiguous rows at one row pitch")
+            x, ldx = x2, x2.stride(0)
+        if not out.is_contiguous() or not weight.is_contiguous():
+            raise B200AwqError("b200awq: program rmsnorm expects contiguous tensors")
         self._ops.append(("rmsnorm", dict(x=x, weight=weight, out=out, eps=float(eps), rows=x.numel() // hidden,
-                                          hidden=hidden)))
+                                          hidden=hidden, ldx=ldx)))
         self._keep += [x, weight, out]
 
     def silu_and_mul(self, out, gate_up):
@@ -177,6 +193,56 @@ class DecodeProgram:
                                        ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc, qdesc=qdesc)))
         self._keep += [qkv, q2, freqs_cis, pos, k_cache, v_cache, q_out] + norm_w
         return q_out
+
+    def mla_rope(self, qkva, freqs, pos, k_cache, n_heads, nope_dim, rope_dim, kv_lora_rank, style, q_out=None):
+        """ext.mla_rope recorded on the fused q_proj | kv_a_proj_with_mqa output qkva [.., H (Dn + Dr) + C + Dr]:
+        q_out [M, H, Dn + Dr] = [q_nope | rotated q_pe] (allocated when not given, and returned) and k_cache[m, *pos, h,
+        Dn:] = the rotated k_pe for every head.  style 0 (DeepSeek-V2): freqs = the complex64 freqs_cis [S_f, Dr/2] of
+        DeepseekV2RotaryEmbedding (or its f32 real view); style 1 (DeepSeek-V3 / Moonlight, rope_interleave): freqs = the
+        f32 (cos, sin) pair [S_f, Dr] of DeepseekV3RotaryEmbedding.  The row keeps its values: record kv_a_layernorm as
+        layernorm_forward_cuda on qkva[..., H (Dn + Dr): H (Dn + Dr) + C] next.
+        The table is read by address when it already is the contiguous [S_f, Dr/2, 2] f32 layout (a contiguous
+        freqs_cis, or its real view).  Otherwise - the (cos, sin) pair of style 1, or a non-contiguous freqs_cis such as
+        the rotary module's own output - it is copied here, and the program keeps that snapshot: after the caller's
+        table changes (a regrown rotary cache), record the program again.  k_cache needs a batch entry per token row,
+        q_out M x H x (Dn + Dr) elements."""
+        self._no_more()
+        self._dev_of(qkva)
+        H, Dn, Dr, C = int(n_heads), int(nope_dim), int(rope_dim), int(kv_lora_rank)
+        row = ext._rows(qkva, H * (Dn + Dr) + C + Dr, "qkva")
+        if row.data_ptr() != qkva.data_ptr():
+            raise B200AwqError("b200awq: mla_rope records qkva by address: pass its rows as they are")
+        M = row.shape[0]
+        if q_out is None:
+            q_out = torch.empty((M, H, Dn + Dr), dtype=torch.float16, device=qkva.device)
+        f = ext._mla_freqs(freqs, Dr, int(style))
+        for t in (f, pos, k_cache, q_out):
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+        desc = ext.mla_descriptor(pos, f, k_cache, None, q_out, M, H, Dn, Dr, 0, C, style)
+        self._ops.append(("mla_rope", dict(row=row, M=M, N=row.shape[1], ldx=row.stride(0) if M > 1 else row.shape[1],
+                                           desc=desc)))
+        self._keep += [qkva, row, f, pos, k_cache, q_out]
+        return q_out
+
+    def mla_kv_cache(self, kv, pos, k_cache, v_cache, n_heads, nope_dim, v_dim):
+        """ext.mla_kv_cache recorded on kv_b_proj's output kv [.., H (Dn + Dv)]: k_cache[m, *pos, h, :Dn] = k_nope,
+        v_cache[m, *pos, h, :Dv] = v.  k_cache may be mla_rope's (the two write disjoint columns of its rows); both
+        caches need a batch entry per token row."""
+        self._no_more()
+        self._dev_of(kv)
+        H, Dn, Dv = int(n_heads), int(nope_dim), int(v_dim)
+        row = ext._rows(kv, H * (Dn + Dv), "kv")
+        if row.data_ptr() != kv.data_ptr():
+            raise B200AwqError("b200awq: mla_kv_cache records kv by address: pass its rows as they are")
+        for t in (pos, k_cache, v_cache):
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+        M = row.shape[0]
+        desc = ext.mla_descriptor(pos, None, k_cache, v_cache, None, M, H, Dn, k_cache.shape[-1] - Dn, Dv, 0, 0)
+        self._ops.append(("mla_kv", dict(row=row, M=M, N=row.shape[1], ldx=row.stride(0) if M > 1 else row.shape[1],
+                                         desc=desc)))
+        self._keep += [kv, row, pos, k_cache, v_cache]
 
     @staticmethod
     def _stacked(w, name):
@@ -421,7 +487,7 @@ class DecodeProgram:
         for i, (kind, o) in enumerate(self._ops):
             c = arr[i]
             if kind == "rmsnorm":
-                c.kind, c.M, c.K, c.eps = _cabi.OP_RMSNORM, o["rows"], o["hidden"], o["eps"]
+                c.kind, c.M, c.K, c.eps, c.ldx = _cabi.OP_RMSNORM, o["rows"], o["hidden"], o["eps"], o["ldx"]
                 c.x, c.weight, c.y = o["x"].data_ptr(), o["weight"].data_ptr(), o["out"].data_ptr()
             elif kind == "silu":
                 c.kind, c.M, c.K = _cabi.OP_SILU_AND_MUL, o["rows"], o["d"]
@@ -439,6 +505,9 @@ class DecodeProgram:
             elif kind == "rope":
                 c.kind, c.M, c.N, c.ldx = _cabi.OP_ROPE_KV, o["M"], o["N"], o["ldx"]
                 c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["desc"])
+            elif kind in ("mla_rope", "mla_kv"):
+                c.kind, c.M, c.N, c.ldx = (_cabi.OP_MLA_ROPE if kind == "mla_rope" else _cabi.OP_MLA_KV), o["M"], o["N"], o["ldx"]
+                c.x, c.weight = o["row"].data_ptr(), ctypes.addressof(o["desc"])
             else:
                 c.kind, c.M, c.K, c.N, c.group_size, c.ldx = _cabi.OP_LINEAR_GEMM, o["M"], o["K"], o["N"], o["G"], o["ldx"]
                 c.x, c.qweight, c.scales, c.qzeros = (o["x"].data_ptr(), o["qweight"].data_ptr(), o["scales"].data_ptr(),
@@ -483,13 +552,13 @@ class DecodeProgram:
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
-            return o["M"] if kind in ("linear", "moe", "add", "rope") else o["rows"]
+            return o["M"] if kind in ("linear", "moe", "add", "rope", "mla_rope", "mla_kv") else o["rows"]
         return 0
 
     @property
     def kernel_ops(self) -> int:
-        """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe / deepseek_moe (gate|up with the routing, down), none per add or
-        rope_kv_cache (they fold into their producer's epilogue); 0 per-op."""
+        """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe / deepseek_moe (gate|up with the routing, down), none per add,
+        rope_kv_cache, mla_rope or mla_kv_cache (they fold into their producer's epilogue); 0 per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
@@ -497,7 +566,8 @@ class DecodeProgram:
         """Kernels launched by one run(): 1 when fused (adds and rope_kv_cache included); per op, one per recorded
         call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), 34 + top_k per softmax
         deepseek_moe (sigmoid: 36 + top_k, + 6 with expert groups, + 3 with norm_topk_prob), one torch.add launch per add
-        and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
+        and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache, one b200awq_mla_rope / b200awq_mla_kv
+        launch per mla_rope / mla_kv_cache.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
         kernel (torch.sort, torch.gather), so the kernel count can be higher."""
         def per_op(kind, o):
             if kind != "moe":
@@ -541,6 +611,9 @@ class DecodeProgram:
                 with ext._DeviceGuard(dev):
                     code = lib.b200awq_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["M"], ext._stream(dev))
                 check(code, "b200awq_rope_kv")
+            elif kind in ("mla_rope", "mla_kv"):
+                ext._mla_call(lib.b200awq_mla_rope if kind == "mla_rope" else lib.b200awq_mla_kv, o["row"], o["desc"],
+                              o["M"], "b200awq_" + kind)
             else:
                 ext.linear_forward("gemm", o["x"], o["qweight"], o["scales"], o["qzeros"], o["G"], o["bias"], out=o["y"])
 

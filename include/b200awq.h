@@ -207,7 +207,9 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  * awq/modules/fused/mlp.py:41-55): RMSNorm -> linear -> ... -> SiLU*mul -> linear.  After a run every buffer
  * named by the ops holds what the per-op entry points above would have left there.
  *
- *   RMSNORM       : x = input row [K], weight [K], y = output [K], eps           (K = hidden)
+ *   RMSNORM       : x = input row [K], weight [K], y = output [K], eps           (K = hidden); M > 1 rows at
+ *                   pitch ldx (0 or K: contiguous; any other pitch, e.g. the c_kv slice of MLA rows, is
+ *                   B200AWQ_EUNSUPPORTED: the caller replays per op)
  *   SILU_AND_MUL  : x = gate|up [2K], y = output [K]                             (K = d)
  *   LINEAR_GEMM   : as b200awq_gemm_forward (GEMM layout)
  * b200awq_program_create returns B200AWQ_EUNSUPPORTED when the sequence does not fit the fused kernel (M != 1,
@@ -309,10 +311,26 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     a partial row of its own.  Logit exchange as QWEN3_MOE, with the unrounded fp32 logits (DESIGN.md 3.5i).
  *     Envelope (else B200AWQ_EUNSUPPORTED): M = 1, E <= 128, top_k <= 8, the shapes of b200awq_deepseek_moe_plan below.
  *     A program that mixes SPARSE_MOE, QWEN3_MOE and DEEPSEEK_MOE blocks replays per op.  An ADD right after it folds
- *     into its down op. */
+ *     into its down op.
+ *
+ *   MLA_ROPE      : the start of DeepSeek-V2 / V3 multi-head latent attention without a q LoRA, on the fused
+ *                   q_proj | kv_a_proj_with_mqa output row [q (H (Dn + Dr)) | c_kv (C) | k_pe (Dr)]: x = that row [M, N]
+ *                   at row pitch ldx, N = H (Dn + Dr) + C + Dr, weight = a b200awq_mla_t descriptor (below).  As
+ *                   b200awq_mla_rope.
+ *   MLA_KV        : the kv_b_proj output [M, H (Dn + Dv)] into the cache: x, ldx, weight as MLA_ROPE, N = H (Dn + Dv).
+ *                   As b200awq_mla_kv.
+ *     Folding: neither adds a kernel op.  Each folds into the finish of the linear recorded immediately before it, whose
+ *     whole output must be its row.  The linear before an MLA_ROPE is re-laid-out in stream
+ *     mode 3 (adjacent pairs, below), so the thread that finishes column 2i also holds 2i + 1 and rotates the pair in
+ *     registers; its y and published row keep the raw values, so kv_a_layernorm is the RMSNORM op recorded on the c_kv
+ *     slice of that y (a source inside the previous op's output).  B200AWQ_EUNSUPPORTED (the caller replays per op) when
+ *     M != 1, the op before is not a plain linear, N does not match the descriptor, Dn, Dr, Dv or C is not a
+ *     multiple of 16, or any other op reads or writes q_out or the caches or writes pos / freqs; the MLA_ROPE and MLA_KV
+ *     ops of one layer may share k_cache (they write disjoint columns).  A program with MLA ops runs the DeepSeek-MoE
+ *     kernel's configuration (a program that also holds SPARSE_MOE or QWEN3_MOE blocks replays per op). */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
-       B200AWQ_OP_DEEPSEEK_MOE = 9 };
+       B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -435,6 +453,40 @@ typedef struct b200awq_qk_norm_rope {
 int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
                             b200awq_stream_t stream);
 
+/* MLA (DeepSeek-V2 / V3 multi-head latent attention, no q LoRA): the glue between the fused q_proj | kv_a_proj_with_mqa
+ * linear and attention, in transformers' arithmetic (DeepseekV2Attention.forward, DeepseekV3Attention.forward with
+ * rope_interleave), for token rows m < M <= 8 writing cache batch entry m at position p = *pos.  Rotary pairs are adjacent
+ * elements (a, b) = (x[2i], x[2i + 1]) with (c, s) = freqs[p, i], i < Dr/2:
+ *   style 0 (V2, apply_rotary_emb's complex64 product):  out[2i] = fp16(fma(a, c, -(b s))), out[2i + 1] = fp16(fma(b, c, a s))
+ *   style 1 (V3, apply_rotary_pos_emb_interleave in fp16, with c16 = fp16(c), s16 = fp16(s)):
+ *            out[i] = fp16(fp16(a c16) + fp16(-b s16)),  out[i + Dr/2] = fp16(fp16(b c16) + fp16(a s16))
+ * b200awq_mla_rope on the row [q (H (Dn + Dr), per head [nope | pe]) | c_kv (C) | k_pe (Dr)]:
+ *   q_out[m, h, :Dn] = q_nope, q_out[m, h, Dn:] = rotate(q_pe), k_cache[m, p, h, Dn:] = rotate(k_pe) for every h;
+ *   c_kv is not written anywhere (kv_a_layernorm reads it from the row).
+ * b200awq_mla_kv on the kv_b_proj row [H (Dn + Dv)], per head [k_nope | v]:
+ *   k_cache[m, p, h, :Dn] = k_nope, v_cache[m, p, h, :Dv] = v.
+ * Nothing is written when *pos is outside [0, min(cache_len, freqs_len)) (b200awq_mla_kv: outside [0, cache_len); it
+ * reads neither freqs nor q_out, style, C; b200awq_mla_rope reads neither v_cache nor its geometry, Dv).  *pos is read on
+ * the device, so a captured CUDA graph replays at whatever position the caller stored there. */
+typedef struct b200awq_mla {
+  int32_t n_heads, nope_dim, rope_dim, v_dim, kv_lora_rank; /* H, Dn, Dr (even), Dv, C */
+  int32_t style;                         /* 0: V2 (interleaved output), 1: V3 (de-interleaved, fp16 arithmetic) */
+  int32_t cache_len;                     /* S: positions of the caches */
+  int32_t freqs_len;                     /* S_f: rows of freqs */
+  int64_t k_batch_stride;                /* elements between two batch entries of k_cache (>= S H (Dn + Dr)) */
+  int64_t v_batch_stride;                /* elements between two batch entries of v_cache (>= S H v_head_stride) */
+  int32_t v_head_stride;                 /* elements between two heads of one v_cache row (>= Dv; e.g. Dn + Dr) */
+  int32_t pad_;
+  const int32_t* pos;                    /* device int32[1]: the position written */
+  const float* freqs;                    /* [S_f, Dr/2, 2] f32 (cos, sin); style 0: view_as_real(freqs_cis) */
+  void* q_out;                           /* [M, H, Dn + Dr] f16 */
+  void* k_cache;                         /* [B >= M, S, H, Dn + Dr] f16 */
+  void* v_cache;                         /* [B >= M, S, H, v_head_stride] f16 */
+} b200awq_mla_t;
+/* ld: row pitch of `row` in elements.  `desc` is a host pointer, read at the call. */
+int b200awq_mla_rope(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream);
+int b200awq_mla_kv(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream);
+
 typedef struct b200awq_program* b200awq_program_t;
 
 int b200awq_program_create(const b200awq_op_t* ops, int n_ops, b200awq_program_t* out);
@@ -496,7 +548,9 @@ int b200awq_comm_destroy(b200awq_comm_t comm);
  * mode 0: set s = columns 16 s .. 16 s + 15; mode 1 (a fused gate|up linear): gate column j and up column j share
  * a lane, so SiLU*mul happens in the producer; mode 2 (a qkv linear followed by ROPE_KV, b200awq_stream_pack_rotary):
  * set s of head h = s / (D / 16) pairs column h D + 8 t + g with h D + D/2 + 8 t + g (t = s % (D / 16)), so RoPE's
- * rotation partners share a lane (requires D % 16 == 0 and N % D == 0).  Requires N % 16 == 0, K % 128 == 0, G in
+ * rotation partners share a lane (requires D % 16 == 0 and N % D == 0); mode 3 (a q_proj | kv_a_proj_with_mqa linear
+ * followed by MLA_ROPE, adjacent pairs): set s pairs column 16 s + 2 g with 16 s + 2 g + 1, so MLA's interleaved rotation
+ * partners share a lane (b200awq_stream_pack with mode 3).  Requires N % 16 == 0, K % 128 == 0, G in
  * {32, 64} or G % 128 == 0.  b200awq_stream_bytes returns 0 for unsupported shapes; the byte count is the same for
  * every mode. */
 size_t b200awq_stream_bytes(int K, int N, int group_size);
