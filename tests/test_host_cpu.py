@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from _toolchain import header_constants, header_layout, mirror_layout
 from oracle import awq_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -163,29 +164,13 @@ def test_torch_port_matches_oracle():
     assert np.array_equal(_bits(w.numpy()), _bits(O.dequantize_gemm(c["qweight"], c["qzeros"], c["scales"], 64)))
 
 
-def test_program_op_struct_matches_header(built, tmp_path):
+def test_program_op_struct_matches_header(built):
     """ctypes mirror of b200awq_op_t vs the C compiler's view of include/b200awq.h (size + every offset)."""
-    import subprocess
-
     from autoawq_b200 import _cabi
 
-    fields = [f[0] for f in _cabi.Op._fields_]
-    src = tmp_path / "layout.c"
-    src.write_text(
-        '#include <stdio.h>\n#include <stddef.h>\n#include "b200awq.h"\nint main(void) {\n'
-        '  printf("%zu", sizeof(b200awq_op_t));\n'
-        + "".join(f'  printf(" %zu", offsetof(b200awq_op_t, {f}));\n' for f in fields)
-        + "  return 0;\n}\n"
-    )
-    exe = tmp_path / "layout"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).decode().split()]
-    assert got[0] == ctypes.sizeof(_cabi.Op)
-    assert got[1:] == [getattr(_cabi.Op, f).offset for f in fields]
-    header = open(os.path.join(ROOT, "include", "b200awq.h")).read()
-    assert (_cabi.OP_RMSNORM, _cabi.OP_LINEAR_GEMM, _cabi.OP_SILU_AND_MUL) == tuple(
-        int(re.search(rf"{n}\s*=\s*(\d+)", header).group(1))
-        for n in ("B200AWQ_OP_RMSNORM", "B200AWQ_OP_LINEAR_GEMM", "B200AWQ_OP_SILU_AND_MUL"))
+    assert header_layout(_cabi.Op, "b200awq_op_t") == mirror_layout(_cabi.Op)
+    assert header_constants("B200AWQ_OP_RMSNORM", "B200AWQ_OP_LINEAR_GEMM", "B200AWQ_OP_SILU_AND_MUL") == (
+        _cabi.OP_RMSNORM, _cabi.OP_LINEAR_GEMM, _cabi.OP_SILU_AND_MUL)
 
 
 def test_program_argument_validation_without_gpu(built):

@@ -4,18 +4,14 @@ and the consumers share (restated here as the device code walks it: every unit o
 exactly once and no bulk copy crosses a slot), the per-expert stream-slice sizes against oracle/stream_format.py, the
 ctypes mirror of b200awq_moe_t, and the register / spill budget of the MoE kernel instantiation."""
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
 import pytest
 
+from _toolchain import entries, header_constants, header_layout, mirror_layout, needs_nvcc
 from autoawq_b200 import _cabi
 from autoawq_b200._cabi import lib
 from oracle import stream_format as SF
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 UPS = {128: 4, 64: 7, 32: 14}       # units per 4288-byte ring stage (kSpStageBytes / unit bytes)
 
 
@@ -95,20 +91,9 @@ def test_expert_slices_match_stream_format(H, I, G):
     assert SF.unit_bytes(G) * (2 * I // 16) * (H // SF.unit_k(G)) == SF.stream_bytes(H, 2 * I, G)
 
 
-def test_moe_struct_matches_header(tmp_path):
-    fields = [f[0] for f in _cabi.Moe._fields_]
-    src = tmp_path / "layout.c"
-    src.write_text(
-        '#include <stdio.h>\n#include <stddef.h>\n#include "b200awq.h"\nint main(void) {\n'
-        '  printf("%zu", sizeof(b200awq_moe_t));\n'
-        + "".join(f'  printf(" %zu", offsetof(b200awq_moe_t, {f}));\n' for f in fields)
-        + "  printf(\" %d\", B200AWQ_OP_SPARSE_MOE);\n  return 0;\n}\n")
-    exe = tmp_path / "layout"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).decode().split()]
-    assert got[0] == ctypes.sizeof(_cabi.Moe)
-    assert got[1:-1] == [getattr(_cabi.Moe, f).offset for f in fields]
-    assert got[-1] == _cabi.OP_SPARSE_MOE
+def test_moe_struct_matches_header():
+    assert header_layout(_cabi.Moe, "b200awq_moe_t") == mirror_layout(_cabi.Moe)
+    assert header_constants("B200AWQ_OP_SPARSE_MOE") == (_cabi.OP_SPARSE_MOE,)
 
 
 def test_moe_op_argument_validation_without_gpu():
@@ -122,19 +107,11 @@ def test_moe_op_argument_validation_without_gpu():
     assert lib.b200awq_moe_plan(8, 2, 4096, 14336, 128, 132, None) == 1
 
 
-@pytest.mark.skipif(shutil.which("nvcc") is None and not os.path.exists("/usr/local/cuda/bin/nvcc"), reason="needs nvcc")
-def test_moe_kernel_register_and_spill_budget(tmp_path):
+@needs_nvcc
+def test_moe_kernel_register_and_spill_budget():
     """The MoE instantiation (288 threads, one CTA per SM) fits the register file and spills nothing."""
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    src = os.path.join(ROOT, "autoawq_b200", "csrc", "program.cu")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xptxas",
-                          "-v", "-c", src, "-o", str(tmp_path / "program.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    log = out.stderr + out.stdout
-    entries = re.findall(r"Compiling entry function '(\S*stream_moe_kernel\S*)'[^\n]*\n[^\n]*\n\s*"
-                         r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) "
-                         r"registers", log)
-    assert len(entries) == 1, log[-1500:]
-    name, stack, st, ld, regs = entries[0]
-    assert int(regs) * (32 + 32 * 8) <= 65536, f"{regs} registers x 288 threads"
-    assert int(st) == 0 and int(ld) == 0 and int(stack) == 0, f"spills {st} / {ld} bytes, stack {stack}"
+    found = entries("program.cu", r"stream_moe_kernel")
+    assert len(found) == 1, found
+    (regs, stack, st, ld), = found.values()
+    assert regs * (32 + 32 * 8) <= 65536, f"{regs} registers x 288 threads"
+    assert st == 0 and ld == 0 and stack == 0, f"spills {st} / {ld} bytes, stack {stack}"

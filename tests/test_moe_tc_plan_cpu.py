@@ -4,18 +4,14 @@ every sorted position must be covered exactly once per 128-column tile, no tile 
 token tile, and the token tiles of one (expert, column tile) must be adjacent (CTAs that run together then share the
 expert's weight slab in L2).  The kernel's register / spill budget comes from ptxas."""
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+from _toolchain import entries, needs_nvcc
 from autoawq_b200._cabi import lib
 from oracle import awq_oracle as O
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BLOCK = 16
 
 
@@ -118,19 +114,12 @@ def test_plan_argument_errors():
     assert ok(block=8) != 0 and ok(E=257) != 0
 
 
-@pytest.mark.skipif(shutil.which("nvcc") is None, reason="needs nvcc")
-def test_moe_tc_kernel_register_and_spill_budget(tmp_path):
+@needs_nvcc
+def test_moe_tc_kernel_register_and_spill_budget():
     """One CTA of 512 threads per SM, accumulators in the consumer warpgroups' registers: registers x 512 must fit the
     64 K register file and nothing may spill."""
-    src = os.path.join(ROOT, "autoawq_b200", "csrc", "gemm_tc.cu")
-    out = subprocess.run(
-        ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xptxas", "-v", "-c", src,
-         "-o", str(tmp_path / "gemm_tc.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    log = out.stderr + out.stdout
-    entries = re.findall(r"Compiling entry function '(\S*moe_tc_kernel\S*)'[^\n]*\n[^\n]*\n\s*(\d+) bytes stack frame, "
-                         r"(\d+) bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) registers", log)
-    assert len(entries) == 6, log[-1500:]          # BT in {32, 64, 128} x 1 or 2 quantisation groups per k-step
-    for name, stack, st, ld, regs in entries:
-        assert int(st) == 0 and int(ld) == 0 and int(stack) == 0, f"{name}: spills"
-        assert int(regs) * 512 <= 65536, f"{name}: {regs} registers x 512 threads"
+    found = entries("gemm_tc.cu", r"moe_tc_kernel")
+    assert len(found) == 6, found          # BT in {32, 64, 128} x 1 or 2 quantisation groups per k-step
+    for name, (regs, stack, st, ld) in found.items():
+        assert st == 0 and ld == 0 and stack == 0, f"{name}: spills"
+        assert regs * 512 <= 65536, f"{name}: {regs} registers x 512 threads"

@@ -4,21 +4,15 @@ header, the folding of a trailing residual add, the register / spill budget of s
 the pre-existing entries against a given revision, the numpy routing oracle (which the GPU tests hold the kernel to)
 against transformers' own route_tokens_to_experts, and the shared-expert loader against packing.stack_deepseek_experts."""
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 import types
 
 import numpy as np
 import pytest
 
+from _fake_ops import add, buf, plan
+from _toolchain import entries, header_constants, header_layout, mirror_layout, needs_nvcc, sass_compare
 from autoawq_b200 import _cabi
 from autoawq_b200._cabi import lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-needs_nvcc = pytest.mark.skipif(not os.path.exists(NVCC), reason="needs nvcc")
 
 
 def route_oracle(logits, top_k, scoring, bias=None, n_group=1, topk_group=1, norm=False, rsf=1.0):
@@ -88,101 +82,68 @@ def test_plan_partial_row_limit():
 
 def _desc(E=64, k=6, H=2048, I=1408, I_s=2816, G=128, scoring=1, n_group=1, topk_group=1):
     """A DEEPSEEK_MOE descriptor with placeholder addresses (the plan makes no CUDA call and reads no tensor)."""
-    base = [0x10000000]
-
-    def addr(nbytes):
-        a = base[0]
-        base[0] += (nbytes + 0xffff) & ~0xffff
-        return a
-
     d = _cabi.DeepseekMoe()
     m = d.moe
     m.E, m.top_k, m.renormalize, m.group_size, m.H, m.I, m.block_size = E, k, 0, G, H, I, 16
     m.sorted_len = k + E * 15
-    m.gate_weight = addr(E * H * 2)
-    m.w1_qweight, m.w1_scales, m.w1_qzeros = addr(E * H * I), addr(E * H // G * 2 * I * 2), addr(E * H // G * I)
-    m.w2_qweight, m.w2_scales, m.w2_qzeros = addr(E * I * H // 2), addr(E * I // G * H * 2), addr(E * I // G * H // 2)
+    m.gate_weight = buf(E * H * 2)
+    m.w1_qweight, m.w1_scales, m.w1_qzeros = buf(E * H * I), buf(E * H // G * 2 * I * 2), buf(E * H // G * I)
+    m.w2_qweight, m.w2_scales, m.w2_qzeros = buf(E * I * H // 2), buf(E * I // G * H * 2), buf(E * I // G * H // 2)
     for f, n in (("logits", E * 4), ("topk_weights", k * 4), ("topk_ids", k * 4), ("token_expert_indices", k * 4),
                  ("sorted_ids", m.sorted_len * 4), ("expert_ids", (k + E) * 4), ("num_tokens_post_pad", 4),
                  ("gate_up", (k * 2 * I + 2 * I_s) * 2), ("act", (k * I + I_s) * 2), ("down", k * H * 2)):
-        setattr(m, f, addr(n))
+        setattr(m, f, buf(n))
     d.scoring, d.n_group, d.topk_group, d.norm_topk_prob, d.routed_scaling_factor = scoring, n_group, topk_group, 1, 2.5
     d.I_s = I_s
-    d.bias = addr(E * 4)
-    d.ws1_qweight, d.ws1_scales, d.ws1_qzeros = addr(H * I_s), addr(H // G * 2 * I_s * 2), addr(H // G * I_s)
-    d.ws2_qweight, d.ws2_scales, d.ws2_qzeros = addr(I_s * H // 2), addr(I_s // G * H * 2), addr(I_s // G * H // 2)
-    d.shared_out = addr(H * 2)
-    return d, addr
+    d.bias = buf(E * 4)
+    d.ws1_qweight, d.ws1_scales, d.ws1_qzeros = buf(H * I_s), buf(H // G * 2 * I_s * 2), buf(H // G * I_s)
+    d.ws2_qweight, d.ws2_scales, d.ws2_qzeros = buf(I_s * H // 2), buf(I_s // G * H * 2), buf(I_s // G * H // 2)
+    d.shared_out = buf(H * 2)
+    return d
 
 
-def _ops(d, addr, with_add=False):
+def _ops(d, with_add=False):
     H = d.moe.H
-    ops = (_cabi.Op * (2 if with_add else 1))()
-    ops[0].kind, ops[0].M, ops[0].K, ops[0].N = _cabi.OP_DEEPSEEK_MOE, 1, H, H
-    ops[0].x, ops[0].y, ops[0].weight = addr(H * 2), addr(H * 2), ctypes.addressof(d)
+    ops = [dict(kind=_cabi.OP_DEEPSEEK_MOE, M=1, K=H, N=H, x=buf(H * 2), y=buf(H * 2), weight=ctypes.addressof(d))]
     if with_add:
-        ops[1].kind, ops[1].M, ops[1].K = _cabi.OP_ADD, 1, H
-        ops[1].x, ops[1].weight, ops[1].y = ops[0].y, addr(H * 2), addr(H * 2)
+        ops.append(add(ops[0]["y"], buf(H * 2), H))
     return ops
 
 
 @pytest.mark.parametrize("with_add", [False, True])
 def test_trailing_add_folds_into_down(with_add):
-    d, addr = _desc()
-    ops = _ops(d, addr, with_add)
-    n = ctypes.c_int()
-    assert lib.b200awq_program_plan(ops, len(ops), 1, 132, 0, ctypes.byref(n)) == 0
-    assert n.value == 2                      # gate|up (with the routing and the shared expert), down (+ the add)
+    d = _desc()
+    assert plan(_ops(d, with_add)) == (0, 2)               # gate|up (with the routing and the shared expert), down (+ the add)
 
 
 @pytest.mark.parametrize("field,value", [("scoring", 2), ("n_group", 0), ("n_group", 5), ("topk_group", 0),
                                          ("topk_group", 9), ("I_s", 100), ("bias", None), ("shared_out", None),
                                          ("ws2_qzeros", None)])
 def test_bad_descriptor_is_einval(field, value):
-    d, addr = _desc(n_group=8, topk_group=4)
+    d = _desc(n_group=8, topk_group=4)
     setattr(d, field, value)
-    ops = _ops(d, addr)
-    n = ctypes.c_int()
-    assert lib.b200awq_program_plan(ops, len(ops), 1, 132, 0, ctypes.byref(n)) == 1
+    assert plan(_ops(d))[0] == 1
 
 
 def test_softmax_needs_no_bias():
-    d, addr = _desc(scoring=0)
+    d = _desc(scoring=0)
     d.bias = None
-    ops = _ops(d, addr)
-    n = ctypes.c_int()
-    assert lib.b200awq_program_plan(ops, len(ops), 1, 132, 0, ctypes.byref(n)) == 0
+    assert plan(_ops(d))[0] == 0
 
 
-def test_layout_and_op_constant_match_header(tmp_path):
-    src = tmp_path / "c.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "b200awq.h"\n'
-                   'int main(void) { printf("%d %zu %zu %zu %zu %zu", B200AWQ_OP_DEEPSEEK_MOE, '
-                   'sizeof(b200awq_deepseek_moe_t), offsetof(b200awq_deepseek_moe_t, scoring), '
-                   'offsetof(b200awq_deepseek_moe_t, bias), offsetof(b200awq_deepseek_moe_t, ws2_qzeros), '
-                   'offsetof(b200awq_deepseek_moe_t, shared_out)); return 0; }\n')
-    exe = tmp_path / "c"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    D = _cabi.DeepseekMoe
-    want = [_cabi.OP_DEEPSEEK_MOE, ctypes.sizeof(D), D.scoring.offset, D.bias.offset, D.ws2_qzeros.offset,
-            D.shared_out.offset]
-    assert [int(v) for v in subprocess.check_output([str(exe)]).decode().split()] == want
+def test_layout_and_op_constant_match_header():
+    assert header_layout(_cabi.DeepseekMoe, "b200awq_deepseek_moe_t") == mirror_layout(_cabi.DeepseekMoe)
+    assert header_constants("B200AWQ_OP_DEEPSEEK_MOE") == (_cabi.OP_DEEPSEEK_MOE,)
 
 
 @needs_nvcc
-def test_entry_register_and_spill_budget(tmp_path):
+def test_entry_register_and_spill_budget():
     """stream_deepseek_moe_kernel (288 threads, one CTA per SM) fits the register file.  It spills at most 8 bytes: two
     per-op values (the thread index and the CTA's first set) stored before the unit loop and reloaded around it, never
     inside it; the other MoE entries spill nothing (test_program_qwen3moe_cpu.py)."""
-    out = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xptxas",
-                          "-v", "-c", os.path.join(ROOT, "autoawq_b200", "csrc", "program.cu"), "-o",
-                          str(tmp_path / "p.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    log = out.stderr + out.stdout
-    m = re.search(r"Compiling entry function '\S*stream_deepseek_moe_kernel\S*'[^\n]*\n[^\n]*\n\s*(\d+) bytes stack "
-                  r"frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) registers", log)
-    assert m
-    stack, st, ld, regs = (int(v) for v in m.groups())
+    found = entries("program.cu", "stream_deepseek_moe_kernel")
+    assert found
+    regs, stack, st, ld = next(iter(found.values()))
     assert regs * (32 + 32 * 8) <= 65536 and st <= 8 and stack <= 8, (regs, st, ld, stack)
 
 
@@ -191,15 +152,7 @@ def test_existing_entries_sass_unchanged():
     """With B200AWQ_SASS_BASE set to a git revision (the commit before this op), every entry both trees have compiles
     to the same SASS (tools/sass_unchanged.py): the DeepSeek code sits behind SP_DEEPSEEK and its own side table.
     Unset, the test is skipped."""
-    base = os.environ.get("B200AWQ_SASS_BASE")
-    if not base:
-        pytest.skip("set B200AWQ_SASS_BASE to a git revision to compare against")
-    if shutil.which("git") is None or subprocess.run(["git", "-C", ROOT, "cat-file", "-e", base + "^{commit}"],
-                                                     capture_output=True).returncode != 0:
-        pytest.skip(f"{base} is not a commit of this checkout")
-    from tools.sass_unchanged import compare
-
-    res = compare(base)
+    res = sass_compare()
     assert res, "no entry to compare"
     assert all(res.values()), [n for n, same in res.items() if not same]
 

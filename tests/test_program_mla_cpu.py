@@ -3,21 +3,17 @@ b200awq_mla_t and the two op constants against the header, the exports, the mode
 oracle, the folding of the MLA chain and every rejection through b200awq_program_plan, the register / spill budget of
 stream_mla_kernel and the SASS of the pre-existing entries against a given revision."""
 import ctypes
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+from _fake_ops import add, buf, linear, plan, rmsnorm
+from _toolchain import entries, header_constants, header_layout, mirror_layout, needs_nvcc, sass, sass_compare
 from autoawq_b200 import _cabi
 from autoawq_b200._cabi import lib
 from oracle import stream_format as SF
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-needs_nvcc = pytest.mark.skipif(not os.path.exists(NVCC), reason="needs nvcc")
+from test_program_deepseek_moe_cpu import _desc
 
 # DeepSeek-V2-Lite / Moonlight-16B-A3B attention: H, Dn, Dr, Dv, C, hidden
 H, DN, DR, DV, C, HID = 16, 128, 64, 128, 512, 2048
@@ -32,20 +28,9 @@ def mode3_columns(N):
     return np.concatenate([16 * s + 2 * g, 16 * s + 2 * g + 1], axis=1)
 
 
-def test_layout_and_op_constants_match_header(tmp_path):
-    src = tmp_path / "c.c"
-    fields = ["style", "cache_len", "freqs_len", "k_batch_stride", "v_batch_stride", "v_head_stride", "pos", "freqs",
-              "q_out", "k_cache", "v_cache"]
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "b200awq.h"\n'
-                   'int main(void) { printf("%d %d %zu' + " %zu" * len(fields) + '", B200AWQ_OP_MLA_ROPE, '
-                   'B200AWQ_OP_MLA_KV, sizeof(b200awq_mla_t)' +
-                   "".join(f", offsetof(b200awq_mla_t, {f})" for f in fields) + "); return 0; }\n")
-    exe = tmp_path / "c"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    M = _cabi.Mla
-    want = [_cabi.OP_MLA_ROPE, _cabi.OP_MLA_KV, ctypes.sizeof(M)] + [getattr(M, f).offset for f in fields]
-    assert [int(v) for v in subprocess.check_output([str(exe)]).decode().split()] == want
-    assert (_cabi.OP_MLA_ROPE, _cabi.OP_MLA_KV) == (10, 11)
+def test_layout_and_op_constants_match_header():
+    assert header_layout(_cabi.Mla, "b200awq_mla_t") == mirror_layout(_cabi.Mla)
+    assert header_constants("B200AWQ_OP_MLA_ROPE", "B200AWQ_OP_MLA_KV") == (_cabi.OP_MLA_ROPE, _cabi.OP_MLA_KV) == (10, 11)
 
 
 def test_exports():
@@ -97,64 +82,33 @@ def permute_linear(qweight, qzeros, scales, perm):
 
 
 # ------------------------------------------------------------------------------------------------ folding (plan)
-class Addr:
-    """Placeholder device addresses (the plan makes no CUDA call and reads no tensor)."""
-
-    def __init__(self):
-        self.base = 0x10000000
-
-    def __call__(self, nbytes):
-        a = self.base
-        self.base += (nbytes + 0xffff) & ~0xffff
-        return a
-
-
-def mla_desc(addr, S=2048, Sf=4096, style=0, v_head=DV, **kw):
+def mla_desc(S=2048, Sf=4096, style=0, v_head=DV, **kw):
     d = _cabi.Mla()
     d.n_heads, d.nope_dim, d.rope_dim, d.v_dim, d.kv_lora_rank, d.style = H, DN, DR, DV, C, style
     d.cache_len, d.freqs_len = S, Sf
     d.k_batch_stride, d.v_batch_stride, d.v_head_stride = S * H * (DN + DR), S * H * v_head, v_head
-    d.pos, d.freqs, d.q_out = addr(4), addr(Sf * DR * 4), addr(H * (DN + DR) * 2)
-    d.k_cache, d.v_cache = addr(S * H * (DN + DR) * 2), addr(S * H * v_head * 2)
+    d.pos, d.freqs, d.q_out = buf(4), buf(Sf * DR * 4), buf(H * (DN + DR) * 2)
+    d.k_cache, d.v_cache = buf(S * H * (DN + DR) * 2), buf(S * H * v_head * 2)
     for k, v in kw.items():
         setattr(d, k, v)
     return d
 
 
-def linear(op, addr, K, N, x, M=1):
-    op.kind, op.M, op.K, op.N, op.group_size, op.ldx = _cabi.OP_LINEAR_GEMM, M, K, N, 128, K
-    op.x, op.y = x, addr(M * N * 2)
-    op.qweight, op.scales, op.qzeros = addr(K * N // 2), addr(K // 128 * N * 2), addr(K // 128 * N // 2)
-
-
-def mla_chain(addr, M=1, d_rope=None, d_kv=None):
+def mla_chain(M=1, d_rope=None, d_kv=None):
     """[norm1, q|kv_a, mla_rope, rmsnorm(c_kv), kv_b, mla_kv]: the start of a DeepSeek attention block (no q LoRA)."""
-    d = d_rope if d_rope is not None else mla_desc(addr)
+    d = d_rope if d_rope is not None else mla_desc()
     dk = d_kv if d_kv is not None else d
-    ops = (_cabi.Op * 6)()
-    h, xn = addr(M * HID * 2), addr(M * HID * 2)
-    ops[0].kind, ops[0].M, ops[0].K, ops[0].eps = _cabi.OP_RMSNORM, M, HID, 1e-6
-    ops[0].x, ops[0].weight, ops[0].y = h, addr(HID * 2), xn
-    linear(ops[1], addr, HID, N_QKVA, xn, M)
-    ops[2].kind, ops[2].M, ops[2].N, ops[2].ldx = _cabi.OP_MLA_ROPE, M, N_QKVA, N_QKVA
-    ops[2].x, ops[2].weight = ops[1].y, ctypes.addressof(d)
-    ops[3].kind, ops[3].M, ops[3].K, ops[3].eps = _cabi.OP_RMSNORM, M, C, 1e-6
-    ops[3].x, ops[3].weight, ops[3].y = ops[1].y + H * (DN + DR) * 2, addr(C * 2), addr(M * C * 2)
-    linear(ops[4], addr, C, N_KV, ops[3].y, M)
-    ops[5].kind, ops[5].M, ops[5].N, ops[5].ldx = _cabi.OP_MLA_KV, M, N_KV, N_KV
-    ops[5].x, ops[5].weight = ops[4].y, ctypes.addressof(dk)
-    return ops, (d, dk)
-
-
-def plan(ops, max_tokens=1, sms=132):
-    n = ctypes.c_int()
-    rc = lib.b200awq_program_plan(ops, len(ops), max_tokens, sms, 0, ctypes.byref(n))
-    return rc, n.value
+    norm1 = rmsnorm(buf(M * HID * 2), HID, M, eps=1e-6)
+    qkva = linear(norm1["y"], HID, N_QKVA, M)
+    rope = dict(kind=_cabi.OP_MLA_ROPE, M=M, N=N_QKVA, ldx=N_QKVA, x=qkva["y"], weight=ctypes.addressof(d))
+    ckv = rmsnorm(qkva["y"] + H * (DN + DR) * 2, C, M, eps=1e-6)
+    kvb = linear(ckv["y"], C, N_KV, M)
+    kv = dict(kind=_cabi.OP_MLA_KV, M=M, N=N_KV, ldx=N_KV, x=kvb["y"], weight=ctypes.addressof(dk))
+    return [norm1, qkva, rope, ckv, kvb, kv], (d, dk)
 
 
 def test_chain_folds_into_two_kernel_ops():
-    addr = Addr()
-    ops, keep = mla_chain(addr)
+    ops, keep = mla_chain()
     assert plan(ops) == (0, 2)          # q|kv_a (+ MLA_ROPE), kv_b (+ kv_a_layernorm as its prologue, + MLA_KV)
 
 
@@ -162,171 +116,134 @@ def test_chain_folds_into_two_kernel_ops():
 def test_v2_lite_segment_plan(style):
     """[o + h, norm2, deepseek_moe + h, norm1', q|kv_a', mla_rope', rmsnorm(c_kv)', kv_b', mla_kv']: accepted at M = 1
     on 132 SMs (o, gate|up, down, q|kv_a', kv_b'), rejected at M = 2."""
-    from test_program_deepseek_moe_cpu import _desc
-
     for M in (1, 2):
-        addr = Addr()
-        dsk, daddr = _desc(scoring=style)
+        dsk = _desc(scoring=style)
         dsk.moe.sorted_len = 6 * M + 64 * 15
-        addr.base = daddr(0) + (1 << 30)
-        ops = (_cabi.Op * 11)()
-        attn, h = addr(M * HID * 2), addr(M * HID * 2)
-        linear(ops[0], addr, HID, HID, attn, M)                         # o_proj
-        ops[1].kind, ops[1].M, ops[1].K = _cabi.OP_ADD, M, HID
-        ops[1].x, ops[1].weight, ops[1].y = ops[0].y, h, addr(M * HID * 2)
-        ops[2].kind, ops[2].M, ops[2].K, ops[2].eps = _cabi.OP_RMSNORM, M, HID, 1e-6
-        ops[2].x, ops[2].weight, ops[2].y = ops[1].y, addr(HID * 2), addr(M * HID * 2)
-        ops[3].kind, ops[3].M, ops[3].K, ops[3].N = _cabi.OP_DEEPSEEK_MOE, M, HID, HID
-        ops[3].x, ops[3].y, ops[3].weight = ops[2].y, addr(M * HID * 2), ctypes.addressof(dsk)
-        ops[4].kind, ops[4].M, ops[4].K = _cabi.OP_ADD, M, HID
-        ops[4].x, ops[4].weight, ops[4].y = ops[3].y, ops[1].y, addr(M * HID * 2)
-        chain, keep = mla_chain(addr, M)
-        for i in range(6):
-            ops[5 + i] = chain[i]
-        ops[5].x = ops[4].y
-        rc, n = plan(ops, max_tokens=M)
+        o = linear(buf(M * HID * 2), HID, HID, M)                        # o_proj
+        h = add(o["y"], buf(M * HID * 2), HID, M)
+        norm2 = rmsnorm(h["y"], HID, M, eps=1e-6)
+        moe = dict(kind=_cabi.OP_DEEPSEEK_MOE, M=M, K=HID, N=HID, x=norm2["y"], y=buf(M * HID * 2),
+                   weight=ctypes.addressof(dsk))
+        out = add(moe["y"], h["y"], HID, M)
+        chain, keep = mla_chain(M)
+        chain[0]["x"] = out["y"]
+        rc, n = plan([o, h, norm2, moe, out] + chain, max_tokens=M)
         assert (rc, n) == ((0, 5) if M == 1 else (2, 0)), (M, rc, n)
-    addr = Addr()
-    ops, keep = mla_chain(addr, 2)
+    ops, keep = mla_chain(2)
     assert plan(ops, max_tokens=2)[0] == 2       # the MLA ops alone at M = 2: per op as well
 
 
 def _reject(mutate, rc=2):
-    addr = Addr()
-    ops, keep = mla_chain(addr)
-    mutate(ops, keep[0], addr)
+    ops, keep = mla_chain()
+    mutate(ops, keep[0])
     assert plan(ops)[0] == rc
 
 
 def test_rejects_op_before_not_a_plain_linear():
-    def glue_in_between(ops, d, addr):   # mla_rope after the rmsnorm instead of after q|kv_a
+    def glue_in_between(ops, d):   # mla_rope after the rmsnorm instead of after q|kv_a
         ops[2], ops[3] = ops[3], ops[2]
     _reject(glue_in_between)
 
-    def first(ops, d, addr):
+    def first(ops, d):
         ops[0] = ops[2]
     _reject(first)
 
 
 def test_rejects_mla_after_a_moe_block():
-    from test_program_deepseek_moe_cpu import _desc
-
-    addr = Addr()
-    dsk, daddr = _desc()
-    d = mla_desc(addr)
+    dsk = _desc()
+    d = mla_desc()
     d.n_heads, d.nope_dim, d.v_dim, d.v_head_stride = 1, 1024, 1024, 1024
-    ops = (_cabi.Op * 2)()
-    ops[0].kind, ops[0].M, ops[0].K, ops[0].N = _cabi.OP_DEEPSEEK_MOE, 1, HID, HID
-    ops[0].x, ops[0].y, ops[0].weight = daddr(HID * 2), daddr(HID * 2), ctypes.addressof(dsk)
-    ops[1].kind, ops[1].M, ops[1].N, ops[1].ldx = _cabi.OP_MLA_KV, 1, HID, HID
-    ops[1].x, ops[1].weight = ops[0].y, ctypes.addressof(d)
-    assert plan(ops)[0] == 2
+    moe = dict(kind=_cabi.OP_DEEPSEEK_MOE, M=1, K=HID, N=HID, x=buf(HID * 2), y=buf(HID * 2), weight=ctypes.addressof(dsk))
+    kv = dict(kind=_cabi.OP_MLA_KV, M=1, N=HID, ldx=HID, x=moe["y"], weight=ctypes.addressof(d))
+    assert plan([moe, kv])[0] == 2
 
 
 @pytest.mark.parametrize("field,value", [("n_heads", 8), ("kv_lora_rank", 256), ("rope_dim", 32)])
 def test_rejects_n_mismatch(field, value):
-    _reject(lambda ops, d, addr: setattr(d, field, value))
+    _reject(lambda ops, d: setattr(d, field, value))
 
 
 @pytest.mark.parametrize("dims", [(120, 64, 128, 512), (128, 56, 128, 512), (128, 64, 120, 512), (128, 64, 128, 520)])
 def test_rejects_dims_not_multiple_of_16(dims):
     dn, dr, dv, c = dims
-    addr = Addr()
-    d = mla_desc(addr, nope_dim=dn, rope_dim=dr, v_dim=dv, kv_lora_rank=c)
+    d = mla_desc(nope_dim=dn, rope_dim=dr, v_dim=dv, kv_lora_rank=c)
     d.k_batch_stride, d.v_batch_stride, d.v_head_stride = 2048 * H * (dn + dr), 2048 * H * dv, dv
-    ops, keep = mla_chain(addr, d_rope=d)
-    ops[1].N = ops[2].N = H * (dn + dr) + c + dr
-    ops[3].x = ops[1].y + H * (dn + dr) * 2
-    ops[3].K = ops[4].K = c
-    ops[4].N = ops[5].N = H * (dn + dv)
-    ops[4].group_size = 8                    # (so that K = C = 520 is still a whole number of groups)
+    ops, keep = mla_chain(d_rope=d)
+    ops[1]["N"] = ops[2]["N"] = H * (dn + dr) + c + dr
+    ops[3]["x"] = ops[1]["y"] + H * (dn + dr) * 2
+    ops[3]["K"] = ops[4]["K"] = c
+    ops[4]["N"] = ops[5]["N"] = H * (dn + dv)
+    ops[4]["group_size"] = 8                 # (so that K = C = 520 is still a whole number of groups)
     assert plan(ops)[0] == 2
 
 
 @pytest.mark.parametrize("what", ["reads q_out", "writes q_out", "writes k_cache", "writes v_cache", "reads v_cache",
                                   "writes pos", "writes freqs"])
 def test_rejects_other_ops_on_outputs_or_writes_of_inputs(what):
-    def mutate(ops, d, addr):
+    def mutate(ops, d):
         tgt = {"reads q_out": d.q_out, "writes q_out": d.q_out, "writes k_cache": d.k_cache + 4096,
                "writes v_cache": d.v_cache, "reads v_cache": d.v_cache, "writes pos": d.pos,
                "writes freqs": d.freqs}[what]
         if what.startswith("reads"):
-            ops[3].x = tgt                   # kv_a_layernorm (kv_b's prologue) reads it instead of c_kv
+            ops[3]["x"] = tgt                # kv_a_layernorm (kv_b's prologue) reads it instead of c_kv
         else:
-            ops[4].y = tgt
-            ops[5].x = tgt
+            ops[4]["y"] = tgt
+            ops[5]["x"] = tgt
     _reject(mutate)
 
 
 def test_rejects_two_mla_ropes_on_one_k_cache():
-    addr = Addr()
-    ops, (d, _) = mla_chain(addr)
-    ops2, (d2, _) = mla_chain(addr)
+    ops, (d, _) = mla_chain()
+    ops2, (d2, _) = mla_chain()
     d2.k_cache = d.k_cache
-    both = (_cabi.Op * 12)(*list(ops), *list(ops2))
+    both = ops + ops2
     assert plan(both)[0] == 2
-    d2.k_cache = addr(2048 * H * (DN + DR) * 2)   # separate caches: two layers' chains in one program fold
+    d2.k_cache = buf(2048 * H * (DN + DR) * 2)   # separate caches: two layers' chains in one program fold
     assert plan(both) == (0, 4)
 
 
 def test_rope_and_kv_may_not_share_k_cache_with_another_geometry():
-    addr = Addr()
-    d = mla_desc(addr)
-    dk = mla_desc(addr, k_cache=d.k_cache, cache_len=1024)
+    d = mla_desc()
+    dk = mla_desc(k_cache=d.k_cache, cache_len=1024)
     dk.k_batch_stride, dk.v_batch_stride = 1024 * H * (DN + DR), 1024 * H * DV
-    ops, keep = mla_chain(addr, d_rope=d, d_kv=dk)
+    ops, keep = mla_chain(d_rope=d, d_kv=dk)
     assert plan(ops)[0] == 2
 
 
 @pytest.mark.parametrize("field", ["pos", "k_cache", "q_out", "freqs"])
 def test_null_pointer_is_einval(field):
-    _reject(lambda ops, d, addr: setattr(d, field, None), rc=1)
+    _reject(lambda ops, d: setattr(d, field, None), rc=1)
 
 
 def test_kv_op_ignores_rope_only_fields():
     """MLA_KV reads neither freqs nor q_out (a descriptor without them folds); MLA_ROPE reads no v_cache."""
-    addr = Addr()
-    d = mla_desc(addr)
-    dk = mla_desc(addr, k_cache=d.k_cache)
+    d = mla_desc()
+    dk = mla_desc(k_cache=d.k_cache)
     dk.freqs, dk.q_out, dk.freqs_len, dk.style = None, None, 0, 7
     d.v_cache, d.v_dim = None, 0
-    ops, keep = mla_chain(addr, d_rope=d, d_kv=dk)
+    ops, keep = mla_chain(d_rope=d, d_kv=dk)
     assert plan(ops) == (0, 2)
 
 
 @pytest.mark.parametrize("style", [0, 1])
 def test_padded_v_cache_folds(style):
     """A v_cache whose heads are padded to Dn + Dr (FlashAttention-2's layout for Dv < Dqk) is accepted."""
-    addr = Addr()
-    d = mla_desc(addr, style=style, v_head=DN + DR)
-    ops, keep = mla_chain(addr, d_rope=d)
+    d = mla_desc(style=style, v_head=DN + DR)
+    ops, keep = mla_chain(d_rope=d)
     assert plan(ops) == (0, 2)
 
 
 # ------------------------------------------------------------------------------------------------ the kernel entry
 @needs_nvcc
-def test_entry_register_and_spill_budget(tmp_path):
+def test_entry_register_and_spill_budget():
     """stream_mla_kernel (288 threads, one CTA per SM) fits the register file: 168 registers, like
     stream_deepseek_moe_kernel, and 12 bytes of spill stores (the DeepSeek entry's 8 and one more value) made before the
     unit loop.  No spill load or store sits inside the unit loop (between its first and last MMA)."""
-    out = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xptxas",
-                          "-v", "-c", os.path.join(ROOT, "autoawq_b200", "csrc", "program.cu"), "-o",
-                          str(tmp_path / "p.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    log = out.stderr + out.stdout
-
-    def budget(name):
-        m = re.search(r"Compiling entry function '\S*" + name + r"\S*'[^\n]*\n[^\n]*\n\s*(\d+) bytes stack "
-                      r"frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) registers", log)
-        assert m, name
-        return tuple(int(v) for v in m.groups())
-
-    stack, st, ld, regs = budget("stream_mla_kernel")
+    found = entries("program.cu", "stream_mla_kernel")
+    assert found
+    regs, stack, st, ld = next(iter(found.values()))
     assert regs * (32 + 32 * 8) <= 65536 and st <= 12 and stack <= 16, (regs, st, ld, stack)
-    cuobjdump = os.path.join(os.path.dirname(NVCC), "cuobjdump")
-    sass = subprocess.run([cuobjdump, "-sass", str(tmp_path / "p.o")], capture_output=True, text=True, check=True).stdout
-    body = re.search(r"Function : \S*stream_mla_kernel\S*\n(.*?)(?=\n\s*Function : |\Z)", sass, re.S).group(1)
-    lines = body.splitlines()
+    lines = sass("program.cu", "stream_mla_kernel").splitlines()
     mma = [i for i, line in enumerate(lines) if "HMMA" in line]
     assert mma
     inside = [line for line in lines[mma[0]:mma[-1]] if re.search(r"\b(LDL|STL)\b", line)]
@@ -338,15 +255,7 @@ def test_existing_entries_sass_unchanged():
     """With B200AWQ_SASS_BASE set to a git revision (the commit before these ops), every entry both trees have compiles
     to the same SASS (tools/sass_unchanged.py): the MLA code sits behind SP_MLA, its own side table and its own pack
     kernel.  Unset, the test is skipped."""
-    base = os.environ.get("B200AWQ_SASS_BASE")
-    if not base:
-        pytest.skip("set B200AWQ_SASS_BASE to a git revision to compare against")
-    if shutil.which("git") is None or subprocess.run(["git", "-C", ROOT, "cat-file", "-e", base + "^{commit}"],
-                                                     capture_output=True).returncode != 0:
-        pytest.skip(f"{base} is not a commit of this checkout")
-    from tools.sass_unchanged import compare
-
-    res = compare(base)
+    res = sass_compare()
     assert res, "no entry to compare"
     assert all(res.values()), [n for n, same in res.items() if not same]
 
@@ -403,12 +312,8 @@ def test_sizes_that_fit_reach_the_device_check():
 def test_row_strided_rmsnorm_replays_per_op(M, ldx, rc):
     """An RMSNORM over rows of a wider tensor (kv_a_layernorm on the c_kv slice of M > 1 rows) is refused by the fused
     kernels, which stage contiguous rows; a contiguous one (ldx 0 or K) folds."""
-    addr = Addr()
-    ops = (_cabi.Op * 2)()
-    ops[0].kind, ops[0].M, ops[0].K, ops[0].eps, ops[0].ldx = _cabi.OP_RMSNORM, M, C, 1e-6, ldx
-    ops[0].x, ops[0].weight, ops[0].y = addr(M * N_QKVA * 2), addr(C * 2), addr(M * C * 2)
-    linear(ops[1], addr, C, N_KV, ops[0].y, M)
-    assert plan(ops, max_tokens=M)[0] == rc
+    ckv = rmsnorm(buf(M * N_QKVA * 2), C, M, eps=1e-6, ldx=ldx)
+    assert plan([ckv, linear(ckv["y"], C, N_KV, M)], max_tokens=M)[0] == rc
 
 
 def test_fuse_mla_input_concatenates_the_two_projections():

@@ -5,20 +5,14 @@ a model of the grid-wide router-logit exchange (program_stream.cuh: kSpQwenEMax)
 The exchange model checks the protocol's design (one writer per word and run, tags that never pass a stale word); it
 does not run the kernel code, which tests/test_gpu_program_qwen3moe.py covers on the GPU."""
 import ctypes
-import os
 import random
-import re
-import shutil
-import subprocess
 
 import pytest
 
+from _fake_ops import add, buf, plan
+from _toolchain import entries, header_constants, needs_nvcc, sass_compare
 from autoawq_b200 import _cabi
 from autoawq_b200._cabi import lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-needs_nvcc = pytest.mark.skipif(not os.path.exists(NVCC), reason="needs nvcc")
 
 
 def _plan(E, k, H, I, G, sms=132):
@@ -55,64 +49,41 @@ def _moe_ops(with_add, kind=None):
     """[QWEN3_MOE (+ ADD of its output and an external residual)] with placeholder addresses (the plan makes no CUDA
     call and reads no tensor)."""
     H, I, E, k = 2048, 768, 128, 8
-    base = [0x10000000]
-
-    def addr(nbytes):
-        a = base[0]
-        base[0] += (nbytes + 0xffff) & ~0xffff
-        return a
-
     d = _cabi.Moe()
     d.E, d.top_k, d.renormalize, d.group_size, d.H, d.I, d.block_size = E, k, 1, 128, H, I, 16
     d.sorted_len = k + E * 15
-    d.gate_weight = addr(E * H * 2)
-    d.w1_qweight, d.w1_scales, d.w1_qzeros = addr(E * H * 2 * I // 2), addr(E * H // 128 * 2 * I * 2), addr(E * 2 * I)
-    d.w2_qweight, d.w2_scales, d.w2_qzeros = addr(E * I * H // 2), addr(E * I // 128 * H * 2), addr(E * H)
+    d.gate_weight = buf(E * H * 2)
+    d.w1_qweight, d.w1_scales, d.w1_qzeros = buf(E * H * 2 * I // 2), buf(E * H // 128 * 2 * I * 2), buf(E * 2 * I)
+    d.w2_qweight, d.w2_scales, d.w2_qzeros = buf(E * I * H // 2), buf(E * I // 128 * H * 2), buf(E * H)
     for f, n in (("logits", E * 2), ("topk_weights", k * 4), ("topk_ids", k * 4), ("token_expert_indices", k * 4),
                  ("sorted_ids", d.sorted_len * 4), ("expert_ids", (k + E) * 4), ("num_tokens_post_pad", 4),
                  ("gate_up", k * 2 * I * 2), ("act", k * I * 2), ("down", k * H * 2)):
-        setattr(d, f, addr(n))
-    ops = (_cabi.Op * (2 if with_add else 1))()
-    ops[0].kind, ops[0].M, ops[0].K, ops[0].N = kind or _cabi.OP_QWEN3_MOE, 1, H, H
-    ops[0].x, ops[0].y, ops[0].weight = addr(H * 2), addr(H * 2), ctypes.addressof(d)
+        setattr(d, f, buf(n))
+    ops = [dict(kind=kind or _cabi.OP_QWEN3_MOE, M=1, K=H, N=H, x=buf(H * 2), y=buf(H * 2), weight=ctypes.addressof(d))]
     if with_add:
-        ops[1].kind, ops[1].M, ops[1].K = _cabi.OP_ADD, 1, H
-        ops[1].x, ops[1].weight, ops[1].y = ops[0].y, addr(H * 2), addr(H * 2)
+        ops.append(add(ops[0]["y"], buf(H * 2), H))
     return ops, d
 
 
 @pytest.mark.parametrize("with_add", [False, True])
 def test_trailing_add_folds_into_down(with_add):
     ops, _keep = _moe_ops(with_add)
-    n = ctypes.c_int()
-    assert lib.b200awq_program_plan(ops, len(ops), 1, 132, 0, ctypes.byref(n)) == 0
-    assert n.value == 2                      # gate|up with the routing, down (+ the add in its finish)
+    assert plan(ops) == (0, 2)               # gate|up with the routing, down (+ the add in its finish)
 
 
-def test_op_constant_matches_header(tmp_path):
-    src = tmp_path / "c.c"
-    src.write_text('#include <stdio.h>\n#include "b200awq.h"\nint main(void) { printf("%d %d", B200AWQ_OP_QWEN3_MOE, '
-                   'B200AWQ_OP_SPARSE_MOE); return 0; }\n')
-    exe = tmp_path / "c"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    assert subprocess.check_output([str(exe)]).decode().split() == [str(_cabi.OP_QWEN3_MOE), str(_cabi.OP_SPARSE_MOE)]
+def test_op_constant_matches_header():
+    assert header_constants("B200AWQ_OP_QWEN3_MOE", "B200AWQ_OP_SPARSE_MOE") == (_cabi.OP_QWEN3_MOE, _cabi.OP_SPARSE_MOE)
 
 
 @needs_nvcc
-def test_moe_entries_register_and_spill_budget(tmp_path):
+def test_moe_entries_register_and_spill_budget():
     """Every MoE-instantiated M = 1 entry (288 threads, one CTA per SM) fits the register file and spills nothing."""
-    out = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xptxas",
-                          "-v", "-c", os.path.join(ROOT, "autoawq_b200", "csrc", "program.cu"), "-o",
-                          str(tmp_path / "p.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    log = out.stderr + out.stdout
     names = ("stream_moe_kernel", "stream_residual_kernel", "stream_rope_kernel", "stream_qknorm_kernel",
              "stream_qwen3moe_kernel")
     for name in names:
-        m = re.search(r"Compiling entry function '\S*" + name + r"\S*'[^\n]*\n[^\n]*\n\s*(\d+) bytes stack frame, (\d+) "
-                      r"bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) registers", log)
-        assert m, name
-        stack, st, ld, regs = (int(v) for v in m.groups())
+        found = entries("program.cu", name)
+        assert found, name
+        regs, stack, st, ld = next(iter(found.values()))
         assert regs * (32 + 32 * 8) <= 65536 and st == 0 and ld == 0 and stack == 0, (name, regs, st, ld, stack)
 
 
@@ -121,15 +92,7 @@ def test_plain_entries_sass_unchanged():
     """With B200AWQ_SASS_BASE set to a git revision (e.g. the commit before a change to the MoE kernels), the SASS of the
     plain and batched stream entries and the pack kernels equals that revision's (tools/sass_unchanged.py).  Unset, the
     test is skipped: which entries a change may touch is the change's own claim, not a property of the tree."""
-    base = os.environ.get("B200AWQ_SASS_BASE")
-    if not base:
-        pytest.skip("set B200AWQ_SASS_BASE to a git revision to compare against")
-    if shutil.which("git") is None or subprocess.run(["git", "-C", ROOT, "cat-file", "-e", base + "^{commit}"],
-                                                     capture_output=True).returncode != 0:
-        pytest.skip(f"{base} is not a commit of this checkout")
-    from tools.sass_unchanged import compare
-
-    res = compare(base, ["stream_program_kernel", "stream_batch_", "stream_pack_kernel", "stream_pack_rotary_kernel"])
+    res = sass_compare(["stream_program_kernel", "stream_batch_", "stream_pack_kernel", "stream_pack_rotary_kernel"])
     assert res, "no entry to compare"
     assert all(res.values()), [n for n, same in res.items() if not same]
 

@@ -6,164 +6,130 @@ The sequences go through b200awq_program_plan: program_create's folding for a 13
 every test discriminates on any machine.  The recorded pointers are fake (aligned integers): the folding only compares
 addresses.  Shapes are Llama-like (4096 columns: 31 sets per SM)."""
 import ctypes
-import os
-import re
-import shutil
-import subprocess
 
-import pytest
-
+from _fake_ops import add, buf, linear, plan, rmsnorm, silu
+from _toolchain import entries, header_constants, needs_nvcc
 from autoawq_b200 import _cabi
 from autoawq_b200._cabi import lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OK, EINVAL, EUNSUPPORTED = 0, 1, 2
 K, N, SMS = 4096, 4096, 132
-_next = [0x10000000]
-
-
-def _buf(nbytes=1 << 16):
-    p = _next[0]
-    _next[0] += (nbytes + 0xffff) & ~0xffff
-    return p
-
-
-def _lin(x, y=None, k=K, n=N):
-    return dict(kind=_cabi.OP_LINEAR_GEMM, M=1, K=k, N=n, group_size=128, ldx=k, x=x, qweight=_buf(), scales=_buf(),
-                qzeros=_buf(), y=y or _buf())
-
-
-def _add(a, b, y=None, k=N):
-    return dict(kind=_cabi.OP_ADD, M=1, K=k, x=a, weight=b, y=y or _buf())
-
-
-def _norm(x, y=None, k=N):
-    return dict(kind=_cabi.OP_RMSNORM, M=1, K=k, x=x, weight=_buf(), y=y or _buf(), eps=1e-5)
 
 
 def _create(ops):
-    arr = (_cabi.Op * len(ops))()
-    for c, o in zip(arr, ops):
-        for f, v in o.items():
-            setattr(c, f, v)
-    kops = ctypes.c_int()
-    return lib.b200awq_program_plan(arr, len(ops), 1, SMS, 0, ctypes.byref(kops))
+    return plan(ops, sms=SMS)[0]
 
 
-def test_op_add_matches_header(tmp_path):
-    src = tmp_path / "k.c"
-    src.write_text('#include <stdio.h>\n#include "b200awq.h"\nint main(void) { printf("%d", B200AWQ_OP_ADD); return 0; }\n')
-    exe = tmp_path / "k"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    assert int(subprocess.check_output([str(exe)])) == _cabi.OP_ADD == 5
+def test_op_add_matches_header():
+    assert header_constants("B200AWQ_OP_ADD") == (_cabi.OP_ADD,) == (5,)
 
 
 def test_add_argument_validation():
-    x = _buf()
-    lin = _lin(x)
-    r = _buf()
-    assert _create([lin, _add(lin["y"], 0)]) == EINVAL
-    assert _create([lin, _add(0, r)]) == EINVAL
-    assert _create([lin, dict(_add(lin["y"], r), y=0)]) == EINVAL
-    assert _create([lin, _add(lin["y"], r, k=0)]) == EINVAL
-    assert _create([lin, _add(lin["y"], r, k=N - 4)]) == EUNSUPPORTED        # K % 8
-    assert _create([lin, _add(lin["y"], r + 8)]) == EUNSUPPORTED             # not 16-byte aligned
+    x = buf()
+    lin = linear(x, K, N)
+    r = buf()
+    assert _create([lin, add(lin["y"], 0, N)]) == EINVAL
+    assert _create([lin, add(0, r, N)]) == EINVAL
+    assert _create([lin, dict(add(lin["y"], r, N), y=0)]) == EINVAL
+    assert _create([lin, add(lin["y"], r, 0)]) == EINVAL
+    assert _create([lin, add(lin["y"], r, N - 4)]) == EUNSUPPORTED        # K % 8
+    assert _create([lin, add(lin["y"], r + 8, N)]) == EUNSUPPORTED             # not 16-byte aligned
 
 
 def test_controls_fold():
-    x, r = _buf(), _buf()
-    lin = _lin(x)
-    assert _create([lin, _add(lin["y"], r)]) == OK                        # external residual
-    assert _create([lin, _add(r, lin["y"])]) == OK                        # either operand order
+    x, r = buf(), buf()
+    lin = linear(x, K, N)
+    assert _create([lin, add(lin["y"], r, N)]) == OK                        # external residual
+    assert _create([lin, add(r, lin["y"], N)]) == OK                        # either operand order
     # the segment shape: o + h_in -> h, norm(h) -> gate|up ... down + h (two kernel ops back)
-    o = _lin(x)
-    h = _add(o["y"], r)
-    nm = _norm(h["y"])
-    a = _lin(nm["y"], k=N)
-    b = _lin(a["y"], k=N)
-    assert _create([o, h, nm, a, b, _add(b["y"], h["y"])]) == OK
+    o = linear(x, K, N)
+    h = add(o["y"], r, N)
+    nm = rmsnorm(h["y"], N)
+    a = linear(nm["y"], N, N)
+    b = linear(a["y"], N, N)
+    assert _create([o, h, nm, a, b, add(b["y"], h["y"], N)]) == OK
     # an op reading the add's output resolves to the producer's row
-    o2 = _lin(x)
-    h2 = _add(o2["y"], r)
-    assert _create([o2, h2, _lin(h2["y"], k=N)]) == OK
+    o2 = linear(x, K, N)
+    h2 = add(o2["y"], r, N)
+    assert _create([o2, h2, linear(h2["y"], N, N)]) == OK
 
 
 def test_add_after_glue_op():
-    x, r = _buf(), _buf()
-    nm = _norm(x)
-    assert _create([nm, _add(nm["y"], r), _lin(nm["y"], k=N)]) == EUNSUPPORTED
+    x, r = buf(), buf()
+    nm = rmsnorm(x, N)
+    assert _create([nm, add(nm["y"], r, N), linear(nm["y"], N, N)]) == EUNSUPPORTED
 
 
 def test_add_after_add():
-    x, r, r2 = _buf(), _buf(), _buf()
-    lin = _lin(x)
-    a1 = _add(lin["y"], r)
-    assert _create([lin, a1, _add(a1["y"], r2)]) == EUNSUPPORTED
+    x, r, r2 = buf(), buf(), buf()
+    lin = linear(x, K, N)
+    a1 = add(lin["y"], r, N)
+    assert _create([lin, a1, add(a1["y"], r2, N)]) == EUNSUPPORTED
 
 
 def test_add_after_gate_up_read_by_silu():
-    x, r = _buf(), _buf()
-    gu = _lin(x, n=2 * N)
-    act = _buf()
-    ops = [gu, _add(gu["y"], r, k=2 * N), dict(kind=_cabi.OP_SILU_AND_MUL, M=1, K=N, x=gu["y"], y=act), _lin(act, k=N)]
+    x, r = buf(), buf()
+    gu = linear(x, K, 2 * N)
+    act = buf()
+    ops = [gu, add(gu["y"], r, 2 * N), silu(gu["y"], N, y=act), linear(act, N, N)]
     assert _create(ops) == EUNSUPPORTED
 
 
 def test_add_with_both_operands_external():
-    x = _buf()
-    lin = _lin(x)
-    assert _create([lin, _add(_buf(), _buf())]) == EUNSUPPORTED
-    assert _create([lin, _add(lin["y"], lin["y"])]) == EUNSUPPORTED        # y + y: no residual
+    x = buf()
+    lin = linear(x, K, N)
+    assert _create([lin, add(buf(), buf(), N)]) == EUNSUPPORTED
+    assert _create([lin, add(lin["y"], lin["y"], N)]) == EUNSUPPORTED        # y + y: no residual
 
 
 def test_in_place_add():
-    x, r = _buf(), _buf()
-    lin = _lin(x)
-    assert _create([lin, _add(lin["y"], r, y=lin["y"])]) == EUNSUPPORTED
-    lin = _lin(x)
-    assert _create([lin, _add(lin["y"], r, y=r)]) == EUNSUPPORTED
+    x, r = buf(), buf()
+    lin = linear(x, K, N)
+    assert _create([lin, add(lin["y"], r, N, y=lin["y"])]) == EUNSUPPORTED
+    lin = linear(x, K, N)
+    assert _create([lin, add(lin["y"], r, N, y=r)]) == EUNSUPPORTED
 
 
 def test_residual_window():
-    x = _buf()
-    chain = [_lin(x)]
+    x = buf()
+    chain = [linear(x, K, N)]
     for _ in range(5):
-        chain.append(_lin(chain[-1]["y"], k=N))
-    assert _create(chain[:5] + [_add(chain[4]["y"], chain[0]["y"])]) == OK               # four kernel ops back
-    assert _create(chain + [_add(chain[5]["y"], chain[0]["y"])]) == EUNSUPPORTED         # five: outside the window
+        chain.append(linear(chain[-1]["y"], N, N))
+    assert _create(chain[:5] + [add(chain[4]["y"], chain[0]["y"], N)]) == OK               # four kernel ops back
+    assert _create(chain + [add(chain[5]["y"], chain[0]["y"], N)]) == EUNSUPPORTED         # five: outside the window
 
 
 def test_residual_the_program_overwrites():
-    x, r = _buf(), _buf()
-    lin = _lin(x)
-    assert _create([lin, _add(lin["y"], r), _lin(_buf(), y=r, k=K)]) == EUNSUPPORTED     # a later linear writes it
-    lin = _lin(x)
-    assert _create([lin, _add(lin["y"], r), _norm(_buf(), y=r), _lin(r, k=N)]) == EUNSUPPORTED   # ... a later glue op
+    x, r = buf(), buf()
+    lin = linear(x, K, N)
+    assert _create([lin, add(lin["y"], r, N), linear(buf(), K, N, y=r)]) == EUNSUPPORTED     # a later linear writes it
+    lin = linear(x, K, N)
+    assert _create([lin, add(lin["y"], r, N), rmsnorm(buf(), N, y=r), linear(r, N, N)]) == EUNSUPPORTED   # ... a later glue op
 
 
 def test_reading_the_raw_output_under_an_add():
-    x, r = _buf(), _buf()
-    lin = _lin(x)
-    assert _create([lin, _add(lin["y"], r), _lin(lin["y"], k=N)]) == EUNSUPPORTED
+    x, r = buf(), buf()
+    lin = linear(x, K, N)
+    assert _create([lin, add(lin["y"], r, N), linear(lin["y"], N, N)]) == EUNSUPPORTED
 
 
 def test_residual_row_rewritten_without_a_staging_wait():
     """Residual of op 1 = op 0's row; op 4 republishes row 0.  With ops 2..4 reading only external buffers nothing makes
     a CTA wait for op 1's finish before it overwrites row 0 (tests/test_stream_residual_model.py)."""
-    x, r = _buf(), _buf()
-    l0 = _lin(x, n=N)
-    l1 = _lin(l0["y"], k=N)
-    tail = [_lin(_buf()) for _ in range(3)]
-    assert _create([l0, l1, _add(l1["y"], l0["y"])] + tail) == EUNSUPPORTED
+    x, r = buf(), buf()
+    l0 = linear(x, K, N)
+    l1 = linear(l0["y"], N, N)
+    tail = [linear(buf(), K, N) for _ in range(3)]
+    assert _create([l0, l1, add(l1["y"], l0["y"], N)] + tail) == EUNSUPPORTED
 
 
 def test_residual_row_rewritten_after_a_staging_wait_folds():
-    x = _buf()
-    l0 = _lin(x, n=N)
-    l1 = _lin(l0["y"], k=N)
-    s = _add(l1["y"], l0["y"])
-    l2 = _lin(s["y"], k=N)                  # stages from op 1: every CTA finished op 1 before anyone passes it
-    tail = [_lin(_buf()) for _ in range(2)]
+    x = buf()
+    l0 = linear(x, K, N)
+    l1 = linear(l0["y"], N, N)
+    s = add(l1["y"], l0["y"], N)
+    l2 = linear(s["y"], N, N)                  # stages from op 1: every CTA finished op 1 before anyone passes it
+    tail = [linear(buf(), K, N) for _ in range(2)]
     assert _create([l0, l1, s, l2] + tail) == OK
 
 
@@ -171,24 +137,24 @@ def test_residual_row_rewritten_after_a_wait_on_a_slice():
     """The wait that orders the CTAs must be on a whole row: op 2 stages only the first half of op 1's sum, so it waits
     for the CTAs owning those columns, and the others may run on to op 4, which republishes row 0 while a CTA owning the
     second half still reads op 0's row as its residual in op 1's finish."""
-    x = _buf()
-    l0 = _lin(x)
-    l1 = _lin(l0["y"], k=N)
-    s = _add(l1["y"], l0["y"])
-    l2 = _lin(s["y"], k=N // 2)
-    tail = [_lin(_buf(), n=2 * N) for _ in range(2)]
+    x = buf()
+    l0 = linear(x, K, N)
+    l1 = linear(l0["y"], N, N)
+    s = add(l1["y"], l0["y"], N)
+    l2 = linear(s["y"], N // 2, N)
+    tail = [linear(buf(), K, 2 * N) for _ in range(2)]
     assert _create([l0, l1, s, l2] + tail) == EUNSUPPORTED
-    l2 = _lin(s["y"], k=N)                  # the whole row: folds
+    l2 = linear(s["y"], N, N)                  # the whole row: folds
     assert _create([l0, l1, s, l2] + tail) == OK
 
 
 def test_residual_row_rewritten_after_a_wait_on_a_narrow_op():
-    x = _buf()
-    l0 = _lin(x, n=1024)                    # 64 sets: fewer than one per SM
-    l1 = _lin(l0["y"], k=1024, n=1024)
-    s = _add(l1["y"], l0["y"], k=1024)
-    l2 = _lin(s["y"], k=1024)
-    assert _create([l0, l1, s, l2] + [_lin(_buf()) for _ in range(2)]) == EUNSUPPORTED
+    x = buf()
+    l0 = linear(x, K, 1024)                    # 64 sets: fewer than one per SM
+    l1 = linear(l0["y"], 1024, 1024)
+    s = add(l1["y"], l0["y"], 1024)
+    l2 = linear(s["y"], 1024, N)
+    assert _create([l0, l1, s, l2] + [linear(buf(), K, N) for _ in range(2)]) == EUNSUPPORTED
 
 
 def test_plan_argument_validation():
@@ -202,38 +168,31 @@ def test_plan_argument_validation():
 def test_external_residual_aliasing_a_moe_buffer():
     """The fused MoE block writes its routing tensors too: none of them may be an external residual."""
     H, I, E, k = 1024, 512, 8, 2
-    x, h = _buf(), _buf()
+    x, h = buf(), buf()
     for field in ("logits", "topk_weights", "topk_ids", "token_expert_indices", "sorted_ids", "expert_ids",
                   "num_tokens_post_pad", "gate_up", "act", "down"):
         d = _cabi.Moe()
         d.E, d.top_k, d.renormalize, d.group_size, d.H, d.I, d.block_size = E, k, 1, 128, H, I, 16
         d.sorted_len = k + E * 15
         for f, _ in _cabi.Moe._fields_[8:]:
-            setattr(d, f, _buf())
-        res = _buf()
+            setattr(d, f, buf())
+        res = buf()
         setattr(d, field, res)
-        nm = _norm(x, k=H)
-        moe = dict(kind=_cabi.OP_SPARSE_MOE, M=1, K=H, N=H, x=nm["y"], y=_buf(), weight=ctypes.addressof(d))
-        pre = _lin(h, n=H)
-        ops = [pre, _add(pre["y"], res, k=H), nm, moe]
+        nm = rmsnorm(x, H)
+        moe = dict(kind=_cabi.OP_SPARSE_MOE, M=1, K=H, N=H, x=nm["y"], y=buf(), weight=ctypes.addressof(d))
+        pre = linear(h, K, H)
+        ops = [pre, add(pre["y"], res, H), nm, moe]
         assert _create(ops) == EUNSUPPORTED, field
-        ops = [pre, _add(pre["y"], _buf(), k=H), nm, moe]
+        ops = [pre, add(pre["y"], buf(), H), nm, moe]
         assert _create(ops) == OK, field
 
 
-@pytest.mark.skipif(shutil.which("nvcc") is None and not os.path.exists("/usr/local/cuda/bin/nvcc"), reason="needs nvcc")
-def test_residual_kernels_register_and_spill_budget(tmp_path):
+@needs_nvcc
+def test_residual_kernels_register_and_spill_budget():
     """One CTA per SM: the residual entries (M = 1: 288 threads; batched: 288 threads) fit the register file and spill
     nothing."""
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    src = os.path.join(ROOT, "autoawq_b200", "csrc", "program.cu")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xptxas",
-                          "-v", "-c", src, "-o", str(tmp_path / "program.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    log = out.stderr + out.stdout
-    entries = re.findall(r"Compiling entry function '(\S*residual_kernel\S*)'[^\n]*\n[^\n]*\n\s*(\d+) bytes stack frame, "
-                         r"(\d+) bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) registers", log)
-    assert len(entries) == 4, log[-1500:]          # stream_residual_kernel, stream_batch_residual_kernel<2|4|8>
-    for name, stack, st, ld, regs in entries:
-        assert int(regs) * (32 + 32 * 8) <= 65536, f"{name}: {regs} registers x 288 threads"
-        assert int(st) == 0 and int(ld) == 0 and int(stack) == 0, f"{name}: spills {st} / {ld}, stack {stack}"
+    found = entries("program.cu", r"residual_kernel")
+    assert len(found) == 4, found          # stream_residual_kernel, stream_batch_residual_kernel<2|4|8>
+    for name, (regs, stack, st, ld) in found.items():
+        assert regs * (32 + 32 * 8) <= 65536, f"{name}: {regs} registers x 288 threads"
+        assert st == 0 and ld == 0 and stack == 0, f"{name}: spills {st} / {ld}, stack {stack}"
