@@ -81,8 +81,8 @@ class QkNormRope(ctypes.Structure):
 
 
 class Mla(ctypes.Structure):
-    """b200awq_mla_t (include/b200awq.h): the descriptor of b200awq_mla_rope / b200awq_mla_kv and of an MLA_ROPE /
-    MLA_KV op's `weight`."""
+    """b200awq_mla_t (include/b200awq.h): the descriptor of b200awq_mla_rope / _kv / _k_rope / _q_rope and of an
+    MLA_ROPE / MLA_KV / MLA_K_ROPE / MLA_Q_ROPE op's `weight`."""
 
     _fields_ = [
         ("n_heads", ctypes.c_int32), ("nope_dim", ctypes.c_int32), ("rope_dim", ctypes.c_int32),
@@ -96,6 +96,7 @@ class Mla(ctypes.Structure):
 
 OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV = 1, 2, 3, 4, 5, 6
 OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE, OP_DEEPSEEK_MOE, OP_MLA_ROPE, OP_MLA_KV = 7, 8, 9, 10, 11
+OP_MLA_K_ROPE, OP_MLA_Q_ROPE = 12, 13
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -126,6 +127,8 @@ SIGNATURES = {
     "b200awq_qk_norm_rope_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(QkNormRope), _c_int, _c_void_p]),
     "b200awq_mla_rope": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
     "b200awq_mla_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
+    "b200awq_mla_k_rope": (_c_int, [_c_void_p, _c_i64, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
+    "b200awq_mla_q_rope": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
     "b200awq_set_knob": (_c_int, [_c_int, _c_int]),
     "b200awq_get_knob": (_c_int, [_c_int]),
     "b200awq_debug_read": (_c_int, [_c_void_p, _c_size_t]),

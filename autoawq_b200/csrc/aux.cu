@@ -3,7 +3,7 @@
 //   silu_and_mul  <- awq_ext.silu_and_mul             (awq/modules/fused/moe.py:76)
 //   rope_kv       <- RoPE.forward + WindowedCache.update_kv (awq/modules/fused/attn.py:53-86,243-267)
 //   mla_rope / mla_kv <- the glue of transformers' DeepseekV2Attention / DeepseekV3Attention between the projections
-//                    and attention (rotary, head split, cache write)
+//                    and attention (rotary, head split, cache write); mla_k_rope / mla_q_rope: the same with a q LoRA
 // fp16 in/out, fp32 math.  Bandwidth-trivial (KBs per decode step); kept simple.
 #include "common.cuh"
 #include "kernels.h"
@@ -173,16 +173,48 @@ __global__ void __launch_bounds__(256)
   mla_kv_col(d, pos, m, c, row[m * ld + c]);
 }
 
-// rope: the fields MLA_ROPE reads (q_out, freqs, style, C), else MLA_KV's (v_cache and its geometry); both read pos and
-// k_cache with its geometry
-int mla_validate(const b200awq_mla_t* d, bool rope) {
-  if (d == nullptr || d->pos == nullptr || d->k_cache == nullptr) return B200AWQ_EINVAL;
+// one thread per (token row, k_pe pair); kpe points at k_pe of token row 0
+__global__ void __launch_bounds__(256)
+    mla_k_rope_kernel(const __half* __restrict__ kpe, int64_t ld, b200awq_mla_t d, int M) {
+  pdl_trigger();
+  pdl_wait();
+  const int pos = mla_pos(d, true);
+  const int pairs = d.rope_dim >> 1;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pos < 0 || i >= (int64_t)M * pairs) return;
+  const int m = static_cast<int>(i / pairs), c = 2 * static_cast<int>(i - (int64_t)m * pairs);
+  const __half* r = kpe + m * ld;
+  mla_k_pair(d, pos, m, c, r[c], r[c + 1]);
+}
+
+// one thread per (token row, column pair) of the q_b_proj row
+__global__ void __launch_bounds__(256)
+    mla_q_rope_kernel(const __half* __restrict__ row, int64_t ld, b200awq_mla_t d, int M) {
+  pdl_trigger();
+  pdl_wait();
+  const int pos = mla_pos(d, true);
+  const int pairs = (d.n_heads * (d.nope_dim + d.rope_dim)) >> 1;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pos < 0 || i >= (int64_t)M * pairs) return;
+  const int m = static_cast<int>(i / pairs), c = 2 * static_cast<int>(i - (int64_t)m * pairs);
+  const __half* r = row + m * ld;
+  mla_q_pair(d, pos, m, c, r[c], r[c + 1]);
+}
+
+// kind: the op (B200AWQ_OP_MLA_*).  Every op reads pos and the head geometry and bounds the position by cache_len; the
+// rotations (MLA_ROPE, MLA_K_ROPE, MLA_Q_ROPE) read freqs and style; MLA_ROPE and MLA_Q_ROPE write q_out; MLA_ROPE,
+// MLA_K_ROPE and MLA_KV write k_cache (with its geometry); MLA_ROPE and MLA_K_ROPE read C (the row's width), MLA_KV
+// v_cache and its geometry
+int mla_validate(const b200awq_mla_t* d, int kind) {
+  const bool rot = kind != B200AWQ_OP_MLA_KV, q = kind == B200AWQ_OP_MLA_ROPE || kind == B200AWQ_OP_MLA_Q_ROPE;
+  const bool k = kind != B200AWQ_OP_MLA_Q_ROPE;
+  if (d == nullptr || d->pos == nullptr || (k && d->k_cache == nullptr)) return B200AWQ_EINVAL;
   if (d->n_heads <= 0 || d->nope_dim <= 0 || d->rope_dim <= 0 || (d->rope_dim % 2) != 0 || d->cache_len <= 0 ||
-      d->k_batch_stride < (int64_t)d->cache_len * d->n_heads * (d->nope_dim + d->rope_dim))
+      (k && d->k_batch_stride < (int64_t)d->cache_len * d->n_heads * (d->nope_dim + d->rope_dim)))
     return B200AWQ_EINVAL;
-  if (rope)
-    return d->q_out == nullptr || d->freqs == nullptr || d->kv_lora_rank <= 0 || (d->style != 0 && d->style != 1) ||
-                   d->freqs_len <= 0
+  if (rot)
+    return (q && d->q_out == nullptr) || d->freqs == nullptr || (k && d->kv_lora_rank <= 0) ||
+                   (d->style != 0 && d->style != 1) || d->freqs_len <= 0
                ? B200AWQ_EINVAL
                : B200AWQ_OK;
   return d->v_cache == nullptr || d->v_dim <= 0 || d->v_head_stride < d->v_dim ||
@@ -200,6 +232,18 @@ cudaError_t mla_rope(const void* row, int64_t ld, const b200awq_mla_t& d, int M,
 cudaError_t mla_kv(const void* row, int64_t ld, const b200awq_mla_t& d, int M, cudaStream_t st) {
   const int64_t n = (int64_t)M * d.n_heads * (d.nope_dim + d.v_dim);
   return launch_kernel(mla_kv_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
+                       reinterpret_cast<const __half*>(row), ld, d, M);
+}
+
+cudaError_t mla_k_rope(const void* row, int64_t ld, int64_t k_pe_col, const b200awq_mla_t& d, int M, cudaStream_t st) {
+  const int64_t n = (int64_t)M * (d.rope_dim / 2);
+  return launch_kernel(mla_k_rope_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
+                       reinterpret_cast<const __half*>(row) + k_pe_col, ld, d, M);
+}
+
+cudaError_t mla_q_rope(const void* row, int64_t ld, const b200awq_mla_t& d, int M, cudaStream_t st) {
+  const int64_t n = (int64_t)M * ((d.n_heads * (d.nope_dim + d.rope_dim)) / 2);
+  return launch_kernel(mla_q_rope_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
                        reinterpret_cast<const __half*>(row), ld, d, M);
 }
 

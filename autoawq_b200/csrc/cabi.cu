@@ -226,9 +226,9 @@ int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_nor
 }
 
 // the MLA ops' common checks; M <= 8 (a decode step's token rows); the row must hold N = n columns at pitch ld
-static int mla_check(const void* row, int64_t ld, const b200awq_mla_t* desc, bool rope, int M, int64_t n) {
+static int mla_check(const void* row, int64_t ld, const b200awq_mla_t* desc, int kind, int M, int64_t n) {
   if (row == nullptr || M < 0) return B200AWQ_EINVAL;
-  const int v = mla_validate(desc, rope);
+  const int v = mla_validate(desc, kind);
   if (v != B200AWQ_OK) return v;
   if (M > 1 && ld < n) return B200AWQ_EINVAL;
   return M > 8 ? B200AWQ_EUNSUPPORTED : B200AWQ_OK;
@@ -236,7 +236,7 @@ static int mla_check(const void* row, int64_t ld, const b200awq_mla_t* desc, boo
 
 int b200awq_mla_rope(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_mla_rope");
-  const int v = mla_check(row, ld, desc, true, M, desc == nullptr ? 0 :
+  const int v = mla_check(row, ld, desc, B200AWQ_OP_MLA_ROPE, M, desc == nullptr ? 0 :
                           (int64_t)desc->n_heads * (desc->nope_dim + desc->rope_dim) + desc->kv_lora_rank + desc->rope_dim);
   if (v != B200AWQ_OK || M == 0) return v;
   return fold(mla_rope(row, ld, *desc, M, static_cast<cudaStream_t>(stream)));
@@ -244,9 +244,26 @@ int b200awq_mla_rope(const void* row, int64_t ld, const b200awq_mla_t* desc, int
 
 int b200awq_mla_kv(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_mla_kv");
-  const int v = mla_check(row, ld, desc, false, M, desc == nullptr ? 0 : (int64_t)desc->n_heads * (desc->nope_dim + desc->v_dim));
+  const int v = mla_check(row, ld, desc, B200AWQ_OP_MLA_KV, M, desc == nullptr ? 0 : (int64_t)desc->n_heads * (desc->nope_dim + desc->v_dim));
   if (v != B200AWQ_OK || M == 0) return v;
   return fold(mla_kv(row, ld, *desc, M, static_cast<cudaStream_t>(stream)));
+}
+
+int b200awq_mla_k_rope(const void* row, int64_t ld, int64_t k_pe_col, const b200awq_mla_t* desc, int M,
+                       b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_mla_k_rope");
+  if (k_pe_col < 0) return B200AWQ_EINVAL;
+  const int v = mla_check(row, ld, desc, B200AWQ_OP_MLA_K_ROPE, M, desc == nullptr ? 0 : k_pe_col + desc->rope_dim);
+  if (v != B200AWQ_OK || M == 0) return v;
+  return fold(mla_k_rope(row, ld, k_pe_col, *desc, M, static_cast<cudaStream_t>(stream)));
+}
+
+int b200awq_mla_q_rope(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_mla_q_rope");
+  const int v = mla_check(row, ld, desc, B200AWQ_OP_MLA_Q_ROPE, M,
+                          desc == nullptr ? 0 : (int64_t)desc->n_heads * (desc->nope_dim + desc->rope_dim));
+  if (v != B200AWQ_OK || M == 0) return v;
+  return fold(mla_q_rope(row, ld, *desc, M, static_cast<cudaStream_t>(stream)));
 }
 
 

@@ -163,9 +163,12 @@ cudaError_t qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200a
                             cudaStream_t st);
 cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
                                int G, int head_dim, cudaStream_t st);
-// B200AWQ_OK, or the code b200awq_mla_rope / b200awq_mla_kv return for a bad descriptor (host only)
-int mla_validate(const struct ::b200awq_mla* d, bool rope);
+// B200AWQ_OK, or the code the stand-alone op of kind (B200AWQ_OP_MLA_*) returns for a bad descriptor (host only)
+int mla_validate(const struct ::b200awq_mla* d, int kind);
 cudaError_t mla_rope(const void* row, int64_t ld, const struct ::b200awq_mla& d, int M, cudaStream_t st);
 cudaError_t mla_kv(const void* row, int64_t ld, const struct ::b200awq_mla& d, int M, cudaStream_t st);
+cudaError_t mla_k_rope(const void* row, int64_t ld, int64_t k_pe_col, const struct ::b200awq_mla& d, int M,
+                       cudaStream_t st);
+cudaError_t mla_q_rope(const void* row, int64_t ld, const struct ::b200awq_mla& d, int M, cudaStream_t st);
 
 }  // namespace b200awq

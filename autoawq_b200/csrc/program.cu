@@ -147,7 +147,7 @@ struct ProgOp {
   int res_op = -1;
   // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights
   b200awq_qk_norm_rope_t qkr = {};
-  // an MLA_ROPE (mla_kind 1) or MLA_KV (2) folded into the finish
+  // an MLA_ROPE (mla_kind 1), MLA_KV (2), MLA_K_ROPE (3) or MLA_Q_ROPE (4) folded into the finish
   b200awq_mla_t mla = {};
   int mla_kind = 0;
 };
@@ -189,11 +189,12 @@ struct FoldedProgram {
 // The kernel entry that runs a program (chosen by stream_build).  M = 1: the plain kernel (8 or 12 consumer warps,
 // knob 9) or the 8-warp kernel of the program's features; M > 1: the batched kernels at MT = sb_mt(M).  Side tables:
 // the M = 1 kernels from kKernMoe on take SpMoe (null without MoE blocks), from kKernResidual on SpRes, from kKernRope on
-// SpRope, from kKernQkNorm on SpQkNorm, kKernDeepseekMoe and kKernMla SpDsk, and kKernMla SpMla; the batched ones take
-// SpRes from kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2 on.  The Qwen3-MoE,
-// DeepSeek-MoE and MLA kernels take every table, with empty entries where an op has no add, rotation or norm.
+// SpRope, from kKernQkNorm on SpQkNorm, kKernDeepseekMoe, kKernMla and kKernMlaLora SpDsk, and the last two SpMla; the
+// batched ones take SpRes from kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2
+// on.  The Qwen3-MoE, DeepSeek-MoE and MLA kernels take every table, with empty entries where an op has no add,
+// rotation or norm.
 enum ProgKernel {
-  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe, kKernMla,
+  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe, kKernMla, kKernMlaLora,
   kKernBatch2, kKernBatch4, kKernBatch8, kKernBatchResidual2, kKernBatchResidual4, kKernBatchResidual8,
   kKernBatchRope2, kKernBatchRope4, kKernBatchRope8, kKernBatchQkNorm2, kKernBatchQkNorm4, kKernBatchQkNorm8
 };
@@ -365,6 +366,7 @@ static cudaError_t upload(T** d, const std::vector<T>& h) {
 // QK_NORM_ROPE_KV ops: as ROPE_KV, and `qkr` carries the norm weights (q_norm_weight != null: SpQkNorm).
 // MLA_ROPE ops (`mla_kind` 1): packed in mode 3, the finish rotates / stores (SpMla); MLA_KV (2): mode 0, the finish
 // stores the cache columns.  Such a program runs stream_mla_kernel, whose MoE blocks are DEEPSEEK_MOE blocks.
+// MLA_K_ROPE / MLA_Q_ROPE (3 / 4): packed in mode 3, on stream_mla_lora_kernel (the same, plus their finishes).
 static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaError_t* err) {
   *err = cudaSuccess;
   const std::vector<ProgOp>& table = f.table;
@@ -423,7 +425,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   };
   for (int i = 0; i < n; ++i)
     if (table[i].moe == 1) mode[i] = 1;
-  bool has_rope = false, has_qkn = false, has_res = false, has_mla = false;
+  bool has_rope = false, has_qkn = false, has_res = false, has_mla = false, has_lora = false;
   for (int i = 0; i < n; ++i) {
     if (table[i].qkr.rope.head_dim != 0) {
       if (mode[i] != 0) return false;   // (program_create rejects a gate|up producer already)
@@ -433,8 +435,9 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     has_qkn = has_qkn || table[i].qkr.q_norm_weight != nullptr;
     if (table[i].mla_kind != 0) {
       if (mode[i] != 0) return false;
-      if (table[i].mla_kind == 1) mode[i] = 3;
+      if (table[i].mla_kind != 2) mode[i] = 3;
       has_mla = true;
+      has_lora = has_lora || table[i].mla_kind >= 3;
     }
   }
   if (has_mla && M != 1) return false;   // (program_create rejects it already)
@@ -450,6 +453,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   const ProgKernel kern =
       M > 1 ? ProgKernel((has_qkn ? kKernBatchQkNorm2 : has_rope ? kKernBatchRope2 : has_res ? kKernBatchResidual2
                                                                                              : kKernBatch2) + mt)
+      : has_lora                         ? kKernMlaLora
       : has_mla                          ? kKernMla
       : mkind == B200AWQ_OP_DEEPSEEK_MOE ? kKernDeepseekMoe
       : mkind == B200AWQ_OP_QWEN3_MOE    ? kKernQwen3Moe
@@ -649,12 +653,13 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
         (table[i].moe == 1 ? dd[table[i].mi].shb_a : dd[table[i].mi].shb_b) = (long long)shared_bytes(i);
       }
     if (e == cudaSuccess) e = upload(&pr->d_moe, md);
-    if (e == cudaSuccess && (kern == kKernDeepseekMoe || kern == kKernMla)) e = upload(&pr->d_dsk, dd);
+    if (e == cudaSuccess && (kern == kKernDeepseekMoe || kern == kKernMla || kern == kKernMlaLora))
+      e = upload(&pr->d_dsk, dd);
   }
   // the side tables the kernel takes (ProgKernel)
-  const bool takes_res = (kern >= kKernResidual && kern <= kKernMla) || kern >= kKernBatchResidual2;
-  const bool takes_rope = (kern >= kKernRope && kern <= kKernMla) || kern >= kKernBatchRope2;
-  const bool takes_qkn = (kern >= kKernQkNorm && kern <= kKernMla) || kern >= kKernBatchQkNorm2;
+  const bool takes_res = (kern >= kKernResidual && kern <= kKernMlaLora) || kern >= kKernBatchResidual2;
+  const bool takes_rope = (kern >= kKernRope && kern <= kKernMlaLora) || kern >= kKernBatchRope2;
+  const bool takes_qkn = (kern >= kKernQkNorm && kern <= kKernMlaLora) || kern >= kKernBatchQkNorm2;
   if (e == cudaSuccess && takes_res) {
     std::vector<SpRes> rd(n);
     for (int i = 0; i < n; ++i) {
@@ -686,13 +691,16 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     }
     if (e == cudaSuccess) e = upload(&pr->d_qkn, qd);
   }
-  if (e == cudaSuccess && kern == kKernMla) {
+  if (e == cudaSuccess && (kern == kKernMla || kern == kKernMlaLora)) {
     std::vector<SpMla> ml(n);
     for (int i = 0; i < n; ++i) {
       ml[i].d = table[i].mla;
       ml[i].kind = table[i].mla_kind;
       const int s = table[i].stage_row;
       if (s >= 0 && table[s].mla_kind == 1 && ops[i].src_op == s) ml[i].wait_words = table[s].N;
+      // stream_mla_lora_kernel polls the previous op's row (program_create: a slice of a K_ROPE row)
+      if (kern == kKernMlaLora && s == i - 1 && ops[i].src_op >= 0 && table[ops[i].src_op].mla_kind == 3)
+        ml[i].wait_words = table[s].N;
     }
     e = upload(&pr->d_mla, ml);
   }
@@ -701,7 +709,8 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   static const void* const entry[] = {
       (const void*)stream_program_kernel<8, 4>, (const void*)stream_moe_kernel, (const void*)stream_residual_kernel,
       (const void*)stream_rope_kernel, (const void*)stream_qknorm_kernel, (const void*)stream_qwen3moe_kernel,
-      (const void*)stream_deepseek_moe_kernel, (const void*)stream_mla_kernel, (const void*)stream_batch_kernel<2>, (const void*)stream_batch_kernel<4>,
+      (const void*)stream_deepseek_moe_kernel, (const void*)stream_mla_kernel, (const void*)stream_mla_lora_kernel,
+      (const void*)stream_batch_kernel<2>, (const void*)stream_batch_kernel<4>,
       (const void*)stream_batch_kernel<8>, (const void*)stream_batch_residual_kernel<2>,
       (const void*)stream_batch_residual_kernel<4>, (const void*)stream_batch_residual_kernel<8>,
       (const void*)stream_batch_rope_kernel<2>, (const void*)stream_batch_rope_kernel<4>,
@@ -894,26 +903,36 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       else pv.qkr.rope = *r;
       continue;
     }
-    if (op.kind == B200AWQ_OP_MLA_ROPE || op.kind == B200AWQ_OP_MLA_KV) {
+    if (op.kind == B200AWQ_OP_MLA_ROPE || op.kind == B200AWQ_OP_MLA_KV || op.kind == B200AWQ_OP_MLA_K_ROPE ||
+        op.kind == B200AWQ_OP_MLA_Q_ROPE) {
       // MLA's rotation / cache stores, folded into the finish of the linear recorded just before it (whose whole output
-      // is the op's row): q_proj | kv_a_proj_with_mqa for MLA_ROPE, kv_b_proj for MLA_KV
-      const bool mrope = op.kind == B200AWQ_OP_MLA_ROPE;
+      // is the op's row): q_proj | kv_a_proj_with_mqa for MLA_ROPE, kv_b_proj for MLA_KV; with a q LoRA,
+      // q_a_proj | kv_a_proj_with_mqa for MLA_K_ROPE and q_b_proj for MLA_Q_ROPE
+      const bool mrope = op.kind == B200AWQ_OP_MLA_ROPE, krope = op.kind == B200AWQ_OP_MLA_K_ROPE;
+      const bool qrope = op.kind == B200AWQ_OP_MLA_Q_ROPE;
       const b200awq_mla_t* d = static_cast<const b200awq_mla_t*>(op.weight);
       if (op.x == nullptr) return B200AWQ_EINVAL;
-      const int v = mla_validate(d, mrope);
+      const int v = mla_validate(d, op.kind);
       if (v != B200AWQ_OK) return v;
       if (M != 1) return B200AWQ_EUNSUPPORTED;
-      if ((d->nope_dim % 16) != 0 || (d->rope_dim % 16) != 0 || (mrope ? d->kv_lora_rank : d->v_dim) % 16 != 0)
+      if ((d->nope_dim % 16) != 0 || (d->rope_dim % 16) != 0 ||
+          (mrope || krope ? d->kv_lora_rank : qrope ? 0 : d->v_dim) % 16 != 0)
         return B200AWQ_EUNSUPPORTED;
-      const int64_t want = mrope ? (int64_t)d->n_heads * (d->nope_dim + d->rope_dim) + d->kv_lora_rank + d->rope_dim
-                                 : (int64_t)d->n_heads * (d->nope_dim + d->v_dim);
-      if (op.N != want) return B200AWQ_EUNSUPPORTED;
+      const int64_t qn = (int64_t)d->n_heads * (d->nope_dim + d->rope_dim);
+      if (krope) {   // [q_a (Cq) | c_kv | k_pe]: Cq = N - C - Dr
+        const int64_t cq = (int64_t)op.N - d->kv_lora_rank - d->rope_dim;
+        if (cq <= 0 || (cq % 16) != 0) return B200AWQ_EUNSUPPORTED;
+      } else {
+        const int64_t want = mrope ? qn + d->kv_lora_rank + d->rope_dim
+                                   : qrope ? qn : (int64_t)d->n_heads * (d->nope_dim + d->v_dim);
+        if (op.N != want) return B200AWQ_EUNSUPPORTED;
+      }
       if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty() || table.back().moe != 0)
         return B200AWQ_EUNSUPPORTED;
       ProgOp& pv = table.back();
       if (op.x != pv.y || op.N != pv.N) return B200AWQ_EUNSUPPORTED;
       pv.mla = *d;
-      pv.mla_kind = mrope ? 1 : 2;
+      pv.mla_kind = mrope ? 1 : krope ? 3 : qrope ? 4 : 2;
       continue;
     }
     if (op.kind == B200AWQ_OP_ADD) {
@@ -1038,6 +1057,11 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     p.stage_row = s >= 0 && p.src == table[s].y && width == (size_t)table[s].N ? s : -1;
     // a slice of an MLA_ROPE producer's row: stream_mla_kernel stages it after the whole row (SpMla::wait_words)
     if (s >= 0 && table[s].mla_kind == 1 && p.prologue != kProSilu) p.stage_row = s;
+    // a slice of an MLA_K_ROPE producer's row (q_b's q_a slice, or kv_b's c_kv slice two ops back):
+    // stream_mla_lora_kernel first polls one word of every set of the previous op's row (SpMla::wait_words), which
+    // shows what staging that whole row shows
+    if (s >= 0 && table[s].mla_kind == 3 && p.prologue != kProSilu && p.stage_row < 0 && table.back().moe == 0)
+      p.stage_row = static_cast<int>(table.size()) - 1;
     table.push_back(p);
   }
   for (const Glue& gl : glues)
@@ -1111,23 +1135,31 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
           return B200AWQ_EUNSUPPORTED;
     }
   }
-  // MLA_ROPE / MLA_KV: the same rule as ROPE_KV for q_out, the caches, pos and (MLA_ROPE) freqs, against every op,
-  // glue record, MoE block and ROPE_KV op.  The MLA_ROPE and MLA_KV ops of one layer may share k_cache: with the same
-  // geometry they write disjoint columns of its rows (k_pe, k_nope).
+  // MLA ops: the same rule as ROPE_KV for q_out, the caches, pos and (the rotations) freqs, against every op, glue
+  // record, MoE block and ROPE_KV op.  A k rotation (MLA_ROPE, MLA_K_ROPE) and an MLA_KV may share k_cache: with the same
+  // geometry they write disjoint columns of its rows (k_pe, k_nope); two k rotations may not.  q LoRA ops (MLA_K_ROPE,
+  // MLA_Q_ROPE) and MLA_ROPE ops do not mix in one program (their kernels poll different rows, SpMla::wait_words).
+  bool has_mla_rope = false, has_mla_lora = false;
+  for (const ProgOp& p : table) {
+    has_mla_rope = has_mla_rope || p.mla_kind == 1;
+    has_mla_lora = has_mla_lora || p.mla_kind >= 3;
+  }
+  if (has_mla_rope && has_mla_lora) return B200AWQ_EUNSUPPORTED;
   auto mla_outs = [&](const ProgOp& p) {
     const b200awq_mla_t& d = p.mla;
-    const bool r = p.mla_kind == 1;
+    const bool q = p.mla_kind == 1 || p.mla_kind == 4, k = p.mla_kind != 4, v = p.mla_kind == 2;
     const size_t kb = ((size_t)(M - 1) * d.k_batch_stride + (size_t)d.cache_len * d.n_heads * (d.nope_dim + d.rope_dim)) * 2;
     const size_t vb = ((size_t)(M - 1) * d.v_batch_stride + (size_t)d.cache_len * d.n_heads * d.v_head_stride) * 2;
     return std::array<std::pair<const void*, size_t>, 3>{
-        {{r ? d.q_out : nullptr, r ? (size_t)M * d.n_heads * (d.nope_dim + d.rope_dim) * 2 : 0},
-         {d.k_cache, kb},
-         {r ? nullptr : d.v_cache, r ? 0 : vb}}};
+        {{q ? d.q_out : nullptr, q ? (size_t)M * d.n_heads * (d.nope_dim + d.rope_dim) * 2 : 0},
+         {k ? d.k_cache : nullptr, k ? kb : 0},
+         {v ? d.v_cache : nullptr, v ? vb : 0}}};
   };
   auto shares_k = [&](const ProgOp& a, const ProgOp& b) {
     const b200awq_mla_t &x = a.mla, &y = b.mla;
-    return a.mla_kind != b.mla_kind && x.k_cache == y.k_cache && x.n_heads == y.n_heads && x.nope_dim == y.nope_dim &&
-           x.rope_dim == y.rope_dim && x.cache_len == y.cache_len && x.k_batch_stride == y.k_batch_stride;
+    return (a.mla_kind == 2) != (b.mla_kind == 2) && x.k_cache == y.k_cache && x.n_heads == y.n_heads &&
+           x.nope_dim == y.nope_dim && x.rope_dim == y.rope_dim && x.cache_len == y.cache_len &&
+           x.k_batch_stride == y.k_batch_stride;
   };
   for (int ri = 0; ri < nt; ++ri) {
     const ProgOp& mp = table[ri];
@@ -1135,7 +1167,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     const b200awq_mla_t& d = mp.mla;
     const auto outs = mla_outs(mp);
     const std::pair<const void*, size_t> ins[2] = {
-        {d.pos, 4}, {mp.mla_kind == 1 ? d.freqs : nullptr, mp.mla_kind == 1 ? (size_t)d.freqs_len * d.rope_dim * 4 : 0}};
+        {d.pos, 4}, {mp.mla_kind != 2 ? d.freqs : nullptr, mp.mla_kind != 2 ? (size_t)d.freqs_len * d.rope_dim * 4 : 0}};
     auto hits_out = [&](const void* p, size_t b) {
       for (const auto& o : outs)
         if (overlaps(o.first, o.second, p, b)) return true;
@@ -1281,6 +1313,7 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     case kKernQwen3Moe: return stream(stream_qwen3moe_kernel, p->d_res, p->d_rope, p->d_qkn);
     case kKernDeepseekMoe: return stream(stream_deepseek_moe_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk);
     case kKernMla: return stream(stream_mla_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk, p->d_mla);
+    case kKernMlaLora: return stream(stream_mla_lora_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk, p->d_mla);
     case kKernBatch2: return batch(stream_batch_kernel<2>);
     case kKernBatch4: return batch(stream_batch_kernel<4>);
     case kKernBatch8: return batch(stream_batch_kernel<8>);

@@ -269,6 +269,9 @@ __device__ __forceinline__ void sp_cols_pairs(int s, int g, int& lo, int& hi) {
 // first waits for one word of every 16-column set of that row (wait_words columns): each is published by the set's owner
 // after it finished every earlier op, as a whole-row staging shows, so program_create's residual rule may count this
 // staging as one (ProgOp::stage_row).
+// stream_mla_lora_kernel adds kind 3 (MLA_K_ROPE: mode 3, k_pe of the row rotated into k_cache) and kind 4 (MLA_Q_ROPE:
+// mode 3, the row rotated into q_out); there wait_words polls the previous op's row (wait_words = its N), which covers
+// kv_b_proj staging the c_kv slice of the K_ROPE row two ops back.
 struct SpMla {
   b200awq_mla_t d;
   int kind;
@@ -672,6 +675,36 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 #define SP_DEEPSEEK 1
 #define SP_MLA 1
 #include "program_stream_body.inc"
+#undef SP_MLA
+#undef SP_DEEPSEEK
+#undef SP_QWEN3
+#undef SP_QKNORM
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with MLA_K_ROPE / MLA_Q_ROPE ops (MLA with a q LoRA; SpMla kinds 3 / 4), with or without DEEPSEEK_MOE
+// blocks: stream_mla_kernel plus SP_MLA_LORA.  The mode-3 finish runs rope.cuh's mla_lora_pair (k_pe of the fused
+// q_a | kv_a row into every head's k row, or q_b's row into q_out), and an op that stages a slice of a K_ROPE op's row
+// first polls one word of every set of the PREVIOUS op's row (SpMla::wait_words; kv_b's source is two ops back).
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_mla_lora_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                           uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                           int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                           const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn,
+                           const SpDsk* __restrict__ dsk, const SpMla* __restrict__ mla) {
+  constexpr int NW = 8, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_QKNORM 1
+#define SP_QWEN3 1
+#define SP_DEEPSEEK 1
+#define SP_MLA 1
+#define SP_MLA_LORA 1
+#include "program_stream_body.inc"
+#undef SP_MLA_LORA
 #undef SP_MLA
 #undef SP_DEEPSEEK
 #undef SP_QWEN3

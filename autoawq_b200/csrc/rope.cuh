@@ -87,8 +87,9 @@ __device__ __forceinline__ void qk_norm_rope_pair(const b200awq_qk_norm_rope_t& 
   rope_pair(q.rope, pos, m, col, wa, wb);
 }
 
-// ---- MLA (B200AWQ_OP_MLA_ROPE / _MLA_KV, include/b200awq.h): the per-pair / per-column steps shared by the stand-alone
-// kernels (aux.cu) and the finish of the decode-program kernel that folds them (program_stream_body.inc under SP_MLA).
+// ---- MLA (B200AWQ_OP_MLA_ROPE / _MLA_KV / _MLA_K_ROPE / _MLA_Q_ROPE, include/b200awq.h): the per-pair / per-column
+// steps shared by the stand-alone kernels (aux.cu) and the finish of the decode-program kernels that fold them
+// (program_stream_body.inc under SP_MLA / SP_MLA_LORA).
 // Reference: transformers 5.5 DeepseekV2Attention.forward (apply_rotary_emb) and DeepseekV3Attention.forward
 // (apply_rotary_pos_emb_interleave).
 
@@ -128,31 +129,57 @@ __device__ __forceinline__ MlaRot mla_rotate(const b200awq_mla_t& d, int pos, in
   return r;
 }
 
-// MLA_ROPE on columns (col, col + 1) of token row m's q_proj | kv_a_proj_with_mqa row (col even; a, b their values):
-// q_nope copied and q_pe rotated into q_out, c_kv nothing, k_pe rotated into the k rows of all H heads at position pos
-__device__ __forceinline__ void mla_rope_pair(const b200awq_mla_t& d, int pos, int m, int col, __half a, __half b) {
-  const int W = d.nope_dim + d.rope_dim, H = d.n_heads, qn = H * W;
-  if (col < qn) {
-    const int h = col / W, i = col - h * W;
-    __half* q = static_cast<__half*>(d.q_out) + ((size_t)m * H + h) * W;
-    if (i < d.nope_dim) {
-      q[i] = a;
-      q[i + 1] = b;
-    } else {
-      const MlaRot r = mla_rotate(d, pos, (i - d.nope_dim) >> 1, a, b);
-      q[d.nope_dim + r.j0] = r.o0;
-      q[d.nope_dim + r.j1] = r.o1;
-    }
-    return;
+// Columns (col, col + 1) of token row m's q row [H (Dn + Dr), per head [nope | pe]] (col even, col < H (Dn + Dr); a, b
+// their values): q_nope copied, q_pe rotated into q_out.  MLA_ROPE's q part and all of MLA_Q_ROPE.
+__device__ __forceinline__ void mla_q_pair(const b200awq_mla_t& d, int pos, int m, int col, __half a, __half b) {
+  const int W = d.nope_dim + d.rope_dim, H = d.n_heads;
+  const int h = col / W, i = col - h * W;
+  __half* q = static_cast<__half*>(d.q_out) + ((size_t)m * H + h) * W;
+  if (i < d.nope_dim) {
+    q[i] = a;
+    q[i + 1] = b;
+  } else {
+    const MlaRot r = mla_rotate(d, pos, (i - d.nope_dim) >> 1, a, b);
+    q[d.nope_dim + r.j0] = r.o0;
+    q[d.nope_dim + r.j1] = r.o1;
   }
-  const int kp = col - qn - d.kv_lora_rank;
-  if (kp < 0) return;
+}
+
+// Elements (kp, kp + 1) of token row m's k_pe (kp even; a, b their values): rotated into the k rows of all H heads at
+// position pos.  MLA_ROPE's k part and all of MLA_K_ROPE.
+__device__ __forceinline__ void mla_k_pair(const b200awq_mla_t& d, int pos, int m, int kp, __half a, __half b) {
+  const int W = d.nope_dim + d.rope_dim, H = d.n_heads, qn = H * W;
   const MlaRot r = mla_rotate(d, pos, kp >> 1, a, b);
   __half* k = static_cast<__half*>(d.k_cache) + (size_t)m * d.k_batch_stride + (size_t)pos * qn + d.nope_dim;
   for (int h = 0; h < H; ++h) {
     k[(size_t)h * W + r.j0] = r.o0;
     k[(size_t)h * W + r.j1] = r.o1;
   }
+}
+
+// MLA_ROPE on columns (col, col + 1) of token row m's q_proj | kv_a_proj_with_mqa row (col even; a, b their values):
+// q_nope copied and q_pe rotated into q_out, c_kv nothing, k_pe rotated into the k rows of all H heads at position pos
+__device__ __forceinline__ void mla_rope_pair(const b200awq_mla_t& d, int pos, int m, int col, __half a, __half b) {
+  const int qn = d.n_heads * (d.nope_dim + d.rope_dim);
+  if (col < qn) {
+    mla_q_pair(d, pos, m, col, a, b);
+    return;
+  }
+  const int kp = col - qn - d.kv_lora_rank;
+  if (kp < 0) return;
+  mla_k_pair(d, pos, m, kp, a, b);
+}
+
+// The mode-3 finish of an op with a q LoRA MLA op folded in (kind 3: MLA_K_ROPE on a row of N columns whose last Dr are
+// k_pe; kind 4: MLA_Q_ROPE), on columns (col, col + 1) of token row m
+__device__ __forceinline__ void mla_lora_pair(const b200awq_mla_t& d, int kind, int pos, int m, int N, int col, __half a,
+                                              __half b) {
+  if (kind == 4) {
+    mla_q_pair(d, pos, m, col, a, b);
+    return;
+  }
+  const int kp = col - (N - d.rope_dim);
+  if (kp >= 0) mla_k_pair(d, pos, m, kp, a, b);
 }
 
 // MLA_KV on column col of token row m's kv_b_proj row (value x): k_nope into k_cache, v into v_cache, at position pos

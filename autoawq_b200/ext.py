@@ -18,7 +18,7 @@ __all__ = [
     "gemv_forward_cuda_decode", "gemm_forward_cuda_prefill", "layernorm_forward_cuda", "silu_and_mul",
     "topk_softmax", "moe_alig_block_size", "grouped_gemm_forward",
     "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "qk_norm_descriptor",
-    "mla_descriptor", "mla_rope", "mla_kv_cache",
+    "mla_descriptor", "mla_rope", "mla_kv_cache", "mla_k_rope", "mla_q_rope",
     "set_knob", "get_knob",
     "B200AwqError",
 ]
@@ -372,23 +372,28 @@ def _mla_freqs(freqs, rope_dim, style):
     return t
 
 
-def mla_descriptor(pos, freqs, k_cache, v_cache, q_out, M, n_heads, nope_dim, rope_dim, v_dim, kv_lora_rank, style):
+def mla_descriptor(pos, freqs, k_cache, v_cache, q_out, M, n_heads, nope_dim, rope_dim, v_dim, kv_lora_rank, style,
+                   cache_len=None):
     """Checks the tensors of the MLA glue for M token rows and returns the b200awq_mla_t.  freqs: the [S_f, Dr/2, 2] f32
     table (_mla_freqs) or None (MLA_KV); k_cache f16 [B >= M, S, H, Dn + Dr] with contiguous [S, H, Dn + Dr] entries;
     v_cache f16 [B >= M, S, H, >= Dv] (padded heads allowed: the head stride is its last dimension) with contiguous
     entries, or None (MLA_ROPE); q_out contiguous f16 [M, H, Dn + Dr] (any shape of M H (Dn + Dr) elements ending in
-    [H, Dn + Dr]) or None (MLA_KV); pos a device int32 tensor of one element.  The kernels write batch entry m and q_out
-    row m for every m < M, so every size is checked against M before a pointer is taken."""
+    [H, Dn + Dr]) or None (MLA_KV); pos a device int32 tensor of one element.  k_cache may be None for MLA_Q_ROPE, which
+    writes no cache: cache_len then gives the cache's S, which still bounds the position.  The kernels write batch
+    entry m and q_out row m for every m < M, so every size is checked against M before a pointer is taken."""
     H, Dn, Dr, Dv, C, M = int(n_heads), int(nope_dim), int(rope_dim), int(v_dim), int(kv_lora_rank), int(M)
     W = Dn + Dr
     d = _cabi.Mla()
     d.n_heads, d.nope_dim, d.rope_dim, d.v_dim, d.kv_lora_rank, d.style = H, Dn, Dr, Dv, C, int(style)
     if pos.dtype != torch.int32 or pos.numel() != 1:
         raise B200AwqError("b200awq: pos must be a device int32 tensor with one element")
-    if (k_cache.dtype != torch.float16 or k_cache.dim() != 4 or tuple(k_cache.shape[2:]) != (H, W)
+    if k_cache is None:
+        if cache_len is None or int(cache_len) <= 0 or v_cache is not None:
+            raise B200AwqError("b200awq: without k_cache, give the cache length (and no v_cache)")
+    elif (k_cache.dtype != torch.float16 or k_cache.dim() != 4 or tuple(k_cache.shape[2:]) != (H, W)
             or k_cache.stride(3) != 1 or k_cache.stride(2) != W or k_cache.stride(1) != H * W):
         raise B200AwqError(f"b200awq: k_cache must be float16 [B, S, {H}, {W}] with contiguous [S, H, D] entries")
-    if k_cache.shape[0] < M:
+    elif k_cache.shape[0] < M:
         raise B200AwqError(f"b200awq: k_cache has {k_cache.shape[0]} batch entries for {M} token rows")
     if v_cache is not None:
         if (v_cache.dtype != torch.float16 or v_cache.dim() != 4 or v_cache.shape[2] != H or v_cache.shape[3] < Dv
@@ -402,8 +407,11 @@ def mla_descriptor(pos, freqs, k_cache, v_cache, q_out, M, n_heads, nope_dim, ro
                               or tuple(q_out.shape[-2:]) != (H, W) or q_out.numel() != M * H * W):
         raise B200AwqError(f"b200awq: q_out must be a contiguous float16 [{M}, {H}, {W}] tensor")
     _require_cuda(pos, k_cache, v_cache, freqs, q_out)
-    d.cache_len, d.k_batch_stride = k_cache.shape[1], k_cache.stride(0)
-    d.pos, d.k_cache = pos.data_ptr(), k_cache.data_ptr()
+    d.pos = pos.data_ptr()
+    if k_cache is None:
+        d.cache_len = int(cache_len)
+    else:
+        d.cache_len, d.k_batch_stride, d.k_cache = k_cache.shape[1], k_cache.stride(0), k_cache.data_ptr()
     if v_cache is not None:
         d.v_batch_stride, d.v_head_stride, d.v_cache = v_cache.stride(0), v_cache.shape[3], v_cache.data_ptr()
     if freqs is not None:
@@ -413,10 +421,11 @@ def mla_descriptor(pos, freqs, k_cache, v_cache, q_out, M, n_heads, nope_dim, ro
     return d
 
 
-def _mla_call(fn, row2, d, M, name):
+def _mla_call(fn, row2, d, M, name, *pre):
+    """fn(row, ld, *pre, desc, M, stream); pre: b200awq_mla_k_rope's k_pe column."""
     ld = row2.stride(0) if M > 1 else row2.shape[1]
     with _DeviceGuard(row2.device):
-        code = fn(row2.data_ptr(), ld, d, M, _stream(row2.device))
+        code = fn(row2.data_ptr(), ld, *pre, d, M, _stream(row2.device))
     check(code, f"{name}(M={M}, H={d.n_heads}, Dn={d.nope_dim}, Dr={d.rope_dim})")
 
 
@@ -450,6 +459,36 @@ def mla_kv_cache(kv, pos, k_cache, v_cache, n_heads, nope_dim, v_dim):
     d = mla_descriptor(pos, None, k_cache, v_cache, None, M, H, Dn, Dr, Dv, 0, 0)
     _require_cuda(kv)
     _mla_call(lib.b200awq_mla_kv, row2, d, M, "b200awq_mla_kv")
+
+
+def mla_k_rope(qkva, freqs, pos, k_cache, n_heads, nope_dim, rope_dim, kv_lora_rank, q_lora_rank, style):
+    """MLA with a q LoRA (DeepseekV2Attention / DeepseekV3Attention with q_lora_rank set), after the fused
+    q_a_proj | kv_a_proj_with_mqa linear: qkva [.., Cq + C + Dr] f16 = [q_a | c_kv | k_pe].  Writes k_cache[m, *pos, h,
+    Dn:] = the rotated k_pe for every head h, for token rows m < M <= 8; nothing when *pos is outside the cache or the
+    table.  freqs and style as mla_rope.  q_a and c_kv are left to q_a_layernorm and kv_a_layernorm."""
+    H, Dn, Dr, C, Cq = int(n_heads), int(nope_dim), int(rope_dim), int(kv_lora_rank), int(q_lora_rank)
+    row2 = _rows(qkva, Cq + C + Dr, "qkva")
+    M = row2.shape[0]
+    f = _mla_freqs(freqs, Dr, int(style))
+    d = mla_descriptor(pos, f, k_cache, None, None, M, H, Dn, Dr, 0, C, style)
+    _require_cuda(qkva)
+    _mla_call(lib.b200awq_mla_k_rope, row2, d, M, "b200awq_mla_k_rope", Cq + C)
+
+
+def mla_q_rope(q, freqs, pos, cache_len, n_heads, nope_dim, rope_dim, style, q_out=None):
+    """MLA with a q LoRA, after q_b_proj: q [.., H (Dn + Dr)] f16.  Writes q_out [M, H, Dn + Dr] = [q_nope | rotated
+    q_pe] per head (allocated when not given, and returned), for token rows m < M <= 8; nothing when *pos is outside
+    [0, min(cache_len, table rows)), the rule mla_k_rope writes the cache by.  freqs and style as mla_rope."""
+    H, Dn, Dr = int(n_heads), int(nope_dim), int(rope_dim)
+    row2 = _rows(q, H * (Dn + Dr), "q")
+    M = row2.shape[0]
+    if q_out is None:
+        q_out = torch.empty((M, H, Dn + Dr), dtype=torch.float16, device=q.device)
+    f = _mla_freqs(freqs, Dr, int(style))
+    d = mla_descriptor(pos, f, None, None, q_out, M, H, Dn, Dr, 0, 0, style, cache_len=cache_len)
+    _require_cuda(q)
+    _mla_call(lib.b200awq_mla_q_rope, row2, d, M, "b200awq_mla_q_rope")
+    return q_out
 
 
 # ------------------------------------------------------------------------------------ MoE (awq_ext surface)

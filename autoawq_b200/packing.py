@@ -171,3 +171,20 @@ def fuse_mla_input(attn):
              for m in (attn.q_proj, attn.kv_a_proj_with_mqa)]
     f = fuse_columns(parts)
     return f.qweight, f.scales, f.qzeros, f.bias
+
+
+def fuse_mla_lora_input(attn):
+    """(qweight, scales, qzeros, bias) of the fused q_a_proj | kv_a_proj_with_mqa linear of a transformers
+    DeepseekV2Attention / DeepseekV3Attention WITH a q LoRA (q_lora_rank set) whose two projections are WQLinear_GEMM
+    modules: both read the hidden state, so one GEMM-layout linear with N = Cq + C + Dr gives the row [q_a | c_kv | k_pe]
+    that DecodeProgram.mla_k_rope takes (loader.fuse_columns' concatenation along N).  bias is None when neither
+    projection has one."""
+    from .loader import fuse_columns
+    from .shard import PackedGemm
+
+    if getattr(attn, "q_lora_rank", None) is None:
+        raise ValueError("fuse_mla_lora_input: the attention has no q LoRA; use fuse_mla_input")
+    parts = [PackedGemm(m.qweight, m.qzeros, m.scales, getattr(m, "bias", None))
+             for m in (attn.q_a_proj, attn.kv_a_proj_with_mqa)]
+    f = fuse_columns(parts)
+    return f.qweight, f.scales, f.qzeros, f.bias

@@ -54,6 +54,11 @@ transformers' order: the fused q_proj | kv_a_proj_with_mqa linear (packing.fuse_
 an RMSNorm on the c_kv slice of that linear's output, kv_b_proj, mla_kv_cache.  Each folds into the finish of the linear
 recorded just before it, so at M = 1 a DeepSeek segment runs as one launch from one attention call to the next
 (DESIGN.md 3.5j).
+
+With a q LoRA (DeepSeek-V2 / V2.5 / V3, MiniCPM3) the order is: the fused q_a_proj | kv_a_proj_with_mqa linear
+(packing.fuse_mla_lora_input), `mla_k_rope`, q_a_layernorm as an RMSNorm on the q_a slice of that linear's output,
+q_b_proj, `mla_q_rope`, kv_a_layernorm on its c_kv slice, kv_b_proj, mla_kv_cache.  At M = 1 the chain is three
+kernel ops of one launch (DESIGN.md 3.5k).
 """
 from __future__ import annotations
 
@@ -63,6 +68,11 @@ import torch
 
 from . import _cabi, ext
 from ._cabi import B200AwqError, Op, check, lib
+
+
+# the recorded MLA ops: kind -> op constant (the stand-alone entry is b200awq_<kind>)
+_MLA_OPS = {"mla_rope": _cabi.OP_MLA_ROPE, "mla_kv": _cabi.OP_MLA_KV, "mla_k_rope": _cabi.OP_MLA_K_ROPE,
+            "mla_q_rope": _cabi.OP_MLA_Q_ROPE}
 
 
 class DecodeProgram:
@@ -243,6 +253,50 @@ class DecodeProgram:
         self._ops.append(("mla_kv", dict(row=row, M=M, N=row.shape[1], ldx=row.stride(0) if M > 1 else row.shape[1],
                                          desc=desc)))
         self._keep += [kv, row, pos, k_cache, v_cache]
+
+    def mla_k_rope(self, qkva, freqs, pos, k_cache, n_heads, nope_dim, rope_dim, kv_lora_rank, q_lora_rank, style):
+        """ext.mla_k_rope recorded on the fused q_a_proj | kv_a_proj_with_mqa output qkva [.., Cq + C + Dr]:
+        k_cache[m, *pos, h, Dn:] = the rotated k_pe for every head.  freqs and style as mla_rope (the same table rules).
+        The row keeps its values: record q_a_layernorm as layernorm_forward_cuda on qkva[..., :Cq] next, then q_b_proj
+        and mla_q_rope, then kv_a_layernorm on qkva[..., Cq:Cq + C].  k_cache needs a batch entry per token row."""
+        self._no_more()
+        self._dev_of(qkva)
+        H, Dn, Dr, C, Cq = int(n_heads), int(nope_dim), int(rope_dim), int(kv_lora_rank), int(q_lora_rank)
+        row = ext._rows(qkva, Cq + C + Dr, "qkva")
+        if row.data_ptr() != qkva.data_ptr():
+            raise B200AwqError("b200awq: mla_k_rope records qkva by address: pass its rows as they are")
+        M = row.shape[0]
+        f = ext._mla_freqs(freqs, Dr, int(style))
+        for t in (f, pos, k_cache):
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+        desc = ext.mla_descriptor(pos, f, k_cache, None, None, M, H, Dn, Dr, 0, C, style)
+        self._ops.append(("mla_k_rope", dict(row=row, M=M, N=row.shape[1], pre=(Cq + C,),
+                                             ldx=row.stride(0) if M > 1 else row.shape[1], desc=desc)))
+        self._keep += [qkva, row, f, pos, k_cache]
+
+    def mla_q_rope(self, q, freqs, pos, cache_len, n_heads, nope_dim, rope_dim, style, q_out=None):
+        """ext.mla_q_rope recorded on q_b_proj's output q [.., H (Dn + Dr)]: q_out [M, H, Dn + Dr] = [q_nope | rotated
+        q_pe] (allocated when not given, and returned).  cache_len: the caches' S, which bounds the position as it does
+        for mla_k_rope.  freqs and style as mla_rope; q_out needs M x H x (Dn + Dr) elements."""
+        self._no_more()
+        self._dev_of(q)
+        H, Dn, Dr = int(n_heads), int(nope_dim), int(rope_dim)
+        row = ext._rows(q, H * (Dn + Dr), "q")
+        if row.data_ptr() != q.data_ptr():
+            raise B200AwqError("b200awq: mla_q_rope records q by address: pass its rows as they are")
+        M = row.shape[0]
+        if q_out is None:
+            q_out = torch.empty((M, H, Dn + Dr), dtype=torch.float16, device=q.device)
+        f = ext._mla_freqs(freqs, Dr, int(style))
+        for t in (f, pos, q_out):
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+        desc = ext.mla_descriptor(pos, f, None, None, q_out, M, H, Dn, Dr, 0, 0, style, cache_len=cache_len)
+        self._ops.append(("mla_q_rope", dict(row=row, M=M, N=row.shape[1], ldx=row.stride(0) if M > 1 else row.shape[1],
+                                             desc=desc)))
+        self._keep += [q, row, f, pos, q_out]
+        return q_out
 
     @staticmethod
     def _stacked(w, name):
@@ -505,8 +559,8 @@ class DecodeProgram:
             elif kind == "rope":
                 c.kind, c.M, c.N, c.ldx = _cabi.OP_ROPE_KV, o["M"], o["N"], o["ldx"]
                 c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["desc"])
-            elif kind in ("mla_rope", "mla_kv"):
-                c.kind, c.M, c.N, c.ldx = (_cabi.OP_MLA_ROPE if kind == "mla_rope" else _cabi.OP_MLA_KV), o["M"], o["N"], o["ldx"]
+            elif kind in _MLA_OPS:
+                c.kind, c.M, c.N, c.ldx = _MLA_OPS[kind], o["M"], o["N"], o["ldx"]
                 c.x, c.weight = o["row"].data_ptr(), ctypes.addressof(o["desc"])
             else:
                 c.kind, c.M, c.K, c.N, c.group_size, c.ldx = _cabi.OP_LINEAR_GEMM, o["M"], o["K"], o["N"], o["G"], o["ldx"]
@@ -552,13 +606,14 @@ class DecodeProgram:
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
-            return o["M"] if kind in ("linear", "moe", "add", "rope", "mla_rope", "mla_kv") else o["rows"]
+            return o["M"] if kind in ("linear", "moe", "add", "rope") or kind in _MLA_OPS else o["rows"]
         return 0
 
     @property
     def kernel_ops(self) -> int:
         """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe / deepseek_moe (gate|up with the routing, down), none per add,
-        rope_kv_cache, mla_rope or mla_kv_cache (they fold into their producer's epilogue); 0 per-op."""
+        rope_kv_cache, mla_rope, mla_kv_cache, mla_k_rope or mla_q_rope (they fold into their producer's epilogue); 0
+        per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
     @property
@@ -567,7 +622,7 @@ class DecodeProgram:
         call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), 34 + top_k per softmax
         deepseek_moe (sigmoid: 36 + top_k, + 6 with expert groups, + 3 with norm_topk_prob), one torch.add launch per add
         and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache, one b200awq_mla_rope / b200awq_mla_kv
-        launch per mla_rope / mla_kv_cache.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
+        / b200awq_mla_k_rope / b200awq_mla_q_rope launch per mla_rope / mla_kv_cache / mla_k_rope / mla_q_rope.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
         kernel (torch.sort, torch.gather), so the kernel count can be higher."""
         def per_op(kind, o):
             if kind != "moe":
@@ -611,9 +666,9 @@ class DecodeProgram:
                 with ext._DeviceGuard(dev):
                     code = lib.b200awq_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["M"], ext._stream(dev))
                 check(code, "b200awq_rope_kv")
-            elif kind in ("mla_rope", "mla_kv"):
-                ext._mla_call(lib.b200awq_mla_rope if kind == "mla_rope" else lib.b200awq_mla_kv, o["row"], o["desc"],
-                              o["M"], "b200awq_" + kind)
+            elif kind in _MLA_OPS:
+                ext._mla_call(getattr(lib, "b200awq_" + kind), o["row"], o["desc"], o["M"], "b200awq_" + kind,
+                              *o.get("pre", ()))
             else:
                 ext.linear_forward("gemm", o["x"], o["qweight"], o["scales"], o["qzeros"], o["G"], o["bias"], out=o["y"])
 

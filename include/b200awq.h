@@ -327,10 +327,22 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     M != 1, the op before is not a plain linear, N does not match the descriptor, Dn, Dr, Dv or C is not a
  *     multiple of 16, or any other op reads or writes q_out or the caches or writes pos / freqs; the MLA_ROPE and MLA_KV
  *     ops of one layer may share k_cache (they write disjoint columns).  A program with MLA ops runs the DeepSeek-MoE
- *     kernel's configuration (a program that also holds SPARSE_MOE or QWEN3_MOE blocks replays per op). */
+ *     kernel's configuration (a program that also holds SPARSE_MOE or QWEN3_MOE blocks replays per op).
+ *
+ *   MLA_K_ROPE    : MLA with a q LoRA (DeepSeek-V2 / V2.5 / V3, MiniCPM3), on the fused q_a_proj | kv_a_proj_with_mqa
+ *                   output row [q_a (Cq) | c_kv (C) | k_pe (Dr)]: x = that row [M, N] at pitch ldx, Cq = N - C - Dr > 0,
+ *                   weight = a b200awq_mla_t.  Writes only k_cache (q_out may be null).  As b200awq_mla_k_rope with
+ *                   k_pe_col = N - Dr.
+ *   MLA_Q_ROPE    : the q_b_proj output [M, H (Dn + Dr)] into q_out = [q_nope | rotated q_pe]: x, ldx, weight as above,
+ *                   N = H (Dn + Dr).  Writes only q_out (k_cache may be null).  As b200awq_mla_q_rope.
+ *     Folding: as MLA_ROPE, each into the finish of the linear recorded immediately before it, packed in mode 3.  The
+ *     chain [q_a|kv_a, MLA_K_ROPE, RMSNORM(q_a slice), q_b, MLA_Q_ROPE, RMSNORM(c_kv slice), kv_b, MLA_KV] is three
+ *     kernel ops; kv_b stages the c_kv slice of the row two ops back.  The rejections of MLA_ROPE apply, Cq must be a
+ *     multiple of 16, two k rotations may not share a k_cache, and a program may not mix MLA_ROPE with these ops. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
-       B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11 };
+       B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11, B200AWQ_OP_MLA_K_ROPE = 12,
+       B200AWQ_OP_MLA_Q_ROPE = 13 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -486,6 +498,16 @@ typedef struct b200awq_mla {
 /* ld: row pitch of `row` in elements.  `desc` is a host pointer, read at the call. */
 int b200awq_mla_rope(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream);
 int b200awq_mla_kv(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream);
+/* MLA with a q LoRA (q = q_b_proj(q_a_layernorm(q_a_proj(h)))): the rotation split in two, same arithmetic and position
+ * rule as b200awq_mla_rope.
+ * b200awq_mla_k_rope on a row whose columns [k_pe_col, k_pe_col + Dr) are k_pe (k_pe_col = Cq + C for the fused
+ *   q_a_proj | kv_a_proj_with_mqa row [q_a | c_kv | k_pe]): k_cache[m, p, h, Dn:] = rotate(k_pe) for every h.  Reads
+ *   neither q_out nor v_cache; C only as the op's row width in a program.
+ * b200awq_mla_q_rope on the q_b_proj row [H (Dn + Dr), per head [nope | pe]]: q_out[m, h, :Dn] = q_nope,
+ *   q_out[m, h, Dn:] = rotate(q_pe).  Reads neither k_cache (cache_len still bounds the position) nor v_cache, C. */
+int b200awq_mla_k_rope(const void* row, int64_t ld, int64_t k_pe_col, const b200awq_mla_t* desc, int M,
+                       b200awq_stream_t stream);
+int b200awq_mla_q_rope(const void* row, int64_t ld, const b200awq_mla_t* desc, int M, b200awq_stream_t stream);
 
 typedef struct b200awq_program* b200awq_program_t;
 
@@ -549,7 +571,7 @@ int b200awq_comm_destroy(b200awq_comm_t comm);
  * a lane, so SiLU*mul happens in the producer; mode 2 (a qkv linear followed by ROPE_KV, b200awq_stream_pack_rotary):
  * set s of head h = s / (D / 16) pairs column h D + 8 t + g with h D + D/2 + 8 t + g (t = s % (D / 16)), so RoPE's
  * rotation partners share a lane (requires D % 16 == 0 and N % D == 0); mode 3 (a q_proj | kv_a_proj_with_mqa linear
- * followed by MLA_ROPE, adjacent pairs): set s pairs column 16 s + 2 g with 16 s + 2 g + 1, so MLA's interleaved rotation
+ * followed by MLA_ROPE, MLA_K_ROPE or MLA_Q_ROPE, adjacent pairs): set s pairs column 16 s + 2 g with 16 s + 2 g + 1, so MLA's interleaved rotation
  * partners share a lane (b200awq_stream_pack with mode 3).  Requires N % 16 == 0, K % 128 == 0, G in
  * {32, 64} or G % 128 == 0.  b200awq_stream_bytes returns 0 for unsupported shapes; the byte count is the same for
  * every mode. */
