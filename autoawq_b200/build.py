@@ -11,7 +11,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libb200awq.so")
 SOURCES = ["cabi.cu", "dequant.cu", "gemv.cu", "gemm_tc.cu", "aux.cu", "program.cu", "moe.cu", "comm.cu"]
-HEADERS = ["common.cuh", "gemv_tile.cuh", "program_stream.cuh", "program_stream_body.inc", "program_batch.cuh", "program_batch_body.inc", "rope.cuh", "kernels.h", os.path.join(ROOT, "include", "b200awq.h")]
+HEADERS = ["common.cuh", "gemv_tile.cuh", "program_stream.cuh", "program_stream_body.inc", "program_batch.cuh", "program_batch_body.inc", "rope.cuh", "layernorm.cuh", "kernels.h", os.path.join(ROOT, "include", "b200awq.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",

@@ -1,12 +1,15 @@
 // Glue kernels the reference's fused modules call through awq_ext (SURVEY.md 8f #1, #2):
 //   rmsnorm       <- awq_ext.layernorm_forward_cuda   (awq/modules/fused/norm.py:33-36)
 //   silu_and_mul  <- awq_ext.silu_and_mul             (awq/modules/fused/moe.py:76)
+//   layer_norm / gelu <- nn.LayerNorm (CohereLayerNorm without a bias) and F.gelu of the LayerNorm blocks
+//                    (Command-R, StarCoder2, MPT)
 //   rope_kv       <- RoPE.forward + WindowedCache.update_kv (awq/modules/fused/attn.py:53-86,243-267)
 //   mla_rope / mla_kv <- the glue of transformers' DeepseekV2Attention / DeepseekV3Attention between the projections
 //                    and attention (rotary, head split, cache write); mla_k_rope / mla_q_rope: the same with a q LoRA
 // fp16 in/out, fp32 math.  Bandwidth-trivial (KBs per decode step); kept simple.
 #include "common.cuh"
 #include "kernels.h"
+#include "layernorm.cuh"
 #include "rope.cuh"
 
 namespace b200awq {
@@ -245,6 +248,80 @@ cudaError_t mla_q_rope(const void* row, int64_t ld, const b200awq_mla_t& d, int 
   const int64_t n = (int64_t)M * ((d.n_heads * (d.nope_dim + d.rope_dim)) / 2);
   return launch_kernel(mla_q_rope_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
                        reinterpret_cast<const __half*>(row), ld, d, M);
+}
+
+// one CTA of 256 threads per row; thread t takes the chunks of 8 columns at 8 t + 2048 p (the order b200awq.h states,
+// which the decode program's LayerNorm staging reproduces: layernorm.cuh has the arithmetic)
+__global__ void __launch_bounds__(256)
+    layer_norm_kernel(const __half* __restrict__ x, int64_t ldx, const __half* __restrict__ w,
+                      const __half* __restrict__ b, __half* __restrict__ out, int K, float eps) {
+  __shared__ float wsum[2][8];
+  pdl_trigger();
+  pdl_wait();
+  const __half* xr = x + (int64_t)blockIdx.x * ldx;
+  __half* orow = out + (int64_t)blockIdx.x * K;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float s = 0.f;
+  for (int c = threadIdx.x * 8; c < K; c += 2048) {
+    const uint4 v = *reinterpret_cast<const uint4*>(xr + c);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) s = ln_sum_pair(s, u32_as_h2((&v.x)[q]));
+  }
+  s = warp_sum(s);
+  if (lane == 0) wsum[0][warp] = s;
+  __syncthreads();
+  float tot = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) tot = __fadd_rn(tot, wsum[0][i]);
+  const float mean = ln_mean(tot, K);
+  s = 0.f;
+  for (int c = threadIdx.x * 8; c < K; c += 2048) {
+    const uint4 v = *reinterpret_cast<const uint4*>(xr + c);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) s = ln_sq_pair(s, u32_as_h2((&v.x)[q]), mean);
+  }
+  s = warp_sum(s);
+  if (lane == 0) wsum[1][warp] = s;
+  __syncthreads();
+  tot = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) tot = __fadd_rn(tot, wsum[1][i]);
+  const float r = ln_rstd(tot, K, eps);
+  for (int c = threadIdx.x * 8; c < K; c += 2048) {
+    const uint4 v = *reinterpret_cast<const uint4*>(xr + c);
+    const uint4 wv = __ldg(reinterpret_cast<const uint4*>(w + c));
+    uint4 bv = make_uint4(0u, 0u, 0u, 0u);
+    if (b != nullptr) bv = __ldg(reinterpret_cast<const uint4*>(b + c));
+    uint4 o;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float2 a = __half22float2(u32_as_h2((&v.x)[q])), wq = __half22float2(u32_as_h2((&wv.x)[q]));
+      const float2 bq = __half22float2(u32_as_h2((&bv.x)[q]));
+      (&o.x)[q] = h2_as_u32(__halves2half2(ln_apply(a.x, mean, r, wq.x, bq.x, b != nullptr),
+                                           ln_apply(a.y, mean, r, wq.y, bq.y, b != nullptr)));
+    }
+    *reinterpret_cast<uint4*>(orow + c) = o;
+  }
+}
+
+// one thread per element; kind 1 = exact, 2 = tanh (layernorm.cuh)
+__global__ void __launch_bounds__(256) gelu_kernel(const __half* __restrict__ x, __half* __restrict__ out, int64_t n,
+                                                   int kind) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = gelu_h(x[i], kind);
+}
+
+cudaError_t layer_norm(const void* x, int64_t ldx, const void* w, const void* b, void* out, int rows, int hidden,
+                       float eps, cudaStream_t st) {
+  return launch_kernel(layer_norm_kernel, dim3(rows), dim3(256), 0, st, reinterpret_cast<const __half*>(x), ldx,
+                       reinterpret_cast<const __half*>(w), reinterpret_cast<const __half*>(b),
+                       reinterpret_cast<__half*>(out), hidden, eps);
+}
+cudaError_t gelu(const void* x, void* out, int64_t n, int approximate, cudaStream_t st) {
+  return launch_kernel(gelu_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
+                       reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(out), n, approximate ? 2 : 1);
 }
 
 cudaError_t rmsnorm(const void* x, const void* w, void* out, int rows, int hidden, float eps, cudaStream_t st) {

@@ -205,6 +205,25 @@ int b200awq_silu_and_mul(const void* gate_up, void* out, int rows, int d, b200aw
   return fold(silu_and_mul(gate_up, out, rows, d, static_cast<cudaStream_t>(stream)));
 }
 
+int b200awq_layer_norm(const void* x, int64_t ldx, const void* weight, const void* bias, void* out, int rows,
+                       int hidden, float eps, b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_layer_norm");
+  if (!x || !weight || !out || rows < 0 || hidden <= 0 || (rows > 1 && ldx < hidden)) return B200AWQ_EINVAL;
+  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  if ((hidden % 8) != 0 || (rows > 1 && (ldx % 8) != 0) || !a16(x) || !a16(weight) || !a16(out) || (bias && !a16(bias)))
+    return B200AWQ_EUNSUPPORTED;   // the fixed summation order works in chunks of 8 columns
+  if (rows == 0) return B200AWQ_OK;
+  return fold(layer_norm(x, rows > 1 ? ldx : hidden, weight, bias, out, rows, hidden, eps,
+                         static_cast<cudaStream_t>(stream)));
+}
+
+int b200awq_gelu(const void* x, void* out, int rows, int n, int approximate, b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_gelu");
+  if (!x || !out || rows < 0 || n <= 0 || (approximate != 0 && approximate != 1)) return B200AWQ_EINVAL;
+  if (rows == 0) return B200AWQ_OK;
+  return fold(gelu(x, out, (int64_t)rows * n, approximate, static_cast<cudaStream_t>(stream)));
+}
+
 int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_rope_kv");
   if (qkv == nullptr || M < 0) return B200AWQ_EINVAL;

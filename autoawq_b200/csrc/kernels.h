@@ -153,6 +153,9 @@ void comm_destroy(Comm* c);
 
 cudaError_t rmsnorm(const void* x, const void* w, void* out, int rows, int hidden, float eps, cudaStream_t st);
 cudaError_t silu_and_mul(const void* gate_up, void* out, int rows, int d, cudaStream_t st);
+cudaError_t layer_norm(const void* x, int64_t ldx, const void* w, const void* b, void* out, int rows, int hidden,
+                       float eps, cudaStream_t st);
+cudaError_t gelu(const void* x, void* out, int64_t n, int approximate, cudaStream_t st);
 // B200AWQ_OK, or the code b200awq_rope_kv returns for a bad descriptor / qkv pitch (host only)
 int rope_validate(const struct ::b200awq_rope* r, int64_t ldqkv);
 cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_rope& r, int M, cudaStream_t st);

@@ -29,11 +29,12 @@
 #include "common.cuh"
 #include "gemv_tile.cuh"
 #include "kernels.h"
+#include "layernorm.cuh"
 #include "rope.cuh"
 
 namespace b200awq {
 
-enum { kProCopy = 0, kProRmsnorm = 1, kProSilu = 2 };
+enum { kProCopy = 0, kProRmsnorm = 1, kProSilu = 2, kProLayernorm = 3 };
 
 // knob 3 = 2: per-op phase timestamps (globaltimer ns) of the first 8 CTAs for the first 32 kernel ops; the slots are
 // listed in program_stream.cuh (SP_STAMP)
@@ -128,7 +129,8 @@ struct ProgOp {
   const __half* bias = nullptr;
   __half* y = nullptr;           // what the op's row publishes (an ADD folded in swaps the linear's y for its output)
   const __half* src = nullptr;   // external source (fp16, global) when !src_prev: COPY x, RMSNORM row, SILU gate|up
-  const __half* norm_w = nullptr;   // RMSNORM weight [K]
+  const __half* norm_w = nullptr;   // RMSNORM / LAYER_NORM weight [K]
+  const __half* ln_b = nullptr;     // LAYER_NORM bias [K], or null
   __half* xout = nullptr;        // where the recorded glue op wanted its result, or null
   int src_off = 0;               // src_prev: first column of the previous op's output this op reads
   int src_prev = 0;              // 1: the source is the previous op's output
@@ -150,6 +152,9 @@ struct ProgOp {
   // an MLA_ROPE (mla_kind 1), MLA_KV (2), MLA_K_ROPE (3) or MLA_Q_ROPE (4) folded into the finish
   b200awq_mla_t mla = {};
   int mla_kind = 0;
+  // a GELU (1) or GELU_TANH (2) folded into the finish: y is the GELU's output (the row publishes it), raw_y the
+  // linear's own, still stored (res_op / res_ext stay unset: no residual)
+  int gelu = 0;
 };
 
 // One MoE op of a folded program (two kernel ops): kind is B200AWQ_OP_SPARSE_MOE, _QWEN3_MOE or _DEEPSEEK_MOE, ds.moe
@@ -189,12 +194,12 @@ struct FoldedProgram {
 // The kernel entry that runs a program (chosen by stream_build).  M = 1: the plain kernel (8 or 12 consumer warps,
 // knob 9) or the 8-warp kernel of the program's features; M > 1: the batched kernels at MT = sb_mt(M).  Side tables:
 // the M = 1 kernels from kKernMoe on take SpMoe (null without MoE blocks), from kKernResidual on SpRes, from kKernRope on
-// SpRope, from kKernQkNorm on SpQkNorm, kKernDeepseekMoe, kKernMla and kKernMlaLora SpDsk, and the last two SpMla; the
+// SpRope, kKernLayerNorm SpLn (and none of the later tables), from kKernQkNorm on SpQkNorm, kKernDeepseekMoe, kKernMla and kKernMlaLora SpDsk, and the last two SpMla; the
 // batched ones take SpRes from kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2
 // on.  The Qwen3-MoE, DeepSeek-MoE and MLA kernels take every table, with empty entries where an op has no add,
 // rotation or norm.
 enum ProgKernel {
-  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe, kKernMla, kKernMlaLora,
+  kKernPlain, kKernMoe, kKernResidual, kKernRope, kKernLayerNorm, kKernQkNorm, kKernQwen3Moe, kKernDeepseekMoe, kKernMla, kKernMlaLora,
   kKernBatch2, kKernBatch4, kKernBatch8, kKernBatchResidual2, kKernBatchResidual4, kKernBatchResidual8,
   kKernBatchRope2, kKernBatchRope4, kKernBatchRope8, kKernBatchQkNorm2, kKernBatchQkNorm4, kKernBatchQkNorm8
 };
@@ -230,13 +235,14 @@ struct Program {
   SpQkNorm* d_qkn = nullptr;
   unsigned long long* d_qkn_part = nullptr;
   SpMla* d_mla = nullptr;
+  SpLn* d_ln = nullptr;
 
   Program() = default;
   Program(const Program&) = delete;
   Program& operator=(const Program&) = delete;
   ~Program() {
     for (void* d : std::initializer_list<void*>{d_sp_ops, d_stream, d_cta, d_rows, d_state, d_moe, d_xlog, d_dsk, d_res,
-                                                d_rope, d_qkn, d_qkn_part, d_mla})
+                                                d_rope, d_qkn, d_qkn_part, d_mla, d_ln})
       cudaFree(d);
   }
 };
@@ -367,6 +373,7 @@ static cudaError_t upload(T** d, const std::vector<T>& h) {
 // MLA_ROPE ops (`mla_kind` 1): packed in mode 3, the finish rotates / stores (SpMla); MLA_KV (2): mode 0, the finish
 // stores the cache columns.  Such a program runs stream_mla_kernel, whose MoE blocks are DEEPSEEK_MOE blocks.
 // MLA_K_ROPE / MLA_Q_ROPE (3 / 4): packed in mode 3, on stream_mla_lora_kernel (the same, plus their finishes).
+// LAYER_NORM prologues (kProLayernorm) and GELU finishes (`gelu` != 0, mode 0): stream_layernorm_kernel (SpLn).
 static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaError_t* err) {
   *err = cudaSuccess;
   const std::vector<ProgOp>& table = f.table;
@@ -441,18 +448,25 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     }
   }
   if (has_mla && M != 1) return false;   // (program_create rejects it already)
-  // residual adds: the producer and an in-program residual must publish plain columns (a mode-1 row holds SiLU*mul)
-  for (int i = 0; i < n; ++i)
+  // residual adds and GELUs: the producer and an in-program residual must publish plain columns (a mode-1 row holds
+  // SiLU*mul)
+  bool has_ln = false;
+  for (int i = 0; i < n; ++i) {
     if (table[i].raw_y != nullptr) {
       if (mode[i] == 1 || (table[i].res_op >= 0 && mode[table[i].res_op] == 1)) return false;
-      has_res = true;
+      has_res = has_res || table[i].gelu == 0;
     }
+    has_ln = has_ln || table[i].gelu != 0 || table[i].prologue == kProLayernorm;
+  }
+  // LAYER_NORM / GELU run on stream_layernorm_kernel only (program_create rejects the rest already)
+  if (has_ln && (M != 1 || has_moe || has_qkn || has_mla)) return false;
   // the kernel: the first of these the program needs (has_qkn implies has_rope; QWEN3_MOE and DEEPSEEK_MOE blocks only
   // exist at M = 1)
   const int mt = sb_mt(M) == 2 ? 0 : (sb_mt(M) == 4 ? 1 : 2);
   const ProgKernel kern =
       M > 1 ? ProgKernel((has_qkn ? kKernBatchQkNorm2 : has_rope ? kKernBatchRope2 : has_res ? kKernBatchResidual2
                                                                                              : kKernBatch2) + mt)
+      : has_ln                           ? kKernLayerNorm
       : has_lora                         ? kKernMlaLora
       : has_mla                          ? kKernMla
       : mkind == B200AWQ_OP_DEEPSEEK_MOE ? kKernDeepseekMoe
@@ -528,7 +542,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
       if (p.xout != nullptr) ops[j].act_out = p.xout;
     } else {
       o.prologue = p.prologue;
-      o.xout = p.prologue == kProRmsnorm ? p.xout : nullptr;
+      o.xout = p.prologue == kProRmsnorm || p.prologue == kProLayernorm ? p.xout : nullptr;
       if (p.prologue == kProCopy && p.xout != nullptr) return false;
       int j = -1;
       if (p.src_prev) j = i - 1;
@@ -547,6 +561,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
         o.ldx = p.src_ld;
       }
     }
+    if (p.gelu != 0) o.act_out = p.y;   // the GELU's output (o.y is the linear's raw y)
     if (p.moe != 0) {
       o.moe = p.moe;
       o.moe_i = p.mi;
@@ -664,7 +679,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     std::vector<SpRes> rd(n);
     for (int i = 0; i < n; ++i) {
       rd[i].op = table[i].res_op;
-      if (table[i].raw_y == nullptr) continue;
+      if (table[i].raw_y == nullptr || table[i].gelu != 0) continue;
       rd[i].out = table[i].y;                       // the ADD's output (the op's y was swapped for it)
       rd[i].ext = static_cast<const __half*>(table[i].res_ext);
     }
@@ -704,11 +719,20 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     }
     e = upload(&pr->d_mla, ml);
   }
+  if (e == cudaSuccess && kern == kKernLayerNorm) {
+    std::vector<SpLn> ln(n);
+    for (int i = 0; i < n; ++i) {
+      ln[i].bias = table[i].prologue == kProLayernorm ? table[i].ln_b : nullptr;
+      ln[i].gelu = table[i].gelu;
+    }
+    e = upload(&pr->d_ln, ln);
+  }
   if (e == cudaSuccess) e = upload(&pr->d_sp_ops, ops);
   // the kernel may use all 227 KB of shared memory (the plain one at both warp counts: knob 9 is read at run time)
   static const void* const entry[] = {
       (const void*)stream_program_kernel<8, 4>, (const void*)stream_moe_kernel, (const void*)stream_residual_kernel,
-      (const void*)stream_rope_kernel, (const void*)stream_qknorm_kernel, (const void*)stream_qwen3moe_kernel,
+      (const void*)stream_rope_kernel, (const void*)stream_layernorm_kernel, (const void*)stream_qknorm_kernel,
+      (const void*)stream_qwen3moe_kernel,
       (const void*)stream_deepseek_moe_kernel, (const void*)stream_mla_kernel, (const void*)stream_mla_lora_kernel,
       (const void*)stream_batch_kernel<2>, (const void*)stream_batch_kernel<4>,
       (const void*)stream_batch_kernel<8>, (const void*)stream_batch_residual_kernel<2>,
@@ -840,6 +864,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     int kind;
     const void* src;
     const void* w;
+    const void* b;   // LAYER_NORM bias, or null
     void* out;
     int width;
     float eps;
@@ -970,13 +995,37 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       pv.y = static_cast<__half*>(op.y);   // the producer's row now publishes the sum
       continue;
     }
-    if (op.kind == B200AWQ_OP_RMSNORM || op.kind == B200AWQ_OP_SILU_AND_MUL) {
+    if (op.kind == B200AWQ_OP_GELU || op.kind == B200AWQ_OP_GELU_TANH) {
+      // y = gelu(x), folded into the finish of the linear recorded just before it, whose whole output x must be (as an
+      // ADD folds: that linear's row then publishes the GELU's output, its raw y is stored on the side)
       if (op.x == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
-      if (op.kind == B200AWQ_OP_RMSNORM && op.weight == nullptr) return B200AWQ_EINVAL;
+      if ((op.K % 8) != 0 || !aligned16(op.x) || !aligned16(op.y)) return B200AWQ_EUNSUPPORTED;
+      if (M != 1 || max_tokens > 1) return B200AWQ_EUNSUPPORTED;   // batched programs replay per op
+      const size_t bytes = rows_bytes(op.K);
+      if (overlaps(op.y, bytes, op.x, bytes)) return B200AWQ_EUNSUPPORTED;   // in place
+      // (an ADD, a glue op or a ROPE_KV / MLA op in between: the op before is not a linear; a MoE block's ops are not
+      // plain linears; a linear carrying an ADD or a GELU already has raw_y)
+      if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty()) return B200AWQ_EUNSUPPORTED;
+      ProgOp& pv = table.back();
+      if (pv.moe != 0 || pv.raw_y != nullptr || op.x != pv.y || op.K != pv.N) return B200AWQ_EUNSUPPORTED;
+      // the output must not overlap what the producer reads (other CTAs may still be staging it) or publishes
+      if (overlaps(op.y, bytes, pv.src, src_bytes(pv)) || (pv.xout != nullptr && overlaps(op.y, bytes, pv.xout, rows_bytes(pv.K))))
+        return B200AWQ_EUNSUPPORTED;
+      if (!glue_write(op.y, bytes, nullptr)) return B200AWQ_EUNSUPPORTED;
+      pv.raw_y = pv.y;
+      pv.gelu = op.kind == B200AWQ_OP_GELU ? 1 : 2;
+      pv.y = static_cast<__half*>(op.y);   // the producer's row now publishes the GELU's output
+      continue;
+    }
+    if (op.kind == B200AWQ_OP_RMSNORM || op.kind == B200AWQ_OP_SILU_AND_MUL || op.kind == B200AWQ_OP_LAYER_NORM) {
+      const bool ln = op.kind == B200AWQ_OP_LAYER_NORM;
+      if (op.x == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
+      if (op.kind != B200AWQ_OP_SILU_AND_MUL && op.weight == nullptr) return B200AWQ_EINVAL;
       // an RMSNORM over rows of a wider tensor (ldx > K): the kernels stage contiguous rows only
-      if (op.kind == B200AWQ_OP_RMSNORM && M > 1 && op.ldx != 0 && op.ldx != op.K) return B200AWQ_EUNSUPPORTED;
+      if (op.kind != B200AWQ_OP_SILU_AND_MUL && M > 1 && op.ldx != 0 && op.ldx != op.K) return B200AWQ_EUNSUPPORTED;
       if ((op.K % 8) != 0 || !aligned16(op.x) || !aligned16(op.y) || (op.weight != nullptr && !aligned16(op.weight)))
         return B200AWQ_EUNSUPPORTED;
+      if (ln && (M != 1 || max_tokens > 1 || (op.bias != nullptr && !aligned16(op.bias)))) return B200AWQ_EUNSUPPORTED;
       const size_t in_bytes = (size_t)M * (op.kind == B200AWQ_OP_SILU_AND_MUL ? 2 : 1) * op.K * 2;
       if (overlaps(op.y, rows_bytes(op.K), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;  // in-place glue op
       if (!glue_write(op.y, rows_bytes(op.K), nullptr)) return B200AWQ_EUNSUPPORTED;
@@ -984,8 +1033,12 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       // its input must not be a buffer only CTA 0 publishes
       for (const Glue& gl : glues)
         if (overlaps(gl.out, glue_out_bytes(gl), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
-      glues.push_back(Glue{op.kind == B200AWQ_OP_RMSNORM ? kProRmsnorm : kProSilu, op.x, op.weight, op.y, op.K, op.eps,
-                           false, true});
+      // a SiLU*mul of a GELU's output: its producer would have to be a mode-1 gate|up
+      if (op.kind == B200AWQ_OP_SILU_AND_MUL)
+        for (const ProgOp& t : table)
+          if (t.gelu != 0 && overlaps(t.y, y_bytes(t), op.x, in_bytes)) return B200AWQ_EUNSUPPORTED;
+      glues.push_back(Glue{op.kind == B200AWQ_OP_RMSNORM ? kProRmsnorm : ln ? kProLayernorm : kProSilu, op.x, op.weight,
+                           ln ? op.bias : nullptr, op.y, op.K, op.eps, false, true});
       continue;
     }
     if (op.kind != B200AWQ_OP_LINEAR_GEMM) return B200AWQ_EINVAL;
@@ -1012,6 +1065,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       p.prologue = hit->kind;
       p.src = static_cast<const __half*>(hit->src);
       p.norm_w = static_cast<const __half*>(hit->w);
+      p.ln_b = static_cast<const __half*>(hit->b);
       p.xout = hit->used ? nullptr : static_cast<__half*>(hit->out);   // published once, by its first consumer
       p.eps = hit->eps;
       p.src_ld = (hit->kind == kProSilu ? 2 : 1) * op.K;   // glue buffers are contiguous rows
@@ -1068,6 +1122,13 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (!gl.used) return B200AWQ_EUNSUPPORTED;   // a glue op nobody consumes would never run
   if (table.empty()) return B200AWQ_EUNSUPPORTED;
   const int nt = static_cast<int>(table.size());
+  // LAYER_NORM / GELU ops run on stream_layernorm_kernel, which has no MoE, q / k norm or MLA steps (no model mixes them)
+  bool has_ln = false, has_other = !moes.empty();
+  for (const ProgOp& t : table) {
+    has_ln = has_ln || t.prologue == kProLayernorm || t.gelu != 0;
+    has_other = has_other || t.qkr.q_norm_weight != nullptr || t.mla_kind != 0;
+  }
+  if (has_ln && has_other) return B200AWQ_EUNSUPPORTED;
   for (const ProgOp& t : table) {
     // an external residual is read at the finish of its op, any time during the run: nothing of the program may write it
     if (t.res_ext == nullptr) continue;
@@ -1309,6 +1370,7 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     case kKernMoe: return stream(stream_moe_kernel);
     case kKernResidual: return stream(stream_residual_kernel, p->d_res);
     case kKernRope: return stream(stream_rope_kernel, p->d_res, p->d_rope);
+    case kKernLayerNorm: return stream(stream_layernorm_kernel, p->d_res, p->d_rope, p->d_ln);
     case kKernQkNorm: return stream(stream_qknorm_kernel, p->d_res, p->d_rope, p->d_qkn);
     case kKernQwen3Moe: return stream(stream_qwen3moe_kernel, p->d_res, p->d_rope, p->d_qkn);
     case kKernDeepseekMoe: return stream(stream_deepseek_moe_kernel, p->d_res, p->d_rope, p->d_qkn, p->d_dsk);

@@ -278,6 +278,15 @@ struct SpMla {
   int wait_words;
 };
 
+// LAYER_NORM / GELU / GELU_TANH folded into a linear (stream_layernorm_kernel): one entry per kernel op in a side table,
+// like SpRope.  bias: the LayerNorm bias of the op's staging prologue (prologue kProLayernorm; null without one);
+// gelu: 1 (exact) or 2 (tanh) when the op's mode-0 finish publishes fp16(gelu(y)) and stores it to act_out, else 0.
+struct SpLn {
+  const __half* bias;
+  int gelu;
+  int pad_;
+};
+
 // phase (b) of a QK_NORM_ROPE_KV finish (SpQkNorm above), shared by the M = 1 and the batched body: item t of this
 // thread (t = ct, ct + nthr, ... < nsets * per_set; per_set = 8 M) is lane group t % 8 of token row (t % per_set) / 8 of
 // local set t / per_set, whose fp16 pair phase (a) kept in part[(ls * kst + m) * 16 + g] / [.. + 8].
@@ -709,6 +718,28 @@ __global__ void __launch_bounds__(32 + 8 * 32, 1)
 #undef SP_DEEPSEEK
 #undef SP_QWEN3
 #undef SP_QKNORM
+#undef SP_ROPE
+#undef SP_RESIDUAL
+}
+
+// M = 1 programs with LAYER_NORM / GELU / GELU_TANH ops (SpLn above; Command-R, StarCoder2 and MPT blocks), with or
+// without residual adds and ROPE_KV ops: stream_rope_kernel plus SP_LAYERNORM, which compiles in the LayerNorm staging
+// (sum of x while staging, the centred sum of squares from the staged row after a CTA barrier, then the normalisation in
+// place) and the GELU of a mode-0 finish.  Neither crosses CTAs.  A program with these ops has no MoE, q / k norm or
+// MLA op (program_create).
+__global__ void __launch_bounds__(32 + 8 * 32, 1)
+    stream_layernorm_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
+                            uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int spw, int dbg,
+                            int l2_ahead, int gate_ahead, const SpMoe* __restrict__ moe, const SpRes* __restrict__ res,
+                            const SpRope* __restrict__ rope, const SpLn* __restrict__ lnt) {
+  constexpr int NW = 8, GR = 4;
+  constexpr bool MOE = true;
+  pdl_wait();
+#define SP_RESIDUAL 1
+#define SP_ROPE 1
+#define SP_LAYERNORM 1
+#include "program_stream_body.inc"
+#undef SP_LAYERNORM
 #undef SP_ROPE
 #undef SP_RESIDUAL
 }

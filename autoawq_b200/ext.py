@@ -16,6 +16,7 @@ from ._cabi import B200AwqError, check, lib
 __all__ = [
     "gemm_forward_cuda", "dequantize_weights_cuda", "gemv_forward_cuda", "gemmv2_forward_cuda",
     "gemv_forward_cuda_decode", "gemm_forward_cuda_prefill", "layernorm_forward_cuda", "silu_and_mul",
+    "layer_norm", "gelu",
     "topk_softmax", "moe_alig_block_size", "grouped_gemm_forward",
     "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "qk_norm_descriptor",
     "mla_descriptor", "mla_rope", "mla_kv_cache", "mla_k_rope", "mla_q_rope",
@@ -239,6 +240,52 @@ def silu_and_mul(out, gate_up):
     with _DeviceGuard(out.device):
         code = lib.b200awq_silu_and_mul(gate_up.data_ptr(), out.data_ptr(), rows, d, _stream(out.device))
     check(code, "b200awq_silu_and_mul")
+
+
+def layer_norm(x, weight, bias, out, eps):
+    """nn.LayerNorm / F.layer_norm over the last dimension of fp16 x, written into `out` (transformers' CohereLayerNorm
+    with bias=None), in the fixed summation order of include/b200awq.h (b200awq_layer_norm): mean, then the centred
+    variance in a second pass, fp32 math, rounded once.  hidden % 8 == 0 and 16-byte aligned tensors."""
+    _require_cuda(x, weight, bias, out)
+    for t, n in ((x, "x"), (weight, "weight"), (bias, "bias"), (out, "out")):
+        if t is not None and t.dtype != torch.float16:
+            raise B200AwqError(f"b200awq: layer_norm expects float16 tensors ({n} is {t.dtype})")
+    hidden = x.shape[-1]
+    if weight.shape != (hidden,) or (bias is not None and bias.shape != (hidden,)):
+        raise B200AwqError(f"b200awq: layer_norm weight / bias must be [{hidden}]")
+    if not weight.is_contiguous() or (bias is not None and not bias.is_contiguous()):
+        raise B200AwqError("b200awq: layer_norm weight / bias must be contiguous")
+    xc = x if x.is_contiguous() else x.contiguous()
+    rows = xc.numel() // hidden if hidden else 0
+    if not out.is_contiguous() or out.numel() != rows * hidden:
+        raise B200AwqError("b200awq: layer_norm output must be contiguous with x's shape")
+    with _DeviceGuard(x.device):
+        code = lib.b200awq_layer_norm(xc.data_ptr(), hidden, weight.data_ptr(),
+                                      bias.data_ptr() if bias is not None else None, out.data_ptr(), rows, hidden,
+                                      float(eps), _stream(x.device))
+    check(code, "b200awq_layer_norm")
+
+
+_GELU_APPROX = {"none": 0, "tanh": 1}
+
+
+def gelu(out, x, approximate="none"):
+    """out = F.gelu(x, approximate=approximate) on fp16 tensors ("tanh": gelu_pytorch_tanh / GELUTanh, StarCoder2;
+    "none": the exact erf form, MPT and Falcon), in torch's CUDA formulas with fp32 math, rounded once."""
+    _require_cuda(out, x)
+    if approximate not in _GELU_APPROX:
+        raise B200AwqError(f"b200awq: gelu approximate must be 'none' or 'tanh', got {approximate!r}")
+    if x.dtype != torch.float16 or out.dtype != torch.float16:
+        raise B200AwqError("b200awq: gelu expects float16 tensors")
+    if x.shape != out.shape or not x.is_contiguous() or not out.is_contiguous():
+        raise B200AwqError("b200awq: gelu expects contiguous tensors of one shape")
+    n = x.shape[-1] if x.dim() else 1
+    rows = x.numel() // n if n else 0
+    if rows == 0:
+        return
+    with _DeviceGuard(out.device):
+        code = lib.b200awq_gelu(x.data_ptr(), out.data_ptr(), rows, n, _GELU_APPROX[approximate], _stream(out.device))
+    check(code, "b200awq_gelu")
 
 
 def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out):

@@ -59,6 +59,20 @@ With a q LoRA (DeepSeek-V2 / V2.5 / V3, MiniCPM3) the order is: the fused q_a_pr
 (packing.fuse_mla_lora_input), `mla_k_rope`, q_a_layernorm as an RMSNorm on the q_a slice of that linear's output,
 q_b_proj, `mla_q_rope`, kv_a_layernorm on its c_kv slice, kv_b_proj, mla_kv_cache.  At M = 1 the chain is three
 kernel ops of one launch (DESIGN.md 3.5k).
+
+`layer_norm(x, weight, bias, out, eps)` records an nn.LayerNorm (bias None: transformers' CohereLayerNorm) and
+`gelu(out, x, approximate)` an F.gelu ("tanh" or "none").  At M = 1 the LayerNorm runs in the staging of every linear
+that reads its output, as layernorm_forward_cuda's RMSNorm does, and the GELU in the finish of the linear recorded just
+before it (DESIGN.md 3.5l).  Programs built with max_tokens > 1 replay them per op.  The recording order of one segment,
+from one attention call to the next:
+
+  * Command-R (CohereBlock, parallel residual): o + x -> h, gate|up(xn) (gate and up concatenated along N, as
+    packing.fuse_qkv concatenates q, k and v), silu_and_mul, down + h -> x', layer_norm(x') -> xn' (no bias), qkv',
+    rope_kv_cache.  xn and xn' may be one buffer.
+  * StarCoder2 (LlamaLikeBlock): o + x -> h, layer_norm(h), c_fc, gelu("tanh"), c_proj + h -> x', layer_norm(x'), qkv',
+    rope_kv_cache.  Every linear has a bias.
+  * MPT (MPTBlock): the StarCoder2 order with gelu("none"), no biases and no rope_kv_cache: ALiBi stays in the caller's
+    attention, so the segment ends at Wqkv.
 """
 from __future__ import annotations
 
@@ -128,6 +142,41 @@ class DecodeProgram:
             raise B200AwqError("b200awq: silu_and_mul expects contiguous [.., 2d] -> [.., d]")
         self._ops.append(("silu", dict(out=out, gate_up=gate_up, rows=out.numel() // d, d=d)))
         self._keep += [out, gate_up]
+
+    def layer_norm(self, x, weight, bias, out, eps):
+        """ext.layer_norm recorded: out = LayerNorm(x) over the last dimension (bias may be None).  x, weight, bias and
+        out are contiguous float16 tensors, captured by address."""
+        self._no_more()
+        self._dev_of(x)
+        hidden = x.shape[-1]
+        for t in (x, weight, bias, out):
+            if t is None:
+                continue
+            if t.device != self._dev:
+                raise B200AwqError("b200awq: a decode program lives on one device")
+            if t.dtype != torch.float16 or not t.is_contiguous():
+                raise B200AwqError("b200awq: layer_norm expects contiguous float16 tensors")
+        if weight.shape != (hidden,) or (bias is not None and bias.shape != (hidden,)) or out.numel() != x.numel():
+            raise B200AwqError(f"b200awq: layer_norm expects weight / bias [{hidden}] and out shaped like x")
+        self._ops.append(("layer_norm", dict(x=x, weight=weight, bias=bias, out=out, eps=float(eps),
+                                             rows=x.numel() // hidden, hidden=hidden)))
+        self._keep += [t for t in (x, weight, bias, out) if t is not None]
+
+    def gelu(self, out, x, approximate="none"):
+        """ext.gelu recorded: out = F.gelu(x, approximate) ("tanh" or "none") on contiguous float16 tensors of one
+        shape.  Fused when x is the whole output of the linear recorded just before it."""
+        self._no_more()
+        self._dev_of(x)
+        if approximate not in ("none", "tanh"):
+            raise B200AwqError(f"b200awq: gelu approximate must be 'none' or 'tanh', got {approximate!r}")
+        if out.device != self._dev:
+            raise B200AwqError("b200awq: a decode program lives on one device")
+        if (x.dtype != torch.float16 or out.dtype != torch.float16 or x.shape != out.shape or not x.is_contiguous()
+                or not out.is_contiguous()):
+            raise B200AwqError("b200awq: gelu expects contiguous float16 tensors of one shape")
+        n = x.shape[-1]
+        self._ops.append(("gelu", dict(x=x, out=out, approximate=approximate, rows=x.numel() // n, n=n)))
+        self._keep += [x, out]
 
     def gemm_forward_cuda(self, x, qweight, scales, qzeros, split_k_iters=8, bias=None):
         self._no_more()
@@ -546,6 +595,13 @@ class DecodeProgram:
             elif kind == "silu":
                 c.kind, c.M, c.K = _cabi.OP_SILU_AND_MUL, o["rows"], o["d"]
                 c.x, c.y = o["gate_up"].data_ptr(), o["out"].data_ptr()
+            elif kind == "layer_norm":
+                c.kind, c.M, c.K, c.eps = _cabi.OP_LAYER_NORM, o["rows"], o["hidden"], o["eps"]
+                c.x, c.weight, c.y = o["x"].data_ptr(), o["weight"].data_ptr(), o["out"].data_ptr()
+                c.bias = o["bias"].data_ptr() if o["bias"] is not None else None
+            elif kind == "gelu":
+                c.kind = _cabi.OP_GELU_TANH if o["approximate"] == "tanh" else _cabi.OP_GELU
+                c.M, c.K, c.x, c.y = o["rows"], o["n"], o["x"].data_ptr(), o["out"].data_ptr()
             elif kind == "add":
                 c.kind, c.M, c.K = _cabi.OP_ADD, o["M"], o["K"]
                 c.x, c.weight, c.y = o["a"].data_ptr(), o["b"].data_ptr(), o["out"].data_ptr()
@@ -602,7 +658,8 @@ class DecodeProgram:
 
     @property
     def tokens(self) -> int:
-        """Token rows per run (M of the recorded ops; 0 before anything was recorded)."""
+        """Token rows per run (M of the recorded ops, the rows of a norm, silu_and_mul, layer_norm or gelu; 0 before
+        anything was recorded)."""
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
@@ -612,7 +669,8 @@ class DecodeProgram:
     @property
     def kernel_ops(self) -> int:
         """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe / deepseek_moe (gate|up with the routing, down), none per add,
-        rope_kv_cache, mla_rope, mla_kv_cache, mla_k_rope or mla_q_rope (they fold into their producer's epilogue); 0
+        rope_kv_cache, mla_rope, mla_kv_cache, mla_k_rope, mla_q_rope or gelu (they fold into their producer's epilogue)
+        and none per layernorm_forward_cuda, silu_and_mul or layer_norm (they fold into their consumers' staging); 0
         per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
 
@@ -622,7 +680,8 @@ class DecodeProgram:
         call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), 34 + top_k per softmax
         deepseek_moe (sigmoid: 36 + top_k, + 6 with expert groups, + 3 with norm_topk_prob), one torch.add launch per add
         and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache, one b200awq_mla_rope / b200awq_mla_kv
-        / b200awq_mla_k_rope / b200awq_mla_q_rope launch per mla_rope / mla_kv_cache / mla_k_rope / mla_q_rope.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
+        / b200awq_mla_k_rope / b200awq_mla_q_rope launch per mla_rope / mla_kv_cache / mla_k_rope / mla_q_rope, one
+        b200awq_layer_norm / b200awq_gelu launch per layer_norm / gelu.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
         kernel (torch.sort, torch.gather), so the kernel count can be higher."""
         def per_op(kind, o):
             if kind != "moe":
@@ -650,6 +709,10 @@ class DecodeProgram:
                 ext.layernorm_forward_cuda(o["x"], o["weight"], o["out"], o["eps"])
             elif kind == "silu":
                 ext.silu_and_mul(o["out"], o["gate_up"])
+            elif kind == "layer_norm":
+                ext.layer_norm(o["x"], o["weight"], o["bias"], o["out"], o["eps"])
+            elif kind == "gelu":
+                ext.gelu(o["out"], o["x"], o["approximate"])
             elif kind == "moe" and o["ds"] is not None:
                 self._deepseek_moe_replay(o)
             elif kind == "moe" and o["hf"]:

@@ -89,6 +89,30 @@ int b200awq_rmsnorm(const void* x, const void* weight, void* out, int rows, int 
 /* out[r, j] = silu(gate_up[r, j]) * gate_up[r, d + j], j < d  (fp32 math, fp16 in/out) */
 int b200awq_silu_and_mul(const void* gate_up, void* out, int rows, int d, b200awq_stream_t stream);
 
+/* LayerNorm (nn.LayerNorm / F.layer_norm on fp16 rows; transformers' CohereLayerNorm when bias is null): for row r of
+ * x (pitch ldx elements, >= hidden) into the contiguous out[r, :], K = hidden, fp32 math:
+ *   mean = S1 / K                                    S1 = sum of x in the order below
+ *   var  = S2 / K                                    S2 = sum of (x - mean)^2 in the same order (a second pass over the
+ *                                                    row, not E[x^2] - mean^2: rows whose mean is large against their
+ *                                                    spread would cancel in that form)
+ *   r    = rsqrtf(var + eps)
+ *   out  = fp16(((x - mean) * r) * w [+ b])          rounded once; no bias add when bias is null
+ * Every operation is one IEEE fp32 operation (no contraction); r is the device's rsqrtf.  Summation order (both sums):
+ * thread t < 256 takes the chunks of 8 consecutive columns c = 8 t + 2048 p, p = 0, 1, ...; within a chunk the pairs
+ * (c + 2q, c + 2q + 1), q = 0..3, in order: s = s + (v0 + v1) for S1, s = s + (d0 d0 + d1 d1) for S2 (d = x - mean);
+ * the 32 lanes of warp w = t / 32 are summed with the xor butterfly at offsets 16, 8, 4, 2, 1; the 8 warp totals are
+ * added to 0 in ascending w.  Requires hidden % 8 == 0, ldx % 8 == 0 and 16-byte aligned x, weight, bias and out
+ * (else B200AWQ_EUNSUPPORTED); out must not overlap x. */
+int b200awq_layer_norm(const void* x, int64_t ldx, const void* weight, const void* bias, void* out, int rows,
+                       int hidden, float eps, b200awq_stream_t stream);
+
+/* GELU, elementwise over rows x n contiguous fp16 values, fp32 math, rounded once (torch's CUDA formulas):
+ *   approximate = 1 (F.gelu(x, approximate="tanh"), gelu_pytorch_tanh):
+ *       fp16(0.5 x (1 + tanhf(kBeta fma(0.044715, x^3, x)))),  kBeta = fp32(sqrt(2 / pi)), x^3 = (x x) x
+ *   approximate = 0 (F.gelu): fp16((0.5 x) (1 + erff(x fp32(sqrt(1/2)))))
+ * out may not partially overlap x (out == x is fine). */
+int b200awq_gelu(const void* x, void* out, int rows, int n, int approximate, b200awq_stream_t stream);
+
 /* ---- MoE (awq/modules/fused/moe.py:45-171; Mixtral: awq/models/mixtral.py:129-158) ------------------------------
  * b200awq_topk_softmax ............ awq_ext.topk_softmax        moe.py:162-167 (fused_topk)
  * b200awq_moe_align_block_size .... awq_ext.moe_alig_block_size moe.py:131-133
@@ -338,11 +362,28 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     Folding: as MLA_ROPE, each into the finish of the linear recorded immediately before it, packed in mode 3.  The
  *     chain [q_a|kv_a, MLA_K_ROPE, RMSNORM(q_a slice), q_b, MLA_Q_ROPE, RMSNORM(c_kv slice), kv_b, MLA_KV] is three
  *     kernel ops; kv_b stages the c_kv slice of the row two ops back.  The rejections of MLA_ROPE apply, Cq must be a
- *     multiple of 16, two k rotations may not share a k_cache, and a program may not mix MLA_ROPE with these ops. */
+ *     multiple of 16, two k rotations may not share a k_cache, and a program may not mix MLA_ROPE with these ops.
+ *
+ *   LAYER_NORM    : as b200awq_layer_norm: x = input row [K] at pitch ldx, weight [K], bias = [K] or null, y = output
+ *                   [K], eps (Command-R's CohereLayerNorm without a bias; StarCoder2's and MPT's nn.LayerNorm).
+ *     Folding: as RMSNORM, into the staging of every later linear that reads its output (a published row, a slice of
+ *     one, or an external buffer); the first such linear stores y.  Its staging sums x while it stages, takes the
+ *     centred sum of squares from the staged row after a CTA barrier and normalises in place: the stand-alone order
+ *     above, bit for bit.
+ *   GELU / GELU_TANH : as b200awq_gelu with approximate 0 / 1: x = the input [K], y = output [K] (MPT and Falcon use
+ *                   GELU; StarCoder2 GELU_TANH).
+ *     Folding: into the finish of the plain linear recorded immediately before it, whose whole output must be x (as
+ *     an ADD folds): the linear's row publishes fp16(gelu(y)), its y and the op's y are both stored, and the next
+ *     linear copies the published row.  The linear keeps mode-0 packing.
+ *     Both fold at M = 1 only.  B200AWQ_EUNSUPPORTED (the caller replays per op) for any program created with
+ *     max_tokens > 1, a program that also holds MoE, QK_NORM_ROPE_KV or MLA ops, a GELU after anything but a plain
+ *     linear (a glue op, an ADD, a ROPE_KV or MLA finish, a MoE block, a linear that already carries an ADD or a GELU),
+ *     a GELU in place or on part of the linear's output, a later read of that linear's raw y, and a SiLU*mul of a GELU's
+ *     output. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
        B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11, B200AWQ_OP_MLA_K_ROPE = 12,
-       B200AWQ_OP_MLA_Q_ROPE = 13 };
+       B200AWQ_OP_MLA_Q_ROPE = 13, B200AWQ_OP_LAYER_NORM = 14, B200AWQ_OP_GELU = 15, B200AWQ_OP_GELU_TANH = 16 };
 
 typedef struct b200awq_op {
   int32_t kind;

@@ -28,7 +28,9 @@ def _nvcc():
 
 
 def _functions(obj):
-    """mangled name -> SASS text (instructions with encodings, addresses and line comments stripped)"""
+    """mangled name -> SASS text (instructions with encodings, addresses and line comments stripped, runs of blanks
+    collapsed: cuobjdump pads every line to the widest instruction of the whole object, so a new kernel elsewhere in
+    program.cu would otherwise change the text of every entry)"""
     cuobjdump = os.path.join(os.path.dirname(_nvcc()), "cuobjdump")
     out = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
     funcs, name, body = {}, None, []
@@ -39,7 +41,7 @@ def _functions(obj):
                 funcs[name] = "\n".join(body)
             name, body = m.group(1), []
         elif name is not None:
-            body.append(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).strip())
+            body.append(" ".join(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).split()))
     if name is not None:
         funcs[name] = "\n".join(body)
     return funcs
