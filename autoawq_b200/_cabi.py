@@ -64,7 +64,7 @@ class Rope(ctypes.Structure):
 
     _fields_ = [
         ("n_heads", ctypes.c_int32), ("n_kv_heads", ctypes.c_int32), ("head_dim", ctypes.c_int32),
-        ("cache_len", ctypes.c_int32), ("freqs_len", ctypes.c_int32), ("pad_", ctypes.c_int32),
+        ("cache_len", ctypes.c_int32), ("freqs_len", ctypes.c_int32), ("rotary_dim", ctypes.c_int32),
         ("cache_batch_stride", ctypes.c_int64), ("pos", ctypes.c_void_p), ("freqs", ctypes.c_void_p),
         ("q_out", ctypes.c_void_p), ("k_cache", ctypes.c_void_p), ("v_cache", ctypes.c_void_p),
     ]
@@ -166,6 +166,8 @@ SIGNATURES = {
     "b200awq_stream_pack": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int, _c_void_p]),
     "b200awq_stream_pack_rotary": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int, _c_int,
                                             _c_void_p]),
+    "b200awq_stream_pack_partial_rotary": (_c_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_int, _c_int, _c_int,
+                                                    _c_int, _c_int, _c_void_p]),
     "b200awq_program_run": (_c_int, [_c_void_p, _c_void_p, _c_size_t, _c_void_p]),
     "b200awq_program_destroy": (_c_int, [_c_void_p]),
 }

@@ -72,7 +72,7 @@ __global__ void __launch_bounds__(256)
   out[i] = __float2half_rn(g / (1.f + __expf(-g)) * u);
 }
 
-// one thread per (token row, head, pair); rope.cuh has the arithmetic
+// one thread per (token row, head, column pair of rope.cuh's rope_cols); rope.cuh has the arithmetic
 __global__ void __launch_bounds__(256)
     rope_kv_kernel(const __half* __restrict__ qkv, int64_t ldqkv, b200awq_rope_t r, int M) {
   pdl_trigger();
@@ -82,9 +82,13 @@ __global__ void __launch_bounds__(256)
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (pos < 0 || i >= (int64_t)M * heads * half) return;
   const int m = static_cast<int>(i / ((int64_t)heads * half));
-  const int p = static_cast<int>(i - (int64_t)m * heads * half), h = p / half, c = h * r.head_dim + (p - h * half);
+  const int p = static_cast<int>(i - (int64_t)m * heads * half), h = p / half;
+  int lo, hi;
+  rope_cols(r.head_dim, rope_rotary_dim(r), p - h * half, lo, hi);
+  lo += h * r.head_dim;
+  hi += h * r.head_dim;
   const __half* row = qkv + m * ldqkv;
-  rope_pair(r, pos, m, c, row[c], row[c + half]);
+  rope_pair(r, pos, m, lo, hi, row[lo], row[hi]);
 }
 
 // one CTA per (token row, head), one thread per pair (a strided loop past 256 pairs); rope.cuh has the arithmetic and
@@ -103,7 +107,8 @@ __global__ void __launch_bounds__(256)
   const __half* row = qkv + (int64_t)m * ldqkv + (int64_t)h * D;
   const int c0 = h * D;
   if (h >= r.n_heads + r.n_kv_heads) {   // v head: not normalised
-    for (int p = threadIdx.x; p < half; p += blockDim.x) rope_pair(r, pos, m, c0 + p, row[p], row[p + half]);
+    for (int p = threadIdx.x; p < half; p += blockDim.x)
+      rope_pair(r, pos, m, c0 + p, c0 + p + half, row[p], row[p + half]);
     return;
   }
   for (int p = threadIdx.x; p < half; p += blockDim.x) {   // blockDim % 8 == 0: a set's 8 lanes run together
@@ -137,7 +142,8 @@ int rope_validate(const b200awq_rope_t* r, int64_t ldqkv) {
       r->v_cache == nullptr)
     return B200AWQ_EINVAL;
   if (r->n_heads <= 0 || r->n_kv_heads <= 0 || r->head_dim <= 0 || (r->head_dim % 2) != 0 || r->cache_len <= 0 ||
-      r->freqs_len <= 0 || r->cache_batch_stride < (int64_t)r->cache_len * r->n_kv_heads * r->head_dim ||
+      r->rotary_dim < 0 || (r->rotary_dim % 2) != 0 || r->rotary_dim > r->head_dim || r->freqs_len <= 0 ||
+      r->cache_batch_stride < (int64_t)r->cache_len * r->n_kv_heads * r->head_dim ||
       ldqkv < (int64_t)(r->n_heads + 2 * r->n_kv_heads) * r->head_dim)
     return B200AWQ_EINVAL;
   return B200AWQ_OK;

@@ -240,6 +240,8 @@ int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_nor
   const int v = qk_norm_validate(desc, ldqkv);
   if (v != B200AWQ_OK) return v;
   if ((desc->rope.head_dim % 16) != 0) return B200AWQ_EUNSUPPORTED;   // the fixed summation order works in sets of 16
+  if (desc->rope.rotary_dim != 0 && desc->rope.rotary_dim != desc->rope.head_dim)
+    return B200AWQ_EUNSUPPORTED;   // full rotary only: no model pairs q / k norm with partial rotary
   if (M == 0) return B200AWQ_OK;
   return fold(qk_norm_rope_kv(qkv, ldqkv, *desc, M, static_cast<cudaStream_t>(stream)));
 }
@@ -352,15 +354,23 @@ int b200awq_stream_pack(const int32_t* qweight, const void* scales, const int32_
   return fold(stream_pack(qweight, scales, qzeros, out, K, N, group_size, mode, static_cast<cudaStream_t>(stream)));
 }
 
-int b200awq_stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K,
-                               int N, int group_size, int head_dim, b200awq_stream_t stream) {
+int b200awq_stream_pack_partial_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out,
+                                       int K, int N, int group_size, int head_dim, int rotary_dim,
+                                       b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_stream_pack_rotary");
   if (!qweight || !scales || !qzeros || !out || head_dim <= 0) return B200AWQ_EINVAL;
+  if (rotary_dim == 0) rotary_dim = head_dim;
+  if (rotary_dim < 2 || (rotary_dim % 2) != 0 || rotary_dim > head_dim) return B200AWQ_EINVAL;
   if (!shape_ok(1, K, N, group_size)) return B200AWQ_EINVAL;
   if (!stream_format_supported(K, N, group_size, 0) || (head_dim % 16) != 0 || (N % head_dim) != 0)
     return B200AWQ_EUNSUPPORTED;
-  return fold(stream_pack_rotary(qweight, scales, qzeros, out, K, N, group_size, head_dim,
+  return fold(stream_pack_rotary(qweight, scales, qzeros, out, K, N, group_size, head_dim, rotary_dim,
                                  static_cast<cudaStream_t>(stream)));
+}
+
+int b200awq_stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K,
+                               int N, int group_size, int head_dim, b200awq_stream_t stream) {
+  return b200awq_stream_pack_partial_rotary(qweight, scales, qzeros, out, K, N, group_size, head_dim, head_dim, stream);
 }
 
 int b200awq_program_run(b200awq_program_t prog, void* workspace, size_t workspace_bytes, b200awq_stream_t stream) {

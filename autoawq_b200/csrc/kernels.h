@@ -165,7 +165,7 @@ int qk_norm_validate(const struct ::b200awq_qk_norm_rope* q, int64_t ldqkv);
 cudaError_t qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_qk_norm_rope& q, int M,
                             cudaStream_t st);
 cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
-                               int G, int head_dim, cudaStream_t st);
+                               int G, int head_dim, int rotary_dim, cudaStream_t st);
 // B200AWQ_OK, or the code the stand-alone op of kind (B200AWQ_OP_MLA_*) returns for a bad descriptor (host only)
 int mla_validate(const struct ::b200awq_mla* d, int kind);
 cudaError_t mla_rope(const void* row, int64_t ld, const struct ::b200awq_mla& d, int M, cudaStream_t st);

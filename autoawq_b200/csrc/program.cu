@@ -327,15 +327,16 @@ static int sp_pick_spw(int nw, bool moe, size_t xs_bytes) {
 }
 
 cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
-                               int G, int head_dim, cudaStream_t st) {
-  if (!stream_format_supported(K, N, G, 0) || head_dim <= 0 || (head_dim % 16) != 0 || (N % head_dim) != 0)
+                               int G, int head_dim, int rotary_dim, cudaStream_t st) {
+  if (!stream_format_supported(K, N, G, 0) || head_dim <= 0 || (head_dim % 16) != 0 || (N % head_dim) != 0 ||
+      rotary_dim < 2 || (rotary_dim % 2) != 0 || rotary_dim > head_dim)
     return cudaErrorNotSupported;
   const int UK = G < 128 ? G : 128;
   const int64_t total = (int64_t)(N / 16) * (K / UK) * ((UK / 16) * 32 + 12);
   const int cap = prog_sm_count() * 16;
   const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
   stream_pack_rotary_kernel<<<blocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros,
-                                                    static_cast<uint8_t*>(out), K, N, G, head_dim);
+                                                    static_cast<uint8_t*>(out), K, N, G, head_dim, rotary_dim);
   return cudaGetLastError();
 }
 
@@ -614,7 +615,8 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     }
     if (mode[i] == 2)
       e = stream_pack_rotary(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K,
-                             table[i].N, table[i].G, table[i].qkr.rope.head_dim, nullptr);
+                             table[i].N, table[i].G, table[i].qkr.rope.head_dim, rope_rotary_dim(table[i].qkr.rope),
+                             nullptr);
     else
       e = stream_pack(table[i].qw_src, table[i].scales, table[i].qzeros, pr->d_stream + woff[i], table[i].K, table[i].N,
                       table[i].G, mode[i], nullptr);
@@ -918,6 +920,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       if (qkn && (qd->q_norm_weight == nullptr || qd->k_norm_weight == nullptr)) return B200AWQ_EINVAL;
       if (qkn && (!aligned16(qd->q_norm_weight) || !aligned16(qd->k_norm_weight))) return B200AWQ_EUNSUPPORTED;
       const int D = r->head_dim;
+      if (qkn && rope_rotary_dim(*r) != D) return B200AWQ_EUNSUPPORTED;   // q / k norm: full rotary only
       if (op.N != (r->n_heads + 2 * r->n_kv_heads) * D || (D % 16) != 0) return B200AWQ_EUNSUPPORTED;
       // (an ADD or a glue op in between: the op before is not a linear; a MoE block's ops are not plain linears)
       if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty() || table.back().moe != 0)
@@ -1159,7 +1162,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (r.head_dim == 0) continue;
     const auto outs = rope_outs(r);
     const size_t wn = q.q_norm_weight != nullptr ? (size_t)r.head_dim * 2 : 0;   // (null, 0: overlaps nothing)
-    const std::pair<const void*, size_t> ins[4] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * r.head_dim * 4},
+    const std::pair<const void*, size_t> ins[4] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * rope_rotary_dim(r) * 4},
                                                    {q.q_norm_weight, wn}, {q.k_norm_weight, wn}};
     auto hits_out = [&](const void* p, size_t b) {
       for (const auto& o : outs)
@@ -1255,7 +1258,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         for (const auto& w : rope_outs(q.rope))
           if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
         const size_t wn = q.q_norm_weight != nullptr ? (size_t)q.rope.head_dim * 2 : 0;
-        if (hits_out(q.rope.pos, 4) || hits_out(q.rope.freqs, (size_t)q.rope.freqs_len * q.rope.head_dim * 4) ||
+        if (hits_out(q.rope.pos, 4) || hits_out(q.rope.freqs, (size_t)q.rope.freqs_len * rope_rotary_dim(q.rope) * 4) ||
             hits_out(q.q_norm_weight, wn) || hits_out(q.k_norm_weight, wn))
           return B200AWQ_EUNSUPPORTED;
       }

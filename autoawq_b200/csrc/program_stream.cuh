@@ -190,8 +190,8 @@ __device__ __forceinline__ float sp_residual(const SpRes& r, const uint32_t* row
 }
 
 // ROPE_KV folded into a qkv linear's finish (stream_rope_kernel / stream_batch_rope_kernel): one entry per kernel op in a
-// side table, like SpRes.  The op is packed in mode 2 (sp_cols_rot, head_dim = r.head_dim); r.head_dim == 0 on every
-// other op.  The descriptor is the recorded b200awq_rope_t (rope.cuh does the arithmetic).
+// side table, like SpRes.  The op is packed in mode 2 (sp_cols_rot with r.head_dim and r's rotary dim); r.head_dim == 0
+// on every other op.  The descriptor is the recorded b200awq_rope_t (rope.cuh does the arithmetic).
 struct SpRope {
   b200awq_rope_t r;
 };
@@ -247,12 +247,14 @@ __device__ __forceinline__ void sp_cols(int mode, int N, int s, int g, int& lo, 
   }
 }
 
-// mode 2 (a qkv linear whose ROPE_KV folds into its finish): set s of head h = s / (D / 16) holds the RoPE pairs
-// lo = h D + 8 t + g, hi = lo + D / 2 (t = s % (D / 16)), so one lane finishes both columns of a rotation
-__device__ __forceinline__ void sp_cols_rot(int D, int s, int g, int& lo, int& hi) {
+// mode 2 (a qkv linear whose ROPE_KV folds into its finish): set s of head h = s / (D / 16) holds the head's column
+// pairs p = 8 t + g (t = s % (D / 16)) of rope.cuh's rope_cols with R rotated columns (lo = h D + p, hi = lo + D / 2
+// for R = D), so one lane finishes both columns of a rotation
+__device__ __forceinline__ void sp_cols_rot(int D, int R, int s, int g, int& lo, int& hi) {
   const int per_head = D >> 4, h = s / per_head, t = s - h * per_head;
-  lo = h * D + 8 * t + g;
-  hi = lo + (D >> 1);
+  rope_cols(D, R, 8 * t + g, lo, hi);
+  lo += h * D;
+  hi += h * D;
 }
 
 // mode 3 (a q_proj | kv_a_proj_with_mqa linear whose MLA_ROPE folds into its finish): set s holds the adjacent pairs
@@ -298,10 +300,10 @@ __device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, in
     const int ls = t / per_set, r = t - ls * per_set, m = r >> 3, gg = r & 7, hd = (set0 + ls) / per_head;
     const float* keep = part + ((size_t)ls * kst + m) * 16;
     int clo, chi;
-    sp_cols_rot(rp.head_dim, set0 + ls, gg, clo, chi);
+    sp_cols_rot(rp.head_dim, rp.head_dim, set0 + ls, gg, clo, chi);   // (full rotary: program_create checks it)
     const __half a = __float2half_rn(keep[gg]), b = __float2half_rn(keep[gg + 8]);
     if (hd >= hqk) {   // v head: not normalised, only appended
-      rope_pair(rp, rpos, m, clo, a, b);
+      rope_pair(rp, rpos, m, clo, chi, a, b);
       continue;
     }
     const unsigned long long* hp = qn->part + (size_t)m * (N >> 4) + (size_t)hd * per_head;
@@ -384,10 +386,10 @@ __global__ void __launch_bounds__(256)
 __global__ void __launch_bounds__(256)
     stream_pack_rotary_kernel(const int32_t* __restrict__ qweight, const __half* __restrict__ scales,
                               const int32_t* __restrict__ qzeros, uint8_t* __restrict__ out, int K, int N, int G,
-                              int head_dim) {
+                              int head_dim, int rotary_dim) {
   pdl_wait();   // (launched without the PDL attribute: a no-op, kept so the kernel stays safe under one)
   sp_pack(qweight, scales, qzeros, out, K, N, G,
-          [=](int s, int g, int& lo, int& hi) { sp_cols_rot(head_dim, s, g, lo, hi); });
+          [=](int s, int g, int& lo, int& hi) { sp_cols_rot(head_dim, rotary_dim, s, g, lo, hi); });
 }
 
 __global__ void __launch_bounds__(256)

@@ -11,29 +11,55 @@
 
 namespace b200awq {
 
-// One pair (column h D + i and h D + D/2 + i, i < D/2) of token row m; `col` = h D + i.  a, b: the fp16 qkv values.
+// R, the rotated columns of a q / k head (b200awq_rope_t.rotary_dim; 0 means D)
+__host__ __device__ __forceinline__ int rope_rotary_dim(const b200awq_rope_t& r) {
+  return r.rotary_dim != 0 ? r.rotary_dim : r.head_dim;
+}
+
+// The column map of a head (include/b200awq.h, b200awq_rope_t): pair p < D/2 of a head of D columns whose first R are
+// rotated -> its columns (lo, hi) within the head.  p < R/2: the rotated pair (p, p + R/2); p >= R/2: the pass-through
+// pair (R + q, R + q + (D - R)/2) with q = p - R/2.  R = D gives (p, p + D/2).  The stand-alone kernel, the mode-2
+// packer and the mode-2 finishes (program_stream.cuh: sp_cols_rot) all pair columns through this one definition.
+__host__ __device__ __forceinline__ void rope_cols(int D, int R, int p, int& lo, int& hi) {
+  const int hr = R >> 1;
+  if (p < hr) {
+    lo = p;
+    hi = p + hr;
+  } else {
+    lo = p + hr;
+    hi = lo + ((D - R) >> 1);
+  }
+}
+
+// One pair of token row m: columns lo = h D + i and hi = h D + j of head h, paired by rope_cols.  a, b: the fp16 qkv
+// values.  A q / k pair with i < R/2 is rotated; every other pair (the pass-through columns, a v head) is copied.
 // The rotation is torch's complex<float> product (c10 complex operator*=: re = a c - b s, im = a s + b c) with the
 // contraction nvcc gives it there, re = fma(a, c, -(b s)) and im = fma(b, c, a s); explicit intrinsics keep -fmad from
 // changing it.  Torch's loops for other shapes differ in a few elements by one fp16 ulp (DESIGN.md 3.5f;
 // tests/test_gpu_program_rope.py compares against RoPE.forward with that bound).
-__device__ __forceinline__ void rope_pair(const b200awq_rope_t& r, int pos, int m, int col, __half a, __half b) {
-  const int D = r.head_dim, half = D >> 1;
-  const int h = col / D, i = col - h * D;
+__device__ __forceinline__ void rope_pair(const b200awq_rope_t& r, int pos, int m, int lo, int hi, __half a, __half b) {
+  const int D = r.head_dim, hr = rope_rotary_dim(r) >> 1;
+  const int h = lo / D, i = lo - h * D, j = hi - h * D;
   const int H = r.n_heads, KV = r.n_kv_heads;
   if (h >= H + KV) {   // v head: unrotated
     __half* v = static_cast<__half*>(r.v_cache) + (size_t)m * r.cache_batch_stride + ((size_t)pos * KV + (h - H - KV)) * D;
     v[i] = a;
-    v[i + half] = b;
+    v[j] = b;
     return;
   }
-  const float2 cs = reinterpret_cast<const float2*>(r.freqs)[(size_t)pos * half + i];
+  __half* dst = h < H ? static_cast<__half*>(r.q_out) + ((size_t)m * H + h) * D
+                      : static_cast<__half*>(r.k_cache) + (size_t)m * r.cache_batch_stride + ((size_t)pos * KV + (h - H)) * D;
+  if (i >= hr) {       // pass-through pair
+    dst[i] = a;
+    dst[j] = b;
+    return;
+  }
+  const float2 cs = reinterpret_cast<const float2*>(r.freqs)[(size_t)pos * hr + i];
   const float fa = __half2float(a), fb = __half2float(b);
   const float re = __fmaf_rn(fa, cs.x, -__fmul_rn(fb, cs.y));
   const float im = __fmaf_rn(fb, cs.x, __fmul_rn(fa, cs.y));
-  __half* dst = h < H ? static_cast<__half*>(r.q_out) + ((size_t)m * H + h) * D
-                      : static_cast<__half*>(r.k_cache) + (size_t)m * r.cache_batch_stride + ((size_t)pos * KV + (h - H)) * D;
   dst[i] = __float2half_rn(re);
-  dst[i + half] = __float2half_rn(im);
+  dst[j] = __float2half_rn(im);
 }
 
 // the position of this step, or -1 when it is outside the cache / the frequency table (then nothing is written)
@@ -68,8 +94,8 @@ __device__ __forceinline__ float qk_head_sum(int nsets, Partial&& partial) {
   return s;
 }
 
-// Qwen3RMSNorm.forward on one pair of fp16 values (column col = h D + i of token row m, partner col + D / 2) of a q
-// or k head with total sum of squares ss, then rope_pair on the result:
+// Qwen3RMSNorm.forward on one pair of fp16 values (column col = h D + i of token row m, partner col + D / 2; full
+// rotary only) of a q or k head with total sum of squares ss, then rope_pair on the result:
 //   r = rsqrtf(ss * inv_d + eps), x' = fp16(w * fp16(x * r))   (hidden_states * torch.rsqrt(variance + eps), .to(fp16),
 //   weight * it: transformers' Qwen3RMSNorm)
 // inv_d = fp32(1 / D), rounded on the host: torch.mean scales its sum by that factor, and ss * inv_d == ss / D for a
@@ -84,7 +110,7 @@ __device__ __forceinline__ void qk_norm_rope_pair(const b200awq_qk_norm_rope_t& 
   const __half nb = __float2half_rn(__fmul_rn(__half2float(b), r));
   const __half wa = __float2half_rn(__fmul_rn(__half2float(w[i]), __half2float(na)));
   const __half wb = __float2half_rn(__fmul_rn(__half2float(w[i + (D >> 1)]), __half2float(nb)));
-  rope_pair(q.rope, pos, m, col, wa, wb);
+  rope_pair(q.rope, pos, m, col, col + (D >> 1), wa, wb);
 }
 
 // ---- MLA (B200AWQ_OP_MLA_ROPE / _MLA_KV / _MLA_K_ROPE / _MLA_Q_ROPE, include/b200awq.h): the per-pair / per-column

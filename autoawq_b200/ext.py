@@ -288,21 +288,32 @@ def gelu(out, x, approximate="none"):
     check(code, "b200awq_gelu")
 
 
-def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out):
+def _rope_dims(freqs, head_dim):
+    """(D, R) of a rotary table [S_f, R/2] (complex64) or [S_f, R/2, 2] (f32) and the head_dim argument (None: D = R)."""
+    R = 2 * (freqs.shape[1] if freqs.dtype == torch.complex64 else freqs.shape[-2])
+    D = R if head_dim is None else int(head_dim)
+    if D < R or D % 2:
+        raise B200AwqError(f"b200awq: head_dim {D} must be even and at least the table's rotary dim {R}")
+    return D, R
+
+
+def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out, head_dim=None):
     """Checks the tensors of one RoPE + KV-cache append and returns (b200awq_rope_t, qkv as [M, N], M).
 
-    qkv [.., (H + 2 KV) D] f16 (rows at a unit stride, any row pitch); freqs: the fp32 [S_f, D/2, 2] real view of
-    RoPE.freqs_cis (awq/modules/fused/attn.py:29-43) or the complex64 [S_f, D/2] table itself; pos: a device int32
-    tensor of one element; k_cache / v_cache: WindowedCache's contiguous-row f16 [B >= M, S, KV, D] (cache.py:5-31);
-    q_out: contiguous f16 with M H D elements.  n_kv_heads = 0 means n_heads, as WindowedCache sizes it."""
+    qkv [.., (H + 2 KV) D] f16 (rows at a unit stride, any row pitch); freqs: the fp32 [S_f, R/2, 2] real view of
+    RoPE(R, ..).freqs_cis (awq/modules/fused/attn.py:29-43) or the complex64 [S_f, R/2] table itself; pos: a device
+    int32 tensor of one element; k_cache / v_cache: WindowedCache's contiguous-row f16 [B >= M, S, KV, D]
+    (cache.py:5-31); q_out: contiguous f16 with M H D elements.  n_kv_heads = 0 means n_heads, as WindowedCache sizes
+    it.  head_dim: D (None: R, full rotary); when larger than R, only the first R columns of each q / k head are
+    rotated (partial rotary, StableLM) and the rest pass through."""
     _require_cuda(qkv, freqs, pos, k_cache, v_cache, q_out)
     H = int(n_heads)
     KV = int(n_kv_heads) or H
     if freqs.dtype == torch.complex64:
         freqs = torch.view_as_real(freqs)
     if freqs.dtype != torch.float32 or freqs.dim() != 3 or freqs.shape[-1] != 2 or not freqs.is_contiguous():
-        raise B200AwqError("b200awq: freqs must be RoPE.freqs_cis (complex64 [S, D/2]) or its contiguous real view")
-    D = 2 * freqs.shape[1]
+        raise B200AwqError("b200awq: freqs must be RoPE.freqs_cis (complex64 [S, R/2]) or its contiguous real view")
+    D, R = _rope_dims(freqs, head_dim)
     N = (H + 2 * KV) * D
     if qkv.dtype != torch.float16 or qkv.shape[-1] != N:
         raise B200AwqError(f"b200awq: qkv must be float16 [.., (n_heads + 2 n_kv_heads) head_dim = {N}]")
@@ -322,7 +333,7 @@ def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_ou
     if q_out.dtype != torch.float16 or not q_out.is_contiguous() or q_out.numel() != M * H * D:
         raise B200AwqError(f"b200awq: q_out must be a contiguous float16 tensor of {M} x {H} x {D} elements")
     r = _cabi.Rope()
-    r.n_heads, r.n_kv_heads, r.head_dim = H, KV, D
+    r.n_heads, r.n_kv_heads, r.head_dim, r.rotary_dim = H, KV, D, R if R < D else 0
     r.cache_len, r.freqs_len = k_cache.shape[1], freqs.shape[0]
     r.cache_batch_stride = k_cache.stride(0)
     r.pos, r.freqs, r.q_out = pos.data_ptr(), freqs.data_ptr(), q_out.data_ptr()
@@ -339,6 +350,8 @@ def qk_norm_descriptor(rope, q_norm, k_norm, device):
     if q_norm is None or k_norm is None:
         raise B200AwqError("b200awq: give both q_norm and k_norm, or neither")
     D = rope.head_dim
+    if rope.rotary_dim not in (0, D):
+        raise B200AwqError("b200awq: q_norm / k_norm need full rotary (head_dim = 2 freqs.shape[1])")
     ws = []
     for name, n in (("q_norm", q_norm), ("k_norm", k_norm)):
         w = getattr(n, "weight", None)
@@ -357,7 +370,8 @@ def qk_norm_descriptor(rope, q_norm, k_norm, device):
     return d, ws
 
 
-def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None, k_norm=None):
+def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None, k_norm=None,
+                  head_dim=None):
     """RoPE.forward on q and k of the fused qkv output and WindowedCache.update_kv of k and v at position *pos
     (awq/modules/fused/attn.py:243-267): writes q_out [M, H, D] and the row `pos` of cache batch entries 0..M-1, nothing
     else (nothing at all when pos is outside the cache or the frequency table).  pos is read on the device: a captured
@@ -365,13 +379,17 @@ def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_
 
     q_norm / k_norm: Qwen3's two Qwen3RMSNorm modules (attn.py:250-253), both or neither.  With them every q head and
     every k head is normalised per token before the rotation (b200awq_qk_norm_rope_kv; the head's sum of squares in the
-    fixed order of include/b200awq.h); v heads are not."""
+    fixed order of include/b200awq.h); v heads are not.  They need full rotary.
+
+    head_dim: D when the heads are wider than the table's rotary dim R = 2 freqs_cis.shape[1] (StableLM's
+    partial_rotary_factor, freqs_cis = RoPE(R, ..).freqs_cis): columns [0, R) of each q / k head are rotated, columns
+    [R, D) are copied unchanged into q_out and k_cache.  None: D = R."""
     H = int(n_heads)
-    D = (freqs_cis.shape[1] if freqs_cis.dtype == torch.complex64 else freqs_cis.shape[-2]) * 2
+    D, _ = _rope_dims(freqs_cis, head_dim)
     if q_out is None:
         M = qkv.numel() // qkv.shape[-1] if qkv.shape[-1] else 0
         q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
-    r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out)
+    r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim)
     qd, _ = qk_norm_descriptor(r, q_norm, k_norm, qkv.device)
     ld = q2.stride(0) if M > 1 else q2.shape[1]
     with _DeviceGuard(qkv.device):
@@ -654,8 +672,9 @@ def stream_pack(qweight, scales, qzeros, mode: int = 0) -> torch.Tensor:
     return out
 
 
-def stream_pack_rotary(qweight, scales, qzeros, head_dim: int) -> torch.Tensor:
-    """The stream format in mode 2 (include/b200awq.h): RoPE's column pairs (i, i + D/2) of every head share a lane.
+def stream_pack_rotary(qweight, scales, qzeros, head_dim: int, rotary_dim=None) -> torch.Tensor:
+    """The stream format in mode 2 (include/b200awq.h): RoPE's column pairs of every head share a lane - (i, i + D/2)
+    for full rotary, (i, i + R/2) and the pass-through pairs after column R for rotary_dim R < D (None: R = D).
     What a decode program packs a qkv linear into when a ROPE_KV op folds into its finish."""
     _require_cuda(qweight, scales, qzeros)
     _check_w(qweight, torch.int32, "qweight")
@@ -668,9 +687,11 @@ def stream_pack_rotary(qweight, scales, qzeros, head_dim: int) -> torch.Tensor:
         raise B200AwqError(f"b200awq: no stream format for K={K}, N={N}, G={G}")
     out = torch.empty(nbytes, dtype=torch.uint8, device=qweight.device)
     with _DeviceGuard(qweight.device):
-        code = lib.b200awq_stream_pack_rotary(qweight.data_ptr(), scales.data_ptr(), qzeros.data_ptr(), out.data_ptr(),
-                                              K, N, G, int(head_dim), _stream(qweight.device))
-    check(code, f"b200awq_stream_pack_rotary(K={K}, N={N}, G={G}, head_dim={head_dim})")
+        code = lib.b200awq_stream_pack_partial_rotary(qweight.data_ptr(), scales.data_ptr(), qzeros.data_ptr(),
+                                                      out.data_ptr(), K, N, G, int(head_dim),
+                                                      int(rotary_dim or head_dim), _stream(qweight.device))
+    check(code, f"b200awq_stream_pack_partial_rotary(K={K}, N={N}, G={G}, head_dim={head_dim}, "
+                f"rotary_dim={rotary_dim})")
     return out
 
 

@@ -73,6 +73,10 @@ from one attention call to the next:
     rope_kv_cache.  Every linear has a bias.
   * MPT (MPTBlock): the StarCoder2 order with gelu("none"), no biases and no rope_kv_cache: ALiBi stays in the caller's
     attention, so the segment ends at Wqkv.
+  * StableLM (StableLmFuser's LlamaLikeBlock with partial_rotary_factor): o + x -> h, layer_norm(h)
+    (post_attention_layernorm, with bias), gate|up (concatenated along N), silu_and_mul, down + h -> x', layer_norm(x')
+    (next input_layernorm), qkv' (with its bias on StableLM-2), rope_kv_cache(..., head_dim=D) with freqs_cis the
+    table of the R = D x partial_rotary_factor rotated columns.  Four kernel ops, one launch at M = 1 (DESIGN.md 3.5m).
 """
 from __future__ import annotations
 
@@ -220,15 +224,17 @@ class DecodeProgram:
         return out
 
     def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None,
-                      k_norm=None):
+                      k_norm=None, head_dim=None):
         """RoPE.forward(xq, xk, start_pos = *pos, seqlen = 1) + cache.update_kv(xv, xk) on the fused qkv output (q heads,
         then k heads, then v heads, as get_attention_shapes slices it): writes q_out [M, H, D] (allocated when not given,
         and returned) and row *pos of k_cache / v_cache batch entries 0..M-1, nothing when *pos is outside the cache or
         freqs_cis.  freqs_cis: the RoPE module's complex64 [S_f, D/2] table (any rope_theta / scaling it was built with
         applies as is).  q_norm / k_norm: Qwen3's two Qwen3RMSNorm modules (.weight fp16 [D], .variance_epsilon), both
         or neither; with them q and k heads are normalised per head before the rotation (ext.rope_kv_cache), and the
-        fused kernel exchanges the heads' sums of squares across CTAs (DESIGN.md 3.5g).  Partial rotary and ALiBi are
-        not this op: the caller keeps those steps."""
+        fused kernel exchanges the heads' sums of squares across CTAs (DESIGN.md 3.5g).  head_dim: D when it is wider
+        than the table's rotary dim R = 2 freqs_cis.shape[1] (partial rotary, StableLM: freqs_cis = RoPE(R, ..)'s
+        table); columns [R, D) of each q / k head pass through unchanged, still inside the qkv linear's finish
+        (DESIGN.md 3.5m).  ALiBi is not this op: the caller keeps that step."""
         self._no_more()
         self._dev_of(qkv)
         H = int(n_heads)
@@ -236,14 +242,14 @@ class DecodeProgram:
             freqs_cis = torch.view_as_real(freqs_cis)
         if freqs_cis.dtype != torch.float32 or freqs_cis.dim() != 3:
             raise B200AwqError("b200awq: freqs_cis must be RoPE.freqs_cis (complex64 [S, D/2]) or its real view")
-        D = 2 * freqs_cis.shape[1]
+        D, _ = ext._rope_dims(freqs_cis, head_dim)
         M = qkv.numel() // qkv.shape[-1] if qkv.shape[-1] else 0
         if q_out is None:
             q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
         for t in (freqs_cis, pos, k_cache, v_cache, q_out):
             if t.device != self._dev:
                 raise B200AwqError("b200awq: a decode program lives on one device")
-        desc, q2, M = ext.rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out)
+        desc, q2, M = ext.rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim)
         if q2.data_ptr() != qkv.data_ptr():
             raise B200AwqError("b200awq: rope_kv_cache records qkv by address: pass its rows as they are")
         qdesc, norm_w = ext.qk_norm_descriptor(desc, q_norm, k_norm, self._dev)

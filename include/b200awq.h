@@ -284,8 +284,9 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *                   N = (H + 2 KV) D.  As b200awq_rope_kv.
  *     Folding: a ROPE_KV adds no kernel op.  It folds into the finish of the linear recorded immediately before it, whose
  *     whole output must be its qkv: that linear is re-laid-out in stream mode 2 (rotary pairs, below), so the thread that
- *     finishes column i of a head also holds column i + D/2 and rotates the pair in registers.  The linear's y and
- *     published row keep the raw qkv values.  B200AWQ_EUNSUPPORTED (the caller replays per op) when the op before it is
+ *     finishes column i < R/2 of a head also holds column i + R/2 and rotates the pair in registers (a pass-through pair
+ *     is copied).  Partial rotary (rotary_dim < D) folds like full rotary, at M = 1 and at max_tokens > 1.  The
+ *     linear's y and published row keep the raw qkv values.  B200AWQ_EUNSUPPORTED (the caller replays per op) when the op before it is
  *     not a plain linear (a glue op, an ADD, a gate|up whose product SiLU*mul reads, a SPARSE_MOE) or already carries an
  *     ADD, when N != (H + 2 KV) D or D % 16 != 0, or when any other op of the program reads or writes q_out or the
  *     caches.
@@ -294,7 +295,8 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *                   (Qwen3RMSNorm q_norm / k_norm, awq/modules/fused/attn.py:250-253).  x, M, N as ROPE_KV, weight = a
  *                   b200awq_qk_norm_rope_t descriptor (below).  As b200awq_qk_norm_rope_kv.
  *     Folding: exactly ROPE_KV's rules and rejections (on the embedded descriptor), plus B200AWQ_EINVAL for a null norm
- *     weight and B200AWQ_EUNSUPPORTED for one that is not 16-byte aligned or that an op of the program writes.  A head's
+ *     weight and B200AWQ_EUNSUPPORTED for one that is not 16-byte aligned or that an op of the program writes, or for
+ *     partial rotary (rotary_dim not 0 or D).  A head's
  *     sums of squares span sets that other CTAs may finish: every CTA publishes the partials of its sets into a buffer
  *     the program owns, then waits for all partials of each q / k head it finishes (DESIGN.md 3.5g).
  *
@@ -463,28 +465,34 @@ typedef struct b200awq_deepseek_moe {
 int b200awq_deepseek_moe_plan(int E, int top_k, int H, int I, int I_s, int group_size, int sm_count, int* out8);
 
 /* RoPE + KV-cache append of one decode step (awq/modules/fused/attn.py:53-86 RoPE.forward, cache.py:41-46
- * WindowedCache.update_kv).  For token row m < M, head h < H + 2 KV and pair i < D/2, with a = qkv[m, h D + i],
- * b = qkv[m, h D + D/2 + i], (c, s) = freqs[pos, i]:
- *   q head (h < H):   q_out[m, h, i] = fp16(fma(a, c, -(b s))), q_out[m, h, i + D/2] = fp16(fma(b, c, a s))
+ * WindowedCache.update_kv), with partial rotary (StableLM's partial_rotary_factor): only the first R = rotary_dim
+ * columns of a q / k head are rotated, the other D - R pass through.  For token row m < M, head h < H + 2 KV and
+ * rotated pair i < R/2, with a = qkv[m, h D + i], b = qkv[m, h D + R/2 + i], (c, s) = freqs[pos, i]:
+ *   q head (h < H):   q_out[m, h, i] = fp16(fma(a, c, -(b s))), q_out[m, h, i + R/2] = fp16(fma(b, c, a s))
  *   k head:           the same rotation into k_cache[m, pos, h - H, .]
- *   v head:           a, b unrotated into v_cache[m, pos, h - H - KV, .]
+ * and every column R <= j < D of a q / k head, and every column of a v head, is copied unchanged into q_out,
+ * k_cache[m, pos, h - H, j] or v_cache[m, pos, h - H - KV, j].  R = D (rotary_dim 0) is full rotary.
  * (the fp32 complex product of RoPE.forward with the FMA contraction torch's CUDA kernel uses, then .type_as(fp16);
  * torch's loops for some shapes round a few elements differently, within one fp16 ulp of this).
  * Nothing else is written; when *pos is outside [0, min(cache_len, freqs_len)) nothing at all.  The kernel reads *pos
- * on the device, so a captured CUDA graph replays at whatever position the caller stored there. */
+ * on the device, so a captured CUDA graph replays at whatever position the caller stored there.
+ * Column pairs: the kernels handle a head as D/2 column pairs; pair p < R/2 is the rotated pair (p, p + R/2), and pair
+ * p >= R/2 with q = p - R/2 is the pass-through pair (R + q, R + q + (D - R)/2) (v heads: the same pairs, copied).
+ * For R = D that is (p, p + D/2).  Stream mode 2 lays a qkv linear out in these pairs (below). */
 typedef struct b200awq_rope {
   int32_t n_heads, n_kv_heads, head_dim; /* H, KV, D (D % 2 == 0) */
   int32_t cache_len;                     /* S: positions of the cache */
   int32_t freqs_len;                     /* S_f: rows of freqs */
-  int32_t pad_;
+  int32_t rotary_dim;                    /* R: rotated columns per q / k head, even, 2 <= R <= D; 0 means D */
   int64_t cache_batch_stride;            /* elements between two batch entries of k_cache / v_cache (>= S KV D) */
   const int32_t* pos;                    /* device int32[1]: the position written (start_pos) */
-  const float* freqs;                    /* [S_f, D/2, 2] f32 (cos, sin): torch.view_as_real(RoPE.freqs_cis) */
+  const float* freqs;                    /* [S_f, R/2, 2] f32 (cos, sin): torch.view_as_real(RoPE(R, ..).freqs_cis) */
   void* q_out;                           /* [M, H, D] f16 */
   void* k_cache;                         /* [B >= M, S, KV, D] f16 */
   void* v_cache;                         /* [B >= M, S, KV, D] f16 */
 } b200awq_rope_t;
-/* ldqkv: row pitch of qkv in elements (>= (H + 2 KV) D).  `rope` is a host pointer, read at the call. */
+/* ldqkv: row pitch of qkv in elements (>= (H + 2 KV) D).  `rope` is a host pointer, read at the call.
+ * B200AWQ_EINVAL for an odd, negative or larger-than-D rotary_dim. */
 int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream);
 
 /* Qwen3's q_norm / k_norm, then RoPE + KV-cache append (awq/modules/fused/attn.py:250-253, then as b200awq_rope_kv).
@@ -495,7 +503,8 @@ int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, 
  * then the rotation and stores of b200awq_rope_kv on x'.  v heads are not normalised.  Summation order: set t of a head
  * (t < D/16) holds the pairs (8 t + g, 8 t + g + D/2), g < 8; s_g = a_g^2 + b_g^2; the set partial is the xor
  * butterfly of the 8 s_g at offsets 4, 2, 1; the head total is the sum of the D/16 set partials in ascending t.
- * Requires D % 16 == 0.  Nothing is written when *pos is outside [0, min(cache_len, freqs_len)). */
+ * Requires D % 16 == 0 and full rotary (rope.rotary_dim 0 or D; else B200AWQ_EUNSUPPORTED).  Nothing is written when
+ * *pos is outside [0, min(cache_len, freqs_len)). */
 typedef struct b200awq_qk_norm_rope {
   b200awq_rope_t rope;
   const void* q_norm_weight;             /* [D] f16 */
@@ -610,8 +619,9 @@ int b200awq_comm_destroy(b200awq_comm_t comm);
  * the unit's scales / zeros), the buffer is set-major, so any partition of the work is a contiguous byte range.
  * mode 0: set s = columns 16 s .. 16 s + 15; mode 1 (a fused gate|up linear): gate column j and up column j share
  * a lane, so SiLU*mul happens in the producer; mode 2 (a qkv linear followed by ROPE_KV, b200awq_stream_pack_rotary):
- * set s of head h = s / (D / 16) pairs column h D + 8 t + g with h D + D/2 + 8 t + g (t = s % (D / 16)), so RoPE's
- * rotation partners share a lane (requires D % 16 == 0 and N % D == 0); mode 3 (a q_proj | kv_a_proj_with_mqa linear
+ * set s of head h = s / (D / 16) holds the column pairs p = 8 t + g (t = s % (D / 16)) of b200awq_rope_t's pairing,
+ * lo = h D + p, hi = lo + D/2 for full rotary (R = D), so RoPE's rotation partners share a lane (requires D % 16 == 0
+ * and N % D == 0; R even, 2 <= R <= D, with no alignment: a set may hold rotated and pass-through pairs); mode 3 (a q_proj | kv_a_proj_with_mqa linear
  * followed by MLA_ROPE, MLA_K_ROPE or MLA_Q_ROPE, adjacent pairs): set s pairs column 16 s + 2 g with 16 s + 2 g + 1, so MLA's interleaved rotation
  * partners share a lane (b200awq_stream_pack with mode 3).  Requires N % 16 == 0, K % 128 == 0, G in
  * {32, 64} or G % 128 == 0.  b200awq_stream_bytes returns 0 for unsupported shapes; the byte count is the same for
@@ -621,6 +631,11 @@ int b200awq_stream_pack(const int32_t* qweight, const void* scales, const int32_
                         int group_size, int mode, b200awq_stream_t stream);
 int b200awq_stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K,
                                int N, int group_size, int head_dim, b200awq_stream_t stream);
+/* Mode 2 for partial rotary: rotary_dim R (even, 2 <= R <= head_dim; 0 means head_dim).  b200awq_stream_pack_rotary is
+ * this with R = head_dim. */
+int b200awq_stream_pack_partial_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out,
+                                       int K, int N, int group_size, int head_dim, int rotary_dim,
+                                       b200awq_stream_t stream);
 
 #ifdef __cplusplus
 }
