@@ -224,26 +224,47 @@ int b200awq_gelu(const void* x, void* out, int rows, int n, int approximate, b20
   return fold(gelu(x, out, (int64_t)rows * n, approximate, static_cast<cudaStream_t>(stream)));
 }
 
-int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream) {
-  NvtxScope nvtx_("b200awq_rope_kv");
-  if (qkv == nullptr || M < 0) return B200AWQ_EINVAL;
+static int rope_kv_call(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, int T, cudaStream_t st) {
+  if (qkv == nullptr || M < 0 || T < 1 || (M % T) != 0) return B200AWQ_EINVAL;
   const int v = rope_validate(rope, ldqkv);
   if (v != B200AWQ_OK) return v;
   if (M == 0) return B200AWQ_OK;
-  return fold(rope_kv(qkv, ldqkv, *rope, M, static_cast<cudaStream_t>(stream)));
+  return fold(rope_kv(qkv, ldqkv, *rope, M, T, st));
 }
 
-int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
-                            b200awq_stream_t stream) {
-  NvtxScope nvtx_("b200awq_qk_norm_rope_kv");
-  if (qkv == nullptr || M < 0) return B200AWQ_EINVAL;
+int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_rope_kv");
+  return rope_kv_call(qkv, ldqkv, rope, M, 1, static_cast<cudaStream_t>(stream));
+}
+
+int b200awq_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, int T,
+                        b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_rope_kv_seq");
+  return rope_kv_call(qkv, ldqkv, rope, M, T, static_cast<cudaStream_t>(stream));
+}
+
+static int qk_norm_rope_kv_call(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M, int T,
+                                cudaStream_t st) {
+  if (qkv == nullptr || M < 0 || T < 1 || (M % T) != 0) return B200AWQ_EINVAL;
   const int v = qk_norm_validate(desc, ldqkv);
   if (v != B200AWQ_OK) return v;
   if ((desc->rope.head_dim % 16) != 0) return B200AWQ_EUNSUPPORTED;   // the fixed summation order works in sets of 16
   if (desc->rope.rotary_dim != 0 && desc->rope.rotary_dim != desc->rope.head_dim)
     return B200AWQ_EUNSUPPORTED;   // full rotary only: no model pairs q / k norm with partial rotary
   if (M == 0) return B200AWQ_OK;
-  return fold(qk_norm_rope_kv(qkv, ldqkv, *desc, M, static_cast<cudaStream_t>(stream)));
+  return fold(qk_norm_rope_kv(qkv, ldqkv, *desc, M, T, st));
+}
+
+int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
+                            b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_qk_norm_rope_kv");
+  return qk_norm_rope_kv_call(qkv, ldqkv, desc, M, 1, static_cast<cudaStream_t>(stream));
+}
+
+int b200awq_qk_norm_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M, int T,
+                                b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_qk_norm_rope_kv_seq");
+  return qk_norm_rope_kv_call(qkv, ldqkv, desc, M, T, static_cast<cudaStream_t>(stream));
 }
 
 // the MLA ops' common checks; M <= 8 (a decode step's token rows); the row must hold N = n columns at pitch ld

@@ -147,8 +147,10 @@ struct ProgOp {
   const void* raw_y = nullptr;
   const void* res_ext = nullptr;
   int res_op = -1;
-  // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights
+  // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights;
+  // rope_T: tokens per sequence (ROPE_KV_SEQ / QK_NORM_ROPE_KV_SEQ: the op's K; 1 for ROPE_KV)
   b200awq_qk_norm_rope_t qkr = {};
+  int rope_T = 1;
   // an MLA_ROPE (mla_kind 1), MLA_KV (2), MLA_K_ROPE (3) or MLA_Q_ROPE (4) folded into the finish
   b200awq_mla_t mla = {};
   int mla_kind = 0;
@@ -195,7 +197,7 @@ struct FoldedProgram {
 // knob 9) or the 8-warp kernel of the program's features; M > 1: the batched kernels at MT = sb_mt(M).  Side tables:
 // the M = 1 kernels from kKernMoe on take SpMoe (null without MoE blocks), from kKernResidual on SpRes, from kKernRope on
 // SpRope, kKernLayerNorm SpLn (and none of the later tables), from kKernQkNorm on SpQkNorm, kKernDeepseekMoe, kKernMla and kKernMlaLora SpDsk, and the last two SpMla; the
-// batched ones take SpRes from kKernBatchResidual2 on, SpRope from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2
+// batched ones take SpRes from kKernBatchResidual2 on, SpRopeSeq from kKernBatchRope2 on, SpQkNorm from kKernBatchQkNorm2
 // on.  The Qwen3-MoE, DeepSeek-MoE and MLA kernels take every table, with empty entries where an op has no add,
 // rotation or norm.
 enum ProgKernel {
@@ -232,6 +234,7 @@ struct Program {
   SpDsk* d_dsk = nullptr;
   SpRes* d_res = nullptr;
   SpRope* d_rope = nullptr;
+  SpRopeSeq* d_rope_seq = nullptr;   // (the batched kernels' table in place of SpRope)
   SpQkNorm* d_qkn = nullptr;
   unsigned long long* d_qkn_part = nullptr;
   SpMla* d_mla = nullptr;
@@ -242,7 +245,7 @@ struct Program {
   Program& operator=(const Program&) = delete;
   ~Program() {
     for (void* d : std::initializer_list<void*>{d_sp_ops, d_stream, d_cta, d_rows, d_state, d_moe, d_xlog, d_dsk, d_res,
-                                                d_rope, d_qkn, d_qkn_part, d_mla, d_ln})
+                                                d_rope, d_rope_seq, d_qkn, d_qkn_part, d_mla, d_ln})
       cudaFree(d);
   }
 };
@@ -687,10 +690,17 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
     }
     e = upload(&pr->d_res, rd);
   }
-  if (e == cudaSuccess && takes_rope) {
+  if (e == cudaSuccess && takes_rope && M == 1) {
     std::vector<SpRope> rp(n);
     for (int i = 0; i < n; ++i) rp[i].r = table[i].qkr.rope;   // (head_dim 0: no rotation)
     e = upload(&pr->d_rope, rp);
+  } else if (e == cudaSuccess && takes_rope) {
+    std::vector<SpRopeSeq> rp(n);
+    for (int i = 0; i < n; ++i) {
+      rp[i].r = table[i].qkr.rope;
+      rp[i].T = table[i].rope_T;
+    }
+    e = upload(&pr->d_rope_seq, rp);
   }
   if (e == cudaSuccess && takes_qkn) {
     // the partials of op i live at [M][N_i / 16] words from its offset; zero tags are never a run's (sp_tag >= 1)
@@ -908,10 +918,15 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     const b200awq_op_t& op = ops[i];
     if (M < 0) M = op.M;
     if (op.M != M) return B200AWQ_EUNSUPPORTED;
-    if (op.kind == B200AWQ_OP_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV) {
+    if (op.kind == B200AWQ_OP_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV || op.kind == B200AWQ_OP_ROPE_KV_SEQ ||
+        op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ) {
       // RoPE + cache append, folded into the finish of the linear recorded just before it (whose whole output is qkv);
-      // QK_NORM_ROPE_KV: the same op on its embedded descriptor, with q / k normalised first
-      const bool qkn = op.kind == B200AWQ_OP_QK_NORM_ROPE_KV;
+      // QK_NORM_ROPE_KV: the same op on its embedded descriptor, with q / k normalised first.  The _SEQ kinds: T = op.K
+      // tokens per sequence (M = B T rows; T > 1 needs M > 1, so only the batched kernels see it)
+      const bool qkn = op.kind == B200AWQ_OP_QK_NORM_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ;
+      const bool seq = op.kind == B200AWQ_OP_ROPE_KV_SEQ || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ;
+      const int T = seq ? op.K : 1;
+      if (T < 1 || (M % T) != 0) return B200AWQ_EINVAL;
       const b200awq_qk_norm_rope_t* qd = qkn ? static_cast<const b200awq_qk_norm_rope_t*>(op.weight) : nullptr;
       const b200awq_rope_t* r = qkn ? (qd != nullptr ? &qd->rope : nullptr) : static_cast<const b200awq_rope_t*>(op.weight);
       if (op.x == nullptr) return B200AWQ_EINVAL;
@@ -929,6 +944,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       if (op.x != pv.y || op.N != pv.N || (M > 1 && op.ldx != op.N)) return B200AWQ_EUNSUPPORTED;
       if (qkn) pv.qkr = *qd;
       else pv.qkr.rope = *r;
+      pv.rope_T = T;
       continue;
     }
     if (op.kind == B200AWQ_OP_MLA_ROPE || op.kind == B200AWQ_OP_MLA_KV || op.kind == B200AWQ_OP_MLA_K_ROPE ||
@@ -1151,8 +1167,11 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   // other op of the program may read or write them, nor write the position / frequency table the finish reads; the
   // producer must not be a gate|up whose product a SiLU*mul reads (its row would hold silu(gate) * up).
   // QK_NORM_ROPE_KV: its two norm weights are reads like the position and the frequency table.
-  auto rope_outs = [&](const b200awq_rope_t& r) {
-    const size_t cache = ((size_t)(M - 1) * r.cache_batch_stride + (size_t)r.cache_len * r.n_kv_heads * r.head_dim) * 2;
+  // (the caches: B = M / T entries)
+  auto rope_outs = [&](const ProgOp& p) {
+    const b200awq_rope_t& r = p.qkr.rope;
+    const size_t cache =
+        ((size_t)(M / p.rope_T - 1) * r.cache_batch_stride + (size_t)r.cache_len * r.n_kv_heads * r.head_dim) * 2;
     return std::array<std::pair<const void*, size_t>, 3>{
         {{r.q_out, (size_t)M * r.n_heads * r.head_dim * 2}, {r.k_cache, cache}, {r.v_cache, cache}}};
   };
@@ -1160,7 +1179,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     const b200awq_qk_norm_rope_t& q = table[ri].qkr;
     const b200awq_rope_t& r = q.rope;
     if (r.head_dim == 0) continue;
-    const auto outs = rope_outs(r);
+    const auto outs = rope_outs(table[ri]);
     const size_t wn = q.q_norm_weight != nullptr ? (size_t)r.head_dim * 2 : 0;   // (null, 0: overlaps nothing)
     const std::pair<const void*, size_t> ins[4] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * rope_rotary_dim(r) * 4},
                                                    {q.q_norm_weight, wn}, {q.k_norm_weight, wn}};
@@ -1187,7 +1206,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       if (o.prologue == kProSilu && overlaps(o.src, src_bytes(o), table[ri].y, y_bytes(table[ri])))
         return B200AWQ_EUNSUPPORTED;   // a SiLU*mul of the qkv output: the producer would be a mode-1 gate|up
       if (j != ri && o.qkr.rope.head_dim != 0)   // another ROPE_KV: its outputs are writes, its inputs reads
-        for (const auto& w : rope_outs(o.qkr.rope))
+        for (const auto& w : rope_outs(o))
           if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
     }
     for (const Glue& gl : glues)
@@ -1255,7 +1274,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         return B200AWQ_EUNSUPPORTED;
       if (o.qkr.rope.head_dim != 0) {   // a ROPE_KV: its outputs are writes, its inputs reads
         const b200awq_qk_norm_rope_t& q = o.qkr;
-        for (const auto& w : rope_outs(q.rope))
+        for (const auto& w : rope_outs(o))
           if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
         const size_t wn = q.q_norm_weight != nullptr ? (size_t)q.rope.head_dim * 2 : 0;
         if (hits_out(q.rope.pos, 4) || hits_out(q.rope.freqs, (size_t)q.rope.freqs_len * rope_rotary_dim(q.rope) * 4) ||
@@ -1385,12 +1404,12 @@ cudaError_t program_run(Program* p, cudaStream_t st) {
     case kKernBatchResidual2: return batch(stream_batch_residual_kernel<2>, p->d_res);
     case kKernBatchResidual4: return batch(stream_batch_residual_kernel<4>, p->d_res);
     case kKernBatchResidual8: return batch(stream_batch_residual_kernel<8>, p->d_res);
-    case kKernBatchRope2: return batch(stream_batch_rope_kernel<2>, p->d_res, p->d_rope);
-    case kKernBatchRope4: return batch(stream_batch_rope_kernel<4>, p->d_res, p->d_rope);
-    case kKernBatchRope8: return batch(stream_batch_rope_kernel<8>, p->d_res, p->d_rope);
-    case kKernBatchQkNorm2: return batch(stream_batch_qknorm_kernel<2>, p->d_res, p->d_rope, p->d_qkn);
-    case kKernBatchQkNorm4: return batch(stream_batch_qknorm_kernel<4>, p->d_res, p->d_rope, p->d_qkn);
-    case kKernBatchQkNorm8: return batch(stream_batch_qknorm_kernel<8>, p->d_res, p->d_rope, p->d_qkn);
+    case kKernBatchRope2: return batch(stream_batch_rope_kernel<2>, p->d_res, p->d_rope_seq);
+    case kKernBatchRope4: return batch(stream_batch_rope_kernel<4>, p->d_res, p->d_rope_seq);
+    case kKernBatchRope8: return batch(stream_batch_rope_kernel<8>, p->d_res, p->d_rope_seq);
+    case kKernBatchQkNorm2: return batch(stream_batch_qknorm_kernel<2>, p->d_res, p->d_rope_seq, p->d_qkn);
+    case kKernBatchQkNorm4: return batch(stream_batch_qknorm_kernel<4>, p->d_res, p->d_rope_seq, p->d_qkn);
+    case kKernBatchQkNorm8: return batch(stream_batch_qknorm_kernel<8>, p->d_res, p->d_rope_seq, p->d_qkn);
   }
   return cudaErrorInvalidValue;   // (not reached: stream_build sets one of the above)
 }

@@ -152,14 +152,14 @@ __global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
 #undef SP_RESIDUAL
 }
 
-// batched programs with a ROPE_KV op (SpRope, program_stream.cuh): the residual kernel plus RoPE + cache append in a
-// mode-2 finish (token row m writes cache batch m)
+// batched programs with a ROPE_KV or ROPE_KV_SEQ op (SpRopeSeq, program_stream.cuh): the residual kernel plus RoPE +
+// cache append in a mode-2 finish (token row m = b T + t writes cache entry b at position *pos + t; T = 1: entry m)
 template <int MT>
 __global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
     stream_batch_rope_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
                              uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int M, int spw,
                              int lmax, int nu_max, int dbg, const SpRes* __restrict__ res,
-                             const SpRope* __restrict__ rope) {
+                             const SpRopeSeq* __restrict__ rope) {
   pdl_wait();
 #define SP_RESIDUAL 1
 #define SP_ROPE 1
@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(32 + kSbWarps * 32, 1)
     stream_batch_qknorm_kernel(const SpOp* __restrict__ ops, const uint32_t* __restrict__ cta_all, int n_ops,
                                uint32_t* __restrict__ rows, int row_stride, int* __restrict__ state, int M, int spw,
                                int lmax, int nu_max, int dbg, const SpRes* __restrict__ res,
-                               const SpRope* __restrict__ rope, const SpQkNorm* __restrict__ qkn) {
+                               const SpRopeSeq* __restrict__ rope, const SpQkNorm* __restrict__ qkn) {
   pdl_wait();
 #define SP_RESIDUAL 1
 #define SP_ROPE 1

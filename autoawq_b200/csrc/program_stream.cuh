@@ -195,6 +195,15 @@ __device__ __forceinline__ float sp_residual(const SpRes& r, const uint32_t* row
 struct SpRope {
   b200awq_rope_t r;
 };
+// The batched kernels' entry (stream_batch_rope_kernel / stream_batch_qknorm_kernel): SpRope's descriptor and T, the
+// tokens per sequence of the op (B200AWQ_OP_ROPE_KV_SEQ's b200awq_op_t.K; 1 for ROPE_KV): token row m = b T + t writes
+// cache entry b at position *r.pos + t (rope.cuh: rope_row_pos).  A table of its own: a wider SpRope would change the
+// M = 1 kernels' table stride, and they only run T = 1.
+struct SpRopeSeq {
+  b200awq_rope_t r;
+  int T;
+  int pad_;
+};
 
 // QK_NORM_ROPE_KV folded into a qkv linear's finish (stream_qknorm_kernel / stream_batch_qknorm_kernel): one entry per
 // kernel op in a side table next to SpRope (whose descriptor is the embedded b200awq_rope_t); part == null on every op
@@ -291,9 +300,11 @@ struct SpLn {
 
 // phase (b) of a QK_NORM_ROPE_KV finish (SpQkNorm above), shared by the M = 1 and the batched body: item t of this
 // thread (t = ct, ct + nthr, ... < nsets * per_set; per_set = 8 M) is lane group t % 8 of token row (t % per_set) / 8 of
-// local set t / per_set, whose fp16 pair phase (a) kept in part[(ls * kst + m) * 16 + g] / [.. + 8].
-__device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, int rpos, const float* part, int kst, int ct,
-                                          int nthr, int nsets, int per_set, int set0, int N, uint32_t tag, int op) {
+// local set t / per_set, whose fp16 pair phase (a) kept in part[(ls * kst + m) * 16 + g] / [.. + 8].  T >= 1 (the
+// batched body): p0 = *pos and T tokens per sequence, each row's entry and position from rope.cuh's rope_row_pos (a row
+// outside the cache writes nothing); T = 0 (the M = 1 body): p0 is the step's position, already checked, entry m.
+__device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, int p0, int T, const float* part, int kst,
+                                          int ct, int nthr, int nsets, int per_set, int set0, int N, uint32_t tag, int op) {
   const b200awq_rope_t& rp = qn->q.rope;
   const int per_head = rp.head_dim >> 4, hqk = rp.n_heads + rp.n_kv_heads;
   for (int t = ct; t < nsets * per_set; t += nthr) {
@@ -302,13 +313,15 @@ __device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, in
     int clo, chi;
     sp_cols_rot(rp.head_dim, rp.head_dim, set0 + ls, gg, clo, chi);   // (full rotary: program_create checks it)
     const __half a = __float2half_rn(keep[gg]), b = __float2half_rn(keep[gg + 8]);
+    int e = m, rpos = p0;
+    if (T > 0 && (rpos = rope_row_pos(rp, p0, T, m, e)) < 0) continue;
     if (hd >= hqk) {   // v head: not normalised, only appended
-      rope_pair(rp, rpos, m, clo, chi, a, b);
+      rope_pair(rp, rpos, m, e, clo, chi, a, b);
       continue;
     }
     const unsigned long long* hp = qn->part + (size_t)m * (N >> 4) + (size_t)hd * per_head;
     const float ss = qk_head_sum(per_head, [&](int u) { return sp_qk_partial(hp + u, tag, op); });
-    qk_norm_rope_pair(qn->q, qn->inv_d, rpos, m, clo, a, b, ss);
+    qk_norm_rope_pair(qn->q, qn->inv_d, rpos, m, e, clo, a, b, ss);
   }
 }
 

@@ -297,7 +297,15 @@ def _rope_dims(freqs, head_dim):
     return D, R
 
 
-def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out, head_dim=None):
+def _seq_len(seq_len):
+    """T of a rope_kv_cache call: None means 1 (one token per sequence)."""
+    T = 1 if seq_len is None else int(seq_len)
+    if T < 1:
+        raise B200AwqError(f"b200awq: seq_len must be at least 1, got {T}")
+    return T
+
+
+def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out, head_dim=None, seq_len=None):
     """Checks the tensors of one RoPE + KV-cache append and returns (b200awq_rope_t, qkv as [M, N], M).
 
     qkv [.., (H + 2 KV) D] f16 (rows at a unit stride, any row pitch); freqs: the fp32 [S_f, R/2, 2] real view of
@@ -305,8 +313,10 @@ def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_ou
     int32 tensor of one element; k_cache / v_cache: WindowedCache's contiguous-row f16 [B >= M, S, KV, D]
     (cache.py:5-31); q_out: contiguous f16 with M H D elements.  n_kv_heads = 0 means n_heads, as WindowedCache sizes
     it.  head_dim: D (None: R, full rotary); when larger than R, only the first R columns of each q / k head are
-    rotated (partial rotary, StableLM) and the rest pass through."""
+    rotated (partial rotary, StableLM) and the rest pass through.  seq_len: T tokens per sequence (None: 1); M must be
+    a multiple of T and the caches need B >= M / T entries."""
     _require_cuda(qkv, freqs, pos, k_cache, v_cache, q_out)
+    T = _seq_len(seq_len)
     H = int(n_heads)
     KV = int(n_kv_heads) or H
     if freqs.dtype == torch.complex64:
@@ -321,9 +331,11 @@ def rope_descriptor(qkv, freqs, pos, k_cache, v_cache, n_heads, n_kv_heads, q_ou
     if q2.stride(-1) != 1:
         raise B200AwqError("b200awq: qkv rows must have a unit stride")
     M = q2.shape[0]
+    if M % T:
+        raise B200AwqError(f"b200awq: {M} qkv rows are not a whole number of sequences of seq_len {T}")
     for name, c in (("k_cache", k_cache), ("v_cache", v_cache)):
-        if c.dtype != torch.float16 or c.dim() != 4 or tuple(c.shape[2:]) != (KV, D) or c.shape[0] < M:
-            raise B200AwqError(f"b200awq: {name} must be float16 [B >= {M}, S, {KV}, {D}]")
+        if c.dtype != torch.float16 or c.dim() != 4 or tuple(c.shape[2:]) != (KV, D) or c.shape[0] < M // T:
+            raise B200AwqError(f"b200awq: {name} must be float16 [B >= {M // T}, S, {KV}, {D}]")
         if c.stride(3) != 1 or c.stride(2) != D or c.stride(1) != KV * D:
             raise B200AwqError(f"b200awq: {name} must have contiguous [S, KV, D] entries")
     if k_cache.shape[1] != v_cache.shape[1] or k_cache.stride(0) != v_cache.stride(0):
@@ -371,7 +383,7 @@ def qk_norm_descriptor(rope, q_norm, k_norm, device):
 
 
 def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None, k_norm=None,
-                  head_dim=None):
+                  head_dim=None, seq_len=None):
     """RoPE.forward on q and k of the fused qkv output and WindowedCache.update_kv of k and v at position *pos
     (awq/modules/fused/attn.py:243-267): writes q_out [M, H, D] and the row `pos` of cache batch entries 0..M-1, nothing
     else (nothing at all when pos is outside the cache or the frequency table).  pos is read on the device: a captured
@@ -383,23 +395,34 @@ def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_
 
     head_dim: D when the heads are wider than the table's rotary dim R = 2 freqs_cis.shape[1] (StableLM's
     partial_rotary_factor, freqs_cis = RoPE(R, ..).freqs_cis): columns [0, R) of each q / k head are rotated, columns
-    [R, D) are copied unchanged into q_out and k_cache.  None: D = R."""
+    [R, D) are copied unchanged into q_out and k_cache.  None: D = R.
+
+    seq_len: T tokens per sequence at consecutive positions (RoPE.forward(xq, xk, start_pos = *pos, seqlen = T) and
+    update_kv of rows *pos .. *pos + T - 1; None or 1: one token, as above).  qkv is then the reference's xqkv view
+    [B, T, N] or its rows [B T, N]; row m = b T + t is token t of sequence b at position *pos + t and writes q_out row m
+    and cache entry b (the caches need B entries).  A row whose position is outside the cache or the table writes
+    nothing; the rest of the step still does (b200awq_rope_kv_seq)."""
     H = int(n_heads)
+    T = _seq_len(seq_len)
     D, _ = _rope_dims(freqs_cis, head_dim)
     if q_out is None:
         M = qkv.numel() // qkv.shape[-1] if qkv.shape[-1] else 0
         q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
-    r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim)
+    r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim, T)
     qd, _ = qk_norm_descriptor(r, q_norm, k_norm, qkv.device)
     ld = q2.stride(0) if M > 1 else q2.shape[1]
     with _DeviceGuard(qkv.device):
-        if qd is None:
-            code = lib.b200awq_rope_kv(q2.data_ptr(), ld, r, M, _stream(qkv.device))
-        else:
-            code = lib.b200awq_qk_norm_rope_kv(q2.data_ptr(), ld, qd, M, _stream(qkv.device))
-    name = "b200awq_rope_kv" if qd is None else "b200awq_qk_norm_rope_kv"
-    check(code, f"{name}(M={M}, H={H}, KV={r.n_kv_heads}, D={D})")
+        code, name = rope_kv_call(q2.data_ptr(), ld, r, qd, M, T, _stream(qkv.device))
+    check(code, f"{name}(M={M}, T={T}, H={H}, KV={r.n_kv_heads}, D={D})")
     return q_out
+
+
+def rope_kv_call(qkv_ptr, ld, desc, qdesc, M, T, stream):
+    """The C entry of one RoPE + KV-cache append: b200awq_rope_kv (qdesc None) or b200awq_qk_norm_rope_kv, their
+    _seq forms for T > 1.  Returns (code, entry name)."""
+    name = ("b200awq_rope_kv" if qdesc is None else "b200awq_qk_norm_rope_kv") + ("_seq" if T > 1 else "")
+    args = (qkv_ptr, ld, desc if qdesc is None else qdesc, M) + ((T,) if T > 1 else ())
+    return getattr(lib, name)(*args, stream), name
 
 
 def _rows(x, N, name):

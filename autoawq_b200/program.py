@@ -48,6 +48,13 @@ the cache row written, and attention reads them directly (DESIGN.md 3.5f).  `pos
 in place between runs (or graph replays).  With `q_norm=` / `k_norm=` (Qwen3's Qwen3RMSNorm modules) it also applies
 Qwen3's per-head q / k norm first, still inside the qkv linear's finish (DESIGN.md 3.5g).
 
+A step of T tokens per sequence (speculative verification of a T-token draft, multi-token prediction, a prompt
+continued in chunks) records the same segment with M = B T rows, in the reference's order (xqkv viewed as [B, T, N]):
+o + x -> h, norm2(h), gate|up, silu, down + h -> out, norm1'(out), qkv', `rope_kv_cache(..., seq_len=T)`.  Row
+m = b T + t is token t of sequence b at position *pos + t, written to cache entry b; attention (with the causal mask
+over the new tokens) stays the caller's, between programs.  `DecodeProgram(max_tokens=B T)` runs the segment as one
+launch (B T <= 8; DESIGN.md 3.5n); advance `pos` by T per step.
+
 `mla_rope(qkva, freqs, pos, k_cache, ...)` and `mla_kv_cache(kv, pos, k_cache, v_cache, ...)` record the glue of
 DeepSeek-V2 / V3 multi-head latent attention (transformers' DeepseekV2Attention / DeepseekV3Attention, no q LoRA) in
 transformers' order: the fused q_proj | kv_a_proj_with_mqa linear (packing.fuse_mla_input), mla_rope, kv_a_layernorm as
@@ -224,7 +231,7 @@ class DecodeProgram:
         return out
 
     def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None,
-                      k_norm=None, head_dim=None):
+                      k_norm=None, head_dim=None, seq_len=None):
         """RoPE.forward(xq, xk, start_pos = *pos, seqlen = 1) + cache.update_kv(xv, xk) on the fused qkv output (q heads,
         then k heads, then v heads, as get_attention_shapes slices it): writes q_out [M, H, D] (allocated when not given,
         and returned) and row *pos of k_cache / v_cache batch entries 0..M-1, nothing when *pos is outside the cache or
@@ -234,7 +241,13 @@ class DecodeProgram:
         fused kernel exchanges the heads' sums of squares across CTAs (DESIGN.md 3.5g).  head_dim: D when it is wider
         than the table's rotary dim R = 2 freqs_cis.shape[1] (partial rotary, StableLM: freqs_cis = RoPE(R, ..)'s
         table); columns [R, D) of each q / k head pass through unchanged, still inside the qkv linear's finish
-        (DESIGN.md 3.5m).  ALiBi is not this op: the caller keeps that step."""
+        (DESIGN.md 3.5m).  ALiBi is not this op: the caller keeps that step.
+
+        seq_len: T tokens per sequence (None or 1: one, as above): RoPE.forward(xq, xk, start_pos = *pos, seqlen = T)
+        and update_kv of rows *pos .. *pos + T - 1.  qkv is the step's [B, T, N] (the reference's xqkv view) or [B T, N]
+        output; row m = b T + t writes q_out row m and cache entry b at position *pos + t, and the caches need B
+        entries.  A program built with max_tokens >= B T folds it into the qkv linear's finish as well (DESIGN.md
+        3.5n); advance pos by T between runs."""
         self._no_more()
         self._dev_of(qkv)
         H = int(n_heads)
@@ -249,12 +262,13 @@ class DecodeProgram:
         for t in (freqs_cis, pos, k_cache, v_cache, q_out):
             if t.device != self._dev:
                 raise B200AwqError("b200awq: a decode program lives on one device")
-        desc, q2, M = ext.rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim)
+        T = ext._seq_len(seq_len)
+        desc, q2, M = ext.rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim, T)
         if q2.data_ptr() != qkv.data_ptr():
             raise B200AwqError("b200awq: rope_kv_cache records qkv by address: pass its rows as they are")
         qdesc, norm_w = ext.qk_norm_descriptor(desc, q_norm, k_norm, self._dev)
         self._ops.append(("rope", dict(qkv=q2, freqs=freqs_cis, pos=pos, k_cache=k_cache, v_cache=v_cache, q_out=q_out,
-                                       H=H, KV=desc.n_kv_heads, M=M, N=q2.shape[1],
+                                       H=H, KV=desc.n_kv_heads, M=M, N=q2.shape[1], T=T,
                                        ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc, qdesc=qdesc)))
         self._keep += [qkv, q2, freqs_cis, pos, k_cache, v_cache, q_out] + norm_w
         return q_out
@@ -615,12 +629,12 @@ class DecodeProgram:
                 c.kind, c.M, c.K, c.N = (_cabi.OP_DEEPSEEK_MOE if o["ds"] is not None else
                                          _cabi.OP_QWEN3_MOE if o["hf"] else _cabi.OP_SPARSE_MOE), o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
-            elif kind == "rope" and o["qdesc"] is not None:
-                c.kind, c.M, c.N, c.ldx = _cabi.OP_QK_NORM_ROPE_KV, o["M"], o["N"], o["ldx"]
-                c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["qdesc"])
             elif kind == "rope":
-                c.kind, c.M, c.N, c.ldx = _cabi.OP_ROPE_KV, o["M"], o["N"], o["ldx"]
-                c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["desc"])
+                qk, seq = o["qdesc"] is not None, o["T"] > 1     # (seq: kinds 17 / 18, with K = T)
+                c.kind = ((_cabi.OP_QK_NORM_ROPE_KV_SEQ if seq else _cabi.OP_QK_NORM_ROPE_KV) if qk else
+                          (_cabi.OP_ROPE_KV_SEQ if seq else _cabi.OP_ROPE_KV))
+                c.M, c.N, c.ldx, c.K = o["M"], o["N"], o["ldx"], o["T"] if seq else 0
+                c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["qdesc"] if qk else o["desc"])
             elif kind in _MLA_OPS:
                 c.kind, c.M, c.N, c.ldx = _MLA_OPS[kind], o["M"], o["N"], o["ldx"]
                 c.x, c.weight = o["row"].data_ptr(), ctypes.addressof(o["desc"])
@@ -727,14 +741,11 @@ class DecodeProgram:
                 self._moe_replay(o)
             elif kind == "add":
                 torch.add(o["a"], o["b"], out=o["out"])
-            elif kind == "rope" and o["qdesc"] is not None:
-                with ext._DeviceGuard(dev):
-                    code = lib.b200awq_qk_norm_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["qdesc"], o["M"], ext._stream(dev))
-                check(code, "b200awq_qk_norm_rope_kv")
             elif kind == "rope":
                 with ext._DeviceGuard(dev):
-                    code = lib.b200awq_rope_kv(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["M"], ext._stream(dev))
-                check(code, "b200awq_rope_kv")
+                    code, name = ext.rope_kv_call(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["qdesc"], o["M"], o["T"],
+                                                  ext._stream(dev))
+                check(code, name)
             elif kind in _MLA_OPS:
                 ext._mla_call(getattr(lib, "b200awq_" + kind), o["row"], o["desc"], o["M"], "b200awq_" + kind,
                               *o.get("pre", ()))

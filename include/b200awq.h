@@ -381,11 +381,22 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     max_tokens > 1, a program that also holds MoE, QK_NORM_ROPE_KV or MLA ops, a GELU after anything but a plain
  *     linear (a glue op, an ADD, a ROPE_KV or MLA finish, a MoE block, a linear that already carries an ADD or a GELU),
  *     a GELU in place or on part of the linear's output, a later read of that linear's raw y, and a SiLU*mul of a GELU's
- *     output. */
+ *     output.
+ *
+ *   ROPE_KV_SEQ / QK_NORM_ROPE_KV_SEQ : ROPE_KV / QK_NORM_ROPE_KV for a step of T tokens per sequence (speculative
+ *                   verification, multi-token prediction, a prompt continued in chunks): the record of kind 6 / 7 with
+ *                   K = T (1 <= T, M % T == 0).  Row m = b T + t of x is token t of sequence b at position *pos + t; it
+ *                   writes q_out row m and cache entry b.  As b200awq_rope_kv_seq / b200awq_qk_norm_rope_kv_seq.
+ *     Folding: the rules and rejections of kind 6 / 7 on the embedded descriptor, with the cache extent of the hazard
+ *     checks taken over B = M / T entries.  B200AWQ_EINVAL for T < 1 or M % T != 0.  T = 1 folds exactly as kind 6 / 7.
+ *     T > 1 means M > 1, so it folds only in a program created with max_tokens >= M, in the segments where ROPE_KV
+ *     folds at M > 1 (RMSNorm staging, residual adds, partial rotary, q / k norm); with LAYER_NORM, GELU, MLA or MoE
+ *     ops the program replays per op (B200AWQ_EUNSUPPORTED), as it does for ROPE_KV at M > 1. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
        B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11, B200AWQ_OP_MLA_K_ROPE = 12,
-       B200AWQ_OP_MLA_Q_ROPE = 13, B200AWQ_OP_LAYER_NORM = 14, B200AWQ_OP_GELU = 15, B200AWQ_OP_GELU_TANH = 16 };
+       B200AWQ_OP_MLA_Q_ROPE = 13, B200AWQ_OP_LAYER_NORM = 14, B200AWQ_OP_GELU = 15, B200AWQ_OP_GELU_TANH = 16,
+       B200AWQ_OP_ROPE_KV_SEQ = 17, B200AWQ_OP_QK_NORM_ROPE_KV_SEQ = 18 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -514,6 +525,20 @@ typedef struct b200awq_qk_norm_rope {
 } b200awq_qk_norm_rope_t;
 int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
                             b200awq_stream_t stream);
+
+/* b200awq_rope_kv / b200awq_qk_norm_rope_kv for a step of T tokens per sequence at consecutive positions
+ * (RoPE.forward(xq, xk, start_pos, seqlen = T) and WindowedCache.update_kv over start_pos .. start_pos + T - 1 for
+ * each of B = M / T sequences; speculative verification, multi-token prediction, a prompt continued in chunks, prefill
+ * at *pos = 0).  Row m = b T + t of qkv is token t of sequence b at position p = *pos + t: it gets exactly the
+ * rotation, copies and norm b200awq_rope_kv / b200awq_qk_norm_rope_kv give one row at p, written to q_out[m] and to
+ * k_cache / v_cache entry b, row p (so the caches need B entries).  A row whose p is outside [0, min(cache_len,
+ * freqs_len)) writes nothing, not even its q_out row; the other rows of the step still write.  Any M (a prefill of T up
+ * to cache_len tokens included).  T = 1 is b200awq_rope_kv / b200awq_qk_norm_rope_kv.  The descriptors are the same;
+ * B200AWQ_EINVAL for T < 1 or M % T != 0, otherwise the return codes of those entries. */
+int b200awq_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, int T,
+                        b200awq_stream_t stream);
+int b200awq_qk_norm_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M, int T,
+                                b200awq_stream_t stream);
 
 /* MLA (DeepSeek-V2 / V3 multi-head latent attention, no q LoRA): the glue between the fused q_proj | kv_a_proj_with_mqa
  * linear and attention, in transformers' arithmetic (DeepseekV2Attention.forward, DeepseekV3Attention.forward with
