@@ -8,7 +8,10 @@
 // and accumulated in fp32 (fhfma: exact product, one fp32 rounding) - one FMA per
 // weight plus 5/8 op of LOP3/SHF unpack.  Zero-point and scale are applied once per (group, column):
 //     y[n] += s[g,n] * ( 2^24 * sum_k x[k] q[k,n]  -  z[g,n] * sum_k x[k] )
-// The cross-thread / cross-CTA (split-K) reduction is fp32; the result is rounded to fp16 once.
+// The cross-thread / cross-CTA (split-K) reduction is fp32; the result is rounded to fp16 once.  Because the fold
+// subtracts z * sum_k x[k] from sums that were already rounded, their rounding error scales with z * sum |x|, not with
+// |q - z| |x|: the bound these kernels meet is oracle/llm_data.forward_tolerance, family code-fold (Omega = 15), and the
+// tensor-pipe GEMVs below family offset-fold (Omega = 1039).
 #include <cuda.h>
 
 #include <atomic>
@@ -38,7 +41,10 @@ constexpr float kScaleB = 1048576.0f;   // 2^20: code read through mask 0x00f000
 // mask 0x00f000f0 as 1024 + 16 q (kind B).  No per-weight zero/scale work at all: the tensor core
 // accumulates S = sum_k x_k * (1024 + c*q_k) in fp32 and the epilogue folds, per (group, column),
 //     y += s * ( S - (1024 + c*z) * sum_k x_k ) / c ,     c = 1 (kind A) or 16 (kind B).
-// The 1024 offset costs ~10 bits of the fp32 accumulator's 24: the result keeps >= 13 bits, above fp16.
+// The 1024 offset costs ~10 bits of the fp32 accumulator's 24, and those bits are lost relative to 1039 sum |x|, not to
+// the result: the error is about 2^-24 r 1039 sum_g s_g sum_{k in g} |x_k| (r roundings on the fold path), which does
+// not shrink with the weights - a column of all-zero weights under large activations comes back small but non-zero.
+// oracle/llm_data.forward_tolerance (family offset-fold) states the bound and derives r.
 //
 // Warp tile = 256 columns x 16 rows: lane (g = lane/4, tig = lane%4) loads uint4 (4 words, 32 columns) at
 // word column 4g for rows 4 tig .. 4 tig + 3 (128 B contiguous per row across the 8 g's).  MMA (w, t)

@@ -7,18 +7,17 @@ x M in {1, 2, 4, 8, 16, 64, 300} (GEMV kernels, the small-batch kernel, the wgmm
 checkpoint layouts (GEMM / GEMV / GEMVFast), through the awq_ext / awq_v2_ext operator surface.  The oracle is
 the fp64 contraction of the bit-exact dequantised weights, evaluated on a strided sample of output columns
 (every 61st + the edges: the full product at M = 300 on 4096x28672 would be 70 GFLOP of fp64 per case; each
-column is an independent dot product, so a column sample checks the same arithmetic); tolerances as in
-test_gpu_parity.py.
+column is an independent dot product, so a column sample checks the same arithmetic); each route held to
+oracle/llm_data.forward_tolerance of the kernel family that ran (oracle/llm_data.*_route_family).
 """
 import numpy as np
 import pytest
 import torch
 
 from oracle import awq_oracle as O
+from oracle import llm_data as L
 
 pytestmark = pytest.mark.gpu
-
-RTOL, WR_GEMV, WR_TC = 2.0**-10, 2.0**-11, 2.0**-16
 SHAPES = [
     ("8b.qkv", 4096, 6144), ("8b.o", 4096, 4096), ("8b.gate_up", 4096, 28672), ("8b.down", 14336, 4096),
     ("70b8.qkv", 8192, 1280), ("70b8.o", 1024, 8192), ("70b8.gate_up", 8192, 7168), ("70b8.down", 3584, 8192),
@@ -35,13 +34,9 @@ def _t(a):
     return torch.from_numpy(np.ascontiguousarray(a)).to(_dev())
 
 
-def _check(y, x, w, cols, wr, what):
-    ref = O.gemm_f64(x, w[:, cols])
-    bud = np.abs(x.astype(np.float64)) @ np.abs(w[:, cols].astype(np.float64))
-    got = np.asarray(y, dtype=np.float64)[:, cols]
-    tol = RTOL * np.abs(ref) + wr * bud + 1e-6
-    bad = np.abs(got - ref) > tol
-    assert not bad.any(), f"{what}: {bad.sum()} / {bad.size} outside tolerance, max err {np.abs(got - ref).max():.3e}"
+def _check(y, x, w, scales, cols, family, what):
+    case = dict(w=w[:, cols], scales=np.asarray(scales)[:, cols], group_size=G, bias=None)
+    L.check_forward(np.asarray(y)[:, cols], x, case, family, what)
 
 
 @pytest.fixture(scope="module")
@@ -72,18 +67,17 @@ def test_all_layouts_all_m_vs_oracle(ext, name, K, N):
     for M in MS:
         x = rng.standard_normal((M, K)).astype(np.float16)
         xt = _t(x)
-        wr = WR_GEMV if M <= 64 else WR_TC   # the M <= 64 kernels fold scale / zero per group in fp32 (see parity tests)
         y = awq_ext.gemm_forward_cuda(xt, qw, sc, qz, 8)
         assert tuple(y.shape) == (M, N)
-        _check(y.cpu().numpy(), x, w, cols, wr, f"{name} gemm layout M={M}")
+        _check(y.cpu().numpy(), x, w, s, cols, L.gemm_route_family(M, K, N, G), f"{name} gemm layout M={M}")
         if M > 8:
             yv = awq_ext.gemmv2_forward_cuda(xt, tvw, tvs, tvz, G, 8)
             yf = awq_v2_ext.gemm_forward_cuda_prefill(xt.unsqueeze(0), tfw, tfs, tfz)[0]
         else:
             yv = awq_ext.gemv_forward_cuda(xt, tvw, tvs, tvz, G)
             yf = awq_v2_ext.gemv_forward_cuda_decode(xt.unsqueeze(1), tfw, tfs, tfz, M, N, K, G)[:, 0]
-        _check(yv.cpu().numpy(), x, w, cols, WR_GEMV if M <= 8 else WR_TC, f"{name} gemv layout M={M}")
-        _check(yf.cpu().numpy(), x, wfast, cols, WR_GEMV, f"{name} fast layout M={M}")
+        _check(yv.cpu().numpy(), x, w, s, cols, L.gemv_route_family(M, K), f"{name} gemv layout M={M}")
+        _check(yf.cpu().numpy(), x, wfast, fs, cols, L.fast_route_family(M), f"{name} fast layout M={M}")
     # dequant at this shape, bit-exact on the sampled columns and on a full-row digest
     wd = awq_ext.dequantize_weights_cuda(qw, sc, qz, 0, 0, 0, False).cpu().numpy()
     assert np.array_equal(wd.view(np.uint16), w.view(np.uint16)), f"{name}: dequant not bit-exact"
