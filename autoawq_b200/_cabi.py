@@ -80,6 +80,13 @@ class QkNormRope(ctypes.Structure):
     ]
 
 
+class RopeOffset(ctypes.Structure):
+    """b200awq_rope_offset_t (include/b200awq.h): the descriptor of b200awq_rope_kv_offset and of a ROPE_KV_OFFSET op's
+    `weight` (null norm weights: no q / k norm)."""
+
+    _fields_ = [("qk", QkNormRope), ("rot_offset", ctypes.c_void_p)]
+
+
 class Mla(ctypes.Structure):
     """b200awq_mla_t (include/b200awq.h): the descriptor of b200awq_mla_rope / _kv / _k_rope / _q_rope and of an
     MLA_ROPE / MLA_KV / MLA_K_ROPE / MLA_Q_ROPE op's `weight`."""
@@ -98,7 +105,7 @@ OP_RMSNORM, OP_LINEAR_GEMM, OP_SILU_AND_MUL, OP_SPARSE_MOE, OP_ADD, OP_ROPE_KV =
 OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE, OP_DEEPSEEK_MOE, OP_MLA_ROPE, OP_MLA_KV = 7, 8, 9, 10, 11
 OP_MLA_K_ROPE, OP_MLA_Q_ROPE = 12, 13
 OP_LAYER_NORM, OP_GELU, OP_GELU_TANH = 14, 15, 16
-OP_ROPE_KV_SEQ, OP_QK_NORM_ROPE_KV_SEQ = 17, 18
+OP_ROPE_KV_SEQ, OP_QK_NORM_ROPE_KV_SEQ, OP_ROPE_KV_OFFSET = 17, 18, 19
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one
@@ -133,6 +140,7 @@ SIGNATURES = {
     "b200awq_rope_kv_seq": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Rope), _c_int, _c_int, _c_void_p]),
     "b200awq_qk_norm_rope_kv_seq": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(QkNormRope), _c_int, _c_int,
                                              _c_void_p]),
+    "b200awq_rope_kv_offset": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(RopeOffset), _c_int, _c_int, _c_void_p]),
     "b200awq_mla_rope": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
     "b200awq_mla_kv": (_c_int, [_c_void_p, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),
     "b200awq_mla_k_rope": (_c_int, [_c_void_p, _c_i64, _c_i64, ctypes.POINTER(Mla), _c_int, _c_void_p]),

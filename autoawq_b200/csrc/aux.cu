@@ -73,17 +73,19 @@ __global__ void __launch_bounds__(256)
 }
 
 // one thread per (token row, head, column pair of rope.cuh's rope_cols); rope.cuh has the arithmetic.  T tokens per
-// sequence: token row m writes cache entry m / T at position *pos + m % T (rope_row_pos)
+// sequence: token row m writes cache entry m / T at position *pos + m % T, rotated at that position plus off[m / T]
+// (off null: plus 0; rope_row_pos)
 __global__ void __launch_bounds__(256)
-    rope_kv_kernel(const __half* __restrict__ qkv, int64_t ldqkv, b200awq_rope_t r, int M, int T) {
+    rope_kv_kernel(const __half* __restrict__ qkv, int64_t ldqkv, b200awq_rope_t r, int M, int T,
+                   const int32_t* __restrict__ off) {
   pdl_trigger();
   pdl_wait();
   const int half = r.head_dim >> 1, heads = r.n_heads + 2 * r.n_kv_heads;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)M * heads * half) return;
   const int m = static_cast<int>(i / ((int64_t)heads * half));
-  int e;
-  const int pos = rope_row_pos(r, *r.pos, T, m, e);
+  int e, rot;
+  const int pos = rope_row_pos(r, *r.pos, T, off, m, e, rot);
   if (pos < 0) return;
   const int p = static_cast<int>(i - (int64_t)m * heads * half), h = p / half;
   int lo, hi;
@@ -91,29 +93,30 @@ __global__ void __launch_bounds__(256)
   lo += h * r.head_dim;
   hi += h * r.head_dim;
   const __half* row = qkv + m * ldqkv;
-  rope_pair(r, pos, m, e, lo, hi, row[lo], row[hi]);
+  rope_pair(r, pos, rot, m, e, lo, hi, row[lo], row[hi]);
 }
 
 // one CTA per (token row, head), one thread per pair (a strided loop past 256 pairs); rope.cuh has the arithmetic and
-// the summation order of the head's sum of squares (set partials into shared memory, then summed in set order).  T as
-// rope_kv_kernel
+// the summation order of the head's sum of squares (set partials into shared memory, then summed in set order).  T and
+// off as rope_kv_kernel
 __global__ void __launch_bounds__(256)
     qk_norm_rope_kv_kernel(const __half* __restrict__ qkv, int64_t ldqkv, b200awq_qk_norm_rope_t q, float inv_d,
-                           int M, int T) {
+                           int M, int T, const int32_t* __restrict__ off) {
   extern __shared__ float qk_part[];   // [D / 16] set partials of this head
   pdl_trigger();
   pdl_wait();
   const b200awq_rope_t& r = q.rope;
   const int D = r.head_dim, half = D >> 1, heads = r.n_heads + 2 * r.n_kv_heads;
   const int m = static_cast<int>(blockIdx.x / heads), h = static_cast<int>(blockIdx.x - (unsigned)m * heads);
-  int e;
-  const int pos = rope_row_pos(r, *r.pos, T, m, e);
-  if (pos < 0 || m >= M) return;
+  if (m >= M) return;
+  int e, rot;
+  const int pos = rope_row_pos(r, *r.pos, T, off, m, e, rot);
+  if (pos < 0) return;
   const __half* row = qkv + (int64_t)m * ldqkv + (int64_t)h * D;
   const int c0 = h * D;
   if (h >= r.n_heads + r.n_kv_heads) {   // v head: not normalised
     for (int p = threadIdx.x; p < half; p += blockDim.x)
-      rope_pair(r, pos, m, e, c0 + p, c0 + p + half, row[p], row[p + half]);
+      rope_pair(r, pos, rot, m, e, c0 + p, c0 + p + half, row[p], row[p + half]);
     return;
   }
   for (int p = threadIdx.x; p < half; p += blockDim.x) {   // blockDim % 8 == 0: a set's 8 lanes run together
@@ -123,7 +126,7 @@ __global__ void __launch_bounds__(256)
   __syncthreads();
   const float ss = qk_head_sum(D >> 4, [&](int t) { return qk_part[t]; });
   for (int p = threadIdx.x; p < half; p += blockDim.x)
-    qk_norm_rope_pair(q, inv_d, pos, m, e, c0 + p, row[p], row[p + half], ss);
+    qk_norm_rope_pair(q, inv_d, pos, rot, m, e, c0 + p, row[p], row[p + half], ss);
 }
 
 int qk_norm_validate(const b200awq_qk_norm_rope_t* q, int64_t ldqkv) {
@@ -135,12 +138,12 @@ int qk_norm_validate(const b200awq_qk_norm_rope_t* q, int64_t ldqkv) {
 }
 
 cudaError_t qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t& q, int M, int T,
-                            cudaStream_t st) {
+                            const int32_t* off, cudaStream_t st) {
   const int half = q.rope.head_dim / 2, heads = q.rope.n_heads + 2 * q.rope.n_kv_heads;
   const int threads = half < 256 ? half : 256;
   return launch_kernel(qk_norm_rope_kv_kernel, dim3(static_cast<unsigned>((int64_t)M * heads)), dim3(threads),
                        (size_t)(q.rope.head_dim / 16) * sizeof(float), st, reinterpret_cast<const __half*>(qkv), ldqkv, q,
-                       1.f / static_cast<float>(q.rope.head_dim), M, T);
+                       1.f / static_cast<float>(q.rope.head_dim), M, T, off);
 }
 
 int rope_validate(const b200awq_rope_t* r, int64_t ldqkv) {
@@ -155,10 +158,11 @@ int rope_validate(const b200awq_rope_t* r, int64_t ldqkv) {
   return B200AWQ_OK;
 }
 
-cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t& r, int M, int T, cudaStream_t st) {
+cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t& r, int M, int T, const int32_t* off,
+                    cudaStream_t st) {
   const int64_t n = (int64_t)M * (r.n_heads + 2 * r.n_kv_heads) * (r.head_dim / 2);
   return launch_kernel(rope_kv_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st,
-                       reinterpret_cast<const __half*>(qkv), ldqkv, r, M, T);
+                       reinterpret_cast<const __half*>(qkv), ldqkv, r, M, T, off);
 }
 
 // one thread per (token row, column pair) of the q_proj | kv_a_proj_with_mqa row; rope.cuh has the arithmetic

@@ -224,27 +224,28 @@ int b200awq_gelu(const void* x, void* out, int rows, int n, int approximate, b20
   return fold(gelu(x, out, (int64_t)rows * n, approximate, static_cast<cudaStream_t>(stream)));
 }
 
-static int rope_kv_call(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, int T, cudaStream_t st) {
+static int rope_kv_call(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, int T, const int32_t* off,
+                        cudaStream_t st) {
   if (qkv == nullptr || M < 0 || T < 1 || (M % T) != 0) return B200AWQ_EINVAL;
   const int v = rope_validate(rope, ldqkv);
   if (v != B200AWQ_OK) return v;
   if (M == 0) return B200AWQ_OK;
-  return fold(rope_kv(qkv, ldqkv, *rope, M, T, st));
+  return fold(rope_kv(qkv, ldqkv, *rope, M, T, off, st));
 }
 
 int b200awq_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_rope_kv");
-  return rope_kv_call(qkv, ldqkv, rope, M, 1, static_cast<cudaStream_t>(stream));
+  return rope_kv_call(qkv, ldqkv, rope, M, 1, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int b200awq_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_rope_t* rope, int M, int T,
                         b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_rope_kv_seq");
-  return rope_kv_call(qkv, ldqkv, rope, M, T, static_cast<cudaStream_t>(stream));
+  return rope_kv_call(qkv, ldqkv, rope, M, T, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 static int qk_norm_rope_kv_call(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M, int T,
-                                cudaStream_t st) {
+                                const int32_t* off, cudaStream_t st) {
   if (qkv == nullptr || M < 0 || T < 1 || (M % T) != 0) return B200AWQ_EINVAL;
   const int v = qk_norm_validate(desc, ldqkv);
   if (v != B200AWQ_OK) return v;
@@ -252,19 +253,30 @@ static int qk_norm_rope_kv_call(const void* qkv, int64_t ldqkv, const b200awq_qk
   if (desc->rope.rotary_dim != 0 && desc->rope.rotary_dim != desc->rope.head_dim)
     return B200AWQ_EUNSUPPORTED;   // full rotary only: no model pairs q / k norm with partial rotary
   if (M == 0) return B200AWQ_OK;
-  return fold(qk_norm_rope_kv(qkv, ldqkv, *desc, M, T, st));
+  return fold(qk_norm_rope_kv(qkv, ldqkv, *desc, M, T, off, st));
 }
 
 int b200awq_qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M,
                             b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_qk_norm_rope_kv");
-  return qk_norm_rope_kv_call(qkv, ldqkv, desc, M, 1, static_cast<cudaStream_t>(stream));
+  return qk_norm_rope_kv_call(qkv, ldqkv, desc, M, 1, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int b200awq_qk_norm_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M, int T,
                                 b200awq_stream_t stream) {
   NvtxScope nvtx_("b200awq_qk_norm_rope_kv_seq");
-  return qk_norm_rope_kv_call(qkv, ldqkv, desc, M, T, static_cast<cudaStream_t>(stream));
+  return qk_norm_rope_kv_call(qkv, ldqkv, desc, M, T, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int b200awq_rope_kv_offset(const void* qkv, int64_t ldqkv, const b200awq_rope_offset_t* desc, int M, int T,
+                           b200awq_stream_t stream) {
+  NvtxScope nvtx_("b200awq_rope_kv_offset");
+  if (desc == nullptr || desc->rot_offset == nullptr) return B200AWQ_EINVAL;
+  const b200awq_qk_norm_rope_t& q = desc->qk;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (q.q_norm_weight == nullptr && q.k_norm_weight == nullptr)   // no q / k norm
+    return rope_kv_call(qkv, ldqkv, &q.rope, M, T, desc->rot_offset, st);
+  return qk_norm_rope_kv_call(qkv, ldqkv, &q, M, T, desc->rot_offset, st);
 }
 
 // the MLA ops' common checks; M <= 8 (a decode step's token rows); the row must hold N = n columns at pitch ld

@@ -158,13 +158,15 @@ cudaError_t layer_norm(const void* x, int64_t ldx, const void* w, const void* b,
 cudaError_t gelu(const void* x, void* out, int64_t n, int approximate, cudaStream_t st);
 // B200AWQ_OK, or the code b200awq_rope_kv returns for a bad descriptor / qkv pitch (host only)
 int rope_validate(const struct ::b200awq_rope* r, int64_t ldqkv);
-// T tokens per sequence (M % T == 0): token row m writes cache entry m / T at position *pos + m % T (T = 1: entry m)
-cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_rope& r, int M, int T, cudaStream_t st);
+// T tokens per sequence (M % T == 0): token row m writes cache entry m / T at position *pos + m % T (T = 1: entry m),
+// rotated at that position plus off[m / T] (off: device int32[M / T] rotary offsets; null: none)
+cudaError_t rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_rope& r, int M, int T, const int32_t* off,
+                    cudaStream_t st);
 // B200AWQ_OK, or the code b200awq_qk_norm_rope_kv returns for a bad descriptor / qkv pitch (host only; D % 16 is
 // checked by the callers)
 int qk_norm_validate(const struct ::b200awq_qk_norm_rope* q, int64_t ldqkv);
 cudaError_t qk_norm_rope_kv(const void* qkv, int64_t ldqkv, const struct ::b200awq_qk_norm_rope& q, int M, int T,
-                            cudaStream_t st);
+                            const int32_t* off, cudaStream_t st);
 cudaError_t stream_pack_rotary(const int32_t* qweight, const void* scales, const int32_t* qzeros, void* out, int K, int N,
                                int G, int head_dim, int rotary_dim, cudaStream_t st);
 // B200AWQ_OK, or the code the stand-alone op of kind (B200AWQ_OP_MLA_*) returns for a bad descriptor (host only)

@@ -148,9 +148,11 @@ struct ProgOp {
   const void* res_ext = nullptr;
   int res_op = -1;
   // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights;
-  // rope_T: tokens per sequence (ROPE_KV_SEQ / QK_NORM_ROPE_KV_SEQ: the op's K; 1 for ROPE_KV)
+  // rope_T: tokens per sequence (ROPE_KV_SEQ / QK_NORM_ROPE_KV_SEQ / ROPE_KV_OFFSET: the op's K; 1 for ROPE_KV);
+  // rot_offset: a ROPE_KV_OFFSET's per-sequence rotary offsets (null for the other kinds)
   b200awq_qk_norm_rope_t qkr = {};
   int rope_T = 1;
+  const int32_t* rot_offset = nullptr;
   // an MLA_ROPE (mla_kind 1), MLA_KV (2), MLA_K_ROPE (3) or MLA_Q_ROPE (4) folded into the finish
   b200awq_mla_t mla = {};
   int mla_kind = 0;
@@ -692,12 +694,16 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
   }
   if (e == cudaSuccess && takes_rope && M == 1) {
     std::vector<SpRope> rp(n);
-    for (int i = 0; i < n; ++i) rp[i].r = table[i].qkr.rope;   // (head_dim 0: no rotation)
+    for (int i = 0; i < n; ++i) {
+      rp[i].r = table[i].qkr.rope;   // (head_dim 0: no rotation)
+      rp[i].rot_offset = table[i].rot_offset;
+    }
     e = upload(&pr->d_rope, rp);
   } else if (e == cudaSuccess && takes_rope) {
     std::vector<SpRopeSeq> rp(n);
     for (int i = 0; i < n; ++i) {
       rp[i].r = table[i].qkr.rope;
+      rp[i].rot_offset = table[i].rot_offset;
       rp[i].T = table[i].rope_T;
     }
     e = upload(&pr->d_rope_seq, rp);
@@ -714,6 +720,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
       qd[i].q = table[i].qkr;
       qd[i].part = pr->d_qkn_part + off;
       qd[i].inv_d = 1.f / static_cast<float>(table[i].qkr.rope.head_dim);
+      qd[i].rot_offset = table[i].rot_offset;
       off += (size_t)M * (table[i].N / 16);
     }
     if (e == cudaSuccess) e = upload(&pr->d_qkn, qd);
@@ -919,16 +926,22 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (M < 0) M = op.M;
     if (op.M != M) return B200AWQ_EUNSUPPORTED;
     if (op.kind == B200AWQ_OP_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV || op.kind == B200AWQ_OP_ROPE_KV_SEQ ||
-        op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ) {
+        op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ || op.kind == B200AWQ_OP_ROPE_KV_OFFSET) {
       // RoPE + cache append, folded into the finish of the linear recorded just before it (whose whole output is qkv);
       // QK_NORM_ROPE_KV: the same op on its embedded descriptor, with q / k normalised first.  The _SEQ kinds: T = op.K
-      // tokens per sequence (M = B T rows; T > 1 needs M > 1, so only the batched kernels see it)
-      const bool qkn = op.kind == B200AWQ_OP_QK_NORM_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ;
-      const bool seq = op.kind == B200AWQ_OP_ROPE_KV_SEQ || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ;
+      // tokens per sequence (M = B T rows; T > 1 needs M > 1, so only the batched kernels see it).  ROPE_KV_OFFSET: the
+      // _SEQ kind its embedded descriptor's norm weights name (both null: no norm), with per-sequence rotary offsets
+      const b200awq_rope_offset_t* od =
+          op.kind == B200AWQ_OP_ROPE_KV_OFFSET ? static_cast<const b200awq_rope_offset_t*>(op.weight) : nullptr;
+      if (op.kind == B200AWQ_OP_ROPE_KV_OFFSET && (od == nullptr || od->rot_offset == nullptr)) return B200AWQ_EINVAL;
+      const bool qkn = op.kind == B200AWQ_OP_QK_NORM_ROPE_KV || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ ||
+                       (od != nullptr && (od->qk.q_norm_weight != nullptr || od->qk.k_norm_weight != nullptr));
+      const bool seq = op.kind == B200AWQ_OP_ROPE_KV_SEQ || op.kind == B200AWQ_OP_QK_NORM_ROPE_KV_SEQ || od != nullptr;
       const int T = seq ? op.K : 1;
       if (T < 1 || (M % T) != 0) return B200AWQ_EINVAL;
-      const b200awq_qk_norm_rope_t* qd = qkn ? static_cast<const b200awq_qk_norm_rope_t*>(op.weight) : nullptr;
-      const b200awq_rope_t* r = qkn ? (qd != nullptr ? &qd->rope : nullptr) : static_cast<const b200awq_rope_t*>(op.weight);
+      const b200awq_qk_norm_rope_t* qd =
+          od != nullptr ? &od->qk : qkn ? static_cast<const b200awq_qk_norm_rope_t*>(op.weight) : nullptr;
+      const b200awq_rope_t* r = qd != nullptr ? &qd->rope : qkn ? nullptr : static_cast<const b200awq_rope_t*>(op.weight);
       if (op.x == nullptr) return B200AWQ_EINVAL;
       const int v = rope_validate(r, M > 1 ? op.ldx : INT64_MAX);   // (one row: no pitch; N is checked below)
       if (v != B200AWQ_OK) return v;
@@ -945,6 +958,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       if (qkn) pv.qkr = *qd;
       else pv.qkr.rope = *r;
       pv.rope_T = T;
+      pv.rot_offset = od != nullptr ? od->rot_offset : nullptr;
       continue;
     }
     if (op.kind == B200AWQ_OP_MLA_ROPE || op.kind == B200AWQ_OP_MLA_KV || op.kind == B200AWQ_OP_MLA_K_ROPE ||
@@ -1166,8 +1180,8 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
   // ROPE_KV: the rotated q and the appended cache rows are written in a finish, while other CTAs run later ops.  No
   // other op of the program may read or write them, nor write the position / frequency table the finish reads; the
   // producer must not be a gate|up whose product a SiLU*mul reads (its row would hold silu(gate) * up).
-  // QK_NORM_ROPE_KV: its two norm weights are reads like the position and the frequency table.
-  // (the caches: B = M / T entries)
+  // QK_NORM_ROPE_KV: its two norm weights are reads like the position and the frequency table; ROPE_KV_OFFSET: its B
+  // rotary offsets too.  (the caches and the offsets: B = M / T entries)
   auto rope_outs = [&](const ProgOp& p) {
     const b200awq_rope_t& r = p.qkr.rope;
     const size_t cache =
@@ -1181,8 +1195,10 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
     if (r.head_dim == 0) continue;
     const auto outs = rope_outs(table[ri]);
     const size_t wn = q.q_norm_weight != nullptr ? (size_t)r.head_dim * 2 : 0;   // (null, 0: overlaps nothing)
-    const std::pair<const void*, size_t> ins[4] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * rope_rotary_dim(r) * 4},
-                                                   {q.q_norm_weight, wn}, {q.k_norm_weight, wn}};
+    const size_t ob = table[ri].rot_offset != nullptr ? (size_t)(M / table[ri].rope_T) * 4 : 0;
+    const std::pair<const void*, size_t> ins[5] = {{r.pos, 4}, {r.freqs, (size_t)r.freqs_len * rope_rotary_dim(r) * 4},
+                                                   {q.q_norm_weight, wn}, {q.k_norm_weight, wn},
+                                                   {table[ri].rot_offset, ob}};
     auto hits_out = [&](const void* p, size_t b) {
       for (const auto& o : outs)
         if (overlaps(o.first, o.second, p, b)) return true;
@@ -1277,8 +1293,9 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
         for (const auto& w : rope_outs(o))
           if (hits_any(w.first, w.second)) return B200AWQ_EUNSUPPORTED;
         const size_t wn = q.q_norm_weight != nullptr ? (size_t)q.rope.head_dim * 2 : 0;
+        const size_t ob = o.rot_offset != nullptr ? (size_t)(M / o.rope_T) * 4 : 0;
         if (hits_out(q.rope.pos, 4) || hits_out(q.rope.freqs, (size_t)q.rope.freqs_len * rope_rotary_dim(q.rope) * 4) ||
-            hits_out(q.q_norm_weight, wn) || hits_out(q.k_norm_weight, wn))
+            hits_out(q.q_norm_weight, wn) || hits_out(q.k_norm_weight, wn) || hits_out(o.rot_offset, ob))
           return B200AWQ_EUNSUPPORTED;
       }
       if (j != ri && o.mla_kind != 0) {   // another MLA op: its outputs are writes (its reads: its own pass of this loop)

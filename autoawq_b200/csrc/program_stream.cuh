@@ -191,19 +191,31 @@ __device__ __forceinline__ float sp_residual(const SpRes& r, const uint32_t* row
 
 // ROPE_KV folded into a qkv linear's finish (stream_rope_kernel / stream_batch_rope_kernel): one entry per kernel op in a
 // side table, like SpRes.  The op is packed in mode 2 (sp_cols_rot with r.head_dim and r's rotary dim); r.head_dim == 0
-// on every other op.  The descriptor is the recorded b200awq_rope_t (rope.cuh does the arithmetic).
+// on every other op.  The descriptor is the recorded b200awq_rope_t (rope.cuh does the arithmetic); rot_offset: a
+// ROPE_KV_OFFSET's per-sequence rotary offsets (null for every other op).
 struct SpRope {
   b200awq_rope_t r;
+  const int32_t* rot_offset;
 };
 // The batched kernels' entry (stream_batch_rope_kernel / stream_batch_qknorm_kernel): SpRope's descriptor and T, the
 // tokens per sequence of the op (B200AWQ_OP_ROPE_KV_SEQ's b200awq_op_t.K; 1 for ROPE_KV): token row m = b T + t writes
-// cache entry b at position *r.pos + t (rope.cuh: rope_row_pos).  A table of its own: a wider SpRope would change the
-// M = 1 kernels' table stride, and they only run T = 1.
+// cache entry b at position *r.pos + t (rope.cuh: rope_row_pos).  A table of its own: the M = 1 kernels only run T = 1.
+// rot_offset as SpRope.
 struct SpRopeSeq {
   b200awq_rope_t r;
+  const int32_t* rot_offset;
   int T;
   int pad_;
 };
+
+// The rotary row of cache row p in the M = 1 finish (one sequence): p plus the offset behind the op's side-table field
+// `field` (SpRope::rot_offset, SpQkNorm::rot_offset; null: none).  The finish derives it again for every pair instead of
+// carrying it from the range check: carried through the pair loop it costs the M = 1 kernels, already at 168
+// registers, a spill; derived here every M = 1 entry keeps the registers and spills it had without offsets.
+__device__ __forceinline__ int sp_rot_row(const int32_t* const* field, int p) {
+  const int32_t* o = *field;
+  return o != nullptr ? p + *o : p;
+}
 
 // QK_NORM_ROPE_KV folded into a qkv linear's finish (stream_qknorm_kernel / stream_batch_qknorm_kernel): one entry per
 // kernel op in a side table next to SpRope (whose descriptor is the embedded b200awq_rope_t); part == null on every op
@@ -216,6 +228,7 @@ struct SpRopeSeq {
 struct SpQkNorm {
   b200awq_qk_norm_rope_t q;
   unsigned long long* part;    // [M][N / 16] published set partials of this op (program-owned)
+  const int32_t* rot_offset;   // SpRope::rot_offset again: phase (b) reads it from here (sp_qk_finish)
   float inv_d;                 // fp32(1 / head_dim), rounded on the host (rope.cuh: qk_norm_rope_pair)
   int pad_;
 };
@@ -301,8 +314,9 @@ struct SpLn {
 // phase (b) of a QK_NORM_ROPE_KV finish (SpQkNorm above), shared by the M = 1 and the batched body: item t of this
 // thread (t = ct, ct + nthr, ... < nsets * per_set; per_set = 8 M) is lane group t % 8 of token row (t % per_set) / 8 of
 // local set t / per_set, whose fp16 pair phase (a) kept in part[(ls * kst + m) * 16 + g] / [.. + 8].  T >= 1 (the
-// batched body): p0 = *pos and T tokens per sequence, each row's entry and position from rope.cuh's rope_row_pos (a row
-// outside the cache writes nothing); T = 0 (the M = 1 body): p0 is the step's position, already checked, entry m.
+// batched body): p0 = *pos and T tokens per sequence, each row's entry, cache row and rotary row from rope.cuh's
+// rope_row_pos (a row out of range writes nothing); T = 0 (the M = 1 body): p0 is the step's cache row, already checked
+// with its rotary row (sp_rot_row), entry m.
 __device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, int p0, int T, const float* part, int kst,
                                           int ct, int nthr, int nsets, int per_set, int set0, int N, uint32_t tag, int op) {
   const b200awq_rope_t& rp = qn->q.rope;
@@ -313,15 +327,16 @@ __device__ __forceinline__ void sp_qk_finish(const SpQkNorm* __restrict__ qn, in
     int clo, chi;
     sp_cols_rot(rp.head_dim, rp.head_dim, set0 + ls, gg, clo, chi);   // (full rotary: program_create checks it)
     const __half a = __float2half_rn(keep[gg]), b = __float2half_rn(keep[gg + 8]);
-    int e = m, rpos = p0;
-    if (T > 0 && (rpos = rope_row_pos(rp, p0, T, m, e)) < 0) continue;
+    int e = m, rpos = p0, rot;
+    if (T == 0) rot = sp_rot_row(&qn->rot_offset, p0);
+    else if ((rpos = rope_row_pos(rp, p0, T, qn->rot_offset, m, e, rot)) < 0) continue;
     if (hd >= hqk) {   // v head: not normalised, only appended
-      rope_pair(rp, rpos, m, e, clo, chi, a, b);
+      rope_pair(rp, rpos, rot, m, e, clo, chi, a, b);
       continue;
     }
     const unsigned long long* hp = qn->part + (size_t)m * (N >> 4) + (size_t)hd * per_head;
     const float ss = qk_head_sum(per_head, [&](int u) { return sp_qk_partial(hp + u, tag, op); });
-    qk_norm_rope_pair(qn->q, qn->inv_d, rpos, m, e, clo, a, b, ss);
+    qk_norm_rope_pair(qn->q, qn->inv_d, rpos, rot, m, e, clo, a, b, ss);
   }
 }
 

@@ -31,16 +31,16 @@ __host__ __device__ __forceinline__ void rope_cols(int D, int R, int p, int& lo,
   }
 }
 
-// One pair of token row m, written to q_out row m and to cache entry e at position pos: columns lo = h D + i and
-// hi = h D + j of head h, paired by rope_cols.  a, b: the fp16 qkv values.  A q / k pair with i < R/2 is rotated; every
-// other pair (the pass-through columns, a v head) is copied.  (e = m for a step of one token per sequence; rope_row_pos
-// gives e and pos for T tokens per sequence.)
+// One pair of token row m, written to q_out row m and to cache entry e at cache row pos, rotated with freqs row rot:
+// columns lo = h D + i and hi = h D + j of head h, paired by rope_cols.  a, b: the fp16 qkv values.  A q / k pair with
+// i < R/2 is rotated; every other pair (the pass-through columns, a v head) is copied.  (rope_row_pos gives e, pos and
+// rot: e = m and rot = pos for a step of one token per sequence without a rotary offset.)
 // The rotation is torch's complex<float> product (c10 complex operator*=: re = a c - b s, im = a s + b c) with the
 // contraction nvcc gives it there, re = fma(a, c, -(b s)) and im = fma(b, c, a s); explicit intrinsics keep -fmad from
 // changing it.  Torch's loops for other shapes differ in a few elements by one fp16 ulp (DESIGN.md 3.5f;
 // tests/test_gpu_program_rope.py compares against RoPE.forward with that bound).
-__device__ __forceinline__ void rope_pair(const b200awq_rope_t& r, int pos, int m, int e, int lo, int hi, __half a,
-                                          __half b) {
+__device__ __forceinline__ void rope_pair(const b200awq_rope_t& r, int pos, int rot, int m, int e, int lo, int hi,
+                                          __half a, __half b) {
   const int D = r.head_dim, hr = rope_rotary_dim(r) >> 1;
   const int h = lo / D, i = lo - h * D, j = hi - h * D;
   const int H = r.n_heads, KV = r.n_kv_heads;
@@ -57,7 +57,7 @@ __device__ __forceinline__ void rope_pair(const b200awq_rope_t& r, int pos, int 
     dst[j] = b;
     return;
   }
-  const float2 cs = reinterpret_cast<const float2*>(r.freqs)[(size_t)pos * hr + i];
+  const float2 cs = reinterpret_cast<const float2*>(r.freqs)[(size_t)rot * hr + i];
   const float fa = __half2float(a), fb = __half2float(b);
   const float re = __fmaf_rn(fa, cs.x, -__fmul_rn(fb, cs.y));
   const float im = __fmaf_rn(fb, cs.x, __fmul_rn(fa, cs.y));
@@ -65,20 +65,16 @@ __device__ __forceinline__ void rope_pair(const b200awq_rope_t& r, int pos, int 
   dst[j] = __float2half_rn(im);
 }
 
-// the position of this step, or -1 when it is outside the cache / the frequency table (then nothing is written)
-__device__ __forceinline__ int rope_pos(const b200awq_rope_t& r) {
-  const int p = *r.pos;
-  return (p >= 0 && p < r.cache_len && p < r.freqs_len) ? p : -1;
-}
-
-// Token row m of a step of T tokens per sequence (B200AWQ_OP_ROPE_KV_SEQ): row m = b T + t is token t of sequence b, so
-// its cache entry is e = b and its position p0 + t (p0 = *r.pos).  Returns that position, or -1 when it is outside
-// the cache / the frequency table (then the row writes nothing; the other rows of the step still do).  T = 1 is
-// rope_pos with e = m.
-__device__ __forceinline__ int rope_row_pos(const b200awq_rope_t& r, int p0, int T, int m, int& e) {
+// Token row m of a step of T tokens per sequence (T = 1: one token, B200AWQ_OP_ROPE_KV): row m = b T + t is token t of
+// sequence b, so its cache entry is e = b, its cache row p = p0 + t (p0 = *r.pos) and its rotary row rot = p + off[b]
+// (off: B200AWQ_OP_ROPE_KV_OFFSET's per-sequence rotary offsets; null: rot = p).  Returns p, or -1 when p is outside the
+// cache or rot outside the frequency table (then the row writes nothing; the other rows of the step still do).
+__device__ __forceinline__ int rope_row_pos(const b200awq_rope_t& r, int p0, int T, const int32_t* off, int m, int& e,
+                                            int& rot) {
   e = m / T;
-  const long long p = (long long)p0 + (m - e * T);
-  return (p >= 0 && p < r.cache_len && p < r.freqs_len) ? static_cast<int>(p) : -1;
+  const long long p = (long long)p0 + (m - e * T), q = off != nullptr ? p + off[e] : p;
+  rot = static_cast<int>(q);
+  return (p >= 0 && p < r.cache_len && q >= 0 && q < r.freqs_len) ? static_cast<int>(p) : -1;
 }
 
 // ---- Qwen3 q_norm / k_norm in front of the rotation (B200AWQ_OP_QK_NORM_ROPE_KV).  The sum of squares of a head is
@@ -108,14 +104,15 @@ __device__ __forceinline__ float qk_head_sum(int nsets, Partial&& partial) {
 }
 
 // Qwen3RMSNorm.forward on one pair of fp16 values (column col = h D + i of token row m, partner col + D / 2; full
-// rotary only) of a q or k head with total sum of squares ss, then rope_pair on the result (cache entry e):
+// rotary only) of a q or k head with total sum of squares ss, then rope_pair on the result (cache entry e, cache row
+// pos, freqs row rot):
 //   r = rsqrtf(ss * inv_d + eps), x' = fp16(w * fp16(x * r))   (hidden_states * torch.rsqrt(variance + eps), .to(fp16),
 //   weight * it: transformers' Qwen3RMSNorm)
 // inv_d = fp32(1 / D), rounded on the host: torch.mean scales its sum by that factor, and ss * inv_d == ss / D for a
 // power-of-two D.  (A device division would also pull its slow-path subroutine into the stream kernels, whose call
 // convention costs the 8-warp kernel a spill.)
-__device__ __forceinline__ void qk_norm_rope_pair(const b200awq_qk_norm_rope_t& q, float inv_d, int pos, int m, int e,
-                                                  int col, __half a, __half b, float ss) {
+__device__ __forceinline__ void qk_norm_rope_pair(const b200awq_qk_norm_rope_t& q, float inv_d, int pos, int rot, int m,
+                                                  int e, int col, __half a, __half b, float ss) {
   const int D = q.rope.head_dim, h = col / D, i = col - h * D;
   const __half* w = static_cast<const __half*>(h < q.rope.n_heads ? q.q_norm_weight : q.k_norm_weight);
   const float r = rsqrtf(__fadd_rn(__fmul_rn(ss, inv_d), q.eps));
@@ -123,7 +120,7 @@ __device__ __forceinline__ void qk_norm_rope_pair(const b200awq_qk_norm_rope_t& 
   const __half nb = __float2half_rn(__fmul_rn(__half2float(b), r));
   const __half wa = __float2half_rn(__fmul_rn(__half2float(w[i]), __half2float(na)));
   const __half wb = __float2half_rn(__fmul_rn(__half2float(w[i + (D >> 1)]), __half2float(nb)));
-  rope_pair(q.rope, pos, m, e, col, col + (D >> 1), wa, wb);
+  rope_pair(q.rope, pos, rot, m, e, col, col + (D >> 1), wa, wb);
 }
 
 // ---- MLA (B200AWQ_OP_MLA_ROPE / _MLA_KV / _MLA_K_ROPE / _MLA_Q_ROPE, include/b200awq.h): the per-pair / per-column

@@ -19,6 +19,7 @@ __all__ = [
     "layer_norm", "gelu",
     "topk_softmax", "moe_alig_block_size", "grouped_gemm_forward",
     "linear_forward", "stream_pack", "stream_pack_rotary", "rope_kv_cache", "rope_descriptor", "qk_norm_descriptor",
+    "rope_offset_descriptor",
     "mla_descriptor", "mla_rope", "mla_kv_cache", "mla_k_rope", "mla_q_rope",
     "set_knob", "get_knob",
     "B200AwqError",
@@ -382,8 +383,26 @@ def qk_norm_descriptor(rope, q_norm, k_norm, device):
     return d, ws
 
 
+def rope_offset_descriptor(desc, qdesc, rope_offset, B, device):
+    """b200awq_rope_offset_t around a b200awq_rope_t (and the b200awq_qk_norm_rope_t of q / k norm, or None) with the
+    per-sequence rotary offsets rope_offset: a contiguous int32 tensor of B elements on `device` (None: returns None,
+    the op without offsets)."""
+    if rope_offset is None:
+        return None
+    if (not isinstance(rope_offset, torch.Tensor) or rope_offset.dtype != torch.int32 or rope_offset.numel() != B
+            or not rope_offset.is_contiguous() or rope_offset.device != device):
+        raise B200AwqError(f"b200awq: rope_offset must be a contiguous int32 tensor of B = {B} elements on {device}")
+    d = _cabi.RopeOffset()
+    if qdesc is not None:
+        d.qk = qdesc
+    else:
+        d.qk.rope = desc
+    d.rot_offset = rope_offset.data_ptr()
+    return d
+
+
 def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None, k_norm=None,
-                  head_dim=None, seq_len=None):
+                  head_dim=None, seq_len=None, rope_offset=None):
     """RoPE.forward on q and k of the fused qkv output and WindowedCache.update_kv of k and v at position *pos
     (awq/modules/fused/attn.py:243-267): writes q_out [M, H, D] and the row `pos` of cache batch entries 0..M-1, nothing
     else (nothing at all when pos is outside the cache or the frequency table).  pos is read on the device: a captured
@@ -401,7 +420,12 @@ def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_
     update_kv of rows *pos .. *pos + T - 1; None or 1: one token, as above).  qkv is then the reference's xqkv view
     [B, T, N] or its rows [B T, N]; row m = b T + t is token t of sequence b at position *pos + t and writes q_out row m
     and cache entry b (the caches need B entries).  A row whose position is outside the cache or the table writes
-    nothing; the rest of the step still does (b200awq_rope_kv_seq)."""
+    nothing; the rest of the step still does (b200awq_rope_kv_seq).
+
+    rope_offset: a device int32 tensor of B = M / T per-sequence rotary offsets (None: none).  Row m = b T + t keeps
+    cache row *pos + t of entry b and is rotated at *pos + t + rope_offset[b] (b200awq_rope_kv_offset): -pad_b for a
+    left-padded batch, rope_deltas[b] for a Qwen2-VL / Qwen2.5-VL text step.  A row writes nothing unless both its
+    cache row and its rotary position are in range.  The offsets are read on the device, as pos is."""
     H = int(n_heads)
     T = _seq_len(seq_len)
     D, _ = _rope_dims(freqs_cis, head_dim)
@@ -410,16 +434,20 @@ def rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_
         q_out = torch.empty((M, H, D), dtype=torch.float16, device=qkv.device)
     r, q2, M = rope_descriptor(qkv, freqs_cis, pos, k_cache, v_cache, H, n_kv_heads, q_out, head_dim, T)
     qd, _ = qk_norm_descriptor(r, q_norm, k_norm, qkv.device)
+    od = rope_offset_descriptor(r, qd, rope_offset, M // T, qkv.device)
     ld = q2.stride(0) if M > 1 else q2.shape[1]
     with _DeviceGuard(qkv.device):
-        code, name = rope_kv_call(q2.data_ptr(), ld, r, qd, M, T, _stream(qkv.device))
+        code, name = rope_kv_call(q2.data_ptr(), ld, r, qd, M, T, _stream(qkv.device), od)
     check(code, f"{name}(M={M}, T={T}, H={H}, KV={r.n_kv_heads}, D={D})")
     return q_out
 
 
-def rope_kv_call(qkv_ptr, ld, desc, qdesc, M, T, stream):
+def rope_kv_call(qkv_ptr, ld, desc, qdesc, M, T, stream, odesc=None):
     """The C entry of one RoPE + KV-cache append: b200awq_rope_kv (qdesc None) or b200awq_qk_norm_rope_kv, their
-    _seq forms for T > 1.  Returns (code, entry name)."""
+    _seq forms for T > 1, and b200awq_rope_kv_offset for any of them with rotary offsets (odesc, which embeds desc /
+    qdesc).  Returns (code, entry name)."""
+    if odesc is not None:
+        return lib.b200awq_rope_kv_offset(qkv_ptr, ld, odesc, M, T, stream), "b200awq_rope_kv_offset"
     name = ("b200awq_rope_kv" if qdesc is None else "b200awq_qk_norm_rope_kv") + ("_seq" if T > 1 else "")
     args = (qkv_ptr, ld, desc if qdesc is None else qdesc, M) + ((T,) if T > 1 else ())
     return getattr(lib, name)(*args, stream), name

@@ -55,6 +55,12 @@ m = b T + t is token t of sequence b at position *pos + t, written to cache entr
 over the new tokens) stays the caller's, between programs.  `DecodeProgram(max_tokens=B T)` runs the segment as one
 launch (B T <= 8; DESIGN.md 3.5n); advance `pos` by T per step.
 
+When a sequence's rotary position differs from its cache row (a left-padded batch: `rope_offset = -pad`; a Qwen2-VL /
+Qwen2.5-VL text step: the M-RoPE delta of each sequence), `rope_kv_cache(..., rope_offset=off)` takes a device int32
+tensor of B per-sequence offsets: row m = b T + t is written to cache row *pos + t of entry b and rotated at *pos + t
++ off[b].  It folds wherever the op without offsets folds (DESIGN.md 3.5o); rewrite `off` in place between runs, like
+`pos`.
+
 `mla_rope(qkva, freqs, pos, k_cache, ...)` and `mla_kv_cache(kv, pos, k_cache, v_cache, ...)` record the glue of
 DeepSeek-V2 / V3 multi-head latent attention (transformers' DeepseekV2Attention / DeepseekV3Attention, no q LoRA) in
 transformers' order: the fused q_proj | kv_a_proj_with_mqa linear (packing.fuse_mla_input), mla_rope, kv_a_layernorm as
@@ -231,7 +237,7 @@ class DecodeProgram:
         return out
 
     def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None,
-                      k_norm=None, head_dim=None, seq_len=None):
+                      k_norm=None, head_dim=None, seq_len=None, rope_offset=None):
         """RoPE.forward(xq, xk, start_pos = *pos, seqlen = 1) + cache.update_kv(xv, xk) on the fused qkv output (q heads,
         then k heads, then v heads, as get_attention_shapes slices it): writes q_out [M, H, D] (allocated when not given,
         and returned) and row *pos of k_cache / v_cache batch entries 0..M-1, nothing when *pos is outside the cache or
@@ -247,7 +253,12 @@ class DecodeProgram:
         and update_kv of rows *pos .. *pos + T - 1.  qkv is the step's [B, T, N] (the reference's xqkv view) or [B T, N]
         output; row m = b T + t writes q_out row m and cache entry b at position *pos + t, and the caches need B
         entries.  A program built with max_tokens >= B T folds it into the qkv linear's finish as well (DESIGN.md
-        3.5n); advance pos by T between runs."""
+        3.5n); advance pos by T between runs.
+
+        rope_offset: a device int32 tensor of B per-sequence rotary offsets (None: none): row m = b T + t keeps cache
+        row *pos + t of entry b and is rotated at *pos + t + rope_offset[b] (ext.rope_kv_cache).  It folds wherever
+        the op without offsets folds (DESIGN.md 3.5o) and is read at every run: rewrite it in place between runs, as
+        pos."""
         self._no_more()
         self._dev_of(qkv)
         H = int(n_heads)
@@ -267,10 +278,14 @@ class DecodeProgram:
         if q2.data_ptr() != qkv.data_ptr():
             raise B200AwqError("b200awq: rope_kv_cache records qkv by address: pass its rows as they are")
         qdesc, norm_w = ext.qk_norm_descriptor(desc, q_norm, k_norm, self._dev)
+        odesc = ext.rope_offset_descriptor(desc, qdesc, rope_offset, M // T, self._dev)
         self._ops.append(("rope", dict(qkv=q2, freqs=freqs_cis, pos=pos, k_cache=k_cache, v_cache=v_cache, q_out=q_out,
                                        H=H, KV=desc.n_kv_heads, M=M, N=q2.shape[1], T=T,
-                                       ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc, qdesc=qdesc)))
+                                       ldx=q2.stride(0) if M > 1 else q2.shape[1], desc=desc, qdesc=qdesc,
+                                       odesc=odesc)))
         self._keep += [qkv, q2, freqs_cis, pos, k_cache, v_cache, q_out] + norm_w
+        if odesc is not None:
+            self._keep.append(rope_offset)
         return q_out
 
     def mla_rope(self, qkva, freqs, pos, k_cache, n_heads, nope_dim, rope_dim, kv_lora_rank, style, q_out=None):
@@ -629,6 +644,9 @@ class DecodeProgram:
                 c.kind, c.M, c.K, c.N = (_cabi.OP_DEEPSEEK_MOE if o["ds"] is not None else
                                          _cabi.OP_QWEN3_MOE if o["hf"] else _cabi.OP_SPARSE_MOE), o["M"], o["H"], o["H"]
                 c.x, c.y, c.weight = o["x"].data_ptr(), o["out"].data_ptr(), ctypes.addressof(o["desc"])
+            elif kind == "rope" and o["odesc"] is not None:   # kind 19, K = T
+                c.kind, c.M, c.N, c.ldx, c.K = _cabi.OP_ROPE_KV_OFFSET, o["M"], o["N"], o["ldx"], o["T"]
+                c.x, c.weight = o["qkv"].data_ptr(), ctypes.addressof(o["odesc"])
             elif kind == "rope":
                 qk, seq = o["qdesc"] is not None, o["T"] > 1     # (seq: kinds 17 / 18, with K = T)
                 c.kind = ((_cabi.OP_QK_NORM_ROPE_KV_SEQ if seq else _cabi.OP_QK_NORM_ROPE_KV) if qk else
@@ -744,7 +762,7 @@ class DecodeProgram:
             elif kind == "rope":
                 with ext._DeviceGuard(dev):
                     code, name = ext.rope_kv_call(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["qdesc"], o["M"], o["T"],
-                                                  ext._stream(dev))
+                                                  ext._stream(dev), o["odesc"])
                 check(code, name)
             elif kind in _MLA_OPS:
                 ext._mla_call(getattr(lib, "b200awq_" + kind), o["row"], o["desc"], o["M"], "b200awq_" + kind,

@@ -391,12 +391,20 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *     checks taken over B = M / T entries.  B200AWQ_EINVAL for T < 1 or M % T != 0.  T = 1 folds exactly as kind 6 / 7.
  *     T > 1 means M > 1, so it folds only in a program created with max_tokens >= M, in the segments where ROPE_KV
  *     folds at M > 1 (RMSNorm staging, residual adds, partial rotary, q / k norm); with LAYER_NORM, GELU, MLA or MoE
- *     ops the program replays per op (B200AWQ_EUNSUPPORTED), as it does for ROPE_KV at M > 1. */
+ *     ops the program replays per op (B200AWQ_EUNSUPPORTED), as it does for ROPE_KV at M > 1.
+ *
+ *   ROPE_KV_OFFSET : ROPE_KV_SEQ / QK_NORM_ROPE_KV_SEQ with a per-sequence rotary offset (left-padded batches, the text
+ *                   steps of Qwen2-VL / Qwen2.5-VL): x, M, N as kind 17 / 18, K = T (1 <= T, M % T == 0), weight = a
+ *                   b200awq_rope_offset_t descriptor (below; null norm weights: no q / k norm).  Row m = b T + t writes
+ *                   cache row *pos + t of entry b, rotated at that row plus rot_offset[b].  As b200awq_rope_kv_offset.
+ *     Folding: wherever kind 17 / 18 fold (at M = 1 in every program where kind 6 / 7 fold), under their rules and
+ *     rejections on the embedded descriptor, plus B200AWQ_EINVAL for a null rot_offset.  rot_offset is a read like
+ *     pos: B200AWQ_EUNSUPPORTED when an op of the program writes any of its B = M / T entries. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
        B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11, B200AWQ_OP_MLA_K_ROPE = 12,
        B200AWQ_OP_MLA_Q_ROPE = 13, B200AWQ_OP_LAYER_NORM = 14, B200AWQ_OP_GELU = 15, B200AWQ_OP_GELU_TANH = 16,
-       B200AWQ_OP_ROPE_KV_SEQ = 17, B200AWQ_OP_QK_NORM_ROPE_KV_SEQ = 18 };
+       B200AWQ_OP_ROPE_KV_SEQ = 17, B200AWQ_OP_QK_NORM_ROPE_KV_SEQ = 18, B200AWQ_OP_ROPE_KV_OFFSET = 19 };
 
 typedef struct b200awq_op {
   int32_t kind;
@@ -539,6 +547,28 @@ int b200awq_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_rope_t* ro
                         b200awq_stream_t stream);
 int b200awq_qk_norm_rope_kv_seq(const void* qkv, int64_t ldqkv, const b200awq_qk_norm_rope_t* desc, int M, int T,
                                 b200awq_stream_t stream);
+
+/* b200awq_rope_kv_seq / b200awq_qk_norm_rope_kv_seq with a per-sequence rotary offset: the rotary position differs from
+ * the cache row.  Row m = b T + t of qkv has cache row p = *pos + t in entry b (as b200awq_rope_kv_seq) and rotary
+ * position r = p + rot_offset[b].  It gets exactly the arithmetic those entries give one row rotated with freqs[r]
+ * (partial rotary, the copied v and, when the norm weights are set, Qwen3's q / k norm), written to q_out[m] and to row
+ * p of cache entry b.  A row writes nothing, not even its q_out row, unless 0 <= p < cache_len and 0 <= r < freqs_len;
+ * the other rows of the step still write.  Uses:
+ *   - a left-padded batch (transformers' position_ids = attention_mask.cumsum(-1) - 1): rot_offset[b] = -pad_b, the
+ *     cache rows staying in lockstep across the batch;
+ *   - a text step of Qwen2-VL / Qwen2.5-VL, whose M-RoPE components are equal for a text token, so the rotation is
+ *     plain rotate-half RoPE at p + rope_deltas[b].
+ * rot_offset is read on the device at every call, as *pos is: a captured CUDA graph uses what the caller last stored
+ * there.  All-zero offsets give the results of b200awq_rope_kv_seq / b200awq_qk_norm_rope_kv_seq byte for byte.
+ * B200AWQ_EINVAL for a null desc or rot_offset, T < 1 or M % T != 0, otherwise the return codes of
+ * b200awq_rope_kv_seq (both norm weights null) or b200awq_qk_norm_rope_kv_seq (B200AWQ_EINVAL for one null weight,
+ * B200AWQ_EUNSUPPORTED for q / k norm with partial rotary or D % 16 != 0). */
+typedef struct b200awq_rope_offset {
+  b200awq_qk_norm_rope_t qk;             /* the rotation; q_norm_weight = k_norm_weight = null: no q / k norm */
+  const int32_t* rot_offset;             /* device int32[B = M / T]: rotary position minus cache row, per sequence */
+} b200awq_rope_offset_t;
+int b200awq_rope_kv_offset(const void* qkv, int64_t ldqkv, const b200awq_rope_offset_t* desc, int M, int T,
+                           b200awq_stream_t stream);
 
 /* MLA (DeepSeek-V2 / V3 multi-head latent attention, no q LoRA): the glue between the fused q_proj | kv_a_proj_with_mqa
  * linear and attention, in transformers' arithmetic (DeepseekV2Attention.forward, DeepseekV3Attention.forward with
