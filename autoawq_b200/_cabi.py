@@ -106,6 +106,7 @@ OP_QK_NORM_ROPE_KV, OP_QWEN3_MOE, OP_DEEPSEEK_MOE, OP_MLA_ROPE, OP_MLA_KV = 7, 8
 OP_MLA_K_ROPE, OP_MLA_Q_ROPE = 12, 13
 OP_LAYER_NORM, OP_GELU, OP_GELU_TANH = 14, 15, 16
 OP_ROPE_KV_SEQ, OP_QK_NORM_ROPE_KV_SEQ, OP_ROPE_KV_OFFSET = 17, 18, 19
+OP_SCALED_ADD = 20
 EUNSUPPORTED = 2
 
 # name -> (restype, argtypes); mirrors include/b200awq.h one to one

@@ -21,6 +21,7 @@
 // mlp) with awq/modules/fused/mlp.py:41-55 (gate/up GEMM, silu*mul, down GEMM), each a separate awq_ext call.
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <cstring>
 #include <utility>
 #include <vector>
@@ -143,10 +144,12 @@ struct ProgOp {
   int stage_row = -1;            // the op whose WHOLE published row this op's staging waits for, or -1
   int moe = 0, mi = -1;          // 1: the gate|up op of MoE block `mi`, 2: its down op (0: a plain linear)
   // an ADD folded into the finish (raw_y != null): raw_y is the linear's own output, still stored; the residual is the
-  // published row of the older op res_op, or res_ext, which no op of the program writes
+  // published row of the older op res_op, or res_ext, which no op of the program writes; res_mul: a SCALED_ADD's
+  // multiplier (the linear's output is scaled before the add), NaN for an ADD
   const void* raw_y = nullptr;
   const void* res_ext = nullptr;
   int res_op = -1;
+  float res_mul = NAN;
   // a ROPE_KV folded into the finish (qkr.rope.head_dim != 0); a QK_NORM_ROPE_KV also sets qkr's norm weights;
   // rope_T: tokens per sequence (ROPE_KV_SEQ / QK_NORM_ROPE_KV_SEQ / ROPE_KV_OFFSET: the op's K; 1 for ROPE_KV);
   // rot_offset: a ROPE_KV_OFFSET's per-sequence rotary offsets (null for the other kinds)
@@ -689,6 +692,7 @@ static bool stream_build(Program* pr, const FoldedProgram& f, int grid, cudaErro
       if (table[i].raw_y == nullptr || table[i].gelu != 0) continue;
       rd[i].out = table[i].y;                       // the ADD's output (the op's y was swapped for it)
       rd[i].ext = static_cast<const __half*>(table[i].res_ext);
+      rd[i].mul = table[i].res_mul;
     }
     e = upload(&pr->d_res, rd);
   }
@@ -993,18 +997,22 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       pv.mla_kind = mrope ? 1 : krope ? 3 : qrope ? 4 : 2;
       continue;
     }
-    if (op.kind == B200AWQ_OP_ADD) {
-      // y = x + weight, folded into the epilogue of the op recorded just before it (a linear / a MoE block's down)
+    if (op.kind == B200AWQ_OP_ADD || op.kind == B200AWQ_OP_SCALED_ADD) {
+      // y = x + weight, folded into the epilogue of the op recorded just before it (a linear / a MoE block's down);
+      // SCALED_ADD: y = x + fp16(weight * eps), weight the producer's output (a linear's only)
+      const bool scaled = op.kind == B200AWQ_OP_SCALED_ADD;
       if (op.x == nullptr || op.weight == nullptr || op.y == nullptr || op.K <= 0) return B200AWQ_EINVAL;
+      if (scaled && !std::isfinite(op.eps)) return B200AWQ_EINVAL;
       if ((op.K % 8) != 0 || !aligned16(op.x) || !aligned16(op.weight) || !aligned16(op.y)) return B200AWQ_EUNSUPPORTED;
       const size_t bytes = rows_bytes(op.K);
       if (overlaps(op.y, bytes, op.x, bytes) || overlaps(op.y, bytes, op.weight, bytes)) return B200AWQ_EUNSUPPORTED;
       if (i == 0 || ops[i - 1].kind != B200AWQ_OP_LINEAR_GEMM || table.empty()) return B200AWQ_EUNSUPPORTED;
       ProgOp& pv = table.back();
+      if (scaled && pv.moe != 0) return B200AWQ_EUNSUPPORTED;
       const void* r;                 // the residual: the operand that is not the producer's whole output
-      if (op.x == pv.y) r = op.weight;
-      else if (op.weight == pv.y) r = op.x;
-      else return B200AWQ_EUNSUPPORTED;  // neither operand is the producer's output (both external)
+      if (op.weight == pv.y) r = op.x;
+      else if (op.x == pv.y && !scaled) r = op.weight;
+      else return B200AWQ_EUNSUPPORTED;  // neither operand is the producer's output (both external), or swapped scaled
       if (op.K != pv.N || overlaps(r, bytes, pv.y, bytes)) return B200AWQ_EUNSUPPORTED;
       // in-program residual: the newest op that wrote any of it must have published exactly it, kSpResWindow ops back
       int res_op = -1;
@@ -1025,6 +1033,7 @@ int program_create(const b200awq_op_t* ops_in, int n_in, int max_tokens, Program
       pv.raw_y = pv.y;
       pv.res_op = res_op;
       pv.res_ext = res_op < 0 ? r : nullptr;
+      if (scaled) pv.res_mul = op.eps;
       pv.y = static_cast<__half*>(op.y);   // the producer's row now publishes the sum
       continue;
     }

@@ -159,14 +159,29 @@ __device__ __forceinline__ uint32_t sp_tag(int base, int op) { return (uint32_t)
 // publishes fp16(fp16(sum [+ bias]) + residual) into its hand-off row and stores it to `out`, and still stores the raw
 // fp16(sum [+ bias]) to its y.  The residual of column c, token row m is ext[m N + c] (a buffer no op of the program
 // writes: ready at launch) when op < 0, else the tagged word of op `op`'s published row (kSpResWindow ops back at most).
+// A SCALED_ADD (mul not NaN) adds fp16(y * mul) instead of y, with the multiply in fp32 (torch's `r + y * a`).
 constexpr int kSpResWindow = 4;                   // largest producer - residual distance in kernel ops (program_create;
                                                   // tests/test_stream_residual_model.py derives it)
 struct SpRes {
   const __half* ext;
   __half* out;
   int op;
-  int pad_;
+  float mul;   // SCALED_ADD's multiplier (finite); NaN for an ADD, which adds y itself
 };
+static_assert(sizeof(SpRes) == 24 && offsetof(SpRes, mul) == 20, "SpRes layout (sp_res_mul)");
+// res[op].mul, read where the finish uses it by a volatile load that also forms the address: neither the multiplier nor
+// a pointer to it is hoisted into a register across the finish loop (the LayerNorm and q / k norm entries have none to
+// spare; their register counts are asserted by the CPU tests)
+__device__ __forceinline__ float sp_res_mul(const SpRes* res, int op) {
+  float v;
+  asm volatile("{\n\t.reg .u64 a;\n\tmad.wide.s32 a, %2, 24, %1;\n\tld.global.nc.f32 %0, [a+20];\n\t}"
+               : "=f"(v) : "l"(res), "r"(op));
+  return v;
+}
+// the linear's operand of the residual add: y for an ADD (mul NaN), fp16(y * mul) for a SCALED_ADD
+__device__ __forceinline__ float sp_res_y(float mul, __half y) {
+  return mul == mul ? __half2float(__float2half_rn(__half2float(y) * mul)) : __half2float(y);
+}
 __device__ __forceinline__ uint32_t ld_relaxed_u32(const void* p) {
   uint32_t r;
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");

@@ -41,6 +41,14 @@ arguments from a loaded block.
 so a layer splits only at attention - [o + h_in -> h, norm2(h), gate|up, silu, down + h -> out, norm1'(out), qkv'] is one
 program (DESIGN.md 3.5e).  Outside the folding rule `run()` replays per op, with `torch.add` for the adds.
 
+`scaled_add(residual, y, a)` records the depth-scaled residual add of MiniCPM / MiniCPM3 (a = scale_depth /
+sqrt(num_hidden_layers)) and Granite (a = residual_multiplier): out = residual + y * a with torch's rounding,
+fp16(r + fp16(y a)) with a in fp32.  It folds where add folds, with y the whole output of the linear recorded just
+before (DESIGN.md 3.5p), so a MiniCPM / Granite segment [o, scaled_add, norm2, gate|up, silu, down, scaled_add,
+norm1', qkv', rope_kv_cache] is one launch, and a MiniCPM3 segment (the same MLP, then the q-LoRA MLA chain below) too.
+Per op it replays torch.mul then torch.add.  The embedding and logit scales and Granite's attention_multiplier (the
+softmax scale) stay with the caller.
+
 `rope_kv_cache(qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads)` records the start of the attention block
 (RoPE.forward on q and k, WindowedCache.update_kv of k and v: awq/modules/fused/attn.py:243-267).  It adds no kernel
 op either: it folds into the finish of the qkv linear recorded just before it, so the segment ends with q rotated and
@@ -94,6 +102,7 @@ from one attention call to the next:
 from __future__ import annotations
 
 import ctypes
+import math
 
 import torch
 
@@ -219,22 +228,43 @@ class DecodeProgram:
         returned.  Fused when one operand is the whole output of the linear / sparse_moe recorded just before and the
         other is a buffer nothing in the program writes, or the output of an op at most four kernel ops back (DESIGN.md
         3.5e states the rule for the rows such a residual is read from)."""
+        out, M, K = self._add_operands(a, b, out, "add")
+        self._ops.append(("add", dict(a=a, b=b, out=out, M=M, K=K)))
+        self._keep += [a, b, out]
+        return out
+
+    def scaled_add(self, residual, y, multiplier, out=None):
+        """out = residual + y * multiplier with torch's rounding on float16 tensors: fp16(r + fp16(y a)), the product in
+        fp32 with a = float32(multiplier).  The depth-scaled residual add of MiniCPM / MiniCPM3 (a = scale_depth /
+        sqrt(num_hidden_layers)) and Granite (a = residual_multiplier).  Tensors and `out` as add.  Fused as add is,
+        with y (not residual) the whole output of the linear recorded just before; after a sparse_moe / qwen3_moe /
+        deepseek_moe, or anywhere add would not fold, run() replays torch.mul then torch.add (DESIGN.md 3.5p)."""
+        mul = float(multiplier)
+        if not math.isfinite(ctypes.c_float(mul).value):        # (the op carries it as a float32)
+            raise B200AwqError(f"b200awq: scaled_add needs a finite multiplier, got {multiplier!r}")
+        out, M, K = self._add_operands(residual, y, out, "scaled_add")
+        scaled = torch.empty_like(y)                  # y * multiplier, the per-op replay's first result
+        self._ops.append(("scaled_add", dict(a=residual, b=y, out=out, M=M, K=K, mul=mul, scaled=scaled)))
+        self._keep += [residual, y, out, scaled]
+        return out
+
+    def _add_operands(self, a, b, out, name):
+        """add's / scaled_add's checks: contiguous float16 tensors of one shape on the program's device.  Returns out
+        (allocated like gemm_forward_cuda's y when None), M and K."""
         self._no_more()
         self._dev_of(a)
         for t in (a, b) + ((out,) if out is not None else ()):
             if t.device != self._dev:
                 raise B200AwqError("b200awq: a decode program lives on one device")
             if t.dtype != torch.float16 or not t.is_contiguous():
-                raise B200AwqError("b200awq: add expects contiguous float16 tensors")
+                raise B200AwqError(f"b200awq: {name} expects contiguous float16 tensors")
         if a.shape != b.shape or (out is not None and out.shape != a.shape):
-            raise B200AwqError(f"b200awq: add expects equal shapes, got {tuple(a.shape)} and {tuple(b.shape)}")
+            raise B200AwqError(f"b200awq: {name} expects equal shapes, got {tuple(a.shape)} and {tuple(b.shape)}")
         K = a.shape[-1]
         M = a.numel() // K
         if out is None:
             out = torch.empty((M, K), dtype=torch.float16, device=a.device).reshape(a.shape)
-        self._ops.append(("add", dict(a=a, b=b, out=out, M=M, K=K)))
-        self._keep += [a, b, out]
-        return out
+        return out, M, K
 
     def rope_kv_cache(self, qkv, freqs_cis, pos, k_cache, v_cache, n_heads, n_kv_heads, q_out=None, q_norm=None,
                       k_norm=None, head_dim=None, seq_len=None, rope_offset=None):
@@ -640,6 +670,9 @@ class DecodeProgram:
             elif kind == "add":
                 c.kind, c.M, c.K = _cabi.OP_ADD, o["M"], o["K"]
                 c.x, c.weight, c.y = o["a"].data_ptr(), o["b"].data_ptr(), o["out"].data_ptr()
+            elif kind == "scaled_add":                       # x: the residual, weight: the scaled operand
+                c.kind, c.M, c.K, c.eps = _cabi.OP_SCALED_ADD, o["M"], o["K"], o["mul"]
+                c.x, c.weight, c.y = o["a"].data_ptr(), o["b"].data_ptr(), o["out"].data_ptr()
             elif kind == "moe":
                 c.kind, c.M, c.K, c.N = (_cabi.OP_DEEPSEEK_MOE if o["ds"] is not None else
                                          _cabi.OP_QWEN3_MOE if o["hf"] else _cabi.OP_SPARSE_MOE), o["M"], o["H"], o["H"]
@@ -701,13 +734,13 @@ class DecodeProgram:
         if self._handle is not None:
             return lib.b200awq_program_tokens(self._handle)
         for kind, o in self._ops:
-            return o["M"] if kind in ("linear", "moe", "add", "rope") or kind in _MLA_OPS else o["rows"]
+            return o["M"] if kind in ("linear", "moe", "add", "scaled_add", "rope") or kind in _MLA_OPS else o["rows"]
         return 0
 
     @property
     def kernel_ops(self) -> int:
         """Ops of the fused kernel: one per linear, two per sparse_moe / qwen3_moe / deepseek_moe (gate|up with the routing, down), none per add,
-        rope_kv_cache, mla_rope, mla_kv_cache, mla_k_rope, mla_q_rope or gelu (they fold into their producer's epilogue)
+        scaled_add, rope_kv_cache, mla_rope, mla_kv_cache, mla_k_rope, mla_q_rope or gelu (they fold into their producer's epilogue)
         and none per layernorm_forward_cuda, silu_and_mul or layer_norm (they fold into their consumers' staging); 0
         per-op."""
         return lib.b200awq_program_num_ops(self._handle) if self._handle is not None else 0
@@ -716,12 +749,14 @@ class DecodeProgram:
     def launches_per_run(self) -> int:
         """Kernels launched by one run(): 1 when fused (adds and rope_kv_cache included); per op, one per recorded
         call, 6 per sparse_moe, 15 + top_k per qwen3_moe (17 + top_k with norm_topk_prob), 34 + top_k per softmax
-        deepseek_moe (sigmoid: 36 + top_k, + 6 with expert groups, + 3 with norm_topk_prob), one torch.add launch per add
-        and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache, one b200awq_mla_rope / b200awq_mla_kv
+        deepseek_moe (sigmoid: 36 + top_k, + 6 with expert groups, + 3 with norm_topk_prob), one torch.add launch per add,
+        two (torch.mul, torch.add) per scaled_add and one b200awq_rope_kv (or b200awq_qk_norm_rope_kv) launch per rope_kv_cache, one b200awq_mla_rope / b200awq_mla_kv
         / b200awq_mla_k_rope / b200awq_mla_q_rope launch per mla_rope / mla_kv_cache / mla_k_rope / mla_q_rope, one
         b200awq_layer_norm / b200awq_gelu launch per layer_norm / gelu.  Per op these count the ext / torch calls of the replay: a torch call may launch more than one
         kernel (torch.sort, torch.gather), so the kernel count can be higher."""
         def per_op(kind, o):
+            if kind == "scaled_add":
+                return 2
             if kind != "moe":
                 return 1
             ds = o["ds"]
@@ -759,6 +794,9 @@ class DecodeProgram:
                 self._moe_replay(o)
             elif kind == "add":
                 torch.add(o["a"], o["b"], out=o["out"])
+            elif kind == "scaled_add":
+                torch.mul(o["b"], o["mul"], out=o["scaled"])
+                torch.add(o["a"], o["scaled"], out=o["out"])
             elif kind == "rope":
                 with ext._DeviceGuard(dev):
                     code, name = ext.rope_kv_call(o["qkv"].data_ptr(), o["ldx"], o["desc"], o["qdesc"], o["M"], o["T"],

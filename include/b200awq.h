@@ -399,12 +399,25 @@ int b200awq_debug_read(void* host_dst, size_t bytes);
  *                   cache row *pos + t of entry b, rotated at that row plus rot_offset[b].  As b200awq_rope_kv_offset.
  *     Folding: wherever kind 17 / 18 fold (at M = 1 in every program where kind 6 / 7 fold), under their rules and
  *     rejections on the embedded descriptor, plus B200AWQ_EINVAL for a null rot_offset.  rot_offset is a read like
- *     pos: B200AWQ_EUNSUPPORTED when an op of the program writes any of its B = M / T entries. */
+ *     pos: B200AWQ_EUNSUPPORTED when an op of the program writes any of its B = M / T entries.
+ *
+ *   SCALED_ADD    : the depth-scaled residual add of MiniCPM / MiniCPM3 (h = residual + h * scale_depth /
+ *                   sqrt(num_hidden_layers)) and Granite (h = residual + h * residual_multiplier): x = the residual,
+ *                   weight = the scaled operand, y = the output, all M contiguous rows of K; eps = the multiplier a
+ *                   (float32).  y = fp16(float(x) + float(fp16(float(weight) * a))): torch's rounding of
+ *                   `residual + hidden * a` on float16 tensors with a Python scalar a (an fp32 opmath multiply, rounded
+ *                   to fp16, then the fp16 add).  A non-finite a, a null pointer or K <= 0: B200AWQ_EINVAL; K % 8 != 0
+ *                   or a pointer not 16-byte aligned: B200AWQ_EUNSUPPORTED.
+ *     Folding: ADD's rules and rejections, with the operands fixed: weight must be the whole output of the linear
+ *     recorded immediately before it, x the residual (an external buffer, or a row published at most 4 kernel ops
+ *     back).  It adds no kernel op; the producer's row carries the sum.  B200AWQ_EUNSUPPORTED (the caller replays per op)
+ *     also after a MoE block's down op, and when the operands are swapped. */
 enum { B200AWQ_OP_RMSNORM = 1, B200AWQ_OP_LINEAR_GEMM = 2, B200AWQ_OP_SILU_AND_MUL = 3, B200AWQ_OP_SPARSE_MOE = 4,
        B200AWQ_OP_ADD = 5, B200AWQ_OP_ROPE_KV = 6, B200AWQ_OP_QK_NORM_ROPE_KV = 7, B200AWQ_OP_QWEN3_MOE = 8,
        B200AWQ_OP_DEEPSEEK_MOE = 9, B200AWQ_OP_MLA_ROPE = 10, B200AWQ_OP_MLA_KV = 11, B200AWQ_OP_MLA_K_ROPE = 12,
        B200AWQ_OP_MLA_Q_ROPE = 13, B200AWQ_OP_LAYER_NORM = 14, B200AWQ_OP_GELU = 15, B200AWQ_OP_GELU_TANH = 16,
-       B200AWQ_OP_ROPE_KV_SEQ = 17, B200AWQ_OP_QK_NORM_ROPE_KV_SEQ = 18, B200AWQ_OP_ROPE_KV_OFFSET = 19 };
+       B200AWQ_OP_ROPE_KV_SEQ = 17, B200AWQ_OP_QK_NORM_ROPE_KV_SEQ = 18, B200AWQ_OP_ROPE_KV_OFFSET = 19,
+       B200AWQ_OP_SCALED_ADD = 20 };
 
 typedef struct b200awq_op {
   int32_t kind;
